@@ -6,7 +6,7 @@ every step's frames are exchanged inside the timed region and the clip is comple
 Prints ONE JSON line on rank 0; DESIGN.md §5 explains every field.  The same line carries, under roofline.extra.configs, short measurements
 of BASELINE configs[1] (render only) and configs[4] (48+48 samples + the torso/background SR head) so that one driver run records them.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 """
 import argparse
@@ -37,7 +37,7 @@ def peaks():
         d = json.load(open(p))
         return {'hbm_gbs': d['hbm_gbs'], 'tf_burst': d['bf16_tflops'], 'tf_sustained': d.get('bf16_tflops_sustained', d['bf16_tflops']),
                 'src': 'measured'}
-    return {'hbm_gbs': 6650.0, 'tf_burst': 1590.0, 'tf_sustained': 1400.0, 'src': 'fallback'}
+    return {'hbm_gbs': 3350.0, 'tf_burst': 989.0, 'tf_sustained': 989.0, 'src': 'H100 SXM data sheet (700 W)'}
 
 
 def ncu_traffic():
@@ -54,7 +54,7 @@ def ncu_traffic():
 
 
 class ClockSampler(threading.Thread):
-    """SM clock / throttle reasons during the timed region (B200_PROFILING.md recipe).  Read through NVML in-process (what nvidia-smi
+    """SM clock / throttle reasons during the timed region.  Read through NVML in-process (what nvidia-smi
     itself calls) every 20 ms: spawning `nvidia-smi` several times a second from a side thread stalled the driver long enough to cost
     the PCIe-bound e2e loop a quarter of its H2D rate.  Falls back to the nvidia-smi query if NVML cannot be loaded."""
     Q = 'clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,' \
@@ -289,6 +289,8 @@ def main():
     ap.add_argument('--no-extra-configs', action='store_true', help='skip the configs[1] / configs[4] mini-benchmarks')
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-graph', action='store_true', help='launch every kernel from Python instead of replaying one CUDA graph per step')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the frames of the last timed step (this rank) as DIR/frames.npy (float32)')
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == 'reference':
@@ -353,8 +355,11 @@ def main():
             exchange_note += 'fell back to the NCCL all-gather'
     eng.prepare(resident)                                                    # one step graph per resident batch: inputs are read in place
 
+    last = {}
+
     def step(i):
-        return eng.step(*resident[i % nb], frame_index=((i - args.warmup) % args.steps) * B if i >= args.warmup else 0)
+        last['frames'] = eng.step(*resident[i % nb], frame_index=((i - args.warmup) % args.steps) * B if i >= args.warmup else 0)
+        return last['frames']
 
     sampler = ClockSampler(local); sampler.start()
     launches0 = L.r3dp_launch_count()
@@ -365,6 +370,10 @@ def main():
     if exchange == 'p2p':
         eng.close_clip()
     fps = world * B * args.steps / (ms / 1e3)
+    if args.dump_outputs:                                                    # before any later run reuses the step's output buffer
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, 'frames.npy'), last['frames'].float().cpu().numpy())
 
     # ---- sustained run: the same loop back to back for --sustain-seconds (power-capped regime)
     sustained = None
@@ -419,7 +428,7 @@ def main():
         us_frame = 1e3 * ms_r / args.steps / B
         extra_cfg['configs[1] render only'] = {
             'value': world * B * args.steps / (ms_r / 1e3), 'unit': 'frames/s (64x64x48 feature images)', 'us_per_frame': us_frame, 'ms_per_step': ms_r / args.steps,
-            'kernel': 'render_stream_kernel (gather || tcgen05 decode || march) + ray generation, limits, depth clamp',
+            'kernel': 'render_stream_kernel (gather || wgmma decode || march) + ray generation, limits, depth clamp',
             'hbm_GBps_algorithmic': RENDER_BYTES_PER_FRAME / (us_frame * 1e-6) / 1e9, 'hbm_frac_of_peak': RENDER_BYTES_PER_FRAME / (us_frame * 1e-6) / 1e9 / peaks()['hbm_gbs'],
             'decoder_TFLOPs_algorithmic': RENDER_GFLOP_PER_FRAME / us_frame * 1e3,
             'note': '26.51 MB / 1.84 GFLOP per frame (SURVEY.md §8d): the HBM floor is loose here, the bound is L2->SM gather traffic + MUFU (DESIGN.md §4)'}
@@ -459,7 +468,7 @@ def main():
             extra_cfg['configs[4] torso+head, 96 samples/ray'] = {
                 'value': world * B / (ms5 / 1e3), 'unit': 'frames/s', 'ms_per_step': ms5, 'ms_per_step_uncached': res5[False],
                 'conv_stack_TFLOPs_algorithmic': WARP_CONV_GFLOP_PER_FRAME * B / res5[False], 'frames_per_step_per_gpu': B,
-                'note': 'render 48+48 (two-pass kernel) + SuperresolutionHybrid8XDC_Warp fuse mode v2 on the tcgen05 conv kernels; torso warper = '
+                'note': 'render 48+48 (two-pass kernel) + SuperresolutionHybrid8XDC_Warp fuse mode v2 on the wgmma conv kernels; torso warper = '
                         'synthetic.StubTorsoModel (the real warper is the caller\'s PyTorch child, out of scope); cached = begin_clip() hoists '
                         'bg_encoder(ref_bg) and the 512->256 resizes (sr_with_ref.py:77-90); TFLOP/s counts the reference\'s 782 GFLOP/frame conv stack over the UNCACHED step'}
             del head5
@@ -472,7 +481,7 @@ def main():
         ex.prepare(resident[:min(nb, 4)])
         kx = max(6, args.steps // 2)
         ms_x = timed_loop(lambda i: ex.step(*resident[i % min(nb, 4)]), kx, 3, barrier, dist, dev) / kx
-        extra_cfg["sr_mode='tc_exact' (fp32-grade SR on tcgen05)"] = {
+        extra_cfg["sr_mode='tc_exact' (fp32-grade SR on wgmma)"] = {
             'value': world * B / (ms_x / 1e3), 'unit': 'frames/s', 'ms_per_step': ms_x,
             'note': 'same step as the headline with split fp16 operands in every SR convolution (x_hi*w_hi + x_lo*w_hi + x_hi*w_lo, fp32 accumulation): '
                     'image within 1e-3*range of the fp32 reference (tests/test_gpu_parity.py::test_sr_full_tc_exact_vs_reference) instead of 2.3e-3 absolute'}
@@ -533,7 +542,7 @@ def main():
     line = {
         'metric': METRIC, 'value': fps, 'unit': 'frames/s', 'n_gpus': world,
         'steps': args.steps, 'warmup': args.warmup, 'ms_per_step': ms / args.steps, 'higher_is_better': True, 'scaling': 'weak',
-        'vs_baseline': None, 'dtype': 'f32 render (decoder GEMMs: split-fp16 operands on tcgen05, f32 accumulate, f32-grade results); SR ' + {'tc': 'f16 operands / f32 accumulate (tcgen05)', 'tc_exact': 'split-f16 operands (3 products) / f32 accumulate (tcgen05), f32-grade results'}.get(sr_mode, 'f32'),
+        'vs_baseline': None, 'dtype': 'f32 render (decoder GEMMs: split-fp16 operands on wgmma, f32 accumulate, f32-grade results); SR ' + {'tc': 'f16 operands / f32 accumulate (wgmma)', 'tc_exact': 'split-f16 operands (3 products) / f32 accumulate (wgmma), f32-grade results'}.get(sr_mode, 'f32'),
         'data': 'synthetic',
         # `config` = the workload (the same keys and values in the reference arm) + the L2 policy / timing statements the timing rules ask for;
         # how this arm runs the workload is under `setup`

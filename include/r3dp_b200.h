@@ -1,5 +1,5 @@
 /*
- * r3dp_b200.h — C ABI of libr3dp_b200.so: the B200 (sm_100a) implementation of Real3D-Portrait's per-frame
+ * r3dp_b200.h — C ABI of libr3dp_b200.so: the H100 (sm_90a) implementation of Real3D-Portrait's per-frame
  * volumetric render + super-resolution hot path.
  *
  * The reference has no C ABI for this path: its boundary is Python `torch.nn.Module.forward` signatures
@@ -43,7 +43,7 @@ typedef struct r3dp_mlp {
 
 int         r3dp_abi_version(void);
 const char* r3dp_last_error(void);
-/* SM count and compute capability of the current device; fails unless it is sm_100. */
+/* SM count and compute capability of the current device; fails unless it is sm_90. */
 int r3dp_device_info(int* sm_count, int* cc_major, int* cc_minor);
 /* Running total of CUDA kernels this library has launched in the process (bench.py's `gpu_launches`). */
 unsigned long long r3dp_launch_count(void);
@@ -109,9 +109,9 @@ int r3dp_decode(const float* feat, int N, int K, int P, int C, const r3dp_mlp_t*
  * (uint8 0/1).  Batch-global quirks are reproduced per call: invalid rays inherit min/max of the valid ray starts
  * (renderer.py:123-126) and depth is clamped to the call-wide [min,max] sample depth (ray_marcher.py:50).
  * workspace: r3dp_render_workspace_bytes(N, M) bytes of scratch.
- * Kernels: single-pass renders (S_imp == 0) run the warp-specialised streaming kernel (render_stream.cu: gather, tcgen05 decoder and
+ * Kernels: single-pass renders (S_imp == 0) run the warp-specialised streaming kernel (render_stream.cu: gather, wgmma decoder and
  * ray march of consecutive 128-sample tiles overlap inside one persistent CTA per SM); importance renders run the CTA-per-ray-tile
- * kernel (render.cu).  Decoder arithmetic: the OSGDecoder GEMMs run on tcgen05 with every fp32 operand split into two fp16 halves (three
+ * kernel (render.cu).  Decoder arithmetic: the OSGDecoder GEMMs run on wgmma with every fp32 operand split into two fp16 halves (three
  * partial products, fp32 accumulation in TMEM) - fp32-grade results (rgb within 2e-6 of the CUDA-core decoder); two-pass shapes whose
  * tiles do not fit use the fp32 CUDA-core decoder.  The prepared decoder operands live in the caller's `workspace`, so calls with
  * different decoders may run concurrently on different streams (each with its own workspace).
@@ -195,8 +195,8 @@ int r3dp_sr_layer_fp32(const float* x, const float* wf, const float* bias, int N
 int r3dp_sr_torgb_fp32(const float* x, const float* wf_rgb, const float* bias, const float* img_in, int N, int I,
                        int H, int W, float* img_out, r3dp_stream_t stream);
 
-/* --------------------------------------------------------------- super-resolution on tensor cores (tcgen05) ---
- * Same layers as above as TMA-fed tcgen05 implicit GEMMs: fp16 operands, fp32 accumulation in TMEM, fp32 epilogue.
+/* --------------------------------------------------------------- super-resolution on tensor cores (wgmma) ------
+ * Same layers as above as TMA-fed wgmma implicit GEMMs: fp16 operands, fp32 accumulation in registers, fp32 epilogue.
  * Activations are NHWC fp16 with channels padded to a multiple of 64; weights are the per-sample folded weights
  * (r3dp_sr_fold_weights) packed to fp16 [Nw][9][O][Ipad] with Nw == N (per-sample styles) or 1 (shared styles).
  * Restrictions (met by SuperresolutionHybrid8XDC): W % 128 == 0, Cout % 128 == 0.
@@ -243,7 +243,7 @@ int r3dp_sr_tc_last_layer_ex(const void* x_f16, const void* wp_f16, const float*
 
 /* ---- fp32-grade tensor-core SR (`sr_mode='tc_exact'`): the same layers with SPLIT fp16 operands ------------------------------------------
  * The reference SR computes in fp32 (networks_stylegan2.py:37-94, conv2d_resample.py:48-145).  These entry points keep that accuracy on
- * tcgen05: every fp32 operand is stored as two fp16 halves v = hi + lo (activations NHWC [N,H,W, 2*Cpad] = [hi | lo]; packed weights
+ * wgmma: every fp32 operand is stored as two fp16 halves v = hi + lo (activations NHWC [N,H,W, 2*Cpad] = [hi | lo]; packed weights
  * [Nw,taps,O, 2*Ipad] = [hi | lo] of w * 2^10) and every convolution accumulates hi*hi + lo*hi + hi*lo in fp32 (three times the MMAs; the
  * dropped lo*lo term is ~2^-22).  Same arguments and meaning as the r3dp_sr_tc_* functions of the same name; tensors are twice as wide. */
 int r3dp_sr_tcx_pack_weights(const float* wf, int Nw, int O, int I, void* packed_f16, r3dp_stream_t stream);

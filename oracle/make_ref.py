@@ -1,11 +1,11 @@
 """Recipe that stages the REFERENCE's own, unmodified Python modules for this path under oracle/_ref/ so that the timed CPU baseline
 (`bench.py --impl reference`, `cpu_baseline`) runs the reference's stock code instead of the oracle port.
 
-    python oracle/make_ref.py            # needs /root/reference (the authoring container); the GPU box only uses the staged files
+    python oracle/make_ref.py            # needs a checkout of the reference (R3DP_REFERENCE); machines without it use the staged files
 
 Nothing is edited: the files are byte-for-byte copies, found as the import closure of the reference classes on the path
 (ImportanceRenderer, RaySampler, OSGDecoder, SuperresolutionHybrid8XDC, SuperresolutionHybrid8XDC_Warp).  oracle/_ref/ is git-ignored
-(reference sources never enter this repository's history) but NOT gpurun-ignored, so it travels to the GPU box with the snapshot.
+(reference sources never enter this repository's history).
 Test infrastructure: only tests/, __graft_entry__ and bench.py's CPU-baseline legs may touch oracle/."""
 import hashlib
 import json

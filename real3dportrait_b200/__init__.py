@@ -1,4 +1,4 @@
-"""real3dportrait_b200 — B200 (sm_100a) implementation of Real3D-Portrait's per-frame volumetric render +
+"""real3dportrait_b200 — H100 (sm_90a) implementation of Real3D-Portrait's per-frame volumetric render +
 super-resolution hot path behind the reference's own module interfaces.
 
 Host side (this package) mirrors the reference classes; all arithmetic is in libr3dp_b200.so (csrc/, C ABI in

@@ -119,7 +119,7 @@ def lib() -> C.CDLL:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f'{LIB_PATH} is missing: build it with `python -m real3dportrait_b200.build` '
-                '(nvcc, sm_100a).  real3dportrait_b200 has no CPU or PyTorch fallback.')
+                '(nvcc, sm_90a).  real3dportrait_b200 has no CPU or PyTorch fallback.')
         L = C.CDLL(LIB_PATH)
         for name, (restype, argtypes) in _SIGNATURES.items():
             fn = getattr(L, name)          # AttributeError here = header and library out of sync

@@ -1,7 +1,7 @@
-"""In-tree build of libr3dp_b200.so (nvcc, sm_100a only).  `python -m real3dportrait_b200.build [--force]`.
+"""In-tree build of libr3dp_b200.so (nvcc, sm_90a only).  `python -m real3dportrait_b200.build [--force]`.
 
 The library is plain CUDA C++ behind a C ABI (include/r3dp_b200.h): no torch headers, no pybind.  nvcc cross-compiles
-without a GPU, so this runs in the authoring container; the built .so travels to the GPU box with the repo snapshot."""
+without a GPU, so the library can be built on a machine without one."""
 from __future__ import annotations
 
 import glob
@@ -16,7 +16,7 @@ LIB_DIR = os.path.join(PKG, 'lib')
 LIB = os.path.join(LIB_DIR, 'libr3dp_b200.so')
 
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+    '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
     '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr',
 ]
 
@@ -58,28 +58,12 @@ def build(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError(f'nvcc failed on {src}:\n{out}')
         if verbose and out:
             print(out)
-    link = [_nvcc(), '-shared', '-o', LIB, *objs, '-gencode', 'arch=compute_100a,code=sm_100a', '-lcudart_static', '-ldl', '-lrt', '-lpthread']
+    link = [_nvcc(), '-shared', '-o', LIB, *objs, '-gencode', 'arch=compute_90a,code=sm_90a', '-lcudart_static', '-ldl', '-lrt', '-lpthread']
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError(f'link failed:\n{r.stdout}')
     return LIB
 
 
-def build_debug_timing() -> str:
-    """lib/libr3dp_b200_dbg.so: the same library with -DR3DP_TC_DEBUG_TIMING=1 (clock64 probes in the conv kernel's MMA and epilogue
-    warps, read by tools/conv_issue_timing.py through R3DP_LIB=<path>).  Never loaded by default."""
-    build()
-    out = os.path.join(LIB_DIR, 'libr3dp_b200_dbg.so')
-    obj = os.path.join(LIB_DIR, 'sr_tc_dbg.o')
-    subprocess.run([_nvcc(), *NVCC_FLAGS, '-DR3DP_TC_DEBUG_TIMING=1', '-c', os.path.join(CSRC, 'sr_tc.cu'), '-o', obj], check=True)
-    objs = [obj] + [os.path.join(LIB_DIR, os.path.basename(s)[:-3] + '.o') for s in sources() if not s.endswith('sr_tc.cu')]
-    subprocess.run([_nvcc(), '-shared', '-o', out, *objs, '-gencode', 'arch=compute_100a,code=sm_100a', '-lcudart_static', '-ldl', '-lrt',
-                    '-lpthread'], check=True)
-    return out
-
-
 if __name__ == '__main__':
-    if '--debug-timing' in sys.argv:
-        print(build_debug_timing())
-    else:
-        print(build(force='--force' in sys.argv, verbose='-v' in sys.argv))
+    print(build(force='--force' in sys.argv, verbose='-v' in sys.argv))

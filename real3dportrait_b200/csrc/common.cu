@@ -19,10 +19,10 @@ void count_launches(int n) { __atomic_fetch_add(&g_launches, (unsigned long long
 int sm_count() {
     static int cached[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     if (cached[dev] == 0) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
         cached[dev] = n;
     }
     return cached[dev];
@@ -44,7 +44,7 @@ extern "C" int r3dp_device_info(int* sm_count, int* cc_major, int* cc_minor) {
     if (sm_count) *sm_count = sms;
     if (cc_major) *cc_major = major;
     if (cc_minor) *cc_minor = minor;
-    R3DP_REQUIRE(major == 10, "libr3dp_b200 is built for sm_100a only; current device is sm_%d%d", major, minor);
+    R3DP_REQUIRE(major == 9 && minor == 0, "libr3dp_b200 is built for sm_90a only; current device is sm_%d%d", major, minor);
     return 0;
 }
 

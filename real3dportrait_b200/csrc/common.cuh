@@ -1,4 +1,4 @@
-// Shared helpers for libr3dp_b200 (sm_100a only).
+// Shared helpers for libr3dp_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -6,8 +6,8 @@
 #include <stdarg.h>
 #include "../../include/r3dp_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libr3dp_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libr3dp_b200 is written for sm_90a (H100) only"
 #endif
 
 namespace r3dp {

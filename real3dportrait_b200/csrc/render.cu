@@ -12,7 +12,7 @@ namespace r3dp {
 
 struct RenderWs;
 __device__ __forceinline__ void init_ws(RenderWs* ws);
-// decoder operand image for tcgen05 (+ the call's workspace header, so that a render needs one set-up launch instead of two)
+// decoder operand image for the tensor cores (+ the call's workspace header, so that a render needs one set-up launch instead of two)
 __global__ void mlp_to_tc_kernel(const r3dp_mlp_t m, MlpTcImage* dst, RenderWs* ws) {
     const int tid = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
     if (tid == 0 && ws != nullptr) init_ws(ws);
@@ -34,8 +34,8 @@ __global__ void mlp_to_tc_kernel(const r3dp_mlp_t m, MlpTcImage* dst, RenderWs* 
     for (int i = tid; i < kHidden; i += nt) dst->b1[i] = m.b1[i];
     for (int i = tid; i < 48; i += nt) dst->b2[i] = i < kOut ? m.b2[i] : 0.f;
 }
-constexpr int kTcThreads = 256;                          // 8 warps: TMEM lane quadrant = warp % 4, column half = warp / 4
-constexpr int kTcMaxTiles = 3;                           // 128-sample tiles per pass (TMEM: 64 columns each)
+constexpr int kTcThreads = 256;                          // 2 warpgroups: warpgroup g takes rows [64 g, 64 g + 64) of every 128-sample tile
+constexpr int kTcMaxTiles = 3;                           // 128-sample tiles per pass
 constexpr int kTcA1Bytes = 51200;                        // 3 x 16 KB A1 tiles; later the [R*ST][33] fp32 decoded rows (<= 384 x 132 B)
 constexpr int kTcA2Bytes = 32768;                        // two 16 KB atoms; before the decode: tap descriptors [nsamp][16]; after: march scratch
 __device__ __forceinline__ void init_ws(RenderWs* ws) {
@@ -106,7 +106,7 @@ __device__ __forceinline__ int ray_of(const RenderArgs& a, int tile, int r) {
 
 // TC = false: decoder weights staged in smem, CUDA-core decoder, two samples per thread (odd shapes that do not fit the tensor-core tiles)
 // (the round-1 constant-bank decoder variants - process-wide state - were removed in round 2; git history keeps them)
-// TC = decoder on tcgen05 (single-pass renders with R*S <= 384; 256 threads, 2 CTAs/SM); see the MlpTcImage comment
+// TC = decoder on wgmma (single-pass renders with R*S <= 384; 256 threads, 2 CTAs/SM); see the MlpTcImage comment
 constexpr int kPfCtas = 32;                            // CTAs of a frame that issue its L2 prefetches
 template <int R, bool TC>
 __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_kernel(const RenderArgs a) {
@@ -120,12 +120,11 @@ __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_ke
     float* cdf = wts + R * ST;                             // [R*ST]          importance cdf
     float* rayf = cdf + R * ST;                            // [R][8]          ox oy oz dx dy dz t0 t1
     int* ord = reinterpret_cast<int*>(rayf + R * 8);       // [R*ST]          depth order of the merged samples
-    // TC layout (1024-aligned): [A1 tiles | decoded rows] [A2 atoms | tap descriptors | march scratch] [W image + biases] dep rayf barriers
+    // TC layout (1024-aligned): [A1 tiles | decoded rows] [A2 atoms | tap descriptors | march scratch] [W image + biases] dep rayf
     uint8_t* a1 = nullptr; uint8_t* a2 = nullptr; uint8_t* wimg = nullptr; float* dsc = nullptr; float* b1s = nullptr; float* b2s = nullptr;
-    uint64_t* bar1 = nullptr; uint64_t* bar2 = nullptr; uint32_t* tmem_slot = nullptr;
     // TC, two passes (importance sampling): the decoded rows of pass 1 must survive pass 2, so they get their own region (and hold the
     // tap descriptors of the samples in flight, like the CUDA-core variants); A2 reuses the (by then consumed) A1 tiles instead:
-    //   [A1 tiles (2) = A2 atoms] [W image + biases] rows dep wts cdf rayf ord barriers
+    //   [A1 tiles (2) = A2 atoms] [W image + biases] rows dep wts cdf rayf ord
     const bool two_pass = TC && a.S_imp > 0;
     if (TC) {
         a1 = tc::align_smem_1024(reinterpret_cast<uint8_t*>(smem));
@@ -139,7 +138,6 @@ __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_ke
             b1s = reinterpret_cast<float*>(wimg + 20480); b2s = b1s + kHidden;
             dep = b2s + 48;
             rayf = dep + R * ST;
-            bar1 = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(a1) + ((reinterpret_cast<uint8_t*>(rayf + R * 8) - a1 + 7) & ~7));
             ord = nullptr;
         } else {
             a2 = a1;
@@ -149,10 +147,7 @@ __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_ke
             dep = rows + R * ST * kRow; wts = dep + R * ST; cdf = wts + R * ST;
             rayf = cdf + R * ST;
             ord = reinterpret_cast<int*>(rayf + R * 8);
-            bar1 = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(a1) + ((reinterpret_cast<uint8_t*>(ord + R * ST) - a1 + 7) & ~7));
         }
-        bar2 = bar1 + kTcMaxTiles;
-        tmem_slot = reinterpret_cast<uint32_t*>(bar2 + kTcMaxTiles);
     }
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -165,27 +160,13 @@ __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_ke
         if (n + a.lookahead < a.N) { prefetch_frame_l2(a.p0, a.H, a.W, n + a.lookahead, tile, kPfCtas); prefetch_frame_l2(a.p1, a.H, a.W, n + a.lookahead, tile, kPfCtas); }
     }
     if (!TC) load_mlp_smem(mlp, a.mlp, tid, kRenderThreads);
-    uint32_t tmem_base = 0;
-    uint32_t tc_par = 0;                                   // bit t = parity of the phase bar1[t] / bar2[t] complete next (one use per pass)
     if (TC) {
-        if (tid == 0) {
-            for (int i = 0; i < kTcMaxTiles; ++i) { tc::mbar_init(&bar1[i], 1); tc::mbar_init(&bar2[i], 1); }
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        if (warp == 0) {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(tmem_slot)), "r"(256) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
         // decoder weight image (pre-swizzled fp16 hi/lo atoms + biases): 20 928 B from L2
         const uint4* src = reinterpret_cast<const uint4*>(a.image);
         uint4* dst = reinterpret_cast<uint4*>(wimg);
         for (int i = tid; i < (int)(sizeof(MlpTcImage) / 16); i += kRenderThreads)       // LDGSTS: lands while the rays / depths / taps are computed
             asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(tc::smem_u32(dst + i)), "l"(src + i) : "memory");
         asm volatile("cp.async.commit_group;" ::: "memory");
-        tc::tc_fence_before();
-        __syncthreads();
-        tc::tc_fence_after();
-        tmem_base = *tmem_slot;
     }
 
     // ---- rays + limits -------------------------------------------------------------------------------------
@@ -289,109 +270,77 @@ __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_ke
             }
         }
         if (TC) {
-            // ---- decoder on the tensor core ---------------------------------------------------------------------------------------------
-            const int nt = (nsamp + 127) >> 7;
-            // barriers t < nt complete once in this pass; a pass with fewer tiles leaves the others untouched, so the parity is kept per
-            // barrier (a wait on the wrong parity of a never-used barrier would fall through)
-            const uint32_t par = tc_par;
-            tc_par ^= (1u << nt) - 1u;
+            // ---- decoder on the tensor core: warpgroup wg computes rows [64 wg, 64 wg + 64) of every 128-sample tile ---------------------
+            const int nt = (nsamp + 127) >> 7, wg = warp >> 2;
             asm volatile("cp.async.wait_group 0;" ::: "memory");                // the weight image has landed
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");        // this thread's A1 (and W) stores -> visible to the async proxy
-            tc::tc_fence_before();
             __syncthreads();
-            const uint32_t a1_s = tc::smem_u32(a1), a2_s = tc::smem_u32(a2), w_s = tc::smem_u32(wimg);
-            if (warp == 0) {                                                   // layer 1 of every tile: 3 partial products x 2 k-steps
-                tc::tc_fence_after();
-                for (int t = 0; t < nt; ++t) {
-                    if (tc::elect_one()) {
-                        uint32_t accum = 0;
+            const uint32_t a1_s = tc::smem_u32(a1) + wg * 8192, a2_s = tc::smem_u32(a2) + wg * 8192, w_s = tc::smem_u32(wimg);
+            auto layer1 = [&](int t, float* acc) {                             // x_hi w_hi + x_lo w_hi + x_hi w_lo, 2 k-steps each
+                uint32_t accum = 0;
 #pragma unroll
-                        for (int term = 0; term < 3; ++term) {
-                            const uint32_t ao = term == 1 ? 64u : 0u, bo = term == 2 ? 64u : 0u;     // x_hi w_hi + x_lo w_hi + x_hi w_lo
+                for (int term = 0; term < 3; ++term) {
+                    const uint32_t ao = term == 1 ? 64u : 0u, bo = term == 2 ? 64u : 0u;
 #pragma unroll
-                            for (int ks = 0; ks < 2; ++ks) {
-                                tc::tc_mma_f16(tmem_base + 64 * t, tc::umma_desc_sw128(a1_s + t * 16384 + ao + ks * 32),
-                                               tc::umma_desc_sw128(w_s + bo + ks * 32), kIdescL1, accum);
-                                accum = 1;
-                            }
-                        }
-                        tc::tc_commit(&bar1[t]);
-                    }
-                    __syncwarp();
-                }
-            }
-            const int qd = warp & 3, g = warp >> 2, trow = qd * 32 + lane;      // TMEM lane quadrant, column half, row of the tile
-            const uint32_t lane_addr = tmem_base + ((uint32_t)(qd * 32) << 16);
-            for (int t = 0; t <= nt; ++t) {
-                if (t < nt) {
-                    tc::mbar_wait(&bar1[t], (par >> t) & 1u);
-                    tc::tc_fence_after();
-                    uint32_t v[32];
-                    tc::tc_ld32(lane_addr + 64 * t + 32 * g, v);                // hidden units [32g, 32g+32) of this sample, pre-activation
-                    uint32_t hi[16], lo[16];
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        const float h0 = softplus_fast(__uint_as_float(v[2 * i]) + b1s[32 * g + 2 * i]);
-                        const float h1 = softplus_fast(__uint_as_float(v[2 * i + 1]) + b1s[32 * g + 2 * i + 1]);
-                        const __half2 hh = __floats2half2_rn(h0, h1);
-                        const float2 hf = __half22float2(hh);
-                        const __half2 ll = __floats2half2_rn(h0 - hf.x, h1 - hf.y);
-                        hi[i] = *reinterpret_cast<const uint32_t*>(&hh); lo[i] = *reinterpret_cast<const uint32_t*>(&ll);
-                    }
-                    if (t >= 1) { tc::mbar_wait(&bar2[t - 1], (par >> (t - 1)) & 1u); tc::tc_fence_after(); }  // layer 2 of the previous tile has read A2
-                    else if (two_pass) tc::mbar_wait(&bar1[nt - 1], (par >> (nt - 1)) & 1u);        // A2 overlays the A1 tiles: every layer-1 MMA must have retired
-                    uint8_t* rp = a2 + (trow >> 3) * 1024 + (trow & 7) * 128;
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        const int off = ((4 * g + c) ^ (trow & 7)) << 4;
-                        *reinterpret_cast<uint4*>(rp + off) = make_uint4(hi[4 * c], hi[4 * c + 1], hi[4 * c + 2], hi[4 * c + 3]);
-                        *reinterpret_cast<uint4*>(rp + 16384 + off) = make_uint4(lo[4 * c], lo[4 * c + 1], lo[4 * c + 2], lo[4 * c + 3]);
-                    }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    tc::tc_fence_before();
-                    __syncthreads();
-                    if (warp == 0) {                                           // layer 2: h_hi w_hi + h_lo w_hi + h_hi w_lo, 4 k-steps each
-                        tc::tc_fence_after();
-                        if (tc::elect_one()) {
-                            uint32_t accum = 0;
-#pragma unroll
-                            for (int term = 0; term < 3; ++term) {
-                                const uint32_t ao = term == 1 ? 16384u : 0u, bo = term == 2 ? (8192u + 6144u) : 8192u;
-#pragma unroll
-                                for (int ks = 0; ks < 4; ++ks) {
-                                    tc::tc_mma_f16(tmem_base + 64 * t, tc::umma_desc_sw128(a2_s + ao + ks * 32),
-                                                   tc::umma_desc_sw128(w_s + bo + ks * 32), kIdescL2, accum);
-                                    accum = 1;
-                                }
-                            }
-                            tc::tc_commit(&bar2[t]);
-                        }
-                        __syncwarp();
+                    for (int ks = 0; ks < 2; ++ks) {
+                        tc::wgmma_m64n64k16(acc, tc::gmma_desc_sw128(a1_s + t * 16384 + ao + ks * 32), tc::gmma_desc_sw128(w_s + bo + ks * 32), accum);
+                        accum = 1;
                     }
                 }
-                if (t >= 1) {
-                    // outputs of tile t-1 (its layer 2 overlapped the epilogue above): bias, sigma raw, colours through the scaled sigmoid
-                    if (t == 1) tc::mbar_wait(&bar1[nt - 1], (par >> (nt - 1)) & 1u);               // rows alias the A1 tiles: every layer-1 MMA must have retired
-                    if (t == nt) tc::mbar_wait(&bar2[nt - 1], (par >> (nt - 1)) & 1u);
-                    tc::tc_fence_after();
-                    uint32_t v[32];
-                    tc::tc_ld32(lane_addr + 64 * (t - 1) + 16 * g, v);
-                    const int sidx = (t - 1) * 128 + trow;
-                    if (sidx < nsamp) {
+            };
+            float h[32], hn[32];                                               // layer-1 accumulators of the current and the next tile
+            tc::wg_fence();
+            layer1(0, h);
+            if (two_pass && nt > 1) layer1(1, hn);                              // A2 overlays the A1 tiles: every layer-1 product is taken first
+            tc::wg_commit();
+            tc::wg_wait<0>();
+            tc::wg_fence_acc<32>(h); tc::wg_fence_acc<32>(hn);
+            for (int t = 0; t < nt; ++t) {
+                // hidden units of tile t: +bias, softplus, re-split into the A2 atoms (row = sample, K = hidden unit)
+#pragma unroll
+                for (int i = 0; i < 32; i += 2) {
+                    const int trow = 64 * wg + tc::acc_row(i), j = tc::acc_col(i);
+                    const float h0 = softplus_fast(h[i] + b1s[j]), h1 = softplus_fast(h[i + 1] + b1s[j + 1]);
+                    const __half2 hh = __floats2half2_rn(h0, h1);
+                    const float2 hf = __half22float2(hh);
+                    const __half2 ll = __floats2half2_rn(h0 - hf.x, h1 - hf.y);
+                    *reinterpret_cast<__half2*>(a2 + sw128_off(trow, j)) = hh;
+                    *reinterpret_cast<__half2*>(a2 + 16384 + sw128_off(trow, j)) = ll;
+                }
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                __syncthreads();
+                float o[24];
+                tc::wg_fence();
+                {                                                              // layer 2: h_hi w_hi + h_lo w_hi + h_hi w_lo, 4 k-steps each
+                    uint32_t accum = 0;
+#pragma unroll
+                    for (int term = 0; term < 3; ++term) {
+                        const uint32_t ao = term == 1 ? 16384u : 0u, bo = term == 2 ? (8192u + 6144u) : 8192u;
+#pragma unroll
+                        for (int ks = 0; ks < 4; ++ks) {
+                            tc::wgmma_m64n48k16(o, tc::gmma_desc_sw128(a2_s + ao + ks * 32), tc::gmma_desc_sw128(w_s + bo + ks * 32), accum);
+                            accum = 1;
+                        }
+                    }
+                }
+                if (!two_pass && t + 1 < nt) layer1(t + 1, hn);                 // A1 tile t+1 is read before the decoded rows of tile t overlay it
+                tc::wg_commit();
+                tc::wg_wait<0>();
+                tc::wg_fence_acc<24>(o); tc::wg_fence_acc<32>(hn);
+                __syncthreads();                                               // both warpgroups are done reading A2 and A1 tile t+1
+                // outputs of tile t: bias, sigma raw, colours through the scaled sigmoid
+#pragma unroll
+                for (int i = 0; i < 24; ++i) {
+                    const int sidx = t * 128 + 64 * wg + tc::acc_row(i), oc = tc::acc_col(i);
+                    if (oc < kOut && sidx < nsamp) {
                         const int r = sidx / kn, k = k0 + (sidx - r * kn);
                         float* out = rows + (size_t)(r * ST + k) * kRow;
-                        if (g == 0) {
-                            out[0] = __uint_as_float(v[0]) + b2s[0];
-#pragma unroll
-                            for (int o = 1; o < 16; ++o) out[o] = sigmoid_fast(__uint_as_float(v[o]) + b2s[o]) * 1.002f - 0.001f;
-                        } else {
-#pragma unroll
-                            for (int o = 16; o < kOut; ++o) out[o] = sigmoid_fast(__uint_as_float(v[o - 16]) + b2s[o]) * 1.002f - 0.001f;
-                        }
+                        out[oc] = oc == 0 ? o[i] + b2s[0] : sigmoid_fast(o[i] + b2s[oc]) * 1.002f - 0.001f;
                     }
                 }
+#pragma unroll
+                for (int i = 0; i < 32; ++i) h[i] = hn[i];
             }
-            tc::tc_fence_before();
             __syncthreads();
             return;
         }
@@ -530,14 +479,6 @@ __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_ke
     // call-wide min/max of the sample depths (ray_marcher.py:50)
     dmin = warp_min(dmin); dmax = warp_max(dmax);
     if (lane == 0 && dmin <= dmax) { atomicMin(&a.ws->d_min, f2ord(dmin)); atomicMax(&a.ws->d_max, f2ord(dmax)); }
-    if (TC) {
-        tc::tc_fence_before();
-        __syncthreads();
-        if (warp == 0) {
-            tc::tc_fence_after();
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256) : "memory");
-        }
-    }
 }
 
 // Stand-alone marcher: one warp per ray, lane = channel (C <= 32 per pass, loops for wider C).
@@ -584,11 +525,11 @@ static int mlp_variant() {                         // R3DP_MLP = tc (default) | 
 
 static size_t render_tc_smem(int R, int S, int S_imp) {
     const int ST = S + S_imp;
-    if (S_imp == 0) return 1024 + kTcA1Bytes + kTcA2Bytes + 20480 + (kHidden + 48) * 4 + (size_t)R * (S + 8) * 4 + 8 + 2 * kTcMaxTiles * 8 + 16;
-    return 1024 + kTcA2Bytes + 20480 + (kHidden + 48) * 4 + (size_t)R * ST * (kRow + 4) * 4 + (size_t)R * 8 * 4 + 8 + 2 * kTcMaxTiles * 8 + 16;
+    if (S_imp == 0) return 1024 + kTcA1Bytes + kTcA2Bytes + 20480 + (kHidden + 48) * 4 + (size_t)R * (S + 8) * 4;
+    return 1024 + kTcA2Bytes + 20480 + (kHidden + 48) * 4 + (size_t)R * ST * (kRow + 4) * 4 + (size_t)R * 8 * 4;
 }
 // the tensor-core decoder needs its CTA tile to fit the A tiles: three 128-sample tiles for single-pass renders (decoded rows overlay
-// them), two per pass for importance renders; and two CTAs per SM (TMEM: 2 x 256 columns)
+// them), two per pass for importance renders; and two CTAs per SM (2 x 113 KB of shared memory)
 static bool render_tc_fits(int R, int S, int S_imp) {
     if (S_imp == 0) return R * S <= 128 * kTcMaxTiles && R * S * kRow * 4 <= kTcA1Bytes;
     const int per_pass = R * (S > S_imp ? S : S_imp);
@@ -615,7 +556,7 @@ static int launch_render_v(const RenderArgs& a, cudaStream_t st) {
 }
 template <int R>
 static int launch_render(const RenderArgs& a, cudaStream_t st) {
-    // tcgen05 decoder when the tile fits, else the smem-weights CUDA-core decoder; both keep the decoder in per-call storage
+    // tensor-core decoder when the tile fits, else the smem-weights CUDA-core decoder; both keep the decoder in per-call storage
     const bool grid_single = a.p0.depth > 1 && a.S_imp == 0;      // tri-grid descriptors (27 floats) do not fit the single-pass [nsamp][16] layout
     if (mlp_variant() == 2 && !grid_single && render_tc_fits(R, a.S, a.S_imp)) return launch_render_tc<R>(a, st);
     return launch_render_v<R>(a, st);

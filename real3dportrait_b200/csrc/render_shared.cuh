@@ -1,6 +1,6 @@
 // Structures shared by the two fused-render translation units:
 //   render.cu         entry points, limits / clamp kernels, the CTA-per-ray-tile kernel (two-pass importance renders, odd shapes)
-//   render_stream.cu  the warp-specialised streaming kernel (single-pass renders: gather || tcgen05 decode || march overlap)
+//   render_stream.cu  the warp-specialised streaming kernel (single-pass renders: gather || wgmma decode || march overlap)
 #pragma once
 #include "render_core.cuh"
 #include "tc_prims.cuh"
@@ -8,14 +8,14 @@
 namespace r3dp {
 
 // ---- tensor-core decoder operand image --------------------------------------------------------------------------------------------
-// The OSG decoder is two GEMMs over the samples: [M x 32] x [32 x 64] -> softplus -> [M x 64] x [64 x 33].  They run on tcgen05 with
-// fp16 operands and fp32 accumulation in TMEM; fp32 accuracy is kept by splitting every operand into two fp16 halves
+// The OSG decoder is two GEMMs over the samples: [M x 32] x [32 x 64] -> softplus -> [M x 64] x [64 x 33].  They run on wgmma with
+// fp16 operands and fp32 accumulation in registers; fp32 accuracy is kept by splitting every operand into two fp16 halves
 // (v = hi + lo exactly to 2^-22 |v|) and summing the three significant partial products hi*hi + lo*hi + hi*lo (lo*lo ~ 2^-22 is dropped).
 // Operand images (K-major, 128-byte swizzle: one 128 B row = 64 fp16, 8-row groups 1024 B apart):
 //   A1 tile  128 samples x [x_hi(32) | x_lo(32)]             written by the gather
 //   W1       64 hidden   x [w_hi(32) | w_lo(32)]             k-steps 0,1 = hi, 2,3 = lo
 //   A2 tile  128 samples x [h_hi(64)] , [h_lo(64)]           two atoms, written by the layer-1 epilogue
-//   W2       48 outputs  x [w_hi(64)] , [w_lo(64)]           two atoms, rows >= 33 are zero (UMMA N must be a multiple of 16)
+//   W2       48 outputs  x [w_hi(64)] , [w_lo(64)]           two atoms, rows >= 33 are zero (N = 48: a multiple of 16)
 struct alignas(16) MlpTcImage {
     uint8_t w1[kHidden * 128];
     uint8_t w2hi[48 * 128];
@@ -24,9 +24,6 @@ struct alignas(16) MlpTcImage {
     float b2[48];
 };
 static_assert(sizeof(MlpTcImage) == 8192 + 6144 + 6144 + 256 + 192, "MlpTcImage layout");
-
-constexpr uint32_t kIdescL1 = (1u << 4) | ((uint32_t)(kHidden >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);    // M128 N64, f16 x f16 -> f32
-constexpr uint32_t kIdescL2 = (1u << 4) | ((uint32_t)(48 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);         // M128 N48
 
 __device__ __forceinline__ uint32_t sw128_off(int row, int k) {                // byte offset of fp16 element (row, k) of a swizzled atom
     return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((((k >> 3) ^ (row & 7))) << 4) + (k & 7) * 2);
@@ -64,14 +61,14 @@ struct RenderArgs {
     int S, S_imp; float box_warp; int white_back;
     const float* u_coarse; const float* u_fine;
     r3dp_mlp_t mlp;
-    const MlpTcImage* image;            // tcgen05 decoder operands (workspace)
+    const MlpTcImage* image;            // tensor-core decoder operands (workspace)
     float* rgb; float* depth; float* wsum;
     const float2* limits; const uint8_t* valid; RenderWs* ws;
     int tiles_per_frame, tile_cols;     // ray tiling of the CTA-per-tile kernel (see ray_of)
     int lookahead;                      // frames of planes streamed DRAM -> L2 ahead of the gather (0 = off)
 };
 
-// DRAM -> L2 prefetch of one frame's planes: share `part` of `parts` (32 KB chunks, round-robin).  ncu (profiles/r2_render_ab.md): the gather is
+// DRAM -> L2 prefetch of one frame's planes: share `part` of `parts` (32 KB chunks, round-robin).  The gather is
 // latency-bound - a warp iteration waits for the slowest of its 48 texel lines, and with cold planes one of them nearly always comes from
 // DRAM.  The TMA unit streams the planes into L2 ahead of the demand loads, which then pay the L2 latency only.
 __device__ __forceinline__ void prefetch_frame_l2(const PlaneSet& ps, int H, int W, int n, int part, int parts) {
@@ -140,26 +137,10 @@ __device__ __forceinline__ void sample_desc(const PlaneSet& ps, int H, int W, fl
     }
 }
 
-// ---- packed 2 x fp32 arithmetic (sm_100 f32x2: one issue slot for two values) and the decoder activations on top of it ----------------------
-__device__ __forceinline__ float2 pk_fma(float2 a, float2 b, float2 c) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rc;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\t"
-        "fma.rn.f32x2 rc, ra, rb, rc;\n\tmov.b64 {%0, %1}, rc;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-    return d;
-}
-__device__ __forceinline__ float2 pk_mul(float2 a, float2 b) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rc;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmul.rn.f32x2 rc, ra, rb;\n\tmov.b64 {%0, %1}, rc;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-    return d;
-}
-__device__ __forceinline__ float2 pk_add(float2 a, float2 b) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rc;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tadd.rn.f32x2 rc, ra, rb;\n\tmov.b64 {%0, %1}, rc;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-    return d;
-}
+// ---- 2 x fp32 arithmetic on value pairs and the decoder activations on top of it --------------------------------------------------------
+__device__ __forceinline__ float2 pk_fma(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 pk_mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 pk_add(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float lg2_approx(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
@@ -179,7 +160,7 @@ __device__ __forceinline__ float2 sigmoid_scaled2(float2 x) {
 }
 
 // tri-plane descriptor in the split layout of the streaming kernel: row[0..2] = the three texel-block offsets, row[4 + 8p .. 11 + 8p] = the four
-// weights of plane p, each stored TWICE (w0 w0 w1 w1 w2 w2 w3 w3) so that one LDS.128 yields two aligned (w,w) pairs for packed f32x2 FMAs
+// weights of plane p, each stored TWICE (w0 w0 w1 w1 w2 w2 w3 w3) so that one LDS.128 yields two aligned (w,w) pairs for float2 FMAs
 __device__ __forceinline__ void sample_desc_split(const PlaneSet& ps, int H, int W, float gx, float gy, float gz, float* row) {
     float t[5];
     tap_desc_s(gx, gy, H, W, 0, ps.row_stride, ps.texel_stride, t);

@@ -1,20 +1,20 @@
 // Streaming fused renderer for single-pass renders (ImportanceRenderer.forward with depth_resolution_importance == 0,
-// renderer.py:118-167): one PERSISTENT, warp-specialised CTA per SM in which the tri-plane gather, the OSG decoder on tcgen05 and the
+// renderer.py:118-167): one PERSISTENT, warp-specialised CTA per SM in which the tri-plane gather, the OSG decoder on wgmma and the
 // ray march of consecutive sample tiles overlap instead of alternating.
 //
 // Work item   = a group of G rays of one frame (G rows of one image column when the rays form an image: planes 1 and 2 are indexed by
 //               (x,z)/(z,x) only, so these rays walk the same texels), streamed front to back in depth chunks of D = 128/G samples per ray.
-// Tile        = the G x D = 128 samples of one chunk = one UMMA M-tile; row = ray_local * D + k_local.
-// Roles (17 warps = 4 whole warpgroups + the MMA warp, mbarrier hand-offs, every ring is filled and drained in tile order):
-//   decode  x4  TMEM -> +bias, softplus (packed f32x2) -> re-split into the A2 atoms; TMEM -> +bias, scaled sigmoid -> fp32 rows (2-deep ring)
+// Tile        = the G x D = 128 samples of one chunk = two 64-row wgmma tiles; row = ray_local * D + k_local.
+// Roles (16 warps = 4 whole warpgroups, mbarrier hand-offs, every ring is filled and drained in tile order):
+//   decode  x4  one warpgroup: layer 1 A1 x W1 (3 partial products x 2 k-steps, M64 N64 K16, twice) -> +bias, softplus -> re-split into the
+//               A2 atoms; layer 2 A2 x W2 (3 x 4, M64 N48) -> +bias, scaled sigmoid -> fp32 rows (2-deep ring)
 //   march   x4  MipRayMarcher2 (ray_marcher.py:26-57) incrementally: alpha / transmittance once per sample (lane = tile row, segmented product
 //               scan), colours with lane = channel; accumulators live in registers across the tiles of an item; only the final [32] features,
-//               weight sum and depth leave the SM.  setmaxnreg: 48 registers
+//               weight sum and depth leave the SM
 //   gather  x8  sample depths (renderer.py:223-226) -> positions -> bilinear tap descriptors (smem) -> all 12 x LDG.128 of a sample in flight ->
-//               packed FMAs -> mean feature as fp16 hi|lo halves straight into the swizzled A1 stage (3-stage ring); depths into a small ring
-//               for the marcher; L2 look-ahead prefetch of the next frames' planes.  setmaxnreg: 120 registers
-//   mma     x1  layer 1: A1 x W1 (3 partial products x 2 k-steps, M128 N64 K16) -> TMEM; layer 2: A2 x W2 (3 x 4, M128 N48) -> TMEM
-// Decoder arithmetic is the split-fp16 scheme of render_shared.cuh (fp32-grade results).  Measured history and ncu tables: profiles/r2_render_ab.md.
+//               FMAs -> mean feature as fp16 hi|lo halves straight into the swizzled A1 stage (3-stage ring); depths into a small ring
+//               for the marcher; L2 look-ahead prefetch of the next frames' planes
+// Decoder arithmetic is the split-fp16 scheme of render_shared.cuh (fp32-grade results).
 #include "render_shared.cuh"
 #include <stdlib.h>
 
@@ -24,14 +24,10 @@ int g_rs_prefetch = -1;                                           // frames of L
 namespace rs {
 
 constexpr int kGatherWarps = 8;
-// warps 0-3 decode (TMEM lane quadrant = warp), 4-7 march, 8-15 gather, 16 MMA: every role is a whole warpgroup (4 aligned warps), so the
-// register file can be re-split with setmaxnreg - the march warps give up registers, the gather warps take them to keep all twelve
-// 16-byte loads of a sample in flight (at the launch-wide 96 ptxas split them into four dependent groups)
+// warps 0-3 decode (the warpgroup that issues the MMAs and holds their accumulators), 4-7 march, 8-15 gather.  512 threads leave 128
+// registers per thread, enough for the gather warps to keep all twelve 16-byte loads of a sample in flight
 constexpr int kFirstGather = 8;
-constexpr int kMmaWarp = kFirstGather + kGatherWarps;
-constexpr int kThreads = (kMmaWarp + 1) * 32;                   // 544
-#define R3DP_RS_REGS_MARCH "48"
-#define R3DP_RS_REGS_GATHER "120"
+constexpr int kThreads = (kFirstGather + kGatherWarps) * 32;    // 512
 constexpr int NS = 3;                                           // A1 stages
 constexpr int NR = 2;                                           // decoded-row buffers
 constexpr int ND = 8;                                           // depth ring slots
@@ -50,25 +46,11 @@ constexpr int kSmem = kOffBar + 512 + 1024;                     // + alignment s
 
 struct Bars {
     uint64_t a1_full[NS], a1_empty[NS];
-    uint64_t l1_done[2], l2_done[2], acc2_empty[2];
-    uint64_t a2_full;
     uint64_t rows_full[NR], rows_empty[NR];
     uint64_t dep_empty[ND], dep_full[ND];
-    uint32_t tmem_slot;
 };
 static_assert(sizeof(Bars) <= 512, "barrier block");
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* b) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(b)) : "memory");
-}
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+using tc::mbar_arrive;
 
 template <int LOG2D>
 __device__ __forceinline__ int ray_index(const RenderArgs& a, int grp, int r) {
@@ -102,16 +84,10 @@ __global__ void __launch_bounds__(kThreads, 1) render_stream_kernel(const Render
     const uint32_t total_tiles = (uint32_t)(my_items * NT);
 
     if (tid == 0) {
-        for (int i = 0; i < NS; ++i) { tc::mbar_init(&B.a1_full[i], kGatherWarps); tc::mbar_init(&B.a1_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { tc::mbar_init(&B.l1_done[i], 1); tc::mbar_init(&B.l2_done[i], 1); tc::mbar_init(&B.acc2_empty[i], 4); }
-        tc::mbar_init(&B.a2_full, 4);
+        for (int i = 0; i < NS; ++i) { tc::mbar_init(&B.a1_full[i], kGatherWarps); tc::mbar_init(&B.a1_empty[i], 4); }
         for (int i = 0; i < NR; ++i) { tc::mbar_init(&B.rows_full[i], 4); tc::mbar_init(&B.rows_empty[i], 4); }
         for (int i = 0; i < ND; ++i) { tc::mbar_init(&B.dep_empty[i], 4); tc::mbar_init(&B.dep_full[i], kGatherWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == kMmaWarp) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(&B.tmem_slot)), "r"(256) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     {   // decoder operand image (pre-swizzled fp16 hi/lo atoms + biases) from the call's workspace
         const uint4* src = reinterpret_cast<const uint4*>(a.image);
@@ -122,14 +98,10 @@ __global__ void __launch_bounds__(kThreads, 1) render_stream_kernel(const Render
         asm volatile("cp.async.wait_group 0;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = B.tmem_slot;
 
-    if (warp >= kFirstGather && warp < kMmaWarp) {
+    if (warp >= kFirstGather) {
         // ===================================================== gather ===========================================================
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 " R3DP_RS_REGS_GATHER ";");
         constexpr int RPW = kSPW >> LOG2D;                                      // rays per gather warp
         static_assert(RPW >= 1, "D must not exceed the samples of one gather warp");
         const int gw = warp - kFirstGather, sub = lane >> 3, cq = lane & 7;
@@ -246,112 +218,85 @@ __global__ void __launch_bounds__(kThreads, 1) render_stream_kernel(const Render
         // call-wide min/max of the sample depths (ray_marcher.py:50)
         dmin = warp_min(dmin); dmax = warp_max(dmax);
         if (lane == 0 && dmin <= dmax) { atomicMin(&a.ws->d_min, f2ord(dmin)); atomicMax(&a.ws->d_max, f2ord(dmax)); }
-    } else if (warp == kMmaWarp) {
-        // ======================================================= MMA ============================================================
+    } else if (warp < 4) {
+        // ====================================================== decode ==========================================================
         const uint32_t a2_s = tc::smem_u32(a2), w_s = tc::smem_u32(wimg);
-        auto issue_l2 = [&](uint32_t p) {                                      // h_hi w_hi + h_lo w_hi + h_hi w_lo, 4 k-steps each
-            tc::mbar_wait(&B.a2_full, p & 1u);
-            tc::mbar_wait(&B.acc2_empty[p & 1u], ((p >> 1) & 1u) ^ 1u);
-            tc::tc_fence_after();
-            const uint32_t acc = tmem_base + 128u * (p & 1u) + 64u;
-            if (tc::elect_one()) {
-                uint32_t accum = 0;
-#pragma unroll
-                for (int term = 0; term < 3; ++term) {
-                    const uint32_t ao = term == 1 ? 16384u : 0u, bo = term == 2 ? (8192u + 6144u) : 8192u;
-#pragma unroll
-                    for (int ks = 0; ks < 4; ++ks) {
-                        tc::tc_mma_f16(acc, tc::umma_desc_sw128(a2_s + ao + ks * 32), tc::umma_desc_sw128(w_s + bo + ks * 32), kIdescL2, accum);
-                        accum = 1;
-                    }
-                }
-                tc::tc_commit(&B.l2_done[p & 1u]);
-            }
-            __syncwarp();
-        };
         for (uint32_t q = 0; q < total_tiles; ++q) {
-            if (q >= 1) issue_l2(q - 1);
             const uint32_t stage = q % NS;
             tc::mbar_wait(&B.a1_full[stage], (q / NS) & 1u);
-            tc::tc_fence_after();
             const uint32_t a1_s = tc::smem_u32(a1) + stage * 16384u;
-            const uint32_t acc = tmem_base + 128u * (q & 1u);
-            if (tc::elect_one()) {                                            // x_hi w_hi + x_lo w_hi + x_hi w_lo, 2 k-steps each
+            float h[2][32];                                                    // tile rows [0, 64) and [64, 128)
+            tc::wg_fence();
+#pragma unroll
+            for (int b = 0; b < 2; ++b) {                                      // x_hi w_hi + x_lo w_hi + x_hi w_lo, 2 k-steps each
                 uint32_t accum = 0;
 #pragma unroll
                 for (int term = 0; term < 3; ++term) {
                     const uint32_t ao = term == 1 ? 64u : 0u, bo = term == 2 ? 64u : 0u;
 #pragma unroll
                     for (int ks = 0; ks < 2; ++ks) {
-                        tc::tc_mma_f16(acc, tc::umma_desc_sw128(a1_s + ao + ks * 32), tc::umma_desc_sw128(w_s + bo + ks * 32), kIdescL1, accum);
+                        tc::wgmma_m64n64k16(h[b], tc::gmma_desc_sw128(a1_s + b * 8192 + ao + ks * 32), tc::gmma_desc_sw128(w_s + bo + ks * 32), accum);
                         accum = 1;
                     }
                 }
-                tc::tc_commit(&B.l1_done[q & 1u]);
-                tc::tc_commit(&B.a1_empty[stage]);
             }
+            tc::wg_commit();
+            tc::wg_wait<0>();
+            tc::wg_fence_acc<32>(h[0]); tc::wg_fence_acc<32>(h[1]);
             __syncwarp();
-        }
-        if (total_tiles) issue_l2(total_tiles - 1);
-    } else if (warp < 4) {
-        // ====================================================== decode ==========================================================
-        const int qd = warp, trow = qd * 32 + lane;
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(qd * 32) << 16);
-        auto epi2 = [&](uint32_t p) {                                          // outputs of tile p: sigma raw, colours through the scaled sigmoid
-            tc::mbar_wait(&B.l2_done[p & 1u], (p >> 1) & 1u);
-            tc::tc_fence_after();
-            uint32_t v[32], v2[16];
-            tc::tc_ld32(lane_addr + 128u * (p & 1u) + 64u, v);
-            tc_ld16(lane_addr + 128u * (p & 1u) + 96u, v2);
-            tc::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&B.acc2_empty[p & 1u]);
-            const uint32_t rb = p % NR;
-            tc::mbar_wait(&B.rows_empty[rb], ((p / NR) & 1u) ^ 1u);
-            float* out = rows + (rb * 128 + trow) * kRowF;
-            out[0] = __uint_as_float(v[0]) + b2s[0];
+            if (lane == 0) mbar_arrive(&B.a1_empty[stage]);
+            // hidden units: +bias, softplus, re-split into the A2 atoms (row = sample of the tile, K = hidden unit)
 #pragma unroll
-            for (int o = 1; o < 33; o += 2) {                                  // outputs 1..32 in pairs (o, o+1); output 32 comes from the second TMEM load
-                const float x1 = o + 1 < 32 ? __uint_as_float(v[o + 1]) : __uint_as_float(v2[0]);
-                const float2 sg = sigmoid_scaled2(pk_add(make_float2(__uint_as_float(v[o]), x1), make_float2(b2s[o], b2s[o + 1])));
-                out[o] = sg.x; out[o + 1] = sg.y;
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&B.rows_full[rb]);
-        };
-        for (uint32_t q = 0; q < total_tiles; ++q) {
-            tc::mbar_wait(&B.l1_done[q & 1u], (q >> 1) & 1u);
-            tc::tc_fence_after();
-            uint8_t* rp = a2 + (trow >> 3) * 1024 + (trow & 7) * 128;
+            for (int b = 0; b < 2; ++b)
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                uint32_t v[32];
-                tc::tc_ld32(lane_addr + 128u * (q & 1u) + 32u * h, v);           // hidden units [32h, 32h+32) of this sample, pre-activation
-                uint32_t hi[16], lo[16];
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float2 bb = *reinterpret_cast<const float2*>(b1s + 32 * h + 2 * i);
-                    const float2 hv = softplus2(pk_add(make_float2(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1])), bb));
+                for (int i = 0; i < 32; i += 2) {
+                    const int trow = 64 * b + tc::acc_row(i), j = tc::acc_col(i);
+                    const float2 bb = *reinterpret_cast<const float2*>(b1s + j);
+                    const float2 hv = softplus2(pk_add(make_float2(h[b][i], h[b][i + 1]), bb));
                     const __half2 hh = __floats2half2_rn(hv.x, hv.y);
                     const float2 hf = __half22float2(hh);
                     const __half2 ll = __floats2half2_rn(hv.x - hf.x, hv.y - hf.y);
-                    hi[i] = *reinterpret_cast<const uint32_t*>(&hh); lo[i] = *reinterpret_cast<const uint32_t*>(&ll);
+                    *reinterpret_cast<__half2*>(a2 + sw128_off(trow, j)) = hh;
+                    *reinterpret_cast<__half2*>(a2 + 16384 + sw128_off(trow, j)) = ll;
                 }
-                if (h == 0 && q >= 1) tc::mbar_wait(&B.l2_done[(q - 1) & 1u], ((q - 1) >> 1) & 1u);     // layer 2 of the previous tile has read A2
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            asm volatile("bar.sync 1, 128;" ::: "memory");                      // the whole A2 tile is written
+            float o[2][24];
+            tc::wg_fence();
 #pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    const int off = ((4 * h + c) ^ (trow & 7)) << 4;
-                    *reinterpret_cast<uint4*>(rp + off) = make_uint4(hi[4 * c], hi[4 * c + 1], hi[4 * c + 2], hi[4 * c + 3]);
-                    *reinterpret_cast<uint4*>(rp + 16384 + off) = make_uint4(lo[4 * c], lo[4 * c + 1], lo[4 * c + 2], lo[4 * c + 3]);
+            for (int b = 0; b < 2; ++b) {                                      // h_hi w_hi + h_lo w_hi + h_hi w_lo, 4 k-steps each
+                uint32_t accum = 0;
+#pragma unroll
+                for (int term = 0; term < 3; ++term) {
+                    const uint32_t ao = term == 1 ? 16384u : 0u, bo = term == 2 ? (8192u + 6144u) : 8192u;
+#pragma unroll
+                    for (int ks = 0; ks < 4; ++ks) {
+                        tc::wgmma_m64n48k16(o[b], tc::gmma_desc_sw128(a2_s + b * 8192 + ao + ks * 32), tc::gmma_desc_sw128(w_s + bo + ks * 32), accum);
+                        accum = 1;
+                    }
                 }
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            tc::tc_fence_before();
+            tc::wg_commit();
+            tc::wg_wait<0>();
+            tc::wg_fence_acc<24>(o[0]); tc::wg_fence_acc<24>(o[1]);
+            asm volatile("bar.sync 1, 128;" ::: "memory");                      // every warp's layer 2 has read A2 before the next tile rewrites it
+            // outputs: sigma raw, colours through the scaled sigmoid
+            const uint32_t rb = q % NR;
+            tc::mbar_wait(&B.rows_empty[rb], ((q / NR) & 1u) ^ 1u);
+#pragma unroll
+            for (int b = 0; b < 2; ++b)
+#pragma unroll
+                for (int i = 0; i < 24; i += 2) {
+                    const int trow = 64 * b + tc::acc_row(i), oc = tc::acc_col(i);
+                    float* out = rows + (rb * 128 + trow) * kRowF;
+                    const float2 sg = sigmoid_scaled2(pk_add(make_float2(o[b][i], o[b][i + 1]), *reinterpret_cast<const float2*>(b2s + oc)));
+                    if (oc == 0) out[0] = o[b][i] + b2s[0];
+                    else if (oc < kOut) out[oc] = sg.x;
+                    if (oc + 1 < kOut) out[oc + 1] = sg.y;
+                }
             __syncwarp();
-            if (lane == 0) mbar_arrive(&B.a2_full);
-            if (q >= 1) epi2(q - 1);
+            if (lane == 0) mbar_arrive(&B.rows_full[rb]);
         }
-        if (total_tiles) epi2(total_tiles - 1);
     } else {
         // ====================================================== march ===========================================================
         // ray_marcher.py:26-57, front to back over the tiles of an item.  Warp mw owns RM = G/4 rays = the 32 tile rows [32 mw, 32 mw + 32).
@@ -359,7 +304,6 @@ __global__ void __launch_bounds__(kThreads, 1) render_stream_kernel(const Render
         //            segmented product scan over the ray's D lanes times the value carried from the previous tile - one softplus / exp per sample,
         //            not one per sample and colour channel;
         //   colours  lane = channel: 32 (ray, sample) pairs per tile, each weight broadcast by a shuffle; acc += w * mid-point colour.
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 " R3DP_RS_REGS_MARCH ";");
         constexpr int RM = G / 4;
         static_assert(RM * D == 32, "one warp marches 32 tile rows");
         const int mw = warp - 4, lj = lane & (D - 1), seg_last = lane | (D - 1);
@@ -422,12 +366,6 @@ __global__ void __launch_bounds__(kThreads, 1) render_stream_kernel(const Render
                 }
             }
         }
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == kMmaWarp) {
-        tc::tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256) : "memory");
     }
 }
 

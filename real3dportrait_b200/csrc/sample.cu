@@ -87,7 +87,7 @@ __global__ void __launch_bounds__(256, 3) trigrid_sample_kernel(const float* __r
 // (zero padding folded into the weights: no bounds checks, no predicated loads) into a 2 KB shared-memory block; then 8 steps of 4 points,
 // 8 lanes x float4 = one 128-byte texel line per tap, ALL twelve 16-byte loads of a point issued before the first use, streaming stores
 // (the output is never re-read here).  The coordinates of the next chunk are requested before this chunk's taps.
-// ncu history (profiles/r2_sample_op.md): descriptors recomputed by all 8 lanes of a point + loads split into dependent groups at 64
+// Earlier forms: descriptors recomputed by all 8 lanes of a point + loads split into dependent groups at 64
 // registers -> 59 % of the HBM peak with 60 % issue-active; MINB = resident CTAs per SM the register allocation targets.
 template <int MINB>
 __global__ void __launch_bounds__(256, MINB) triplane_sample_kernel(const float* __restrict__ planes, int N, int H, int W,

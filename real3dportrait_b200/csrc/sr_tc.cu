@@ -1,15 +1,14 @@
-// Tensor-core super-resolution path for sm_100a: the modulated 3x3 convolutions of SuperresolutionHybrid8XDC (197.6 GFLOP/frame,
-// SURVEY.md §8d) and the plain convolutions of the torso head as TMA-fed tcgen05 implicit GEMMs.
+// Tensor-core super-resolution path for sm_90a: the modulated 3x3 convolutions of SuperresolutionHybrid8XDC (197.6 GFLOP/frame,
+// SURVEY.md §8d) and the plain convolutions of the torso head as TMA-fed wgmma implicit GEMMs.
 //
 //   activations  NHWC fp16, channels padded to a multiple of 64 (one 128-byte swizzle row = 64 channels)
 //   weights      per-sample folded (modulated+demodulated) fp16, packed [n][tap][Cout][Cin_pad]  (K-major B operand)
-//   accumulate   fp32 in TMEM; epilogue in fp32 (bias, lrelu*sqrt2, ToRGB + skip) then fp16 / fp32 stores
+//   accumulate   fp32 in registers; epilogue in fp32 (bias, lrelu*sqrt2, ToRGB + skip) then fp16 / fp32 stores
 //
-// The conv kernel (conv_tc3_kernel): persistent CTA PAIRS (cta_group::2): M256 x N128 x K16 MMAs, half weight tile per CTA, A row strips
-// reused by the horizontal taps through row-shifted descriptors, double-buffered TMEM accumulators, 8 epilogue warps.  (Its two
-// predecessors - one tile per CTA, and the same persistent design on single CTAs - were removed in round 2; see git history.)
+// The conv kernel (conv_tc3_kernel): persistent CTAs, M64 x N128 x K16 warpgroup MMAs (two consumer warpgroups = 128 pixels), A row strips
+// reused by the horizontal taps through row-shifted descriptors and by the R output rows of a tile.
 // The im2col is done by TMA itself: every (tap, 64-channel chunk) of the K loop is a box load at the tap's shifted
-// coordinates, zero-filled outside the image (= the conv's zero padding); one elected lane issues the MMAs.
+// coordinates, zero-filled outside the image (= the conv's zero padding).
 //
 // The stride-2 transposed convolution of the up layers (conv2d_resample.py:116-133) keeps the reference's operation order for large Cin:
 // four output-parity phases (4/2/2/1 taps) as units of ONE launch -> (2H+1)x(2W+1) fp16 result -> fir_tma_kernel (TMA-staged 4x4 FIR +
@@ -27,11 +26,9 @@
 namespace r3dp {
 namespace tc {
 
-constexpr int BM = 128, BN = 128, BK = 64, UMMA_K = 16;
+constexpr int BM = 128, BN = 128, BK = 64;
 constexpr float kSplitWeightScale = 1024.0f;       // split-fp16 weights are stored x 2^10: their lo halves (|w| 2^-11) stay normal fp16 numbers
 
-// kind::f16 instruction descriptor: D=f32 (bit 4), A=B=f16 (0), both K-major, N>>3 at [17,23), M>>4 at [24,29)
-constexpr uint32_t kIdesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
 
 struct Taps {
     int n;
@@ -59,18 +56,16 @@ struct ConvArgs {
 // =====================================================================================================================
 // Persistent implicit-GEMM conv design (shared by conv_tc3_kernel<R>): R output rows (R x 128 pixels) x 128 couts per tile.
 //
-// Why: ncu on the first one-tile-per-CTA kernel showed 58 % tensor-pipe activity on the largest layer, L2 at 65 % / 92 % hits: not L2-bound, but
-// with 128x128 tiles the two smem operands cost 128 B/clk of shared-memory reads per MMA, the same port TMA fills.  This design cuts the
-// fill traffic and the per-tile overheads:
-//   * an input ROW STRIP {64 ch, 130 px} is loaded once per 64-channel chunk and serves all horizontal taps (the UMMA smem
+// The design cuts the operand fill traffic and the per-tile overheads:
+//   * an input ROW STRIP {64 ch, 130 px} is loaded once per 64-channel chunk and serves all horizontal taps (the wgmma smem
 //     descriptor starts 128 B x shift later; the 128-byte swizzle is a function of the ABSOLUTE smem address, so the descriptor's
-//     base_offset stays 0 - verified on B200) and the R output rows that touch it vertically;
+//     base_offset stays 0) and the R output rows that touch it vertically;
 //   * every weight tile {64 ch, 128 couts} of a tap is used by R MMA groups before it is released;
-//   * persistent CTAs, accumulators double-buffered in TMEM (R x 128 columns x 2), so the epilogue of tile i overlaps tile i+1;
+//   * persistent CTAs;
 //   * the four output-parity phases of a transposed conv are units of ONE launch;
 //   * a unit = (image, phase, row group, x block); the CTA loops over the cout blocks of its unit so that ToRGB partial sums of a
 //     256-channel layer stay in registers (block0's ToRGB is fused like the last layer's).
-// Two mbarrier rings (A strips, B taps) are filled by one TMA lane in exactly the order the MMA lane consumes them.
+// Two mbarrier rings (A strips, B taps) are filled by one TMA lane in exactly the order the consumer warpgroups use them.
 // =====================================================================================================================
 constexpr int A2_ROWS = 130, A2_BYTES = A2_ROWS * 128, A2_SLOT = 17408;       // 17 x 1024: every slot keeps the swizzle alignment
 struct Taps2 {
@@ -137,34 +132,10 @@ __device__ __forceinline__ float upsampled_skip_bf(const float* __restrict__ ip,
     return fmaf(ky1, r1, fmaf(ky0, r0, 0.f));
 }
 
-// packed 2 x fp32 arithmetic (sm_100 f32x2): one issue slot for two lanes of the epilogue's bias / lrelu / ToRGB work
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rc;\n\t"
-        "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\t"
-        "fma.rn.f32x2 rc, ra, rb, rc;\n\t"
-        "mov.b64 {%0, %1}, rc;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-    return d;
-}
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rc;\n\t"
-        "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\t"
-        "mul.rn.f32x2 rc, ra, rb;\n\t"
-        "mov.b64 {%0, %1}, rc;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-    return d;
-}
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rc;\n\t"
-        "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\t"
-        "add.rn.f32x2 rc, ra, rb;\n\t"
-        "mov.b64 {%0, %1}, rc;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-    return d;
-}
+// 2 x fp32 arithmetic on the value pairs of the epilogue's bias / lrelu / ToRGB work
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
 __device__ __forceinline__ uint4 pack_half8(const float* f) {
     __half2 h0 = __floats2half2_rn(f[0], f[1]), h1 = __floats2half2_rn(f[2], f[3]);
@@ -189,45 +160,22 @@ __device__ __forceinline__ void store_half32(__half* dst, const float* f) {
 }
 
 // =====================================================================================================================
-// conv_tc3_kernel<R>: the v2 kernel on CTA PAIRS (thread-block cluster of 2 = one TPC, tcgen05 cta_group::2).
-// ncu on v1/v2: with 128x128 single-CTA tiles every MMA pulls 4 KB (A) + 4 KB (B) from shared memory per 64 clk = 128 B/clk, the
-// whole smem port, which TMA also needs for the fills -> tensor pipe stuck at ~58 %.  A pair computes M = 256 pixels (each CTA's
-// own 128-pixel strips) x N = 128 couts per instruction and each CTA keeps only HALF of the weight tile (64 couts): 6 KB per 64 clk
-// per SM.  Protocol: both CTAs run the same producer/epilogue loops on neighbouring units; all "full" barriers live in the leader
-// (rank 0) and receive the TMA bytes of both CTAs (cp.async.bulk.tensor.cta_group::2, peer bit cleared in the barrier address);
-// the leader's MMA lane issues tcgen05.mma.cta_group::2 and releases ring slots / publishes accumulators in BOTH CTAs with
-// multicast tcgen05.commit; the epilogue warps of both CTAs arrive on the leader's accumulator-empty barrier.
+// conv_tc3_kernel<R>: one CTA per unit stream, three warpgroups.  Warpgroup 0: one TMA lane (the other warps idle); warpgroups 1 and 2:
+// consumers, warpgroup c computes pixels [64 (c-1), 64 (c-1) + 64) of every output row of the tile x all 128 couts (wgmma M64 N128 K16,
+// fp32 accumulators in registers: R x 64 per thread).  After the K loop of a cout block the accumulators of each row go through a padded
+// fp32 staging tile in shared memory so that the epilogue keeps its thread-per-pixel layout (bias, activation, ToRGB sums, coalesced
+// fp16 stores).  Ring slots are released one MMA group late (wgmma.wait_group 1), so the tensor core always has the next tap queued.
 // =====================================================================================================================
-constexpr int kThreads3 = 64 + 256;                                          // TMA warp, MMA warp, 8 epilogue warps
-constexpr int B3_BYTES = (BN / 2) * BK * 2;                                  // 64 couts x 64 ch fp16 = 8 KB per CTA
-constexpr uint32_t kIdesc3 = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);    // M = 256 across the pair
+constexpr int kThreads3 = 384;                                               // TMA warpgroup + 2 consumer warpgroups
+constexpr int B3_BYTES = BN * BK * 2;                                        // 128 couts x 64 ch fp16 = 16 KB
+constexpr int kStageRow = BN + 8;                                            // fp32 staging row (pixel): 136 floats, conflict-free fragment stores
 template <int R> struct Cfg3 {
-    static constexpr int NA = (R > 2) ? 7 : 8, NB = 8;   // R = 4 gives up one strip slot so the staging buffer fits in 227 KB
-    static constexpr int NACC = (R * BN * 2 <= 512) ? 2 : 1;
-    static constexpr int TMEM_COLS = (R * BN * NACC <= 128) ? 128 : (R * BN * NACC <= 256 ? 256 : 512);
-    static constexpr int TAIL = (R > 2 ? 12288 : 8192);                      // barriers, bias, ToRGB weights, [R][128][3] partial sums
+    static constexpr int NA = 4, NB = 4;
+    static constexpr int TAIL = 8192;                                        // barriers, bias, ToRGB weights, [R][128][3] partial sums
     static constexpr int STAGE = 8 * 32 * 64;                                // fp16 store staging: 8 epilogue warps x 32 px x 64 B
-    static constexpr int SMEM = NA * A2_SLOT + NB * B3_BYTES + 1024 + TAIL + STAGE;
+    static constexpr int ACC = BM * kStageRow * 4;                           // fp32 accumulator staging of one output row
+    static constexpr int SMEM = NA * A2_SLOT + NB * B3_BYTES + 1024 + TAIL + STAGE + ACC;
 };
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tc_commit_2sm(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
 
 template <int R, bool SPLIT>
 __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_constant__ CUtensorMap tmA,
@@ -242,46 +190,32 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
     uint64_t* a_empty = a_full + C::NA;
     uint64_t* b_full = a_empty + C::NA;
     uint64_t* b_empty = b_full + C::NB;
-    uint64_t* acc_full = b_empty + C::NB;
-    uint64_t* acc_empty = acc_full + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
     float* s_bias = reinterpret_cast<float*>(tail + 512);                    // [256]
     float* s_wrgb = s_bias + 256;                                            // [3][n_blocks*128]
     float* s_part = s_wrgb + 768;                                            // [R][128][3] ToRGB partial sums of the second column group
     uint4* s_stage = reinterpret_cast<uint4*>(tail + C::TAIL);               // [8 warps][32 px][4 x 16 B] fp16 store staging (XOR-swizzled)
+    float* s_acc = reinterpret_cast<float*>(tail + C::TAIL + C::STAGE);      // [128 px][kStageRow] fp32 accumulators of one output row
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint32_t cta_rank;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(cta_rank));
-    const bool leader = cta_rank == 0;
     const int units_per_image = a.n_phases * a.row_groups * a.tiles_x;
 
-    if (warp == 0 && lane == 0) {
-        for (int i = 0; i < C::NA; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1); }
-        for (int i = 0; i < C::NB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 16); }
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < C::NA; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 256); }
+        for (int i = 0; i < C::NB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 256); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(C::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    if (warp >= 2) {
-        const int t = threadIdx.x - 64;
+    if (warp >= 4) {
+        const int t = threadIdx.x - 128;
         for (int e = t; e < a.n_blocks * BN && e < 256; e += 256) s_bias[e] = a.bias ? a.bias[e] : 0.f;
     }
-    tc_fence_before();
     __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     // unit index -> (image n, phase, row group, x block); x fastest so neighbouring CTAs share strips in L2
     // Multi-phase launches with an even number of x blocks (the 4/2/2/1-tap phases of a transposed conv at W = 256): phases are interleaved,
-    // slot = rg * n_phases + p' with ph = (p' + rg) mod n_phases, so that at any moment the CTA pairs are spread over all phases (the 1- and
-    // 2-tap phases need 60-80 B/clk/SM of operands, above the L2 share of an SM, the 4-tap phase 40) and every pair sees every phase.
+    // slot = rg * n_phases + p' with ph = (p' + rg) mod n_phases, so that at any moment the CTAs are spread over all phases (the 1- and
+    // 2-tap phases need more operand bandwidth per MMA than the 4-tap phase) and every CTA sees every phase.
     const bool mix = a.phase_mix && a.n_phases > 1 && (a.tiles_x & 1) == 0;
     auto decode = [&](int unit, int& n, int& ph, int& row0, int& col0) {
         n = unit / units_per_image; int r = unit - n * units_per_image;
@@ -292,11 +226,11 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
         row0 = rg * R; col0 = xb * BM;
     };
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ===== TMA producer (one lane): strips and taps in consumption order =====
-        if (lane == 0) {
+        if (warp == 0 && lane == 0) {
             uint32_t aq = 0, bq = 0;                                         // running strip / tap sequence numbers
-            for (int unit = (blockIdx.x & ~1) + (int)cta_rank; unit < a.total_units; unit += gridDim.x) {
+            for (int unit = blockIdx.x; unit < a.total_units; unit += gridDim.x) {
                 int n, ph, row0, col0; decode(unit, n, ph, row0, col0);
                 const Taps2& tp = a.ph[ph].taps;
                 const int DY = tp.ngroups;
@@ -311,125 +245,47 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
                             for (int s = s_lo; s <= s_hi; ++s, ++aq) {
                                 const int slot = aq % C::NA;
                                 mbar_wait(&a_empty[slot], ((aq / C::NA) & 1) ^ 1);
-                                if (leader) mbar_expect_tx(&a_full[slot], 2 * A2_BYTES);
-                                tma_load_4d_2sm(a_ring + slot * A2_SLOT, &tmA, &a_full[slot], kc * BK, col0 - 1, row0 + tp.dy_min + s, n);
+                                mbar_expect_tx(&a_full[slot], A2_BYTES);
+                                tma_load_4d(a_ring + slot * A2_SLOT, &tmA, &a_full[slot], kc * BK, col0 - 1, row0 + tp.dy_min + s, n);
                             }
                             for (int t = tp.gstart[d]; t < tp.gstart[d + 1]; ++t, ++bq) {
                                 const int slot = bq % C::NB;
                                 mbar_wait(&b_empty[slot], ((bq / C::NB) & 1) ^ 1);
-                                if (leader) mbar_expect_tx(&b_full[slot], 2 * B3_BYTES);
-                                tma_load_4d_2sm(b_ring + slot * B3_BYTES, &tmB, &b_full[slot], kb * BK, nblk * BN + (int)cta_rank * (BN / 2), tp.widx[t], wn);
+                                mbar_expect_tx(&b_full[slot], B3_BYTES);
+                                tma_load_4d(b_ring + slot * B3_BYTES, &tmB, &b_full[slot], kb * BK, nblk * BN, tp.widx[t], wn);
                             }
                         }
                     }
             }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer: the leader CTA issues for the pair (M = 256: rows 0-127 from CTA0's strips, 128-255 from CTA1's) =====
-        if (leader) {
-        uint32_t aq = 0, bq = 0, it = 0;
-#if R3DP_TC_DEBUG_TIMING
-        long long t_acc = 0, t_a = 0, t_b = 0, t_issue = 0, t_tot0 = clock64(), tt; unsigned long long ns0, ns1; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns0));
-#define DT_BEGIN() tt = clock64()
-#define DT_END(x) x += clock64() - tt
-#else
-#define DT_BEGIN()
-#define DT_END(x)
-#endif
-        for (int unit = (blockIdx.x & ~1) + (int)cta_rank; unit < a.total_units; unit += gridDim.x) {
-            int n, ph, row0, col0; decode(unit, n, ph, row0, col0);
-            const Taps2& tp = a.ph[ph].taps;
-            const int DY = tp.ngroups, NS = R + DY - 1;
-            for (int nblk = 0; nblk < a.n_blocks; ++nblk, ++it) {
-                const int buf = it % C::NACC;
-                DT_BEGIN();
-                mbar_wait(&acc_empty[buf], (((it / C::NACC) & 1) ^ 1));
-                tc_fence_after();
-                DT_END(t_acc);
-                const uint32_t acc0 = tmem_base + buf * (R * BN);
-                const int K3 = SPLIT ? 3 * a.k_chunks : a.k_chunks;
-                for (int kc = 0; kc < K3; ++kc) {
-                    const uint32_t a_base = aq;                               // sequence number of strip 0 of this chunk
-                    for (int d = 0; d < DY; ++d) {
-                        const int s_lo = d == 0 ? 0 : R - 1 + d, s_hi = R - 1 + d;
-                        DT_BEGIN();
-                        for (int s = s_lo; s <= s_hi; ++s, ++aq) mbar_wait(&a_full[aq % C::NA], (aq / C::NA) & 1);
-                        DT_END(t_a);
-                        for (int t = tp.gstart[d]; t < tp.gstart[d + 1]; ++t, ++bq) {
-                            const int bslot = bq % C::NB;
-                            DT_BEGIN();
-                            mbar_wait(&b_full[bslot], (bq / C::NB) & 1);
-                            tc_fence_after();
-                            DT_END(t_b);
-                            DT_BEGIN();
-                            {
-                                const uint64_t db = umma_desc_sw128(smem_u32(b_ring + bslot * B3_BYTES));
-                                const int sh = tp.shift[t];
-                                const uint32_t first = (uint32_t)(kc | t);
-                                uint64_t da[R];
-#pragma unroll
-                                for (int j = 0; j < R; ++j) da[j] = umma_desc_sw128(smem_u32(a_ring + ((a_base + j + d) % C::NA) * A2_SLOT) + 128 * sh);
-                                if (elect_one()) {
-                                    // k-step outer, row inner: consecutive MMAs accumulate into DIFFERENT TMEM tiles
-#pragma unroll
-                                    for (int k = 0; k < BK / UMMA_K; ++k) {
-#pragma unroll
-                                        for (int j = 0; j < R; ++j)
-                                            tc_mma_f16_2sm(acc0 + j * BN, da[j] + (uint64_t)(2 * k), db + (uint64_t)(2 * k), kIdesc3, first | (uint32_t)k);
-                                    }
-                                    tc_commit_2sm(&b_empty[bslot]);
-                                }
-                            }
-                            __syncwarp();
-                            DT_END(t_issue);
-                        }
-                        // strips no later group needs: strip d after group d; everything left after the last group
-                        if (d < DY - 1) {
-                            if (elect_one()) tc_commit_2sm(&a_empty[(a_base + d) % C::NA]);
-                        } else {
-                            for (int s = DY - 1; s < NS; ++s) { if (elect_one()) tc_commit_2sm(&a_empty[(a_base + s) % C::NA]); }
-                        }
-                        __syncwarp();
-                    }
-                }
-                if (elect_one()) tc_commit_2sm(&acc_full[buf]);
-                __syncwarp();
-            }
-        }
-#if R3DP_TC_DEBUG_TIMING
-        if (lane == 0 && a.debug) {
-            atomicAdd((unsigned long long*)a.debug + 0, (unsigned long long)t_acc); atomicAdd((unsigned long long*)a.debug + 1, (unsigned long long)t_a);
-            atomicAdd((unsigned long long*)a.debug + 2, (unsigned long long)t_b); atomicAdd((unsigned long long*)a.debug + 3, (unsigned long long)t_issue);
-            atomicAdd((unsigned long long*)a.debug + 4, (unsigned long long)(clock64() - t_tot0)); atomicAdd((unsigned long long*)a.debug + 5, 1ull);
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns1)); atomicAdd((unsigned long long*)a.debug + 6, ns1 - ns0); atomicAdd((unsigned long long*)a.debug + 7, (unsigned long long)it);
-        }
-#endif
         }
     } else {
-        // ===== epilogue: warps 2..9; warp w reads TMEM lanes [32*(w%4), +32); warps 2-5 take columns 0-63 of each accumulator, 6-9 columns 64-127 =====
-        const int q = warp & 3, m = q * 32 + lane;
-        const int cg = (warp - 2) >> 2;                                       // column group
+        // ===== consumers: warpgroup wg = 0, 1 multiplies pixels [64 wg, 64 wg + 64) of each row; then the epilogue =====
+        const int wg = (warp >> 2) - 1;
+        const int q = warp & 3, m = q * 32 + lane;                           // epilogue: pixel m of the row, column group cg
+        const int cg = wg;
         const bool want_rgb = (a.mode == kToRgbFinal) || (a.mode == kActRgb);
         const int CW = a.n_blocks * BN;                                      // channels ToRGB sums over
         float brgb[3] = {0.f, 0.f, 0.f};
         if (want_rgb) { brgb[0] = a.brgb[0]; brgb[1] = a.brgb[1]; brgb[2] = a.brgb[2]; }
-        uint32_t it = 0;
         int n_loaded = -1;
-#if R3DP_TC_DEBUG_TIMING
-        long long e_full = 0, e_ld = 0, e_math = 0, e_xchg = 0, e_fin = 0, e_pre = 0, e_tot0 = clock64(), et;
-#define ET_BEGIN() et = clock64()
-#define ET_END(x) x += clock64() - et
-#else
-#define ET_BEGIN()
-#define ET_END(x)
-#endif
-        for (int unit = (blockIdx.x & ~1) + (int)cta_rank; unit < a.total_units; unit += gridDim.x) {
+        uint32_t aq = 0, bq = 0;
+        // slots read by the most recently committed MMA group, released once the NEXT group has been committed and this one has retired
+        int pend_b = -1; uint32_t pend_a0 = 0, pend_an = 0;
+        auto release_pending = [&]() {
+            if (pend_b >= 0) mbar_arrive(&b_empty[pend_b]);
+            for (uint32_t s = 0; s < pend_an; ++s) mbar_arrive(&a_empty[(pend_a0 + s) % C::NA]);
+            pend_b = -1; pend_an = 0;
+        };
+        float acc[R][64];
+        for (int unit = blockIdx.x; unit < a.total_units; unit += gridDim.x) {
             int n, ph, row0, col0; decode(unit, n, ph, row0, col0);
             const Phase2& P = a.ph[ph];
+            const Taps2& tp = P.taps;
+            const int DY = tp.ngroups, NS = R + DY - 1;
             const int wn = a.w_shared ? 0 : n;
             if (want_rgb && wn != n_loaded) {
                 asm volatile("bar.sync 1, 256;" ::: "memory");               // all eight epilogue warps are done with the old weights
-                for (int e = threadIdx.x - 64; e < 3 * CW; e += 256) s_wrgb[e] = a.wrgb[(size_t)wn * 3 * CW + e];
+                for (int e = threadIdx.x - 128; e < 3 * CW; e += 256) s_wrgb[e] = a.wrgb[(size_t)wn * 3 * CW + e];
                 asm volatile("bar.sync 1, 256;" ::: "memory");
                 n_loaded = wn;
             }
@@ -437,10 +293,8 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
             float2 rgb2[R][3];                                               // ToRGB sums, even / odd channels in the two halves
 #pragma unroll
             for (int j = 0; j < R; ++j) { rgb2[j][0] = make_float2(0.f, 0.f); rgb2[j][1] = make_float2(0.f, 0.f); rgb2[j][2] = make_float2(0.f, 0.f); }
-            ET_BEGIN();
-            // skip-image taps of this thread's pixels, fetched by the SECOND column group (it idles at the exchange barrier anyway) and
-            // added to its partial sums.  Issued before the accumulator wait, all loads in one basic block (clamped addresses, zero
-            // weights outside the image), so their L2 latency overlaps and hides behind the MMAs.
+            // skip-image taps of this thread's pixels, fetched by the SECOND column group and added to its partial sums (clamped addresses,
+            // zero weights outside the image: the loads are independent)
             float skipv[R][3];
 #pragma unroll
             for (int j = 0; j < R; ++j) { skipv[j][0] = 0.f; skipv[j][1] = 0.f; skipv[j][2] = 0.f; }
@@ -458,57 +312,81 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
                     const int x0 = (X - 1) >> 1;
                     const float kx0 = (x0 >= 0 && x0 < w) ? ((X & 1) ? 0.75f : 0.25f) : 0.f, kx1 = (x0 + 1 < w) ? ((X & 1) ? 0.25f : 0.75f) : 0.f;
                     const int xa = min(max(x0, 0), w - 1), xb = min(max(x0 + 1, 0), w - 1);
-                    float v[R][3][4], ky0[R], ky1[R];
 #pragma unroll
                     for (int j = 0; j < R; ++j) {
                         const int Y = (row0 + j) * a.oy_mul + P.oy_off, y0 = (Y - 1) >> 1;
-                        ky0[j] = (y0 >= 0 && y0 < h) ? ((Y & 1) ? 0.75f : 0.25f) : 0.f;
-                        ky1[j] = (y0 + 1 < h) ? ((Y & 1) ? 0.25f : 0.75f) : 0.f;
+                        const float ky0 = (y0 >= 0 && y0 < h) ? ((Y & 1) ? 0.75f : 0.25f) : 0.f;
+                        const float ky1 = (y0 + 1 < h) ? ((Y & 1) ? 0.25f : 0.75f) : 0.f;
                         const int ya = min(max(y0, 0), h - 1), yb = min(max(y0 + 1, 0), h - 1);
 #pragma unroll
-                        for (int c = 0; c < 3; ++c) {
+                        for (int c = 0; c < 3; ++c) {                        // the fma order of upsampled_skip
                             const float* ip = a.img_prev + ((size_t)n * 3 + c) * h * w;
-                            v[j][c][0] = __ldg(ip + ya * w + xa); v[j][c][1] = __ldg(ip + ya * w + xb);
-                            v[j][c][2] = __ldg(ip + yb * w + xa); v[j][c][3] = __ldg(ip + yb * w + xb);
+                            const float v0 = __ldg(ip + ya * w + xa), v1 = __ldg(ip + ya * w + xb), v2 = __ldg(ip + yb * w + xa), v3 = __ldg(ip + yb * w + xb);
+                            const float r0 = fmaf(kx1, v1, fmaf(kx0, v0, 0.f)), r1 = fmaf(kx1, v3, fmaf(kx0, v2, 0.f));
+                            skipv[j][c] = fmaf(ky1, r1, fmaf(ky0, r0, 0.f));
                         }
                     }
-#pragma unroll
-                    for (int j = 0; j < R; ++j)
-#pragma unroll
-                        for (int c = 0; c < 3; ++c) {                        // the fma order of upsampled_skip
-                            const float r0 = fmaf(kx1, v[j][c][1], fmaf(kx0, v[j][c][0], 0.f)), r1 = fmaf(kx1, v[j][c][3], fmaf(kx0, v[j][c][2], 0.f));
-                            skipv[j][c] = fmaf(ky1[j], r1, fmaf(ky0[j], r0, 0.f));
-                        }
                 }
             }
-            ET_END(e_pre);
-            for (int nblk = 0; nblk < a.n_blocks; ++nblk, ++it) {
-                const int buf = it % C::NACC;
-                ET_BEGIN();
-                mbar_wait(&acc_full[buf], (it / C::NACC) & 1);
-                tc_fence_after();
-                ET_END(e_full);
+            for (int nblk = 0; nblk < a.n_blocks; ++nblk) {
+                // ---- K loop: (channel chunk) x (dy group) x (tap), R rows per tap, 4 k-steps of 16 channels ----
+                const int K3 = SPLIT ? 3 * a.k_chunks : a.k_chunks;
+                for (int kc = 0; kc < K3; ++kc) {
+                    const uint32_t a_base = aq;                               // sequence number of strip 0 of this chunk
+                    for (int d = 0; d < DY; ++d) {
+                        const int s_lo = d == 0 ? 0 : R - 1 + d, s_hi = R - 1 + d;
+                        for (int s = s_lo; s <= s_hi; ++s, ++aq) mbar_wait(&a_full[aq % C::NA], (aq / C::NA) & 1);
+                        for (int t = tp.gstart[d]; t < tp.gstart[d + 1]; ++t, ++bq) {
+                            const int bslot = bq % C::NB;
+                            mbar_wait(&b_full[bslot], (bq / C::NB) & 1);
+                            const uint64_t db = gmma_desc_sw128(smem_u32(b_ring + bslot * B3_BYTES));
+                            const int sh = tp.shift[t];
+                            const uint32_t first = (uint32_t)(kc | t);
+                            uint64_t da[R];
+#pragma unroll
+                            for (int j = 0; j < R; ++j) da[j] = gmma_desc_sw128(smem_u32(a_ring + ((a_base + j + d) % C::NA) * A2_SLOT) + 128 * (64 * wg + sh));
+                            wg_fence();
+#pragma unroll
+                            for (int k = 0; k < BK / 16; ++k) {
+#pragma unroll
+                                for (int j = 0; j < R; ++j) wgmma_m64n128k16(acc[j], da[j] + (uint64_t)(2 * k), db + (uint64_t)(2 * k), first | (uint32_t)k);
+                            }
+                            wg_commit();
+                            wg_wait<1>();                                     // the previous group has retired: its slots can be refilled
+                            release_pending();
+                            pend_b = bslot;
+                        }
+                        // strips no later group needs: strip d after group d; everything left after the last group
+                        if (d < DY - 1) { pend_a0 = a_base + d; pend_an = 1; }
+                        else { pend_a0 = a_base + DY - 1; pend_an = (uint32_t)(NS - (DY - 1)); }
+                    }
+                }
+                wg_wait<0>();
+#pragma unroll
+                for (int j = 0; j < R; ++j) wg_fence_acc<64>(acc[j]);
+                release_pending();
+                // ---- epilogue, one output row at a time through the fp32 staging tile ----
 #pragma unroll
                 for (int j = 0; j < R; ++j) {
+#pragma unroll
+                    for (int i = 0; i < 64; i += 2)
+                        *reinterpret_cast<float2*>(s_acc + (64 * wg + acc_row(i)) * kStageRow + acc_col(i)) = make_float2(acc[j][i], acc[j][i + 1]);
+                    asm volatile("bar.sync 4, 256;" ::: "memory");
                     const int row = row0 + j;
                     const int Y = row * a.oy_mul + P.oy_off;
                     const bool row_ok = (row < P.rows) && (Y < a.out_H);
                     const bool in_img = row_ok && (X < a.out_W);
-                    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + buf * (R * BN) + j * BN;
 #pragma unroll 1
                     for (int c0 = cg * (BN / 2); c0 < (cg + 1) * (BN / 2); c0 += 32) {
-                        uint32_t r[32];
-                        ET_BEGIN();
-                        tc_ld32(taddr + c0, r);
-                        ET_END(e_ld);
-                        ET_BEGIN();
                         float2 f2[16];
+                        const float4* src = reinterpret_cast<const float4*>(s_acc + m * kStageRow + c0);
                         const float2 sc2 = make_float2(a.acc_scale, a.acc_scale);
-                        if (a.mode == kStoreRaw) {
 #pragma unroll
-                            for (int i = 0; i < 16; ++i) {
-                                f2[i] = make_float2(__uint_as_float(r[2 * i]), __uint_as_float(r[2 * i + 1]));
-                                if (SPLIT) f2[i] = mul2(f2[i], sc2);
+                        for (int i = 0; i < 8; ++i) { const float4 v = src[i]; f2[2 * i] = make_float2(v.x, v.y); f2[2 * i + 1] = make_float2(v.z, v.w); }
+                        if (a.mode == kStoreRaw) {
+                            if (SPLIT) {
+#pragma unroll
+                                for (int i = 0; i < 16; ++i) f2[i] = mul2(f2[i], sc2);
                             }
                         } else {
                             // bias, leaky relu as max(v, v*slope) (slope <= 1), gain: bias_act lrelu*sqrt2 | nn.LeakyReLU | linear
@@ -516,8 +394,7 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
                             const float2 sl2 = make_float2(a.act_slope, a.act_slope), g2 = make_float2(a.act_gain, a.act_gain);
 #pragma unroll
                             for (int i = 0; i < 16; ++i) {
-                                const float2 acc2 = make_float2(__uint_as_float(r[2 * i]), __uint_as_float(r[2 * i + 1]));
-                                const float2 v = SPLIT ? fma2(acc2, sc2, b2[i]) : add2(acc2, b2[i]);
+                                const float2 v = SPLIT ? fma2(f2[i], sc2, b2[i]) : add2(f2[i], b2[i]);
                                 const float2 t = mul2(v, sl2);
                                 f2[i] = mul2(make_float2(fmaxf(v.x, t.x), fmaxf(v.y, t.y)), g2);
                             }
@@ -527,7 +404,7 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
                             // NHWC fp16 store through smem: the thread owns a pixel (32 channels = 64 B); written directly, every
                             // STG.128 of the warp would touch 32 different lines.  Staged, 4 lanes write one pixel's 64 contiguous bytes.
                             // Split mode: a second pass stores the fp16 remainders (v - fp16(v)) lo_off channels further.
-                            uint4* st = s_stage + (warp - 2) * 128;
+                            uint4* st = s_stage + (warp - 4) * 128;
                             const int sw = (lane >> 1) & 3;
                             constexpr int passes = SPLIT ? 2 : 1;
 #pragma unroll
@@ -568,19 +445,17 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
 #pragma unroll
                             for (int c = 0; c < 3; ++c) {
                                 const float4* w4 = reinterpret_cast<const float4*>(s_wrgb + c * CW + nblk * BN + c0);
-                                float2 acc = rgb2[j][c];
+                                float2 accr = rgb2[j][c];
 #pragma unroll
                                 for (int j4 = 0; j4 < 8; ++j4) {
                                     const float4 w = w4[j4];
-                                    acc = fma2(f2[2 * j4], make_float2(w.x, w.y), acc);
-                                    acc = fma2(f2[2 * j4 + 1], make_float2(w.z, w.w), acc);
+                                    accr = fma2(f2[2 * j4], make_float2(w.x, w.y), accr);
+                                    accr = fma2(f2[2 * j4 + 1], make_float2(w.z, w.w), accr);
                                 }
-                                rgb2[j][c] = acc;
+                                rgb2[j][c] = accr;
                             }
                         }
-                        ET_END(e_math);
                     }
-                    ET_BEGIN();
                     if (want_rgb && nblk == a.n_blocks - 1) {
                         // the two column groups hold partial ToRGB sums of the same pixel: group 1 hands its sums to group 0 through smem
                         if (cg == 1) {
@@ -594,8 +469,6 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
                         }
                         asm volatile("bar.sync 3, 256;" ::: "memory");
                     }
-                    ET_END(e_xchg);
-                    ET_BEGIN();
                     if (want_rgb && nblk == a.n_blocks - 1 && in_img && cg == 0) {
 #pragma unroll
                         for (int c = 0; c < 3; ++c) {
@@ -608,29 +481,10 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
                                 a.img_out[(((size_t)n * 3 + c) * a.img_H + Y) * a.img_W + X] = v;
                         }
                     }
-                    ET_END(e_fin);
+                    asm volatile("bar.sync 5, 256;" ::: "memory");               // the staging tile is free for the next row
                 }
-                // this warp is done reading the accumulator buffer
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(&acc_empty[buf]) & 0xFEFFFFFFu) : "memory");
             }
         }
-#if R3DP_TC_DEBUG_TIMING
-        if (lane == 0 && a.debug && (warp == 2 || warp == 6) && cta_rank == 0) {
-            unsigned long long* d = a.debug + 8 + (warp == 6 ? 8 : 0);
-            atomicAdd(d + 0, (unsigned long long)e_full); atomicAdd(d + 1, (unsigned long long)e_ld); atomicAdd(d + 2, (unsigned long long)e_math);
-            atomicAdd(d + 3, (unsigned long long)e_xchg); atomicAdd(d + 4, (unsigned long long)e_fin); atomicAdd(d + 5, (unsigned long long)(clock64() - e_tot0));
-            atomicAdd(d + 6, (unsigned long long)it); atomicAdd(d + 7, (unsigned long long)e_pre);
-        }
-#endif
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                     // the peer's smem/TMEM must stay alive until every MMA that reads it has retired
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(C::TMEM_COLS) : "memory");
     }
 }
 
@@ -745,13 +599,9 @@ constexpr int FIR_TW = 32, FIR_TH = 8, FIR_SEG = 32, FIR_BW = FIR_TW + 3, FIR_BH
 constexpr int FIR_BOX8_BYTES = FIR_BW * FIR_TH * 128;
 constexpr int FIR_BOX_BYTES = FIR_BW * FIR_BH * 128, FIR_SLOT = (FIR_BOX_BYTES + 1023) / 1024 * 1024;
 constexpr int FIR_SMEM = 2 * FIR_SLOT + 1024 + 64;
-// packed 2 x fp32 FMA (sm_100 fma.rn.f32x2): (d0,d1) += (a0,a1) * (b0,b1)
+// (d0,d1) += (a0,a1) * (b0,b1)
 __device__ __forceinline__ void ffma2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-    asm("{\n\t.reg .b64 ra, rb, rc;\n\t"
-        "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%0, %1};\n\t"
-        "fma.rn.f32x2 rc, ra, rb, rc;\n\t"
-        "mov.b64 {%0, %1}, rc;\n\t}"
-        : "+f"(d0), "+f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
+    d0 = __fmaf_rn(a0, b0, d0); d1 = __fmaf_rn(a1, b1, d1);
 }
 // Work item = a strip of FIR_TW px x FIR_SEG output rows of one 64-channel group, streamed as FIR_SEG / FIR_TH chunks: the first box has the
 // 3 halo rows (35 px x 11 rows), the following boxes only new rows (35 x 8) - the 4-row register window simply keeps rolling across the
@@ -836,7 +686,7 @@ __global__ void __launch_bounds__(256) fir_tma_kernel(const __grid_constant__ CU
                     for (int j = 0; j < 4; ++j) {
                         float2 f = __half22float2(h[j]);
                         if (SPLIT) { const float2 g = __half22float2(hl[j]); f.x += g.x; f.y += g.y; }
-                        ffma2(win[3][2 * j], win[3][2 * j + 1], k4[v], k4[v], f.x, f.y);  // packed f32x2: the kernel is issue-bound
+                        ffma2(win[3][2 * j], win[3][2 * j + 1], k4[v], k4[v], f.x, f.y);
                     }
                 }
                 const int gy = gy0 + ry;
@@ -1021,11 +871,8 @@ static void prof_mark(cudaStream_t st) {
 
 static unsigned long long* g_debug_buf = nullptr;
 static int g_debug_launch = 0;
-static int tc_rows() {                         // R3DP_TC_ROWS = 1 | 2 | 4 output rows per tile (default 2: double-buffered accumulators)
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("R3DP_TC_ROWS"); v = e ? atoi(e) : 2; if (v != 1 && v != 2 && v != 4) v = 2; }
-    return v;
-}
+// output rows per tile: each consumer thread holds R x 64 fp32 accumulators; at R = 2 they no longer fit the 168 registers of a 384-thread CTA
+constexpr int kConvRows = 1;
 
 template <int R, bool SPLIT>
 static int launch_conv3_rs(const CUtensorMap& tmA, const CUtensorMap& tmB, Conv2Args a, int max_rows, cudaStream_t st) {
@@ -1033,18 +880,11 @@ static int launch_conv3_rs(const CUtensorMap& tmA, const CUtensorMap& tmB, Conv2
     R3DP_CUDA(cudaFuncSetAttribute(conv_tc3_kernel<R, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
     a.debug = g_debug_buf ? g_debug_buf + 24 * (g_debug_launch++ % 32) : nullptr;
     a.row_groups = (max_rows + R - 1) / R;
-    if ((a.row_groups * a.tiles_x) & 1) a.row_groups += 1;       // the two CTAs of a pair must work on units of the same (image, phase)
     a.total_units = a.n_images * a.n_phases * a.row_groups * a.tiles_x;
-    int grid = a.total_units < sm_count() ? a.total_units : sm_count();
-    grid &= ~1;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads3); cfg.dynamicSmemBytes = C::SMEM; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
+    const int grid = a.total_units < sm_count() ? a.total_units : sm_count();
     prof_mark(st);
-    R3DP_CUDA(cudaLaunchKernelEx(&cfg, conv_tc3_kernel<R, SPLIT>, tmA, tmB, a));
+    conv_tc3_kernel<R, SPLIT><<<grid, kThreads3, C::SMEM, st>>>(tmA, tmB, a);
+    R3DP_LAUNCH_CHECK();
     prof_mark(st);
     count_launches(1);
     return 0;
@@ -1079,14 +919,14 @@ static int run_conv2(const void* x, int N, int H, int W, int Cp, const void* wp,
     CUtensorMap tmA, tmB;
     const uint64_t Cphys = (uint64_t)Cp * (a.split ? 2 : 1);                      // split: [hi | lo] halves of Cp channels each
     if (make_map_4d_box(&tmA, x, Cphys, (uint64_t)W, (uint64_t)H, (uint64_t)N, A2_ROWS)) return 1;
-    if (make_map_4d_box(&tmB, wp, Cphys, (uint64_t)O, (uint64_t)n_taps, (uint64_t)Nw, BN / 2)) return 1;
+    if (make_map_4d_box(&tmB, wp, Cphys, (uint64_t)O, (uint64_t)n_taps, (uint64_t)Nw, BN)) return 1;
     if (a.split) { R3DP_REQUIRE(a.residual == nullptr, "conv_tc3: the residual epilogue is not built for split operands"); a.acc_scale = 1.0f / kSplitWeightScale; a.lo_off = a.out_C; a.out_C *= 2; }
     else { a.acc_scale = 1.0f; a.lo_off = 0; }
     a.k_chunks = Cp / BK; a.tiles_x = W / BM; a.n_blocks = O / BN; a.n_images = N; a.w_shared = (Nw == 1);
     { static int mixv = -1; if (mixv < 0) { const char* e = getenv("R3DP_TC_MIX"); mixv = (e && e[0] == '0') ? 0 : 1; } a.phase_mix = mixv; }      // A/B knob
     if (a.act_gain == 0.f) { a.act_slope = 0.2f; a.act_gain = 1.4142135623730951f; }      // default: bias_act lrelu
     R3DP_REQUIRE(a.n_blocks >= 1 && a.n_blocks <= 2, "conv_tc3: 128 or 256 output channels");
-    return tc_rows() == 1 ? launch_conv3_r<1>(tmA, tmB, a, max_rows, st) : (tc_rows() == 4 ? launch_conv3_r<4>(tmA, tmB, a, max_rows, st) : launch_conv3_r<2>(tmA, tmB, a, max_rows, st));
+    return launch_conv3_r<kConvRows>(tmA, tmB, a, max_rows, st);
 }
 
 // v1-style single-phase description -> v2 launch

@@ -422,6 +422,6 @@ class FrameEngine:
             capi.check(L.r3dp_sr_tc_prof_read(C.byref(ms), C.byref(n)))
             L.r3dp_sr_tc_prof(0)
             conv_ms, conv_n = float(ms.value), int(n.value)
-        kernel = 'conv_tc3_kernel<2> (tcgen05 cta_group::2 implicit-GEMM conv)' if tc else 'conv_taps_kernel (fp32 CUDA-core direct conv)'
+        kernel = 'conv_tc3_kernel<1> (wgmma implicit-GEMM conv)' if tc else 'conv_taps_kernel (fp32 CUDA-core direct conv)'
         return {'stages': stages, 'sr_conv_ms': stages.get('sr_conv', float('nan')), 'total_ms': a.elapsed_time(b), 'sr_kernel': kernel,
                 'conv_kernel_ms': conv_ms, 'conv_launches': conv_n}

@@ -1,5 +1,5 @@
 """Tensor-core execution of SuperresolutionHybrid8XDC.forward (superresolution.py:348-359): the same layers as the
-fp32 modules in superresolution.py, run as tcgen05 implicit GEMMs (csrc/sr_tc.cu) on NHWC fp16 activations with fp32
+fp32 modules in superresolution.py, run as wgmma implicit GEMMs (csrc/sr_tc.cu) on NHWC fp16 activations with fp32
 accumulation.  Weights are folded (modulated + demodulated) in fp32 per sample, exactly as the reference does, and only
 then rounded to fp16.  Stated tolerance vs the fp32 reference: see tests/test_gpu_parity.py::test_sr_full_tc."""
 from __future__ import annotations

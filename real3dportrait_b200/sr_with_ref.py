@@ -3,7 +3,7 @@ fusing SR head of OSAvatarSECC_Img2plane_Torso, BASELINE config 5).
 
 Same constructor arguments, child-module names (`block0/1`, `torso_encoder`, `bg_encoder`, `head_torso_alpha_predictor`,
 `fuse_head_torso_convs`, `head_torso_block`, `fuse_fg_bg_convs`, `torso_model`) and `forward` signature/return as the reference, so
-released checkpoints load with strict=True.  The conv stack (782 GFLOP/frame, SURVEY.md §8d) runs on the tcgen05 kernels of
+released checkpoints load with strict=True.  The conv stack (782 GFLOP/frame, SURVEY.md §8d) runs on the tensor-core kernels of
 csrc/sr_tc.cu; the torso warper `torso_model` (WarpBasedTorsoModelMediaPipe, SURVEY.md §2 #11: out of scope) stays the caller's
 PyTorch module and is called as an opaque child exactly where the reference calls it.  Supported configuration = the released one
 (egs/os_avatar/real3d_orig/secc_img2plane_torso_orig.yaml:26-30): torso_model_version v2, htbsr_head_weight_fuse_mode v2."""

@@ -4,7 +4,7 @@ modules/eg3ds/models/superresolution.py:331-359 and modules/eg3ds/models/network
 Module / parameter / buffer names equal the reference's, so `load_state_dict(strict=True)` of released checkpoints
 works.  forward() orchestrates libr3dp_b200 calls; two arithmetic modes (`sr_mode`):
   'fp32'  exact CUDA-core path (parity anchor, matches the reference to fp32 re-association noise),
-  'tc'    tensor-core path (tcgen05, fp16 operands, fp32 accumulate) — the fast path, own stated tolerance.
+  'tc'    tensor-core path (wgmma, fp16 operands, fp32 accumulate) — the fast path, own stated tolerance.
 Inference only: noise_mode must be 'none' (as in img2plane_baseline.py:113,144), fp32 parameters."""
 from __future__ import annotations
 

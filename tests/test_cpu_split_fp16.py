@@ -1,4 +1,4 @@
-"""The tensor-core OSG decoder (render.cu, MlpTcImage) feeds tcgen05 with fp16 operands and still claims fp32-grade results: every fp32
+"""The tensor-core OSG decoder (render.cu, MlpTcImage) feeds wgmma with fp16 operands and still claims fp32-grade results: every fp32
 operand is split as v = hi + lo (two fp16 numbers) and the products hi*hi + lo*hi + hi*lo are accumulated in fp32.  This CPU test
 restates that arithmetic with numpy on decoder-shaped data (SURVEY.md Appendix A: 32 -> 64 softplus -> 33, gains 1/sqrt(fan_in)) and
 bounds its error against float64, next to plain fp32 and plain fp16 evaluations of the same layer."""

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box with -m gpu): the CUDA path, called through the C ABI via the host mirror,
+"""GPU parity tests (run on an H100 with -m gpu): the CUDA path, called through the C ABI via the host mirror,
 against (a) fixtures produced by the reference's own modules and (b) the CPU oracle on fresh seeded inputs.
 
 Tolerances (stated, per BASELINE.json north_star): rendered RGB max-abs-diff < 1e-3 — we assert a 10x tighter 1e-4
@@ -48,7 +48,7 @@ def test_render_small_vs_reference(golden, name):
 
 def test_sample_and_decode_vs_reference(golden):
     g = golden('sample_small')
-    planes, coords = g['planes'].to(DEV), g['coords'].to(DEV)
+    planes, coords = golden('render_small')['planes'].to(DEV), g['coords'].to(DEV)          # the fixtures share their planes
     feat = r3.sample_from_planes(r3.generate_planes(), planes, coords, padding_mode='zeros', box_warp=1.0)
     assert feat.shape == g['feat'].shape and _maxdiff(feat, g['feat']) < 1e-5
     dec = _decoder(mlp_of(g))
@@ -143,9 +143,9 @@ def test_sr_full_fp32_vs_reference(golden):
     fimg = orc.feature_image(golden('render_full48')['rgb'], 64).to(DEV)
     sr = r3.SuperresolutionHybrid8XDC(channels=32, img_resolution=512, sr_num_fp16_res=0, sr_antialias=True, sr_mode='fp32')
     sr.load_state_dict(syn.make_sr_params(seed=5), strict=True)
-    img = sr.to(DEV)(fimg[:, :3], fimg, torch.ones(1, 14, 512, device=DEV), noise_mode='none')
-    ref = golden('sr_full')['image']
-    assert img.shape == (1, 3, 512, 512)
+    img = sr.to(DEV)(fimg[:, :3], fimg, torch.ones(1, 14, 512, device=DEV), noise_mode='none')[..., ::2, ::2]
+    ref = golden('sr_full')['image_s2']
+    assert img.shape == (1, 3, 256, 256)
     assert _maxdiff(img, ref) < 1e-3 * float(ref.abs().max())
 
 
@@ -175,7 +175,7 @@ def test_render_head_vs_oracle_with_per_sample_styles():
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# tensor-core SR path (tcgen05, fp16 operands / fp32 accumulate).  Stated tolerances:
+# tensor-core SR path (wgmma, fp16 operands / fp32 accumulate).  Stated tolerances:
 #   single layer vs fp32 math on the SAME fp16-rounded operands: 2e-3 * max|y|  (only the fp16 rounding of the output differs)
 #   full SR image vs the fp32 reference: max-abs < 5e-3 and PSNR > 70 dB (measured 2.3e-3 .. 3.4e-3, 72.8 dB on range [-2.2, 1.1])
 # ---------------------------------------------------------------------------------------------------------------------
@@ -220,8 +220,8 @@ def test_sr_full_tc_vs_reference(golden):
     fimg = orc.feature_image(golden('render_full48')['rgb'], 64).to(DEV)
     sr = r3.SuperresolutionHybrid8XDC(channels=32, img_resolution=512, sr_num_fp16_res=0, sr_antialias=True, sr_mode='tc')
     sr.load_state_dict(syn.make_sr_params(seed=5), strict=True)
-    img = sr.to(DEV)(fimg[:, :3], fimg, torch.ones(1, 14, 512, device=DEV), noise_mode='none')
-    ref = golden('sr_full')['image']
+    img = sr.to(DEV)(fimg[:, :3], fimg, torch.ones(1, 14, 512, device=DEV), noise_mode='none')[..., ::2, ::2]
+    ref = golden('sr_full')['image_s2']
     err = _maxdiff(img, ref)
     mse = float(((img.cpu() - ref) ** 2).mean())
     psnr = 10 * torch.log10(torch.tensor(float(ref.max() - ref.min()) ** 2 / mse)).item()
@@ -249,8 +249,8 @@ def test_sr_full_tc_exact_vs_reference(golden):
     fimg = orc.feature_image(golden('render_full48')['rgb'], 64).to(DEV)
     sr = r3.SuperresolutionHybrid8XDC(channels=32, img_resolution=512, sr_num_fp16_res=0, sr_antialias=True, sr_mode='tc_exact')
     sr.load_state_dict(syn.make_sr_params(seed=5), strict=True)
-    img = sr.to(DEV)(fimg[:, :3], fimg, torch.ones(1, 14, 512, device=DEV), noise_mode='none')
-    ref = golden('sr_full')['image']
+    img = sr.to(DEV)(fimg[:, :3], fimg, torch.ones(1, 14, 512, device=DEV), noise_mode='none')[..., ::2, ::2]
+    ref = golden('sr_full')['image_s2']
     err, rng = _maxdiff(img, ref), float(ref.max() - ref.min())
     print(f'tc_exact SR: max-abs {err:.3e} on range {rng:.2f}')
     assert err < 1e-3 * rng, (err, rng)
@@ -295,8 +295,8 @@ def test_torso_head_vs_reference(golden):
     with torch.no_grad():
         img, ret = m(fimg[:, :3].contiguous(), fimg, torch.ones(1, 14, 512, device=DEV), inp['ref_torso_rgb'], inp['ref_bg_rgb'], wimg, inp['segmap'],
                      inp['kp_s'], inp['kp_d'], noise_mode='none')
-    ref = golden('sr_warp_full')['image']
     assert 'occlusion_2' in ret and img.shape == (1, 3, 512, 512)
+    img, ref = img[..., ::2, ::2], golden('sr_warp_full')['image_s2']
     err = _maxdiff(img, ref)
     mse = float(((img.cpu() - ref) ** 2).mean())
     psnr = 10 * torch.log10(torch.tensor(float(ref.max() - ref.min()) ** 2 / mse)).item()
@@ -321,7 +321,7 @@ def test_torso_head_other_fuse_modes_vs_reference(golden, mode):
     with torch.no_grad():
         img, ret = m(fimg[:, :3].contiguous(), fimg, torch.ones(1, 14, 512, device=DEV), inp['ref_torso_rgb'], inp['ref_bg_rgb'], fx['weights_img'].to(DEV),
                      inp['segmap'], inp['kp_s'], inp['kp_d'], noise_mode='none')
-    ref = fx['image']
+    img, ref = img[..., ::2, ::2], fx['image_s2']
     err = _maxdiff(img, ref)
     mse = float(((img.cpu() - ref) ** 2).mean())
     psnr = 10 * torch.log10(torch.tensor(float(ref.max() - ref.min()) ** 2 / mse)).item()
@@ -497,7 +497,7 @@ def test_render_plane_layouts_and_two_plane_sets_vs_oracle():
 
 @pytest.mark.parametrize('S,S_imp,M', [(12, 24, 64), (48, 24, 32), (24, 48, 32)])
 def test_two_pass_decoder_unequal_tile_counts_vs_oracle(S, S_imp, M):
-    """Importance renders whose two passes need DIFFERENT numbers of 128-sample tcgen05 tiles per CTA (12+24 at 8 rays/CTA: 1 then 2 tiles;
+    """Importance renders whose two passes need DIFFERENT numbers of 128-sample tensor-core tiles per CTA (12+24 at 8 rays/CTA: 1 then 2 tiles;
     48+24 at 4 rays/CTA: 2 then 1): the per-barrier parity bookkeeping of the two-pass decoder."""
     N = 2
     g = torch.Generator().manual_seed(S * 100 + S_imp)
@@ -609,7 +609,8 @@ def test_trigrid_v2_vs_reference(golden):
     against fixtures produced by the reference's own sample_from_trigrids / ImportanceRenderer."""
     g = golden('render_trigrid')
     D = g['depth_slices']
-    grids, coords = g['planes'].to(DEV), g['coords'].to(DEV)
+    grids = torch.randn(2, 3, 32 * D, 32, 32, generator=torch.Generator().manual_seed(g['planes_seed'])).to(DEV)
+    coords = g['coords'].to(DEV)
     feat = r3.sample_from_trigrids(r3.generate_planes(), grids, coords, padding_mode='zeros', box_warp=1.0, triplane_depth=D)
     assert feat.shape == g['feat'].shape and _maxdiff(feat, g['feat']) < 1e-5
     cl = r3.grids_to_channels_last(grids, D)
@@ -635,8 +636,8 @@ def test_large_sr_tc_vs_reference(golden):
     sr = r3.SuperresolutionHybrid8XDC(channels=32, img_resolution=512, sr_num_fp16_res=0, sr_antialias=True, large_sr=True, sr_mode='tc',
                                       resblocks_in_large_sr=2)
     sr.load_state_dict(syn.make_sr_large_params(seed=8, n_res=2), strict=True)
-    img = sr.to(DEV)(fimg[:, :3], fimg, torch.ones(1, 14, 512, device=DEV), noise_mode='none')
-    ref = golden('sr_large')['image']
+    img = sr.to(DEV)(fimg[:, :3], fimg, torch.ones(1, 14, 512, device=DEV), noise_mode='none')[..., ::2, ::2]
+    ref = golden('sr_large')['image_s2']
     err, psnr, rng = _maxdiff(img, ref), _psnr(img, ref), float(ref.max() - ref.min())
     print(f'large_sr (tc): max-abs {err:.3e} on range {rng:.1f}, PSNR {psnr:.1f} dB')
     assert err < 2e-3 * rng and psnr > 68.0, (err, psnr)

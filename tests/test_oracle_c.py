@@ -54,7 +54,7 @@ def test_c_rays_and_gather_vs_reference_fixture(clib, golden):
     clib.orc_gen_rays(_p(np.ascontiguousarray(c2w.numpy().reshape(N, 16))), _p(np.ascontiguousarray(K.numpy().reshape(N, 9))), N, res, _p(ro), _p(rd))
     assert float(np.abs(ro - g['ray_o'].numpy()).max()) < 1e-6 and float(np.abs(rd - g['ray_d'].numpy()).max()) < 1e-6
     s = golden('sample_small')
-    pl, co = np.ascontiguousarray(s['planes'].numpy()), np.ascontiguousarray(s['coords'].numpy())
+    pl, co = np.ascontiguousarray(g['planes'].numpy()), np.ascontiguousarray(s['coords'].numpy())     # the fixtures share their planes
     out = np.zeros((2, 3, 500, 32), np.float32)
     clib.orc_sample_planes(_p(pl), 2, 32, 32, _p(co), 500, C.c_float(1.0), _p(out))
     assert float(np.abs(out - s['feat'].numpy()).max()) < 1e-5

@@ -1,6 +1,6 @@
 #!/bin/bash
 # N GPUs of one box: exchange paths bit for bit, then the bench with the p2p exchange and with the NCCL all-gather.
-#   gpurun --gpus 2 --timeout 1800 -- 'bash tools/gpu_multi.sh 2'      (N = 8 is charged 8x: keep it short)
+#   bash tools/gpu_multi.sh 2
 N=${1:-2}
 mkdir -p gpurun_out
 TR="python -m torch.distributed.run --nnodes=1 --nproc-per-node $N --master-addr 127.0.0.1"

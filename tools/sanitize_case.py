@@ -1,6 +1,6 @@
 """Small end-to-end case for compute-sanitizer (memcheck / racecheck are ~100x slower: tiny shapes).
     compute-sanitizer --tool memcheck python tools/sanitize_case.py
-Covers: streaming render kernel (single pass), two-pass tcgen05 render kernel, tri-grid variant, tensor-core SR (all four conv launches,
+Covers: streaming render kernel (single pass), two-pass tensor-core render kernel, tri-grid variant, tensor-core SR (all four conv launches,
 FIR, edge) with fp16 and with split operands, uint8 epilogue, stand-alone sampler."""
 import os
 import sys
