@@ -54,7 +54,7 @@ struct ConvArgs {
 };
 
 // =====================================================================================================================
-// Persistent implicit-GEMM conv design (shared by conv_tc3_kernel<R>): R output rows (R x 128 pixels) x 128 couts per tile.
+// Persistent implicit-GEMM conv design (conv_tc3_kernel): R = kConvRows output rows (R x 128 pixels) x 128 couts per tile.
 //
 // The design cuts the operand fill traffic and the per-tile overheads:
 //   * an input ROW STRIP {64 ch, 130 px} is loaded once per 64-channel chunk and serves all horizontal taps (the wgmma smem
@@ -132,20 +132,6 @@ __device__ __forceinline__ float upsampled_skip_bf(const float* __restrict__ ip,
     return fmaf(ky1, r1, fmaf(ky0, r0, 0.f));
 }
 
-// 2 x fp32 arithmetic on the value pairs of the epilogue's bias / lrelu / ToRGB work
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
-__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
-
-__device__ __forceinline__ uint4 pack_half8(const float* f) {
-    __half2 h0 = __floats2half2_rn(f[0], f[1]), h1 = __floats2half2_rn(f[2], f[3]);
-    __half2 h2 = __floats2half2_rn(f[4], f[5]), h3 = __floats2half2_rn(f[6], f[7]);
-    uint4 pk;
-    pk.x = *reinterpret_cast<uint32_t*>(&h0); pk.y = *reinterpret_cast<uint32_t*>(&h1);
-    pk.z = *reinterpret_cast<uint32_t*>(&h2); pk.w = *reinterpret_cast<uint32_t*>(&h3);
-    return pk;
-}
-
 __device__ __forceinline__ void store_half32(__half* dst, const float* f) {
     uint4* d4 = reinterpret_cast<uint4*>(dst);
 #pragma unroll
@@ -160,27 +146,32 @@ __device__ __forceinline__ void store_half32(__half* dst, const float* f) {
 }
 
 // =====================================================================================================================
-// conv_tc3_kernel<R>: one CTA per unit stream, three warpgroups.  Warpgroup 0: one TMA lane (the other warps idle); warpgroups 1 and 2:
-// consumers, warpgroup c computes pixels [64 (c-1), 64 (c-1) + 64) of every output row of the tile x all 128 couts (wgmma M64 N128 K16,
-// fp32 accumulators in registers: R x 64 per thread).  After the K loop of a cout block the accumulators of each row go through a padded
-// fp32 staging tile in shared memory so that the epilogue keeps its thread-per-pixel layout (bias, activation, ToRGB sums, coalesced
-// fp16 stores).  Ring slots are released one MMA group late (wgmma.wait_group 1), so the tensor core always has the next tap queued.
+// conv_tc3_kernel: one CTA per unit stream, three warpgroups.  Warpgroup 0 hands most of its registers to the consumers (setmaxnreg 40) and
+// one lane of it issues the TMA loads; warpgroups 1 and 2 (setmaxnreg 232) are the consumers: warpgroup c computes pixels
+// [64 (c-1), 64 (c-1) + 64) of both output rows of the tile x all 128 couts (wgmma M64 N128 K16, fp32 accumulators in registers:
+// kConvRows x 64 per thread).  The epilogue works on the accumulator fragments: bias and activation per column in registers, ToRGB as
+// per-thread partial dot products summed over the quad, fp16 stores through a per-warp swizzled tile.  Ring slots are released one MMA
+// group late (wgmma.wait_group 1), so the tensor core always has the next tap queued.
 // =====================================================================================================================
+constexpr int kConvRows = 2;                                                 // output rows per tile
 constexpr int kThreads3 = 384;                                               // TMA warpgroup + 2 consumer warpgroups
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;                       // 128 x 40 + 256 x 232 <= 64 K registers
 constexpr int B3_BYTES = BN * BK * 2;                                        // 128 couts x 64 ch fp16 = 16 KB
-constexpr int kStageRow = BN + 8;                                            // fp32 staging row (pixel): 136 floats, conflict-free fragment stores
-template <int R> struct Cfg3 {
-    static constexpr int NA = 4, NB = 4;
-    static constexpr int TAIL = 8192;                                        // barriers, bias, ToRGB weights, [R][128][3] partial sums
-    static constexpr int STAGE = 8 * 32 * 64;                                // fp16 store staging: 8 epilogue warps x 32 px x 64 B
-    static constexpr int ACC = BM * kStageRow * 4;                           // fp32 accumulator staging of one output row
-    static constexpr int SMEM = NA * A2_SLOT + NB * B3_BYTES + 1024 + TAIL + STAGE + ACC;
+struct Cfg3 {
+    // ring depths: what the 227 KB of shared memory leave.  A 3x3 chunk needs kConvRows + 2 = 4 strips and 3 x 3 taps, so 6-deep rings let
+    // the producer fill the next chunk while the current one drains.
+    static constexpr int NA = 6, NB = 6;
+    static constexpr int TAIL = 8192;                                        // barriers, bias, ToRGB weights
+    static constexpr int STAGE = 8 * 8 * BN * 2;                             // fp16 store staging: 8 consumer warps x 8 px x 128 couts
+    static constexpr int SMEM = NA * A2_SLOT + NB * B3_BYTES + 1024 + TAIL + STAGE;
 };
+static_assert(Cfg3::SMEM <= 227 * 1024, "conv_tc3: shared memory over the sm_90 per-block limit");
 
-template <int R, bool SPLIT>
+template <bool SPLIT>
 __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                const __grid_constant__ CUtensorMap tmB, const Conv2Args a) {
-    using C = Cfg3<R>;
+    using C = Cfg3;
+    constexpr int R = kConvRows;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = align_smem_1024(smem_raw);
     uint8_t* a_ring = smem;
@@ -192,9 +183,7 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
     uint64_t* b_empty = b_full + C::NB;
     float* s_bias = reinterpret_cast<float*>(tail + 512);                    // [256]
     float* s_wrgb = s_bias + 256;                                            // [3][n_blocks*128]
-    float* s_part = s_wrgb + 768;                                            // [R][128][3] ToRGB partial sums of the second column group
-    uint4* s_stage = reinterpret_cast<uint4*>(tail + C::TAIL);               // [8 warps][32 px][4 x 16 B] fp16 store staging (XOR-swizzled)
-    float* s_acc = reinterpret_cast<float*>(tail + C::TAIL + C::STAGE);      // [128 px][kStageRow] fp32 accumulators of one output row
+    uint4* s_stage = reinterpret_cast<uint4*>(tail + C::TAIL);               // [8 warps][8 px][16 x 16 B] fp16 store staging (XOR-swizzled)
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int units_per_image = a.n_phases * a.row_groups * a.tiles_x;
@@ -227,7 +216,8 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
     };
 
     if (warp < 4) {
-        // ===== TMA producer (one lane): strips and taps in consumption order =====
+        setmaxnreg_dec<kProducerRegs>();
+        // ===== TMA producer (one lane): strips and taps in consumption order; the other three warps are done =====
         if (warp == 0 && lane == 0) {
             uint32_t aq = 0, bq = 0;                                         // running strip / tap sequence numbers
             for (int unit = blockIdx.x; unit < a.total_units; unit += gridDim.x) {
@@ -259,10 +249,11 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
             }
         }
     } else {
+        setmaxnreg_inc<kConsumerRegs>();
         // ===== consumers: warpgroup wg = 0, 1 multiplies pixels [64 wg, 64 wg + 64) of each row; then the epilogue =====
+        // The thread holds fragment rows (tile pixels) pix + 8 h, h = 0, 1, and columns (couts) 8 i + 2 quad + e of the cout block.
         const int wg = (warp >> 2) - 1;
-        const int q = warp & 3, m = q * 32 + lane;                           // epilogue: pixel m of the row, column group cg
-        const int cg = wg;
+        const int quad = lane & 3, pix = 64 * wg + 16 * (warp & 3) + (lane >> 2);
         const bool want_rgb = (a.mode == kToRgbFinal) || (a.mode == kActRgb);
         const int CW = a.n_blocks * BN;                                      // channels ToRGB sums over
         float brgb[3] = {0.f, 0.f, 0.f};
@@ -284,21 +275,25 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
             const int DY = tp.ngroups, NS = R + DY - 1;
             const int wn = a.w_shared ? 0 : n;
             if (want_rgb && wn != n_loaded) {
-                asm volatile("bar.sync 1, 256;" ::: "memory");               // all eight epilogue warps are done with the old weights
+                asm volatile("bar.sync 1, 256;" ::: "memory");               // all eight consumer warps are done with the old weights
                 for (int e = threadIdx.x - 128; e < 3 * CW; e += 256) s_wrgb[e] = a.wrgb[(size_t)wn * 3 * CW + e];
                 asm volatile("bar.sync 1, 256;" ::: "memory");
                 n_loaded = wn;
             }
-            const int gcol = col0 + m, X = gcol * a.ox_mul + P.ox_off;
-            float2 rgb2[R][3];                                               // ToRGB sums, even / odd channels in the two halves
+            // ToRGB: after the quad sum, lane quad = h (h = 0, 1) finishes pixel pix + 8 h of every row
+            const bool rgb_lane = want_rgb && quad < 2;
+            const int X = (col0 + pix + 8 * quad) * a.ox_mul + P.ox_off;
+            float rgb[R][2][3];
 #pragma unroll
-            for (int j = 0; j < R; ++j) { rgb2[j][0] = make_float2(0.f, 0.f); rgb2[j][1] = make_float2(0.f, 0.f); rgb2[j][2] = make_float2(0.f, 0.f); }
-            // skip-image taps of this thread's pixels, fetched by the SECOND column group and added to its partial sums (clamped addresses,
-            // zero weights outside the image: the loads are independent)
+            for (int j = 0; j < R; ++j)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) { rgb[j][h][0] = 0.f; rgb[j][h][1] = 0.f; rgb[j][h][2] = 0.f; }
+            // skip-image taps of the finishing lanes' pixels, fetched before the K loop (clamped addresses, zero weights outside the image:
+            // the loads are independent)
             float skipv[R][3];
 #pragma unroll
             for (int j = 0; j < R; ++j) { skipv[j][0] = 0.f; skipv[j][1] = 0.f; skipv[j][2] = 0.f; }
-            if (want_rgb && cg == 1 && a.img_prev) {
+            if (rgb_lane && a.img_prev) {
                 if (a.skip_same_res) {
                     const int Xc = min(X, a.img_W - 1);
 #pragma unroll
@@ -365,114 +360,110 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
 #pragma unroll
                 for (int j = 0; j < R; ++j) wg_fence_acc<64>(acc[j]);
                 release_pending();
-                // ---- epilogue, one output row at a time through the fp32 staging tile ----
+                // ---- epilogue on the fragments: d[4 i + 2 h + e] of row j is pixel pix + 8 h, cout nblk * 128 + 8 i + 2 quad + e ----
+                if (a.mode == kStoreRaw) {
+                    if (SPLIT) {
 #pragma unroll
-                for (int j = 0; j < R; ++j) {
+                        for (int j = 0; j < R; ++j)
 #pragma unroll
-                    for (int i = 0; i < 64; i += 2)
-                        *reinterpret_cast<float2*>(s_acc + (64 * wg + acc_row(i)) * kStageRow + acc_col(i)) = make_float2(acc[j][i], acc[j][i + 1]);
-                    asm volatile("bar.sync 4, 256;" ::: "memory");
-                    const int row = row0 + j;
-                    const int Y = row * a.oy_mul + P.oy_off;
-                    const bool row_ok = (row < P.rows) && (Y < a.out_H);
-                    const bool in_img = row_ok && (X < a.out_W);
-#pragma unroll 1
-                    for (int c0 = cg * (BN / 2); c0 < (cg + 1) * (BN / 2); c0 += 32) {
-                        float2 f2[16];
-                        const float4* src = reinterpret_cast<const float4*>(s_acc + m * kStageRow + c0);
-                        const float2 sc2 = make_float2(a.acc_scale, a.acc_scale);
+                            for (int i = 0; i < 64; ++i) acc[j][i] = __fmul_rn(acc[j][i], a.acc_scale);
+                    }
+                } else {
+                    // bias, leaky relu as max(v, v*slope) (slope <= 1), gain: bias_act lrelu*sqrt2 | nn.LeakyReLU | linear
 #pragma unroll
-                        for (int i = 0; i < 8; ++i) { const float4 v = src[i]; f2[2 * i] = make_float2(v.x, v.y); f2[2 * i + 1] = make_float2(v.z, v.w); }
-                        if (a.mode == kStoreRaw) {
-                            if (SPLIT) {
+                    for (int i = 0; i < 16; ++i) {
+                        const float2 b2 = *reinterpret_cast<const float2*>(s_bias + nblk * BN + 8 * i + 2 * quad);
 #pragma unroll
-                                for (int i = 0; i < 16; ++i) f2[i] = mul2(f2[i], sc2);
-                            }
-                        } else {
-                            // bias, leaky relu as max(v, v*slope) (slope <= 1), gain: bias_act lrelu*sqrt2 | nn.LeakyReLU | linear
-                            const float2* b2 = reinterpret_cast<const float2*>(s_bias + nblk * BN + c0);
-                            const float2 sl2 = make_float2(a.act_slope, a.act_slope), g2 = make_float2(a.act_gain, a.act_gain);
+                        for (int j = 0; j < R; ++j)
 #pragma unroll
-                            for (int i = 0; i < 16; ++i) {
-                                const float2 v = SPLIT ? fma2(f2[i], sc2, b2[i]) : add2(f2[i], b2[i]);
-                                const float2 t = mul2(v, sl2);
-                                f2[i] = mul2(make_float2(fmaxf(v.x, t.x), fmaxf(v.y, t.y)), g2);
-                            }
-                        }
-                        const float* f = reinterpret_cast<const float*>(f2);
-                        if (a.mode != kToRgbFinal) {
-                            // NHWC fp16 store through smem: the thread owns a pixel (32 channels = 64 B); written directly, every
-                            // STG.128 of the warp would touch 32 different lines.  Staged, 4 lanes write one pixel's 64 contiguous bytes.
-                            // Split mode: a second pass stores the fp16 remainders (v - fp16(v)) lo_off channels further.
-                            uint4* st = s_stage + (warp - 4) * 128;
-                            const int sw = (lane >> 1) & 3;
-                            constexpr int passes = SPLIT ? 2 : 1;
+                            for (int h = 0; h < 2; ++h)
 #pragma unroll
-                            for (int pass = 0; pass < passes; ++pass) {
-                                if (pass == 0) {
+                                for (int e = 0; e < 2; ++e) {
+                                    float& x = acc[j][4 * i + 2 * h + e];
+                                    const float b = e ? b2.y : b2.x;
+                                    const float v = SPLIT ? __fmaf_rn(x, a.acc_scale, b) : __fadd_rn(x, b);
+                                    x = __fmul_rn(fmaxf(v, __fmul_rn(v, a.act_slope)), a.act_gain);
+                                }
+                    }
+                }
+                if (a.mode != kToRgbFinal) {
+                    // NHWC fp16 store through smem, 8 pixels of the warp at a time: the fragment's 4-byte pairs go to pixel row lane / 4,
+                    // 16-byte chunk i ^ (lane / 4) (conflict-free), then each half-warp writes one pixel's 256 contiguous bytes.
+                    // Split mode: a second pass stores the fp16 remainders (v - fp16(v)) lo_off channels further.
+                    uint4* st = s_stage + (warp - 4) * 128;
+                    uint32_t* st32 = reinterpret_cast<uint32_t*>(st);
+                    const int sr = lane >> 2;
+                    constexpr int passes = SPLIT ? 2 : 1;
 #pragma unroll
-                                    for (int v = 0; v < 4; ++v) st[lane * 4 + (v ^ sw)] = pack_half8(f + 8 * v);
-                                } else {
+                    for (int j = 0; j < R; ++j) {
+                        const int row = row0 + j, Y = row * a.oy_mul + P.oy_off;
+                        const bool row_ok = (row < P.rows) && (Y < a.out_H);
 #pragma unroll
-                                    for (int v = 0; v < 4; ++v) {
-                                        float lo[8];
+                        for (int pass = 0; pass < passes; ++pass)
 #pragma unroll
-                                        for (int e = 0; e < 8; ++e) lo[e] = f[8 * v + e] - __half2float(__float2half_rn(f[8 * v + e]));
-                                        st[lane * 4 + (v ^ sw)] = pack_half8(lo);
-                                    }
+                            for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                                for (int i = 0; i < 16; ++i) {
+                                    float x0 = acc[j][4 * i + 2 * h], x1 = acc[j][4 * i + 2 * h + 1];
+                                    if (pass) { x0 = x0 - __half2float(__float2half_rn(x0)); x1 = x1 - __half2float(__float2half_rn(x1)); }
+                                    const __half2 hv = __floats2half2_rn(x0, x1);
+                                    st32[sr * 64 + (i ^ sr) * 4 + quad] = *reinterpret_cast<const uint32_t*>(&hv);
                                 }
                                 __syncwarp();
 #pragma unroll
-                                for (int i = 0; i < 4; ++i) {
-                                    const int p = i * 8 + (lane >> 2), cch = lane & 3;
-                                    uint4 pk = st[p * 4 + (cch ^ ((p >> 1) & 3))];
-                                    const int Xp = (col0 + q * 32 + p) * a.ox_mul + P.ox_off;
+                                for (int it = 0; it < 4; ++it) {
+                                    const int p = 2 * it + (lane >> 4), cch = lane & 15;
+                                    uint4 pk = st[p * 16 + (cch ^ p)];
+                                    const int Xp = (col0 + pix - sr + p + 8 * h) * a.ox_mul + P.ox_off;
                                     if (row_ok && Xp < a.out_W) {
-                                        const size_t eo = ((size_t)n * a.out_H + Y) * a.out_W * a.out_C + nblk * BN + (size_t)Xp * a.out_C + c0 + cch * 8 + pass * a.lo_off;
+                                        const size_t eo = ((size_t)n * a.out_H + Y) * a.out_W * a.out_C + nblk * BN + (size_t)Xp * a.out_C + cch * 8 + pass * a.lo_off;
                                         if (a.residual) {          // ResBlock2d: out = act(conv) + x (superresolution.py:283-288), same NHWC fp16 layout as the output
                                             const uint4 rv = __ldg(reinterpret_cast<const uint4*>(a.residual + eo));
-                                            __half2* ph = reinterpret_cast<__half2*>(&pk); const __half2* rh = reinterpret_cast<const __half2*>(&rv);
+                                            __half2* ph2 = reinterpret_cast<__half2*>(&pk); const __half2* rh = reinterpret_cast<const __half2*>(&rv);
 #pragma unroll
-                                            for (int e = 0; e < 4; ++e) { const float2 x = __half22float2(ph[e]), r = __half22float2(rh[e]); ph[e] = __floats2half2_rn(x.x + r.x, x.y + r.y); }
+                                            for (int e = 0; e < 4; ++e) { const float2 x = __half22float2(ph2[e]), r = __half22float2(rh[e]); ph2[e] = __floats2half2_rn(x.x + r.x, x.y + r.y); }
                                         }
                                         *reinterpret_cast<uint4*>(a.out + eo) = pk;
                                     }
                                 }
                                 __syncwarp();
                             }
-                        }
-                        if (want_rgb) {
-#pragma unroll
-                            for (int c = 0; c < 3; ++c) {
-                                const float4* w4 = reinterpret_cast<const float4*>(s_wrgb + c * CW + nblk * BN + c0);
-                                float2 accr = rgb2[j][c];
-#pragma unroll
-                                for (int j4 = 0; j4 < 8; ++j4) {
-                                    const float4 w = w4[j4];
-                                    accr = fma2(f2[2 * j4], make_float2(w.x, w.y), accr);
-                                    accr = fma2(f2[2 * j4 + 1], make_float2(w.z, w.w), accr);
-                                }
-                                rgb2[j][c] = accr;
-                            }
-                        }
                     }
-                    if (want_rgb && nblk == a.n_blocks - 1) {
-                        // the two column groups hold partial ToRGB sums of the same pixel: group 1 hands its sums to group 0 through smem
-                        if (cg == 1) {
+                }
+                if (want_rgb) {
+                    // per-thread partial dot products over the thread's 32 couts of this block, carried across the cout blocks
 #pragma unroll
-                            for (int c = 0; c < 3; ++c) s_part[(j * BM + m) * 3 + c] = (rgb2[j][c].x + rgb2[j][c].y) + skipv[j][c];
-                        }
-                        asm volatile("bar.sync 2, 256;" ::: "memory");
-                        if (cg == 0) {
+                    for (int c = 0; c < 3; ++c)
 #pragma unroll
-                            for (int c = 0; c < 3; ++c) rgb2[j][c].x = (rgb2[j][c].x + rgb2[j][c].y) + s_part[(j * BM + m) * 3 + c];
+                        for (int i = 0; i < 16; ++i) {
+                            const float2 w2 = *reinterpret_cast<const float2*>(s_wrgb + c * CW + nblk * BN + 8 * i + 2 * quad);
+#pragma unroll
+                            for (int j = 0; j < R; ++j)
+#pragma unroll
+                                for (int h = 0; h < 2; ++h)
+                                    rgb[j][h][c] = fmaf(acc[j][4 * i + 2 * h + 1], w2.y, fmaf(acc[j][4 * i + 2 * h], w2.x, rgb[j][h][c]));
                         }
-                        asm volatile("bar.sync 3, 256;" ::: "memory");
-                    }
-                    if (want_rgb && nblk == a.n_blocks - 1 && in_img && cg == 0) {
+                }
+            }
+            if (want_rgb) {
+                // the four lanes of a quad hold the partial sums of the same two pixels
+#pragma unroll
+                for (int j = 0; j < R; ++j)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
 #pragma unroll
                         for (int c = 0; c < 3; ++c) {
-                            float v = rgb2[j][c].x + brgb[c];
+                            rgb[j][h][c] += __shfl_xor_sync(0xffffffffu, rgb[j][h][c], 1);
+                            rgb[j][h][c] += __shfl_xor_sync(0xffffffffu, rgb[j][h][c], 2);
+                        }
+                if (rgb_lane) {
+#pragma unroll
+                    for (int j = 0; j < R; ++j) {
+                        const int row = row0 + j, Y = row * a.oy_mul + P.oy_off;
+                        if (row >= P.rows || Y >= a.out_H || X >= a.out_W) continue;
+#pragma unroll
+                        for (int c = 0; c < 3; ++c) {
+                            float v = ((quad ? rgb[j][1][c] : rgb[j][0][c]) + skipv[j][c]) + brgb[c];
                             if (a.out_clamp) v = fminf(fmaxf(v, -1.0f), 1.0f);
                             if (a.img_out_u8)          // torch: ((x + 1) / 2 * 255.).int() -> uint8, every step rounded in fp32, truncation
                                 a.img_out_u8[(((size_t)n * a.img_H + Y) * a.img_W + X) * 3 + c] =
@@ -481,7 +472,6 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
                                 a.img_out[(((size_t)n * 3 + c) * a.img_H + Y) * a.img_W + X] = v;
                         }
                     }
-                    asm volatile("bar.sync 5, 256;" ::: "memory");               // the staging tile is free for the next row
                 }
             }
         }
@@ -871,27 +861,19 @@ static void prof_mark(cudaStream_t st) {
 
 static unsigned long long* g_debug_buf = nullptr;
 static int g_debug_launch = 0;
-// output rows per tile: each consumer thread holds R x 64 fp32 accumulators; at R = 2 they no longer fit the 168 registers of a 384-thread CTA
-constexpr int kConvRows = 1;
-
-template <int R, bool SPLIT>
-static int launch_conv3_rs(const CUtensorMap& tmA, const CUtensorMap& tmB, Conv2Args a, int max_rows, cudaStream_t st) {
-    using C = Cfg3<R>;
-    R3DP_CUDA(cudaFuncSetAttribute(conv_tc3_kernel<R, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
+template <bool SPLIT>
+static int launch_conv3_s(const CUtensorMap& tmA, const CUtensorMap& tmB, Conv2Args a, int max_rows, cudaStream_t st) {
+    R3DP_CUDA(cudaFuncSetAttribute(conv_tc3_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg3::SMEM));
     a.debug = g_debug_buf ? g_debug_buf + 24 * (g_debug_launch++ % 32) : nullptr;
-    a.row_groups = (max_rows + R - 1) / R;
+    a.row_groups = (max_rows + kConvRows - 1) / kConvRows;
     a.total_units = a.n_images * a.n_phases * a.row_groups * a.tiles_x;
     const int grid = a.total_units < sm_count() ? a.total_units : sm_count();
     prof_mark(st);
-    conv_tc3_kernel<R, SPLIT><<<grid, kThreads3, C::SMEM, st>>>(tmA, tmB, a);
+    conv_tc3_kernel<SPLIT><<<grid, kThreads3, Cfg3::SMEM, st>>>(tmA, tmB, a);
     R3DP_LAUNCH_CHECK();
     prof_mark(st);
     count_launches(1);
     return 0;
-}
-template <int R>
-static int launch_conv3_r(const CUtensorMap& tmA, const CUtensorMap& tmB, const Conv2Args& a, int max_rows, cudaStream_t st) {
-    return a.split ? launch_conv3_rs<R, true>(tmA, tmB, a, max_rows, st) : launch_conv3_rs<R, false>(tmA, tmB, a, max_rows, st);
 }
 
 // taps given as (dy, dx, widx) lists -> sorted/grouped Taps2 (dy groups are contiguous for 3x3 and every transposed-conv phase)
@@ -926,7 +908,7 @@ static int run_conv2(const void* x, int N, int H, int W, int Cp, const void* wp,
     { static int mixv = -1; if (mixv < 0) { const char* e = getenv("R3DP_TC_MIX"); mixv = (e && e[0] == '0') ? 0 : 1; } a.phase_mix = mixv; }      // A/B knob
     if (a.act_gain == 0.f) { a.act_slope = 0.2f; a.act_gain = 1.4142135623730951f; }      // default: bias_act lrelu
     R3DP_REQUIRE(a.n_blocks >= 1 && a.n_blocks <= 2, "conv_tc3: 128 or 256 output channels");
-    return launch_conv3_r<kConvRows>(tmA, tmB, a, max_rows, st);
+    return a.split ? launch_conv3_s<true>(tmA, tmB, a, max_rows, st) : launch_conv3_s<false>(tmA, tmB, a, max_rows, st);
 }
 
 // v1-style single-phase description -> v2 launch

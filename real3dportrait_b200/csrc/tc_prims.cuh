@@ -38,6 +38,12 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, u
         "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
         ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
+// per-thread register budget of a warp-specialised CTA; every warp of an aligned warpgroup executes the call.  A producer warpgroup gives
+// registers back (dec), then the consumer warpgroups take them (inc blocks until the pool has enough).
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 // one lane of the (fully active) warp
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
