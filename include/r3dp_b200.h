@@ -266,6 +266,24 @@ int r3dp_sr_tcx_last_layer(const void* x_f16, const void* wp_f16, const float* b
  * head_torso_alpha_predictor of fuse mode v3, whose output is thresholded (sr_with_ref.py:129-143) and therefore wants fp32-grade arithmetic. */
 int r3dp_sr_tcx_conv(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
                      int act, void* y_f16, r3dp_stream_t stream);
+/* The torso head (SuperresolutionHybrid8XDC_Warp) and large_sr in split form.  Same arguments as the r3dp_sr_tc_* / r3dp_sr_* twin; every fp16 tensor is
+ * [hi | lo] (twice as wide, lo half at half the pixel stride) and every output is written as hi = fp16(v), lo = fp16(v - hi) of the full fp32 value v.
+ * r3dp_sr_tcx_conv_res            residual [N,H,W,2*O] summed to fp32 and added to the activated value BEFORE the hi/lo split (ResBlock2d)
+ * r3dp_sr_tcx_layer_torgb_noup    SynthesisBlockNoUp tail; ToRGB over the fp32 activation
+ * r3dp_sr_tcx_alpha_cat_ex        out [N,H,W,2*(Ca+Cb)] = split of cat[xa*alpha, xb*(1-alpha)]; stride_a / stride_b are the physical pixel strides
+ * r3dp_sr_tcx_alpha_mix           out [N,H,W,2*C] = split of xa*alpha + xb*(1-alpha); strides as above
+ * r3dp_sr_tcx_torgb_ex            x [N,H,W,2*C]: the dot product runs over hi + lo in fp32 */
+int r3dp_sr_tcx_conv_res(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
+                         int act, const void* residual_f16, void* y_f16, r3dp_stream_t stream);
+int r3dp_sr_tcx_layer_torgb_noup(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
+                                 const float* img_prev, int N, int Nw, int I, int O, int H, int W, void* y_f16, float* img_out,
+                                 r3dp_stream_t stream);
+int r3dp_sr_tcx_alpha_cat_ex(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, int xb_shared, const float* alpha,
+                             int N, int H, int W, void* out_f16, r3dp_stream_t stream);
+int r3dp_sr_tcx_alpha_mix(const void* xa_f16, int stride_a, const void* xb_f16, int stride_b, const float* alpha, int C, int N, int H, int W,
+                          void* out_f16, r3dp_stream_t stream);
+int r3dp_sr_tcx_torgb_ex(const void* x_f16, const float* wrgb, const float* brgb, const float* img_prev, int same_res, int N, int Nw, int C,
+                         int H, int W, float* img_out, r3dp_stream_t stream);
 
 /* Measurement hooks (bench.py): time every tensor-core conv launch with a CUDA-event pair on its launching stream. */
 int r3dp_sr_tc_prof(int enable);

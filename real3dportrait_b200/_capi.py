@@ -88,6 +88,11 @@ _SIGNATURES = {
     'r3dp_sr_tc_input_nhwc_rgb': (_I, [_P, _I, _I, _I, _I, _I, _P, _P, _I, _P]),
     'r3dp_sr_tc_conv': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     'r3dp_sr_tcx_conv': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
+    'r3dp_sr_tcx_conv_res': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
+    'r3dp_sr_tcx_layer_torgb_noup': (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
+    'r3dp_sr_tcx_alpha_cat_ex': (_I, [_P, _I, _I, _P, _I, _I, _I, _P, _I, _I, _I, _P, _P]),
+    'r3dp_sr_tcx_alpha_mix': (_I, [_P, _I, _P, _I, _P, _I, _I, _I, _I, _P, _P]),
+    'r3dp_sr_tcx_torgb_ex': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P]),
     'r3dp_sr_alpha_mix': (_I, [_P, _I, _P, _I, _P, _I, _I, _I, _I, _P, _P]),
     'r3dp_sr_alpha_gate': (_I, [_P, _I, _I, _P, _I, _I, _I, _P, _P]),
     'r3dp_sr_tc_conv_res': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),

@@ -386,6 +386,27 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
                                 }
                     }
                 }
+                if (SPLIT && a.residual) {
+                    // ResBlock2d with split operands: the residual [hi | lo] (the output's layout) is summed to fp32 and added to the activated
+                    // value BEFORE the hi/lo split, so the stored pair is the split of the full fp32 sum
+#pragma unroll
+                    for (int j = 0; j < R; ++j) {
+                        const int row = row0 + j, Y = row * a.oy_mul + P.oy_off;
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const int Xr = (col0 + pix + 8 * h) * a.ox_mul + P.ox_off;
+                            if (row >= P.rows || Y >= a.out_H || Xr >= a.out_W) continue;
+                            const __half* rp = a.residual + (((size_t)n * a.out_H + Y) * a.out_W + Xr) * a.out_C + nblk * BN + 2 * quad;
+#pragma unroll
+                            for (int i = 0; i < 16; ++i) {
+                                const float2 rh = __half22float2(__ldg(reinterpret_cast<const __half2*>(rp + 8 * i)));
+                                const float2 rl = __half22float2(__ldg(reinterpret_cast<const __half2*>(rp + a.lo_off + 8 * i)));
+                                acc[j][4 * i + 2 * h] += rh.x + rl.x;
+                                acc[j][4 * i + 2 * h + 1] += rh.y + rl.y;
+                            }
+                        }
+                    }
+                }
                 if (a.mode != kToRgbFinal) {
                     // NHWC fp16 store through smem, 8 pixels of the warp at a time: the fragment's 4-byte pairs go to pixel row lane / 4,
                     // 16-byte chunk i ^ (lane / 4) (conflict-free), then each half-warp writes one pixel's 256 contiguous bytes.
@@ -417,7 +438,7 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
                                     const int Xp = (col0 + pix - sr + p + 8 * h) * a.ox_mul + P.ox_off;
                                     if (row_ok && Xp < a.out_W) {
                                         const size_t eo = ((size_t)n * a.out_H + Y) * a.out_W * a.out_C + nblk * BN + (size_t)Xp * a.out_C + cch * 8 + pass * a.lo_off;
-                                        if (a.residual) {          // ResBlock2d: out = act(conv) + x (superresolution.py:283-288), same NHWC fp16 layout as the output
+                                        if (!SPLIT && a.residual) {          // ResBlock2d: out = act(conv) + x (superresolution.py:283-288), same NHWC fp16 layout as the output
                                             const uint4 rv = __ldg(reinterpret_cast<const uint4*>(a.residual + eo));
                                             __half2* ph2 = reinterpret_cast<__half2*>(&pk); const __half2* rh = reinterpret_cast<const __half2*>(&rv);
 #pragma unroll
@@ -758,6 +779,8 @@ __global__ void __launch_bounds__(256) upconv_edge_split_kernel(const __half* __
 
 // ToRGB for the first block: x NHWC fp16 [N][H][W][C] -> img_out NCHW fp32 = upsample2d(img_prev) + conv1x1 + bias.  One warp per
 // 32 consecutive pixels is wasteful on loads, so: one thread per pixel, 16-byte channel vectors, weights in smem.
+// SPLIT: x is [N][H][W][2C] = [hi | lo]; the dot product runs over hi + lo in fp32.
+template <bool SPLIT>
 __global__ void __launch_bounds__(256) torgb_f16_kernel(const __half* __restrict__ x, const float* __restrict__ wrgb, const float* __restrict__ brgb,
                                                         const float* __restrict__ img_prev, int H, int W, int C, int w_shared, int same_res,
                                                         float* __restrict__ img_out) {
@@ -769,14 +792,18 @@ __global__ void __launch_bounds__(256) torgb_f16_kernel(const __half* __restrict
     const int pix = blockIdx.x * blockDim.x + threadIdx.x;
     if (pix >= H * W) return;
     const int Y = pix / W, X = pix - Y * W;
-    const uint4* xp = reinterpret_cast<const uint4*>(x + ((size_t)n * H * W + pix) * C);
+    const uint4* xp = reinterpret_cast<const uint4*>(x + ((size_t)n * H * W + pix) * (SPLIT ? 2 * C : C));
     float r = 0.f, g = 0.f, b = 0.f;
     for (int c8 = 0; c8 < C / 8; ++c8) {
         const uint4 raw = __ldg(xp + c8);
         const __half2* h = reinterpret_cast<const __half2*>(&raw);
+        uint4 rawl = make_uint4(0, 0, 0, 0);
+        if (SPLIT) rawl = __ldg(xp + C / 8 + c8);
+        const __half2* hl = reinterpret_cast<const __half2*>(&rawl);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            const float2 f = __half22float2(h[j]);
+            float2 f = __half22float2(h[j]);
+            if (SPLIT) { const float2 fl = __half22float2(hl[j]); f.x += fl.x; f.y += fl.y; }
             const int c = c8 * 8 + 2 * j;
             r = fmaf(f.x, s_w[c], r); r = fmaf(f.y, s_w[c + 1], r);
             g = fmaf(f.x, s_w[C + c], g); g = fmaf(f.y, s_w[C + c + 1], g);
@@ -902,7 +929,7 @@ static int run_conv2(const void* x, int N, int H, int W, int Cp, const void* wp,
     const uint64_t Cphys = (uint64_t)Cp * (a.split ? 2 : 1);                      // split: [hi | lo] halves of Cp channels each
     if (make_map_4d_box(&tmA, x, Cphys, (uint64_t)W, (uint64_t)H, (uint64_t)N, A2_ROWS)) return 1;
     if (make_map_4d_box(&tmB, wp, Cphys, (uint64_t)O, (uint64_t)n_taps, (uint64_t)Nw, BN)) return 1;
-    if (a.split) { R3DP_REQUIRE(a.residual == nullptr, "conv_tc3: the residual epilogue is not built for split operands"); a.acc_scale = 1.0f / kSplitWeightScale; a.lo_off = a.out_C; a.out_C *= 2; }
+    if (a.split) { a.acc_scale = 1.0f / kSplitWeightScale; a.lo_off = a.out_C; a.out_C *= 2; }
     else { a.acc_scale = 1.0f; a.lo_off = 0; }
     a.k_chunks = Cp / BK; a.tiles_x = W / BM; a.n_blocks = O / BN; a.n_images = N; a.w_shared = (Nw == 1);
     { static int mixv = -1; if (mixv < 0) { const char* e = getenv("R3DP_TC_MIX"); mixv = (e && e[0] == '0') ? 0 : 1; } a.phase_mix = mixv; }      // A/B knob
@@ -1075,16 +1102,25 @@ extern "C" int r3dp_sr_tc_last_layer(const void* x_f16, const void* wp_f16, cons
 }
 
 // ToRGB of a non-final block: x NHWC fp16 [N][H][W][C] -> img_out NCHW fp32 [N][3][H][W] (+ upsample2d(img_prev) + bias).
-extern "C" int r3dp_sr_tc_torgb_ex(const void* x_f16, const float* wrgb, const float* brgb, const float* img_prev, int same_res, int N, int Nw, int C,
-                                   int H, int W, float* img_out, r3dp_stream_t stream) {
+static int torgb_impl(const void* x_f16, const float* wrgb, const float* brgb, const float* img_prev, int same_res, int N, int Nw, int C,
+                      int H, int W, float* img_out, int split, r3dp_stream_t stream) {
     R3DP_REQUIRE(x_f16 && wrgb && brgb && img_out, "sr_tc_torgb: null pointer");
     R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && C % 8 == 0 && H % 2 == 0 && W % 2 == 0, "sr_tc_torgb: bad shape");
     dim3 grid((H * W + 255) / 256, N);
-    torgb_f16_kernel<<<grid, 256, 3 * C * sizeof(float), as_stream(stream)>>>(reinterpret_cast<const __half*>(x_f16), wrgb, brgb, img_prev, H, W, C,
-                                                                              Nw == 1, same_res, img_out);
+    auto kern = split ? torgb_f16_kernel<true> : torgb_f16_kernel<false>;
+    kern<<<grid, 256, 3 * C * sizeof(float), as_stream(stream)>>>(reinterpret_cast<const __half*>(x_f16), wrgb, brgb, img_prev, H, W, C,
+                                                                  Nw == 1, same_res, img_out);
     R3DP_LAUNCH_CHECK();
     count_launches(1);
     return 0;
+}
+extern "C" int r3dp_sr_tc_torgb_ex(const void* x_f16, const float* wrgb, const float* brgb, const float* img_prev, int same_res, int N, int Nw, int C,
+                                   int H, int W, float* img_out, r3dp_stream_t stream) {
+    return torgb_impl(x_f16, wrgb, brgb, img_prev, same_res, N, Nw, C, H, W, img_out, 0, stream);
+}
+extern "C" int r3dp_sr_tcx_torgb_ex(const void* x_f16, const float* wrgb, const float* brgb, const float* img_prev, int same_res, int N, int Nw, int C,
+                                    int H, int W, float* img_out, r3dp_stream_t stream) {
+    return torgb_impl(x_f16, wrgb, brgb, img_prev, same_res, N, Nw, C, H, W, img_out, 1, stream);
 }
 extern "C" int r3dp_sr_tc_torgb(const void* x_f16, const float* wrgb, const float* brgb, const float* img_prev, int N, int Nw, int C, int H,
                                 int W, float* img_out, r3dp_stream_t stream) {
@@ -1295,6 +1331,11 @@ extern "C" int r3dp_sr_tcx_conv(const void* x_f16, const void* wp_f16, const flo
                                 int act, void* y_f16, r3dp_stream_t stream) {
     return conv_res_impl(x_f16, wp_f16, bias, N, Nw, I, O, H, W, ksize, act, nullptr, y_f16, 1, stream);
 }
+// ... with the residual in the output's [hi | lo] layout, added to the activated fp32 value before the split (ResBlock2d of large_sr)
+extern "C" int r3dp_sr_tcx_conv_res(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
+                                    int act, const void* residual_f16, void* y_f16, r3dp_stream_t stream) {
+    return conv_res_impl(x_f16, wp_f16, bias, N, Nw, I, O, H, W, ksize, act, residual_f16, y_f16, 1, stream);
+}
 extern "C" int r3dp_sr_tc_conv(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
                                int act, void* y_f16, r3dp_stream_t stream) {
     return r3dp_sr_tc_conv_res(x_f16, wp_f16, bias, N, Nw, I, O, H, W, ksize, act, nullptr, y_f16, stream);
@@ -1302,9 +1343,9 @@ extern "C" int r3dp_sr_tc_conv(const void* x_f16, const void* wp_f16, const floa
 
 // SynthesisBlockNoUp tail (superresolution.py:159-258): conv3x3 (modulated, up == 1) + bias/lrelu -> y, and img_out = img_prev (SAME resolution)
 // + ToRGB(y) + brgb.
-extern "C" int r3dp_sr_tc_layer_torgb_noup(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
-                                           const float* img_prev, int N, int Nw, int I, int O, int H, int W, void* y_f16, float* img_out,
-                                           r3dp_stream_t stream) {
+static int layer_torgb_noup_impl(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
+                                 const float* img_prev, int N, int Nw, int I, int O, int H, int W, void* y_f16, float* img_out, int split,
+                                 r3dp_stream_t stream) {
     R3DP_REQUIRE(x_f16 && wp_f16 && bias && wrgb && brgb && y_f16 && img_out, "sr_tc_layer_torgb_noup: null pointer");
     R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && W % BM == 0 && O % BN == 0 && O <= 256, "sr_tc_layer_torgb_noup: bad shape");
     const int Ip = (I + 63) / 64 * 64;
@@ -1317,10 +1358,24 @@ extern "C" int r3dp_sr_tc_layer_torgb_noup(const void* x_f16, const void* wp_f16
     a.ph[0].rows = H;
     a.mode = kActRgb; a.out = reinterpret_cast<__half*>(y_f16); a.out_H = H; a.out_W = W; a.out_C = O; a.oy_mul = a.ox_mul = 1;
     a.bias = bias; a.wrgb = wrgb; a.brgb = brgb; a.img_prev = img_prev; a.img_out = img_out; a.img_H = H; a.img_W = W; a.skip_same_res = 1;
+    a.split = split;
     return run_conv2(x_f16, N, H, W, Ip, wp_f16, Nw, O, a, H, as_stream(stream));
+}
+extern "C" int r3dp_sr_tc_layer_torgb_noup(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
+                                           const float* img_prev, int N, int Nw, int I, int O, int H, int W, void* y_f16, float* img_out,
+                                           r3dp_stream_t stream) {
+    return layer_torgb_noup_impl(x_f16, wp_f16, bias, wrgb, brgb, img_prev, N, Nw, I, O, H, W, y_f16, img_out, 0, stream);
+}
+extern "C" int r3dp_sr_tcx_layer_torgb_noup(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
+                                            const float* img_prev, int N, int Nw, int I, int O, int H, int W, void* y_f16, float* img_out,
+                                            r3dp_stream_t stream) {
+    return layer_torgb_noup_impl(x_f16, wp_f16, bias, wrgb, brgb, img_prev, N, Nw, I, O, H, W, y_f16, img_out, 1, stream);
 }
 
 // out[n,y,x,:] = [ xa[n,y,x,0:Ca] * alpha[n,y,x] , xb[n,y,x,0:Cb] * (1 - alpha[n,y,x]) ]   (sr_with_ref.py:111,122: alpha-cat fusion), fp16 NHWC
+// SPLIT: xa / xb hold [hi | lo] halves (lo at half their pixel stride); hi + lo is scaled in fp32 and the output is the [hi | lo] layout of the
+// (Ca + Cb)-channel result: out [N,H,W, 2 (Ca + Cb)], lo at channel Ca + Cb.
+template <bool SPLIT>
 __global__ void alpha_cat_kernel(const __half* __restrict__ xa, int Ca, int sa, const __half* __restrict__ xb, int Cb, int sb,
                                  long long hw_b, const float* __restrict__ alpha, long long npix, __half* __restrict__ out) {
     const int cv = (Ca + Cb) / 8;
@@ -1330,25 +1385,53 @@ __global__ void alpha_cat_kernel(const __half* __restrict__ xa, int Ca, int sa, 
     const float al = alpha[pix];
     const bool first = c8 * 8 < Ca;
     const long long pb = hw_b > 0 ? pix % hw_b : pix;                    // xb holds one frame shared by the batch
-    const uint4 raw = __ldg(reinterpret_cast<const uint4*>(first ? xa + pix * sa + c8 * 8 : xb + pb * sb + (c8 * 8 - Ca)));
+    const __half* src = first ? xa + pix * sa + c8 * 8 : xb + pb * sb + (c8 * 8 - Ca);
+    const uint4 raw = __ldg(reinterpret_cast<const uint4*>(src));
     const float m = first ? al : 1.0f - al;
     const __half2* h = reinterpret_cast<const __half2*>(&raw);
     uint4 pk; __half2* ph = reinterpret_cast<__half2*>(&pk);
+    if (!SPLIT) {
 #pragma unroll
-    for (int j = 0; j < 4; ++j) { const float2 f = __half22float2(h[j]); ph[j] = __floats2half2_rn(f.x * m, f.y * m); }
-    *reinterpret_cast<uint4*>(out + idx * 8) = pk;
+        for (int j = 0; j < 4; ++j) { const float2 f = __half22float2(h[j]); ph[j] = __floats2half2_rn(f.x * m, f.y * m); }
+        *reinterpret_cast<uint4*>(out + idx * 8) = pk;
+        return;
+    }
+    const uint4 rawl = __ldg(reinterpret_cast<const uint4*>(src + (first ? sa : sb) / 2));
+    const __half2* hl = reinterpret_cast<const __half2*>(&rawl);
+    uint4 pl; __half2* pq = reinterpret_cast<__half2*>(&pl);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const float2 f = __half22float2(h[j]), g = __half22float2(hl[j]);
+        const float v0 = (f.x + g.x) * m, v1 = (f.y + g.y) * m;
+        ph[j] = __floats2half2_rn(v0, v1);
+        const float2 hf = __half22float2(ph[j]);
+        pq[j] = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
+    }
+    __half* dst = out + pix * 2 * (Ca + Cb) + c8 * 8;
+    *reinterpret_cast<uint4*>(dst) = pk;
+    *reinterpret_cast<uint4*>(dst + Ca + Cb) = pl;
 }
-extern "C" int r3dp_sr_alpha_cat_ex(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, int xb_shared,
-                                    const float* alpha, int N, int H, int W, void* out_f16, r3dp_stream_t stream) {
+static int alpha_cat_impl(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, int xb_shared,
+                          const float* alpha, int N, int H, int W, void* out_f16, int split, r3dp_stream_t stream) {
     R3DP_REQUIRE(xa_f16 && xb_f16 && alpha && out_f16, "sr_alpha_cat: null pointer");
-    R3DP_REQUIRE(N > 0 && H > 0 && W > 0 && Ca % 8 == 0 && Cb % 8 == 0 && stride_a >= Ca && stride_b >= Cb && stride_a % 8 == 0 && stride_b % 8 == 0,
-                 "sr_alpha_cat: bad shape");
+    const int wide = split ? 2 : 1;
+    R3DP_REQUIRE(N > 0 && H > 0 && W > 0 && Ca % 8 == 0 && Cb % 8 == 0 && stride_a >= wide * Ca && stride_b >= wide * Cb &&
+                 stride_a % (8 * wide) == 0 && stride_b % (8 * wide) == 0, "sr_alpha_cat: bad shape");
     const long long npix = (long long)N * H * W, total = npix * ((Ca + Cb) / 8);
-    alpha_cat_kernel<<<(unsigned)((total + 255) / 256), 256, 0, as_stream(stream)>>>(reinterpret_cast<const __half*>(xa_f16), Ca, stride_a,
+    auto kern = split ? alpha_cat_kernel<true> : alpha_cat_kernel<false>;
+    kern<<<(unsigned)((total + 255) / 256), 256, 0, as_stream(stream)>>>(reinterpret_cast<const __half*>(xa_f16), Ca, stride_a,
         reinterpret_cast<const __half*>(xb_f16), Cb, stride_b, xb_shared ? (long long)H * W : 0ll, alpha, npix, reinterpret_cast<__half*>(out_f16));
     R3DP_LAUNCH_CHECK();
     count_launches(1);
     return 0;
+}
+extern "C" int r3dp_sr_alpha_cat_ex(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, int xb_shared,
+                                    const float* alpha, int N, int H, int W, void* out_f16, r3dp_stream_t stream) {
+    return alpha_cat_impl(xa_f16, Ca, stride_a, xb_f16, Cb, stride_b, xb_shared, alpha, N, H, W, out_f16, 0, stream);
+}
+extern "C" int r3dp_sr_tcx_alpha_cat_ex(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, int xb_shared,
+                                        const float* alpha, int N, int H, int W, void* out_f16, r3dp_stream_t stream) {
+    return alpha_cat_impl(xa_f16, Ca, stride_a, xb_f16, Cb, stride_b, xb_shared, alpha, N, H, W, out_f16, 1, stream);
 }
 extern "C" int r3dp_sr_alpha_cat(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, const float* alpha, int N,
                                  int H, int W, void* out_f16, r3dp_stream_t stream) {
@@ -1428,6 +1511,8 @@ extern "C" int r3dp_sr_resize_aa_down2(const float* x, int N, int C, int h_out, 
 }
 
 // out[n,y,x,0:C] = xa * alpha + xb * (1 - alpha)  (htbsr_head_weight_fuse_mode v1, sr_with_ref.py:98: plain alpha blend of the head and torso features), fp16 NHWC
+// SPLIT: xa / xb hold [hi | lo] halves (lo at half their pixel stride); the blend of hi + lo runs in fp32, out [N,H,W,2C] = [hi | lo]
+template <bool SPLIT>
 __global__ void alpha_mix_kernel(const __half* __restrict__ xa, int sa, const __half* __restrict__ xb, int sb, const float* __restrict__ alpha, int C,
                                  long long npix, __half* __restrict__ out) {
     const int cv = C / 8;
@@ -1438,20 +1523,47 @@ __global__ void alpha_mix_kernel(const __half* __restrict__ xa, int sa, const __
     const uint4 ra = __ldg(reinterpret_cast<const uint4*>(xa + pix * sa + c8 * 8)), rb = __ldg(reinterpret_cast<const uint4*>(xb + pix * sb + c8 * 8));
     const __half2* ha = reinterpret_cast<const __half2*>(&ra); const __half2* hb = reinterpret_cast<const __half2*>(&rb);
     uint4 pk; __half2* ph = reinterpret_cast<__half2*>(&pk);
+    if (!SPLIT) {
 #pragma unroll
-    for (int j = 0; j < 4; ++j) { const float2 a = __half22float2(ha[j]), b = __half22float2(hb[j]); ph[j] = __floats2half2_rn(a.x * al + b.x * (1.0f - al), a.y * al + b.y * (1.0f - al)); }
-    *reinterpret_cast<uint4*>(out + idx * 8) = pk;
+        for (int j = 0; j < 4; ++j) { const float2 a = __half22float2(ha[j]), b = __half22float2(hb[j]); ph[j] = __floats2half2_rn(a.x * al + b.x * (1.0f - al), a.y * al + b.y * (1.0f - al)); }
+        *reinterpret_cast<uint4*>(out + idx * 8) = pk;
+        return;
+    }
+    const uint4 rla = __ldg(reinterpret_cast<const uint4*>(xa + pix * sa + sa / 2 + c8 * 8)), rlb = __ldg(reinterpret_cast<const uint4*>(xb + pix * sb + sb / 2 + c8 * 8));
+    const __half2* la = reinterpret_cast<const __half2*>(&rla); const __half2* lb = reinterpret_cast<const __half2*>(&rlb);
+    uint4 pl; __half2* pq = reinterpret_cast<__half2*>(&pl);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const float2 a = __half22float2(ha[j]), b = __half22float2(hb[j]), al2 = __half22float2(la[j]), bl2 = __half22float2(lb[j]);
+        const float v0 = (a.x + al2.x) * al + (b.x + bl2.x) * (1.0f - al), v1 = (a.y + al2.y) * al + (b.y + bl2.y) * (1.0f - al);
+        ph[j] = __floats2half2_rn(v0, v1);
+        const float2 hf = __half22float2(ph[j]);
+        pq[j] = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
+    }
+    __half* dst = out + pix * 2 * C + c8 * 8;
+    *reinterpret_cast<uint4*>(dst) = pk;
+    *reinterpret_cast<uint4*>(dst + C) = pl;
 }
-extern "C" int r3dp_sr_alpha_mix(const void* xa_f16, int stride_a, const void* xb_f16, int stride_b, const float* alpha, int C, int N, int H, int W,
-                                 void* out_f16, r3dp_stream_t stream) {
-    R3DP_REQUIRE(xa_f16 && xb_f16 && alpha && out_f16 && N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && stride_a >= C && stride_b >= C &&
-                 stride_a % 8 == 0 && stride_b % 8 == 0, "sr_alpha_mix: bad arguments");
+static int alpha_mix_impl(const void* xa_f16, int stride_a, const void* xb_f16, int stride_b, const float* alpha, int C, int N, int H, int W,
+                          void* out_f16, int split, r3dp_stream_t stream) {
+    const int wide = split ? 2 : 1;
+    R3DP_REQUIRE(xa_f16 && xb_f16 && alpha && out_f16 && N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && stride_a >= wide * C && stride_b >= wide * C &&
+                 stride_a % (8 * wide) == 0 && stride_b % (8 * wide) == 0, "sr_alpha_mix: bad arguments");
     const long long npix = (long long)N * H * W, total = npix * (C / 8);
-    alpha_mix_kernel<<<(unsigned)((total + 255) / 256), 256, 0, as_stream(stream)>>>(reinterpret_cast<const __half*>(xa_f16), stride_a,
+    auto kern = split ? alpha_mix_kernel<true> : alpha_mix_kernel<false>;
+    kern<<<(unsigned)((total + 255) / 256), 256, 0, as_stream(stream)>>>(reinterpret_cast<const __half*>(xa_f16), stride_a,
         reinterpret_cast<const __half*>(xb_f16), stride_b, alpha, C, npix, reinterpret_cast<__half*>(out_f16));
     R3DP_LAUNCH_CHECK();
     count_launches(1);
     return 0;
+}
+extern "C" int r3dp_sr_alpha_mix(const void* xa_f16, int stride_a, const void* xb_f16, int stride_b, const float* alpha, int C, int N, int H, int W,
+                                 void* out_f16, r3dp_stream_t stream) {
+    return alpha_mix_impl(xa_f16, stride_a, xb_f16, stride_b, alpha, C, N, H, W, out_f16, 0, stream);
+}
+extern "C" int r3dp_sr_tcx_alpha_mix(const void* xa_f16, int stride_a, const void* xb_f16, int stride_b, const float* alpha, int C, int N, int H, int W,
+                                     void* out_f16, r3dp_stream_t stream) {
+    return alpha_mix_impl(xa_f16, stride_a, xb_f16, stride_b, alpha, C, N, H, W, out_f16, 1, stream);
 }
 
 // out[n,0,y,x] = min(sigmoid(logit), cap[n,0,y,x]) with logit = channel 0 of an NHWC fp16 tensor (+ its lo half lo_off channels further when lo_off > 0):

@@ -97,15 +97,16 @@ def pack_plain(conv: torch.nn.Conv2d, in_tensor_channels: int, out_pad: int = 12
     return packed, bias, k
 
 
-def conv_plain(x16: torch.Tensor, packed, act: int, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
+def conv_plain(x16: torch.Tensor, packed, act: int, residual: Optional[torch.Tensor] = None, split: bool = False) -> torch.Tensor:
     """x16 [N,H,W,Ct] fp16 -> [N,H,W,Opad] fp16; act 0 linear, 2 nn.LeakyReLU(0.01), 3 ReLU; residual (same shape as the output) is added
-    after the activation (ResBlock2d)."""
+    after the activation (ResBlock2d).  split: [hi | lo] tensors of twice the channels, weights from pack_plain(split=True)."""
     wp, bias, k = packed
     N, H, W, Ct = x16.shape
-    y = torch.empty(N, H, W, wp.shape[2], device=x16.device, dtype=torch.float16)
+    wide = 2 if split else 1
+    y = torch.empty(N, H, W, wp.shape[2] * wide, device=x16.device, dtype=torch.float16)
     with capi.region('sr_conv'):
-        capi.check(capi.lib().r3dp_sr_tc_conv_res(capi.ptr(x16, torch.float16), capi.ptr(wp, torch.float16), capi.ptr(bias), N, 1, Ct, wp.shape[2], H, W, k, act,
-                                                  capi.ptr(residual, torch.float16), capi.ptr(y, torch.float16), capi.stream()))
+        capi.check(_fn('conv_res', split)(capi.ptr(x16, torch.float16), capi.ptr(wp, torch.float16), capi.ptr(bias), N, 1, Ct // wide, wp.shape[2], H, W, k,
+                                          act, capi.ptr(residual, torch.float16), capi.ptr(y, torch.float16), capi.stream()))
     return y
 
 
@@ -139,8 +140,6 @@ def forward(sr, rgb: Optional[torch.Tensor], x: torch.Tensor, ws3: Optional[torc
     N = x.shape[0]
     split = getattr(sr, 'sr_mode', 'tc') == 'tc_exact'          # fp32-grade: split fp16 operands, three MMAs per product
     wide = 2 if split else 1
-    if split and getattr(sr, 'large_sr', False):
-        raise NotImplementedError("large_sr runs with sr_mode='tc' (its residual epilogue is not built for split operands)")
     prep = getattr(sr, 'static_prepared', None)
     if prep is not None and prep.split != split:
         prep = None
@@ -172,7 +171,7 @@ def forward(sr, rgb: Optional[torch.Tensor], x: torch.Tensor, ws3: Optional[torc
                                             capi.ptr(prep.wrgb0), capi.ptr(capi.f32(b0.torgb.bias)), capi.ptr(rgb0), N, Nw, 256, 256, 256, 256,
                                             capi.ptr(a1, torch.float16), capi.ptr(img1), capi.stream()))
     if getattr(sr, 'large_sr', False):
-        return _forward_large_tail(sr, a1, img1, prep, out_clamp, out_uint8)
+        return _forward_large_tail(sr, a1, img1, prep, out_clamp, out_uint8, split)
     a2 = layer(a1, b1.conv0, wp[2], 2, split)
     out = torch.empty(N, 512, 512, 3, device=x.device, dtype=torch.uint8) if out_uint8 else torch.empty(N, 3, 512, 512, device=x.device)
     with capi.region('sr_conv'):                               # block1.conv1 + block1.torgb: the 128-channel activation is never written
@@ -183,45 +182,45 @@ def forward(sr, rgb: Optional[torch.Tensor], x: torch.Tensor, ws3: Optional[torc
     return out
 
 
-def _large_packed(sr):
-    """Packed plain convolutions of the large_sr residual blocks / to_rgb layers (cached until the parameters are reloaded)."""
+def _large_packed(sr, split: bool = False):
+    """Packed plain convolutions of the large_sr residual blocks / to_rgb layers (cached until the parameters are reloaded or the mode changes)."""
     c = getattr(sr, '_large_cache', None)
-    if c is None:
-        c = {}
+    if c is None or c['split'] != split:
+        c = {'split': split}
         for name, blk, ch in (('b0', sr.block0, 256), ('b1', sr.block1, 128)):
-            c[name] = [(pack_plain(rb.conv1, ch), pack_plain(rb.conv2, ch)) for rb in blk.resblocks]
+            c[name] = [(pack_plain(rb.conv1, ch, split=split), pack_plain(rb.conv2, ch, split=split)) for rb in blk.resblocks]
             c[name + '_rgb'] = (blk.to_rgb.weight.detach().float().reshape(1, 3, ch).contiguous(), blk.to_rgb.bias.detach().float().contiguous())
         sr._large_cache = c
     return c
 
 
-def _forward_large_tail(sr, a1, img1, prep, out_clamp, out_uint8):
+def _forward_large_tail(sr, a1, img1, prep, out_clamp, out_uint8, split: bool = False):
     """LargeSynthesisBlock0/1.forward after the first SynthesisBlock (superresolution.py:296-329): residual blocks on the block output,
-    `rgb = rgb + to_rgb(x)`, then the second block the same way.  x stays NHWC fp16, rgb fp32 NCHW."""
+    `rgb = rgb + to_rgb(x)`, then the second block the same way.  x stays NHWC fp16 ([hi | lo] when split), rgb fp32 NCHW."""
     if out_uint8:
         raise NotImplementedError('uint8 frames are written by the standard SR\'s last epilogue; large_sr returns fp32')
-    L = capi.lib()
-    lp = _large_packed(sr)
+    lp = _large_packed(sr, split)
     _, b1 = _sblocks(sr)
     N, Nw, wp = a1.shape[0], prep.Nw, prep.wp
+    wide = 2 if split else 1
 
     def tail(x16, img, key, ch, res):
         for c1, c2 in lp[key]:
-            t = conv_plain(x16, c1, 3)
-            x16 = conv_plain(t, c2, 3, residual=x16)
+            t = conv_plain(x16, c1, 3, split=split)
+            x16 = conv_plain(t, c2, 3, residual=x16, split=split)
         wrgb, brgb = lp[key + '_rgb']
         out = torch.empty(N, 3, res, res, device=x16.device)
-        capi.check(L.r3dp_sr_tc_torgb_ex(capi.ptr(x16, torch.float16), capi.ptr(wrgb), capi.ptr(brgb), capi.ptr(img), 1, N, 1, ch, res, res, capi.ptr(out),
-                                         capi.stream()))
+        capi.check(_fn('torgb_ex', split)(capi.ptr(x16, torch.float16), capi.ptr(wrgb), capi.ptr(brgb), capi.ptr(img), 1, N, 1, ch, res, res,
+                                          capi.ptr(out), capi.stream()))
         return x16, out
 
     x16, img1 = tail(a1, img1, 'b0', 256, 256)
-    a2 = layer(x16, b1.conv0, wp[2], 2)
-    a3 = torch.empty(N, 512, 512, 128, device=a1.device, dtype=torch.float16)
+    a2 = layer(x16, b1.conv0, wp[2], 2, split)
+    a3 = torch.empty(N, 512, 512, 128 * wide, device=a1.device, dtype=torch.float16)
     img2 = torch.empty(N, 3, 512, 512, device=a1.device)
     with capi.region('sr_conv'):
-        capi.check(L.r3dp_sr_tc_layer_torgb(capi.ptr(a2, torch.float16), capi.ptr(wp[3], torch.float16), capi.ptr(capi.f32(b1.conv1.bias)),
-                                            capi.ptr(prep.wrgb1), capi.ptr(capi.f32(b1.torgb.bias)), capi.ptr(img1), N, Nw, 128, 128, 512, 512,
-                                            capi.ptr(a3, torch.float16), capi.ptr(img2), capi.stream()))
+        capi.check(_fn('layer_torgb', split)(capi.ptr(a2, torch.float16), capi.ptr(wp[3], torch.float16), capi.ptr(capi.f32(b1.conv1.bias)),
+                                             capi.ptr(prep.wrgb1), capi.ptr(capi.f32(b1.torgb.bias)), capi.ptr(img1), N, Nw, 128, 128, 512, 512,
+                                             capi.ptr(a3, torch.float16), capi.ptr(img2), capi.stream()))
     _, out = tail(a3, img2, 'b1', 128, 512)
     return out.clamp_(-1, 1) if out_clamp else out

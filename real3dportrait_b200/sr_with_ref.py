@@ -43,8 +43,8 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
                  **block_kwargs):
         block_kwargs.setdefault('sr_mode', 'tc')
         super().__init__(channels, img_resolution, sr_num_fp16_res, sr_antialias, **block_kwargs)
-        if self.sr_mode != 'tc':
-            raise NotImplementedError('the torso head is built on the tensor-core path only (sr_mode="tc")')
+        if self.sr_mode not in ('tc', 'tc_exact'):
+            raise NotImplementedError('the torso head is built on the tensor-core path only (sr_mode="tc" | "tc_exact")')
         hp = dict(hp or {})
         self.hparams = {'torso_model_version': hp.get('torso_model_version', 'v2'), 'htbsr_head_weight_fuse_mode': hp.get('htbsr_head_weight_fuse_mode', 'v2'),
                         'htbsr_head_threshold': float(hp.get('htbsr_head_threshold', 0.9)), 'weight_fuse': hp.get('weight_fuse', True)}
@@ -70,17 +70,25 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         self._clip_cache = None
         self.static_prepared_warp = None
 
+    @property
+    def _split(self) -> bool:
+        """sr_mode='tc_exact': every activation of the head is a [hi | lo] pair of fp16 tensors, every conv runs with split operands."""
+        return self.sr_mode == 'tc_exact'
+
     # ---- weight preparation ------------------------------------------------------------------------------------------------
     def _plain(self) -> Dict[str, tuple]:
-        if self._plain_cache is None:
+        sp = self._split
+        if self._plain_cache is None or self._plain_cache['split'] != sp:
             te, bg, ff = self.torso_encoder, self.bg_encoder, self.fuse_fg_bg_convs
             self._plain_cache = {
-                'te': _pack_plain(te[0], 64), 'bg0': _pack_plain(bg[0], 64), 'bg2': _pack_plain(bg[2], 128), 'bg4': _pack_plain(bg[4], 256),
-                'ff0': _pack_plain(ff[0], 512), 'ff2': _pack_plain(ff[2], 128), 'ff4': _pack_plain(ff[4], 256),
+                'split': sp,
+                'te': _pack_plain(te[0], 64, split=sp), 'bg0': _pack_plain(bg[0], 64, split=sp), 'bg2': _pack_plain(bg[2], 128, split=sp),
+                'bg4': _pack_plain(bg[4], 256, split=sp),
+                'ff0': _pack_plain(ff[0], 512, split=sp), 'ff2': _pack_plain(ff[2], 128, split=sp), 'ff4': _pack_plain(ff[4], 256, split=sp),
             }
             if self.fuse_mode != 'v1':
                 fh = self.fuse_head_torso_convs
-                self._plain_cache.update({'fh0': _pack_plain(fh[0], 512), 'fh2': _pack_plain(fh[2], 256)})
+                self._plain_cache.update({'fh0': _pack_plain(fh[0], 512, split=sp), 'fh2': _pack_plain(fh[2], 256, split=sp)})
             if self.fuse_mode == 'v3':                             # the mask predictor runs with split fp16 operands (its output is thresholded)
                 ap = self.head_torso_alpha_predictor
                 self._plain_cache.update({'ap0': sr_tc.pack_plain(ap[0], 64, split=True), 'ap2': sr_tc.pack_plain(ap[2], 128, split=True),
@@ -109,12 +117,14 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         return y
 
     @staticmethod
-    def _alpha_cat(xa16, Ca, xb16, Cb, alpha) -> torch.Tensor:
-        """cat[xa*alpha, xb*(1-alpha)]; xb may hold ONE frame shared by the whole batch (per-clip constant features)."""
+    def _alpha_cat(xa16, Ca, xb16, Cb, alpha, split: bool = False) -> torch.Tensor:
+        """cat[xa*alpha, xb*(1-alpha)]; xb may hold ONE frame shared by the whole batch (per-clip constant features).  split: [hi | lo] inputs,
+        output = the [hi | lo] layout of the (Ca + Cb)-channel result."""
         N, H, W, _ = xa16.shape
-        out = torch.empty(N, H, W, Ca + Cb, device=xa16.device, dtype=torch.float16)
-        capi.check(capi.lib().r3dp_sr_alpha_cat_ex(capi.ptr(xa16, torch.float16), Ca, xa16.shape[-1], capi.ptr(xb16, torch.float16), Cb, xb16.shape[-1],
-                                                   int(xb16.shape[0] == 1 and N > 1), capi.ptr(alpha), N, H, W, capi.ptr(out, torch.float16), capi.stream()))
+        out = torch.empty(N, H, W, (Ca + Cb) * (2 if split else 1), device=xa16.device, dtype=torch.float16)
+        fn = capi.lib().r3dp_sr_tcx_alpha_cat_ex if split else capi.lib().r3dp_sr_alpha_cat_ex
+        capi.check(fn(capi.ptr(xa16, torch.float16), Ca, xa16.shape[-1], capi.ptr(xb16, torch.float16), Cb, xb16.shape[-1],
+                      int(xb16.shape[0] == 1 and N > 1), capi.ptr(alpha), N, H, W, capi.ptr(out, torch.float16), capi.stream()))
         return out
 
     # ---- per-clip constants (SURVEY.md §8f #2) -------------------------------------------------------------------------------------------
@@ -124,13 +134,17 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         (sr_with_ref.py:77-90): the two antialiased 512->256 resizes and bg_encoder(ref_bg) (96.9 GFLOP/frame).  ref_* [1,3,512,512].
         Until end_clip(), forward() ignores its ref_torso_rgb / ref_bg_rgb arguments and uses these."""
         assert ref_torso_rgb.shape[0] == 1 and ref_bg_rgb.shape[0] == 1, 'one reference image per clip'
-        plain = self._plain()
+        plain, sp = self._plain(), self._split
         t256, b256 = self._aa_down2(ref_torso_rgb), self._aa_down2(ref_bg_rgb)
-        x_bg = self._conv(self._conv(self._conv(sr_tc.to_nhwc_f16(b256, 256), plain['bg0'], 2), plain['bg2'], 2), plain['bg4'], 0)
-        self._clip_cache = {'ref_torso_256': t256, 'ref_bg_256': b256, 'x_bg': x_bg}
+        self._clip_cache = {'ref_torso_256': t256, 'ref_bg_256': b256, 'x_bg': self._bg_features(b256, plain, sp), 'split': sp}
 
     def end_clip(self) -> None:
         self._clip_cache = None
+
+    def _bg_features(self, ref_bg_256, plain, split: bool) -> torch.Tensor:
+        """bg_encoder(ref_bg) on the tensor cores: [N,256,256,256] fp16 ([N,256,256,512] = [hi | lo] when split)."""
+        x = sr_tc.to_nhwc_f16(ref_bg_256, 256, split)
+        return self._conv(self._conv(self._conv(x, plain['bg0'], 2, split), plain['bg2'], 2, split), plain['bg4'], 0, split)
 
     @staticmethod
     def _blend(a, b, alpha) -> torch.Tensor:
@@ -162,21 +176,27 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         if ref_torso_rgb.shape[-1] != 512 or ref_bg_rgb.shape[-1] != 512:
             raise NotImplementedError('reference images must be 512x512 (antialiased 1/2 resize is the only down-scaling built)')
         ws3 = ws[:, -1:, :].expand(N, 3, -1)
+        sp = self._split
+        wide = 2 if sp else 1
         prep = getattr(self, 'static_prepared_warp', None)
+        if prep is not None and prep['main'].split != sp:
+            prep = None
         with capi.region('sr_prep'):
             if prep is None:
                 shared = N == 1 or getattr(self, 'assume_shared_styles', False)
                 wsel = ws3[:1] if shared else ws3
-                prep = {'main': sr_tc.Prepared(self, wsel)}
+                prep = {'main': sr_tc.Prepared(self, wsel, sp)}
                 if self.fuse_mode != 'v1':
-                    prep.update({'ht0': sr_tc.pack_for(self.head_torso_block.conv0, wsel[:, 0]), 'ht1': sr_tc.pack_for(self.head_torso_block.conv1, wsel[:, 1]),
+                    prep.update({'ht0': sr_tc.pack_for(self.head_torso_block.conv0, wsel[:, 0], sp), 'ht1': sr_tc.pack_for(self.head_torso_block.conv1, wsel[:, 1], sp),
                                  'htrgb': self.head_torso_block.torgb.folded_weight(wsel[:, 2])})
             plain = self._plain()
-            x0 = sr_tc.to_nhwc_f16(x, self.input_resolution)
+            x0 = sr_tc.to_nhwc_f16(x, self.input_resolution, sp)
             rgb0 = self._resize(rgb, self.input_resolution) if rgb.shape[-1] != self.input_resolution else capi.f32(rgb)
             rgb_256 = self._resize(rgb0, 256)
             weights_256 = self._resize(weights_img.detach(), 256)
             cc = self._clip_cache
+            if cc is not None and cc['split'] != sp:                    # begun in another sr_mode: run uncached
+                cc = None
             if cc is None:
                 ref_torso_256, ref_bg_256 = self._aa_down2(ref_torso_rgb), self._aa_down2(ref_bg_rgb)
             else:                                                        # per-clip constants, one frame broadcast over the batch (0.8 MB copies)
@@ -184,29 +204,29 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         main, Nw = prep['main'], prep['main'].Nw
         b0, b1, hb = self.block0, self.block1, getattr(self, 'head_torso_block', None)
         # block0: 128^2 -> 256^2 head features + head rgb
-        a0 = sr_tc.layer(x0, b0.conv0, main.wp[0], 2)
-        xh = torch.empty(N, 256, 256, 256, device=x.device, dtype=torch.float16)
+        a0 = sr_tc.layer(x0, b0.conv0, main.wp[0], 2, sp)
+        xh = torch.empty(N, 256, 256, 256 * wide, device=x.device, dtype=torch.float16)
         rgb_h = torch.empty(N, 3, 256, 256, device=x.device)
         with capi.region('sr_conv'):
-            capi.check(L.r3dp_sr_tc_layer_torgb(capi.ptr(a0, torch.float16), capi.ptr(main.wp[1], torch.float16), capi.ptr(capi.f32(b0.conv1.bias)),
+            capi.check(sr_tc._fn('layer_torgb', sp)(capi.ptr(a0, torch.float16), capi.ptr(main.wp[1], torch.float16), capi.ptr(capi.f32(b0.conv1.bias)),
                                                 capi.ptr(main.wrgb0), capi.ptr(capi.f32(b0.torgb.bias)), capi.ptr(rgb0), N, Nw, 256, 256, 256, 256,
                                                 capi.ptr(xh, torch.float16), capi.ptr(rgb_h), capi.stream()))
         # torso warper: the caller's PyTorch module (opaque child, sr_with_ref.py:84-87)
         with capi.region('torso_model'):
             rgb_torso, facev2v_ret = self.torso_model(ref_torso_256, segmap, kp_s, kp_d, rgb_256.detach(), weights_256.detach(), cal_loss=True,
                                                       target_torso_mask=target_torso_mask)
-        x_torso = self._conv(sr_tc.to_nhwc_f16(facev2v_ret['deformed_torso_hid'], 256), plain['te'], 0)               # 1x1, 64 -> 256
+        x_torso = self._conv(sr_tc.to_nhwc_f16(facev2v_ret['deformed_torso_hid'], 256, sp), plain['te'], 0, sp)       # 1x1, 64 -> 256
         if cc is None:
-            x_bg = self._conv(self._conv(self._conv(sr_tc.to_nhwc_f16(ref_bg_256, 256), plain['bg0'], 2), plain['bg2'], 2), plain['bg4'], 0)
+            x_bg = self._bg_features(ref_bg_256, plain, sp)
         else:
-            x_bg = cc['x_bg']                                            # [1,256,256,256] fp16, read by every frame of the batch
+            x_bg = cc['x_bg']                                            # [1,256,256,256 (x2 split)] fp16, read by every frame of the batch
         thr = float(self.hparams['htbsr_head_threshold'])
         if self.fuse_mode == 'v1':
             # head/torso fusion v1 (sr_with_ref.py:96-98): plain alpha blend of the rgb images AND of the feature maps; no fusing convs, no head_torso_block
             alpha = weights_256
             rgb_p2 = self._blend(rgb_h, rgb_torso, alpha)
-            xp = torch.empty(N, 256, 256, 256, device=x.device, dtype=torch.float16)
-            capi.check(L.r3dp_sr_alpha_mix(capi.ptr(xh, torch.float16), xh.shape[-1], capi.ptr(x_torso, torch.float16), x_torso.shape[-1], capi.ptr(alpha), 256,
+            xp = torch.empty(N, 256, 256, 256 * wide, device=x.device, dtype=torch.float16)
+            capi.check((L.r3dp_sr_tcx_alpha_mix if sp else L.r3dp_sr_alpha_mix)(capi.ptr(xh, torch.float16), xh.shape[-1], capi.ptr(x_torso, torch.float16), x_torso.shape[-1], capi.ptr(alpha), 256,
                                            N, 256, 256, capi.ptr(xp, torch.float16), capi.stream()))
         else:
             if self.fuse_mode == 'v3':
@@ -226,12 +246,12 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
                 alpha = weights_256                                 # v2, sr_with_ref.py:108-109 (the masked assignment is a no-op)
             # alpha-cat fusion of the head and torso features (sr_with_ref.py:110-113 | 133-136)
             rgb_p = self._blend(rgb_h, rgb_torso, alpha)
-            xf = self._conv(self._conv(self._alpha_cat(xh, 256, x_torso, 256, alpha), plain['fh0'], 2), plain['fh2'], 0)
-            c0 = sr_tc.layer(xf, hb.conv0, prep['ht0'], 1)
-            xp = torch.empty(N, 256, 256, 256, device=x.device, dtype=torch.float16)
+            xf = self._conv(self._conv(self._alpha_cat(xh, 256, x_torso, 256, alpha, sp), plain['fh0'], 2, sp), plain['fh2'], 0, sp)
+            c0 = sr_tc.layer(xf, hb.conv0, prep['ht0'], 1, sp)
+            xp = torch.empty(N, 256, 256, 256 * wide, device=x.device, dtype=torch.float16)
             rgb_p2 = torch.empty(N, 3, 256, 256, device=x.device)
             with capi.region('sr_conv'):
-                capi.check(L.r3dp_sr_tc_layer_torgb_noup(capi.ptr(c0, torch.float16), capi.ptr(prep['ht1'], torch.float16), capi.ptr(capi.f32(hb.conv1.bias)),
+                capi.check(sr_tc._fn('layer_torgb_noup', sp)(capi.ptr(c0, torch.float16), capi.ptr(prep['ht1'], torch.float16), capi.ptr(capi.f32(hb.conv1.bias)),
                                                          capi.ptr(prep['htrgb']), capi.ptr(capi.f32(hb.torgb.bias)), capi.ptr(rgb_p), N, Nw, 256, 256, 256, 256,
                                                          capi.ptr(xp, torch.float16), capi.ptr(rgb_p2), capi.stream()))
         # person / background fusion, sr_with_ref.py:115-124
@@ -241,12 +261,13 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         capi.check(L.r3dp_sr_person_occlusion(capi.ptr(alpha), capi.ptr(torso_occ), thr, N, 256, 256,
                                               capi.ptr(person), capi.stream()))
         rgb_f = self._blend(rgb_p2, ref_bg_256, person)
-        xg = self._conv(self._conv(self._conv(self._alpha_cat(xp, 256, x_bg, 256, person), plain['ff0'], 2), plain['ff2'], 2), plain['ff4'], 0)
+        xg = self._alpha_cat(xp, 256, x_bg, 256, person, sp)
+        xg = self._conv(self._conv(self._conv(xg, plain['ff0'], 2, sp), plain['ff2'], 2, sp), plain['ff4'], 0, sp)
         # block1: 256^2 -> 512^2
-        a2 = sr_tc.layer(xg, b1.conv0, main.wp[2], 2)
+        a2 = sr_tc.layer(xg, b1.conv0, main.wp[2], 2, sp)
         out = torch.empty(N, 3, 512, 512, device=x.device)
         with capi.region('sr_conv'):
-            capi.check(L.r3dp_sr_tc_last_layer(capi.ptr(a2, torch.float16), capi.ptr(main.wp[3], torch.float16), capi.ptr(capi.f32(b1.conv1.bias)),
-                                               capi.ptr(main.wrgb1), capi.ptr(capi.f32(b1.torgb.bias)), capi.ptr(rgb_f), N, Nw, 128, 512, 512,
-                                               capi.ptr(out), capi.stream()))
+            capi.check((L.r3dp_sr_tcx_last_layer if sp else L.r3dp_sr_tc_last_layer_ex)(
+                capi.ptr(a2, torch.float16), capi.ptr(main.wp[3], torch.float16), capi.ptr(capi.f32(b1.conv1.bias)), capi.ptr(main.wrgb1),
+                capi.ptr(capi.f32(b1.torgb.bias)), capi.ptr(rgb_f), N, Nw, 128, 512, 512, capi.ptr(out), None, 0, capi.stream()))
         return out, facev2v_ret

@@ -4,7 +4,8 @@ modules/eg3ds/models/superresolution.py:331-359 and modules/eg3ds/models/network
 Module / parameter / buffer names equal the reference's, so `load_state_dict(strict=True)` of released checkpoints
 works.  forward() orchestrates libr3dp_b200 calls; two arithmetic modes (`sr_mode`):
   'fp32'  exact CUDA-core path (parity anchor, matches the reference to fp32 re-association noise),
-  'tc'    tensor-core path (wgmma, fp16 operands, fp32 accumulate) — the fast path, own stated tolerance.
+  'tc'    tensor-core path (wgmma, fp16 operands, fp32 accumulate) — the fast path, own stated tolerance,
+  'tc_exact'  the same kernels with split fp16 operands (hi + lo) — fp32-grade results (also for large_sr and the torso head).
 Inference only: noise_mode must be 'none' (as in img2plane_baseline.py:113,144), fp32 parameters."""
 from __future__ import annotations
 
@@ -177,7 +178,7 @@ class SuperresolutionHybrid8XDC(torch.nn.Module):
     def __init__(self, channels, img_resolution, sr_num_fp16_res, sr_antialias, large_sr=False, sr_mode='fp32', resblocks_in_large_sr=None,
                  **block_kwargs):
         """large_sr=True (superresolution.py:263-345) needs `resblocks_in_large_sr` (the reference reads hparams['resblocks_in_large_sr']) and
-        runs on the tensor-core path only."""
+        runs on the tensor-core path only (sr_mode 'tc' or 'tc_exact')."""
         super().__init__()
         assert img_resolution == 512
         if sr_num_fp16_res > 0:
@@ -188,8 +189,8 @@ class SuperresolutionHybrid8XDC(torch.nn.Module):
         self.input_resolution = 128
         self.sr_antialias = sr_antialias
         if self.large_sr:
-            if sr_mode != 'tc' or resblocks_in_large_sr is None:
-                raise NotImplementedError("large_sr is built on the tensor-core path (sr_mode='tc') and needs resblocks_in_large_sr")
+            if sr_mode not in ('tc', 'tc_exact') or resblocks_in_large_sr is None:
+                raise NotImplementedError("large_sr is built on the tensor-core path (sr_mode='tc' | 'tc_exact') and needs resblocks_in_large_sr")
             self.block0 = LargeSynthesisBlock0(channels, False, int(resblocks_in_large_sr), **block_kwargs)
             self.block1 = LargeSynthesisBlock1(False, int(resblocks_in_large_sr), **block_kwargs)
         else:

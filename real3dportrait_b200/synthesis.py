@@ -38,8 +38,9 @@ class RenderHead(torch.nn.Module):
         self.decoder = OSGDecoder(c, {'decoder_lr_mul': 1, 'decoder_output_dim': c})
         sr_kwargs = dict(channels=c, img_resolution=hp['final_resolution'], sr_num_fp16_res=0, sr_antialias=True, channel_base=hp['base_channel'],
                          channel_max=hp['max_channel'], fused_modconv_default='inference_only')
-        if self.torso:
-            self.superresolution = SuperresolutionHybrid8XDC_Warp(hp=hp, torso_model=torso_model, sr_mode='tc', **sr_kwargs)
+        if self.torso:                                               # tensor-core only: 'tc_exact' is kept, every other mode runs as 'tc'
+            torso_mode = 'tc_exact' if sr_mode == 'tc_exact' else 'tc'
+            self.superresolution = SuperresolutionHybrid8XDC_Warp(hp=hp, torso_model=torso_model, sr_mode=torso_mode, **sr_kwargs)
         else:
             self.superresolution = SuperresolutionHybrid8XDC(sr_mode=sr_mode, **sr_kwargs)
         self.renderer = ImportanceRenderer(hp=hp)

@@ -1,7 +1,8 @@
 """Small end-to-end case for compute-sanitizer (memcheck / racecheck are ~100x slower: tiny shapes).
     compute-sanitizer --tool memcheck python tools/sanitize_case.py
 Covers: streaming render kernel (single pass), two-pass tensor-core render kernel, tri-grid variant, tensor-core SR (all four conv launches,
-FIR, edge) with fp16 and with split operands, uint8 epilogue, stand-alone sampler."""
+FIR, edge) with fp16 and with split operands, uint8 epilogue, stand-alone sampler, the torso head (`warp`: alpha-cat / blend kernels, plain convs,
+SynthesisBlockNoUp tail, per-clip cache) and large_sr (`large`: residual epilogue, plain ToRGB), both in 'tc' and 'tc_exact'."""
 import os
 import sys
 
@@ -52,6 +53,32 @@ def main():
             img = sr(fimg[:, :3].contiguous(), fimg, torch.ones(1, 14, 512, device=dev), noise_mode='none', out_uint8=u8)
             torch.cuda.synchronize()
             print('sr', mode, u8, float(img.float().abs().mean()))
+    for mode in (('tc', 'tc_exact') if what in ('all', 'warp') else ()):
+        m = r3.SuperresolutionHybrid8XDC_Warp(channels=32, img_resolution=512, sr_num_fp16_res=0, sr_antialias=True, hp=syn.WARP_HPARAMS, sr_mode=mode,
+                                              torso_model=syn.StubTorsoModel())
+        m.load_state_dict(syn.make_sr_warp_params(seed=6), strict=True)
+        m = m.to(dev).eval()
+        fimg = (torch.rand(1, 32, 64, 64, generator=g) * 2 - 1).to(dev)
+        wimg = torch.rand(1, 1, 64, 64, generator=g).to(dev)
+        inp = {k: v.to(dev) for k, v in syn.make_warp_inputs(1, seed=7).items()}
+        args = (fimg[:, :3].contiguous(), fimg, torch.ones(1, 14, 512, device=dev), inp['ref_torso_rgb'], inp['ref_bg_rgb'], wimg, inp['segmap'],
+                inp['kp_s'], inp['kp_d'])
+        with torch.no_grad():
+            img, _ = m(*args, noise_mode='none')
+            m.begin_clip(inp['ref_torso_rgb'], inp['ref_bg_rgb'])
+            img_c, _ = m(*args, noise_mode='none')
+            m.end_clip()
+        torch.cuda.synchronize()
+        print('warp', mode, float(img.abs().mean()), float(img_c.abs().mean()))
+    for mode in (('tc', 'tc_exact') if what in ('all', 'large') else ()):
+        sr = r3.SuperresolutionHybrid8XDC(channels=32, img_resolution=512, sr_num_fp16_res=0, sr_antialias=True, large_sr=True, sr_mode=mode,
+                                          resblocks_in_large_sr=1)
+        sr.load_state_dict(syn.make_sr_large_params(seed=8, n_res=1), strict=True)
+        sr = sr.to(dev).eval()
+        fimg = (torch.rand(1, 32, 64, 64, generator=g) * 2 - 1).to(dev)
+        img = sr(fimg[:, :3].contiguous(), fimg, torch.ones(1, 14, 512, device=dev), noise_mode='none')
+        torch.cuda.synchronize()
+        print('large', mode, float(img.abs().mean()))
 
 
 if __name__ == '__main__':
