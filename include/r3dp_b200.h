@@ -329,6 +329,15 @@ int r3dp_sr_blend(const float* a, const float* b, const float* alpha, int N, int
 int r3dp_sr_person_occlusion(const float* head_alpha, const float* torso_occlusion, float threshold, int N, int H, int W, float* out,
                              r3dp_stream_t stream);
 int r3dp_sr_resize_aa_down2(const float* x, int N, int C, int h_out, int w_out, float* y, r3dp_stream_t stream);
+/* The torso head's inputs straight from the renderer's channels-last output, in one launch (modules/real3d/super_resolution/sr_with_ref.py:70-78):
+ *   x_nhwc [N,h,w,C] fp32 (C % 8 == 0), wsum [N,h*w,1] fp32 (the layout of the weight image [N,1,h,w]), h, w <= size <= 256
+ *   y_f16   [N,size,size,Cpad] fp16 = r3dp_sr_tc_input_nhwc's output ([hi | lo] when split != 0)
+ *   rgb0    [N,3,size,size] fp32   = the resize of channels 0..2 (rgb_out of r3dp_sr_tc_input_nhwc_rgb)
+ *   rgb_256 [N,3,256,256] fp32     = r3dp_sr_resize_bilinear(rgb0, 256)            (sr_with_ref.py:77)
+ *   w_256   [N,1,256,256] fp32     = r3dp_sr_resize_bilinear(weight image, 256)    (sr_with_ref.py:78)
+ * Every output is bit-identical to that three-launch sequence. */
+int r3dp_sr_warp_input(const float* x_nhwc, const float* wsum, int N, int C, int h, int w, int size, void* y_f16, float* rgb0, float* rgb_256,
+                       float* w_256, int split, r3dp_stream_t stream);
 
 #ifdef __cplusplus
 }

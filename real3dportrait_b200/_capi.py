@@ -103,6 +103,7 @@ _SIGNATURES = {
     'r3dp_sr_blend': (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P]),
     'r3dp_sr_person_occlusion': (_I, [_P, _P, _F, _I, _I, _I, _P, _P]),
     'r3dp_sr_resize_aa_down2': (_I, [_P, _I, _I, _I, _I, _P, _P]),
+    'r3dp_sr_warp_input': (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _I, _P]),
     'r3dp_sr_tc_prof': (_I, [_I]),
     'r3dp_sr_tc_debug_buffer': (_I, [_P]),
     'r3dp_sr_tc_prof_read': (_I, [C.POINTER(C.c_float), C.POINTER(_I)]),

@@ -68,6 +68,23 @@ __device__ __forceinline__ float softplus_fast(float x) {
 }
 __device__ __forceinline__ float sigmoid_fast(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
 
+// Bilinear up-resize (F.interpolate, align_corners=False; antialias is the identity for scale >= 1).  Every resize kernel goes through
+// these two helpers.  The multiply-adds are spelled out with intrinsics: left to the compiler, `a * (1 - t) + b * t` is contracted into
+// fma(a, 1 - t, b * t) in one kernel and fma(b, t, a * (1 - t)) in another, and two kernels that must agree bit for bit would not.
+// bilinear_coord: output index o of an n -> size resize -> source indices i0, i1 and weight t of i1.
+__device__ __forceinline__ void bilinear_coord(int o, int n, int size, int& i0, int& i1, float& t) {
+    const float s = fmaxf(__fmaf_rn((float)o + 0.5f, (float)n / (float)size, -0.5f), 0.f);
+    i0 = min((int)s, n - 1);
+    i1 = min(i0 + 1, n - 1);
+    t = s - (float)i0;
+}
+// a<row><col>: the four source values at (y0,x0), (y1,x0), (y0,x1), (y1,x1)
+__device__ __forceinline__ float bilinear_mix(float a00, float a10, float a01, float a11, float ty, float tx) {
+    const float r0 = __fmaf_rn(a00, 1.f - ty, __fmul_rn(a10, ty));
+    const float r1 = __fmaf_rn(a01, 1.f - ty, __fmul_rn(a11, ty));
+    return __fmaf_rn(r0, 1.f - tx, __fmul_rn(r1, tx));
+}
+
 __device__ __forceinline__ float warp_min(float v) {
 #pragma unroll
     for (int o = 16; o; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o));

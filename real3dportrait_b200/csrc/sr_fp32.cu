@@ -54,15 +54,12 @@ __global__ void sr_resize_kernel(const float* __restrict__ x, int NC, int h, int
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (long long)NC * size * size) return;
     const int ox = (int)(idx % size), oy = (int)((idx / size) % size); const long long nc = idx / ((long long)size * size);
-    const float sy = fmaxf(((float)oy + 0.5f) * ((float)h / (float)size) - 0.5f, 0.f);
-    const float sx = fmaxf(((float)ox + 0.5f) * ((float)w / (float)size) - 0.5f, 0.f);
-    const int y0 = min((int)sy, h - 1), x0 = min((int)sx, w - 1);
-    const int y1 = min(y0 + 1, h - 1), x1 = min(x0 + 1, w - 1);
-    const float ty = sy - (float)y0, tx = sx - (float)x0;
+    int y0, y1, x0, x1;
+    float ty, tx;
+    bilinear_coord(oy, h, size, y0, y1, ty);
+    bilinear_coord(ox, w, size, x0, x1, tx);
     const float* p = x + nc * h * w;
-    const float r0 = p[y0 * w + x0] * (1.f - ty) + p[y1 * w + x0] * ty;
-    const float r1 = p[y0 * w + x1] * (1.f - ty) + p[y1 * w + x1] * ty;
-    y[idx] = r0 * (1.f - tx) + r1 * tx;
+    y[idx] = bilinear_mix(p[y0 * w + x0], p[y1 * w + x0], p[y0 * w + x1], p[y1 * w + x1], ty, tx);
 }
 
 // ---- direct convolution over a tap list ---------------------------------------------------------------------------

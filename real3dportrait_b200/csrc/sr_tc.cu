@@ -529,14 +529,12 @@ __global__ void resize_to_nhwc_f16_kernel(const float* __restrict__ x, int N, in
     const int n = (int)(idx / ((long long)Cp * size * size));
     float v = 0.f;
     if (c < C) {
-        const float sy = fmaxf(((float)oy + 0.5f) * ((float)h / (float)size) - 0.5f, 0.f);
-        const float sx = fmaxf(((float)ox + 0.5f) * ((float)w / (float)size) - 0.5f, 0.f);
-        const int y0 = min((int)sy, h - 1), x0 = min((int)sx, w - 1), y1 = min(y0 + 1, h - 1), x1 = min(x0 + 1, w - 1);
-        const float ty = sy - (float)y0, tx = sx - (float)x0;
+        int y0, y1, x0, x1;
+        float ty, tx;
+        bilinear_coord(oy, h, size, y0, y1, ty);
+        bilinear_coord(ox, w, size, x0, x1, tx);
         const float* p = x + ((size_t)n * C + c) * h * w;
-        const float r0 = p[y0 * w + x0] * (1.f - ty) + p[y1 * w + x0] * ty;
-        const float r1 = p[y0 * w + x1] * (1.f - ty) + p[y1 * w + x1] * ty;
-        v = r0 * (1.f - tx) + r1 * tx;
+        v = bilinear_mix(p[y0 * w + x0], p[y1 * w + x0], p[y0 * w + x1], p[y1 * w + x1], ty, tx);
     }
     if (!split) { y[idx] = __float2half_rn(v); return; }
     __half hi, lo;
@@ -1158,20 +1156,18 @@ extern "C" int r3dp_sr_tcx_layer_torgb(const void* x_f16, const void* wp_f16, co
 }
 
 // bilinear up-resize of a CHANNELS-LAST fp32 image [N,h,w,C] (e.g. the renderer's [N,M,32] output viewed as an image) to
-// NHWC fp16 [N,size,size,Cpad]: one thread = one output pixel x 8 channels.
-__global__ void resize_nhwc_to_f16_kernel(const float* __restrict__ x, int N, int C, int h, int w, int size, int Cp, int split, __half* __restrict__ y,
-                                          float* __restrict__ rgb_out) {
+// NHWC fp16 [N,size,size,Cpad]: one thread = one output pixel x 8 channels.  idx < N * size * size * Cp / 8.
+__device__ __forceinline__ void resize_nhwc_to_f16_item(long long idx, const float* __restrict__ x, int C, int h, int w, int size, int Cp, int split,
+                                                        __half* __restrict__ y, float* __restrict__ rgb_out) {
     const int cv = Cp / 8;
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= (long long)N * size * size * cv) return;
     const int c8 = (int)(idx % cv); const int ox = (int)((idx / cv) % size); const int oy = (int)((idx / ((long long)cv * size)) % size);
     const int n = (int)(idx / ((long long)cv * size * size));
     float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (c8 * 8 < C) {
-        const float sy = fmaxf(((float)oy + 0.5f) * ((float)h / (float)size) - 0.5f, 0.f);
-        const float sx = fmaxf(((float)ox + 0.5f) * ((float)w / (float)size) - 0.5f, 0.f);
-        const int y0 = min((int)sy, h - 1), x0 = min((int)sx, w - 1), y1 = min(y0 + 1, h - 1), x1 = min(x0 + 1, w - 1);
-        const float ty = sy - (float)y0, tx = sx - (float)x0;
+        int y0, y1, x0, x1;
+        float ty, tx;
+        bilinear_coord(oy, h, size, y0, y1, ty);
+        bilinear_coord(ox, w, size, x0, x1, tx);
         const float* b = x + (size_t)n * h * w * C + c8 * 8;
         const float4* p00 = reinterpret_cast<const float4*>(b + ((size_t)y0 * w + x0) * C);
         const float4* p10 = reinterpret_cast<const float4*>(b + ((size_t)y1 * w + x0) * C);
@@ -1183,10 +1179,7 @@ __global__ void resize_nhwc_to_f16_kernel(const float* __restrict__ x, int N, in
             const float e00[4] = {a00.x, a00.y, a00.z, a00.w}, e10[4] = {a10.x, a10.y, a10.z, a10.w};
             const float e01[4] = {a01.x, a01.y, a01.z, a01.w}, e11[4] = {a11.x, a11.y, a11.z, a11.w};
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const float r0 = e00[j] * (1.f - ty) + e10[j] * ty, r1 = e01[j] * (1.f - ty) + e11[j] * ty;
-                v[q * 4 + j] = r0 * (1.f - tx) + r1 * tx;
-            }
+            for (int j = 0; j < 4; ++j) v[q * 4 + j] = bilinear_mix(e00[j], e10[j], e01[j], e11[j], ty, tx);
         }
     }
     if (rgb_out != nullptr && c8 == 0) {                       // channels 0..2 = the raw RGB image the SR takes beside the features (secc_img2plane.py:126), fp32 NCHW
@@ -1205,6 +1198,55 @@ __global__ void resize_nhwc_to_f16_kernel(const float* __restrict__ x, int N, in
     *reinterpret_cast<uint4*>(y + pix + Cp + c8 * 8) = pl;
 }
 
+__global__ void resize_nhwc_to_f16_kernel(const float* __restrict__ x, int N, int C, int h, int w, int size, int Cp, int split, __half* __restrict__ y,
+                                          float* __restrict__ rgb_out) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)N * size * size * (Cp / 8)) return;
+    resize_nhwc_to_f16_item(idx, x, C, h, w, size, Cp, split, y, rgb_out);
+}
+
+// The torso head's inputs from the renderer's output in one launch (sr_with_ref.py:70-78).  Threads [0, n_feat) write x0 and rgb0 exactly as
+// resize_nhwc_to_f16_kernel does; thread n_feat + p writes pixel p of rgb_256 = resize(rgb0, 256) and of w_256 = resize(wsum as [N,1,h,w], 256).
+// rgb0 is written by other threads of the same launch, so its four source values are recomputed from x with the same helpers: same bits.
+constexpr int kWarpRes = 256;
+__global__ void warp_input_kernel(const float* __restrict__ x, const float* __restrict__ wsum, int N, int C, int h, int w, int size, int Cp, int split,
+                                  __half* __restrict__ y, float* __restrict__ rgb0, float* __restrict__ rgb_256, float* __restrict__ w_256) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long n_feat = (long long)N * size * size * (Cp / 8);
+    if (idx < n_feat) { resize_nhwc_to_f16_item(idx, x, C, h, w, size, Cp, split, y, rgb0); return; }
+    const long long p = idx - n_feat;
+    if (p >= (long long)N * kWarpRes * kWarpRes) return;
+    const int ox = (int)(p % kWarpRes), oy = (int)((p / kWarpRes) % kWarpRes), n = (int)(p / ((long long)kWarpRes * kWarpRes));
+    int y0, y1, x0, x1;
+    float ty, tx;
+    bilinear_coord(oy, size, kWarpRes, y0, y1, ty);
+    bilinear_coord(ox, size, kWarpRes, x0, x1, tx);
+    const int ry[2] = {y0, y1}, rx[2] = {x0, x1};
+    float a[3][2][2];                                          // rgb0[c][ry[i]][rx[j]]
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+            int sy0, sy1, sx0, sx1;
+            float sty, stx;
+            bilinear_coord(ry[i], h, size, sy0, sy1, sty);
+            bilinear_coord(rx[j], w, size, sx0, sx1, stx);
+            const float* b = x + (size_t)n * h * w * C;
+#pragma unroll
+            for (int c = 0; c < 3; ++c)
+                a[c][i][j] = bilinear_mix(__ldg(b + ((size_t)sy0 * w + sx0) * C + c), __ldg(b + ((size_t)sy1 * w + sx0) * C + c),
+                                          __ldg(b + ((size_t)sy0 * w + sx1) * C + c), __ldg(b + ((size_t)sy1 * w + sx1) * C + c), sty, stx);
+        }
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+        rgb_256[(((size_t)n * 3 + c) * kWarpRes + oy) * kWarpRes + ox] = bilinear_mix(a[c][0][0], a[c][1][0], a[c][0][1], a[c][1][1], ty, tx);
+    bilinear_coord(oy, h, kWarpRes, y0, y1, ty);
+    bilinear_coord(ox, w, kWarpRes, x0, x1, tx);
+    const float* q = wsum + (size_t)n * h * w;
+    w_256[((size_t)n * kWarpRes + oy) * kWarpRes + ox] = bilinear_mix(__ldg(q + y0 * w + x0), __ldg(q + y1 * w + x0), __ldg(q + y0 * w + x1),
+                                                                      __ldg(q + y1 * w + x1), ty, tx);
+}
+
 static int input_nhwc_impl(const float* x_nhwc, int N, int C, int h, int w, int size, void* y_f16, float* rgb_out, int split, r3dp_stream_t stream) {
     R3DP_REQUIRE(x_nhwc && y_f16, "sr_tc_input_nhwc: null pointer");
     R3DP_REQUIRE(N > 0 && C > 0 && C % 8 == 0 && h > 0 && w > 0 && size >= h && size >= w, "sr_tc_input_nhwc: bad shape (C %% 8 == 0, up-scaling only)");
@@ -1221,6 +1263,19 @@ extern "C" int r3dp_sr_tcx_input_nhwc(const float* x_nhwc, int N, int C, int h, 
 extern "C" int r3dp_sr_tc_input_nhwc_rgb(const float* x_nhwc, int N, int C, int h, int w, int size, void* y_f16, float* rgb_out, int split, r3dp_stream_t stream) {
     R3DP_REQUIRE(rgb_out != nullptr && C >= 3, "sr_tc_input_nhwc_rgb: needs rgb_out and at least 3 channels");
     return input_nhwc_impl(x_nhwc, N, C, h, w, size, y_f16, rgb_out, split != 0, stream);
+}
+extern "C" int r3dp_sr_warp_input(const float* x_nhwc, const float* wsum, int N, int C, int h, int w, int size, void* y_f16, float* rgb0,
+                                  float* rgb_256, float* w_256, int split, r3dp_stream_t stream) {
+    R3DP_REQUIRE(x_nhwc && wsum && y_f16 && rgb0 && rgb_256 && w_256, "sr_warp_input: null pointer");
+    R3DP_REQUIRE(N > 0 && C >= 3 && C % 8 == 0 && h > 0 && w > 0 && size >= h && size >= w && size <= kWarpRes,
+                 "sr_warp_input: bad shape (C >= 3, C %% 8 == 0, h, w <= size <= %d)", kWarpRes);
+    const int Cp = (C + 63) / 64 * 64;
+    const long long total = (long long)N * size * size * (Cp / 8) + (long long)N * kWarpRes * kWarpRes;
+    warp_input_kernel<<<(unsigned)((total + 255) / 256), 256, 0, as_stream(stream)>>>(x_nhwc, wsum, N, C, h, w, size, Cp, split != 0,
+                                                                                     reinterpret_cast<__half*>(y_f16), rgb0, rgb_256, w_256);
+    R3DP_LAUNCH_CHECK();
+    count_launches(1);
+    return 0;
 }
 
 // ---- composed up-convolution for small Cin -------------------------------------------------------------------------------

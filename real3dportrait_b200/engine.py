@@ -9,7 +9,11 @@ only exchange between ranks is the reassembly of the output clip:
   exchange='none'       frames stay on their rank
 
 With out_uint8 the last SR epilogue writes uint8 HWC video frames (the reference's ((x+1)/2*255).int() conversion, real3d_infer.py:519),
-4x fewer bytes to exchange or copy to the host."""
+4x fewer bytes to exchange or copy to the host.
+
+With torso_model=... the engine runs the torso head (OSAvatarSECC_Img2plane_Torso, SuperresolutionHybrid8XDC_Warp): begin_clip() takes the
+constants of a clip (ref_torso_img, bg_img, segmap, kp_s; real3d_infer.py:463-467) and every step takes the frames' kp_d.  The torso warper is
+the caller's PyTorch module; it need not be capturable: by default a step replays two graphs around an eager warper call."""
 from __future__ import annotations
 
 import contextlib
@@ -95,20 +99,45 @@ def _frames_of(planes) -> int:
     return planes.dims[0] if isinstance(planes, PlanesCL) else planes.shape[0]
 
 
+class _TorsoGraphs:
+    """One torso step as two CUDA graphs around an eager torso_model call: graph A (render, SR prep, block0, the warper's inputs), the
+    warper on the current stream, its three outputs copied into graph B's static inputs (the caching allocator does not keep their
+    addresses), graph B (the rest of the head)."""
+
+    def __init__(self, sr, a, st, b_in, b):
+        self.sr, self.a, self.st, self.b_in, self.b = sr, a, st, b_in, b
+
+    def replay(self) -> None:
+        self.a.replay()
+        rgb_torso, ret = self.sr.run_torso(self.st)
+        for dst, src in zip(self.b_in, (rgb_torso, ret['deformed_torso_hid'], ret['occlusion_2'])):
+            dst.copy_(src)
+        self.b.replay()
+
+
 class FrameEngine:
     """batch: frames per step; static_styles: the SR styles are constant (Real3D passes ws == 1, img2plane_baseline.py:142) so
-    the folded fp16 weights are prepared once per parameter load; use_graph: replay the whole step as ONE CUDA graph."""
+    the folded fp16 weights are prepared once per parameter load; use_graph: replay the step as CUDA graphs.
+    torso_model: run the torso head with this warper (WarpBasedTorsoModelMediaPipe or a module with its forward signature);
+    warper_in_graph: capture the warper inside the step's single graph (only for capturable warpers; the default runs it eagerly
+    between two graphs)."""
 
     def __init__(self, batch: int = 4, sr_mode: str = 'fp32', device=None, world: int = 1, rank: int = 0, dist=None, hp: Optional[dict] = None,
-                 static_styles: bool = True, use_graph: bool = True, out_uint8: bool = False, exchange: str = 'allgather'):
+                 static_styles: bool = True, use_graph: bool = True, out_uint8: bool = False, exchange: str = 'allgather',
+                 torso_model: Optional[torch.nn.Module] = None, warper_in_graph: bool = False):
         assert exchange in ('allgather', 'p2p', 'none')
         self.batch, self.world, self.rank, self.dist = batch, world, rank, dist
         self.device = device if device is not None else torch.device('cuda', torch.cuda.current_device())
-        self.head = RenderHead(hp=hp, sr_mode=sr_mode).to(self.device).eval()
+        self.head = RenderHead(hp=hp, sr_mode=sr_mode, torso_model=torso_model).to(self.device).eval()
         self.static_styles, self.use_graph = static_styles, use_graph
+        self.torso, self.warper_in_graph = self.head.torso, bool(warper_in_graph)
         self.out_uint8 = bool(out_uint8)
-        if self.out_uint8 and sr_mode not in ('tc', 'tc_exact'):
+        if self.out_uint8 and self.head.superresolution.sr_mode not in ('tc', 'tc_exact'):     # the head's effective mode: a torso head maps 'fp32' to 'tc'
             raise NotImplementedError('uint8 frames are written by the tensor-core SR epilogue (sr_mode="tc")')
+        # fuse mode v3 thresholds the head mask at a host-side quantile (sr_with_ref.py:141-143): its steps cannot be captured
+        self.eager_reason = ('fuse mode v3 reads a host-side quantile of the head mask every step'
+                             if self.torso and self.head.superresolution.fuse_mode == 'v3' else None)
+        self._consts = None               # torso head: the clip's constants (begin_clip)
         self.exchange = exchange if world > 1 else 'none'
         self.graph = None
         self.launches_per_step = 0
@@ -131,27 +160,80 @@ class FrameEngine:
         self.head.load_state_dict(sd, strict=True)
         self.graph = None
         self.inplace = {}
+        self._consts = None                                            # loading dropped the head's per-clip cache: begin_clip() again
         sr = self.head.superresolution
         sr.static_prepared = None
-        if self.static_styles and sr.sr_mode in ('tc', 'tc_exact') and not self.head.torso:
+        if self.static_styles and sr.sr_mode in ('tc', 'tc_exact'):
             from . import sr_tc
             ones = torch.ones(1, 3, self.head.hparams['w_dim'], device=self.device)
             with torch.no_grad():
-                sr.static_prepared = sr_tc.Prepared(sr, ones, sr.sr_mode == 'tc_exact')
+                if self.torso:
+                    sr.static_prepared_warp = sr.prepare_styles(ones)
+                else:
+                    sr.static_prepared = sr_tc.Prepared(sr, ones, sr.sr_mode == 'tc_exact')
 
+    # ---- torso head: per-clip constants --------------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def _body(self, planes, cameras, u_coarse, u_fine=None) -> torch.Tensor:
+    def begin_clip(self, ref_torso_img: torch.Tensor, bg_img: torch.Tensor, segmap: torch.Tensor, kp_s: torch.Tensor) -> None:
+        """The constants of a clip (real3d_infer.py:463-467): ref_torso_img, bg_img [1,3,512,512], segmap [1,6,512,512], kp_s [1,68,3].
+        Runs the head's per-clip cache (bg_encoder(bg_img), the two antialiased resizes) and keeps the [batch,...] broadcasts every step
+        reads.  A later begin_clip() refills these buffers in place, so graphs captured for an earlier clip render the new one."""
+        if not self.torso:
+            raise ValueError('begin_clip() is for the torso head: FrameEngine(torso_model=...)')
+        if not (ref_torso_img.shape[0] == bg_img.shape[0] == segmap.shape[0] == kp_s.shape[0] == 1):
+            raise ValueError('one set of clip constants: ref_torso_img, bg_img, segmap and kp_s have batch size 1')
+        B = self.batch
+        if not self.head.superresolution.begin_clip(ref_torso_img, bg_img, batch=B, in_place=True):
+            self.graph, self.inplace = None, {}                       # new constant buffers: graphs captured earlier read the old ones
+        bc = {'segmap': segmap.expand(B, -1, -1, -1), 'kp_s': kp_s.expand(B, -1, -1)}
+        if self._consts is None:
+            self._consts = {k: v.to(self.device, torch.float32).contiguous() for k, v in bc.items()}
+        else:
+            for k, v in bc.items():
+                self._consts[k].copy_(v)
+        self._consts.update({'ref_torso_img': ref_torso_img, 'bg_img': bg_img})
+
+    def end_clip(self) -> None:
+        """Release the clip's constants, and the graphs that read them."""
+        if self.torso:
+            self.head.superresolution.end_clip()
+        self._consts = None
+        self.graph, self.inplace = None, {}
+
+    def _cond(self, kp_d: torch.Tensor) -> Dict[str, torch.Tensor]:
+        c = self._consts
+        return {'ref_torso_img': c['ref_torso_img'], 'bg_img': c['bg_img'], 'segmap': c['segmap'], 'kp_s': c['kp_s'], 'kp_d': kp_d}
+
+    def _check_kp_d(self, kp_d) -> None:
+        if not self.torso:
+            if kp_d is not None:
+                raise ValueError('kp_d is the per-frame condition of the torso head: this engine runs the plain head (no torso_model)')
+            return
+        if self._consts is None:
+            raise RuntimeError('torso head: call begin_clip(ref_torso_img, bg_img, segmap, kp_s) before the first step')
+        if kp_d is None:
+            raise ValueError('torso head: every step needs kp_d [B,68,3]')
+
+    @staticmethod
+    def _over(u_coarse, u_fine) -> Dict[str, torch.Tensor]:
         over = {'u_coarse': u_coarse}
         if u_fine is not None:
             over['u_fine'] = u_fine
-        return self.head.synthesis(planes, cameras, lean=True, out_uint8=self.out_uint8, **over)['image']
+        return over
 
-    def _capture_graph(self, planes, cameras, u_coarse, u_fine=None):
+    @torch.no_grad()
+    def _body(self, planes, cameras, u_coarse, u_fine=None, kp_d=None) -> torch.Tensor:
+        cond = self._cond(kp_d) if self.torso else None
+        return self.head.synthesis(planes, cameras, cond=cond, lean=True, out_uint8=self.out_uint8, **self._over(u_coarse, u_fine))['image']
+
+    def _capture_graph(self, planes, cameras, u_coarse, u_fine=None, kp_d=None):
+        if self.torso and not self.warper_in_graph:
+            return self._capture_split(planes, cameras, u_coarse, u_fine, kp_d)
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(2):                                       # warm-up outside capture: lazy inits (func attributes, driver entry points)
-                self._body(planes, cameras, u_coarse, u_fine)
+                self._body(planes, cameras, u_coarse, u_fine, kp_d)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
@@ -159,9 +241,35 @@ class FrameEngine:
             self._pool = torch.cuda.graph_pool_handle()               # all step graphs share one pool: they never run concurrently
         c0 = capi.lib().r3dp_launch_count()
         with torch.cuda.graph(g, pool=self._pool):
-            out = self._body(planes, cameras, u_coarse, u_fine)
+            out = self._body(planes, cameras, u_coarse, u_fine, kp_d)
         self.launches_per_step = int(capi.lib().r3dp_launch_count() - c0)      # libr3dp kernels inside one replay
         return g, out
+
+    def _capture_split(self, planes, cameras, u_coarse, u_fine, kp_d):
+        """Torso step as graph A -> eager warper -> graph B (see _TorsoGraphs); returns (graphs, output buffer)."""
+        sr, over = self.head.superresolution, self._over(u_coarse, u_fine)
+        pre = lambda: self.head.torso_pre(planes, cameras, self._cond(kp_d), self.out_uint8, **over)   # noqa: E731
+        side = torch.cuda.Stream(device=self.device)
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side), torch.no_grad():
+            for _ in range(2):                                       # warm-up outside capture, as in _capture_graph
+                st = pre()
+                rgb_torso, ret = sr.run_torso(st)
+                sr.forward_post(st, rgb_torso, ret)
+            b_in = tuple(capi.f32(t).clone() for t in (rgb_torso, ret['deformed_torso_hid'], ret['occlusion_2']))
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        if self._pool is None:
+            self._pool = torch.cuda.graph_pool_handle()
+        a, b = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+        c0 = capi.lib().r3dp_launch_count()
+        with torch.no_grad():
+            with torch.cuda.graph(a, pool=self._pool):
+                st = pre()
+            with torch.cuda.graph(b, pool=self._pool):
+                out = sr.forward_post(st, b_in[0], {'deformed_torso_hid': b_in[1], 'occlusion_2': b_in[2]})
+        self.launches_per_step = int(capi.lib().r3dp_launch_count() - c0)
+        return _TorsoGraphs(sr, a, st, b_in, b), out
 
     def _needs_fine(self) -> bool:
         return int(self.head.rendering_kwargs['depth_resolution_importance'] or 0) > 0
@@ -181,32 +289,42 @@ class FrameEngine:
         """Zero-copy steps for RESIDENT inputs: capture one step graph per (planes, cameras, u_coarse[, u_fine]) tuple that reads those very
         buffers, so `step()` on them replays without first copying the planes into static graph inputs.  `planes` may be the reference's
         [B,3,32,H,W] tensor (repacked inside the step), a PlanesCL the producer wrote channels-last (no repack), or a (cano, secc) pair.
-        The tensors are kept referenced (their addresses stay valid); refill them in place between steps.  Returns the number of graphs held."""
-        if not self.use_graph:
+        The tensors are kept referenced (their addresses stay valid); refill them in place between steps.  Returns the number of graphs held.
+        The torso head takes (planes, cameras, u_coarse, u_fine, kp_d) tuples; its graphs read kp_d [B,68,3] in place too.  Under fuse mode v3
+        the steps run eagerly (see `eager_reason`) and nothing is captured."""
+        if not self.use_graph or self.eager_reason is not None:
             return 0
         for item in inputs:
             planes, cameras, u_coarse = item[:3]
             u_fine = item[3] if len(item) > 3 else None
+            kp_d = item[4] if len(item) > 4 else None
+            self._check_kp_d(kp_d)
             k = (_ptr_key(planes), cameras.data_ptr(), u_coarse.data_ptr(), _ptr_key(u_fine))
+            if self.torso:
+                k += (kp_d.data_ptr(),)
             if k in self.inplace or len(self.inplace) >= max_graphs or _frames_of(planes) not in (self.batch, 1):
                 continue
             if self._needs_fine() and u_fine is None:
                 raise ValueError('this head renders with importance samples: prepare() needs u_fine [B*M, S_imp] in every input tuple')
-            g, out = self._capture_graph(planes, cameras, u_coarse, u_fine)
-            self.inplace[k] = (g, out, (planes, cameras, u_coarse, u_fine))
+            g, out = self._capture_graph(planes, cameras, u_coarse, u_fine, kp_d)
+            self.inplace[k] = (g, out, (planes, cameras, u_coarse, u_fine, kp_d))
         return len(self.inplace)
 
     @torch.no_grad()
     def step(self, planes, cameras: torch.Tensor, u_coarse: Optional[torch.Tensor] = None, u_fine: Optional[torch.Tensor] = None,
-             frame_index: Optional[int] = None) -> torch.Tensor:
+             frame_index: Optional[int] = None, *, kp_d: Optional[torch.Tensor] = None) -> torch.Tensor:
         """planes [B,3,32,256,256] | PlanesCL | (cano, secc); cameras [B,25]; u_coarse [B,4096,S,1], u_fine [B*4096,S_imp] (drawn here if None)
         -> this rank's frames: fp32 [B,3,512,512] in [-1,1] or uint8 [B,512,512,3]; with exchange='allgather' the gathered
         [world*B,...] (rank-major); with exchange='p2p' the frames are additionally pushed into the open clip at `frame_index`.
+        kp_d [B,68,3]: the frames' driving key points, the torso head's only per-frame condition (torso engines only).
         The returned tensor is reused by the next step."""
+        self._check_kp_d(kp_d)
         drawn = u_coarse is None or (u_fine is None and self._needs_fine())
         u_coarse, u_fine = self._draw(cameras.shape[0], cameras.device, u_coarse, u_fine)
-        graphable = self.use_graph and capi.PROF is None and cameras.shape[0] == self.batch
+        graphable = self.use_graph and capi.PROF is None and cameras.shape[0] == self.batch and self.eager_reason is None
         key = (_ptr_key(planes), cameras.data_ptr(), u_coarse.data_ptr(), _ptr_key(u_fine))
+        if self.torso:
+            key += (kp_d.data_ptr(),)
         hit = self.inplace.get(key) if (graphable and self.inplace and not drawn) else None
         if hit is not None:
             hit[0].replay()
@@ -214,14 +332,16 @@ class FrameEngine:
         elif graphable and isinstance(planes, torch.Tensor):
             if self.graph is None:
                 self.s_in = (planes.clone(), cameras.clone(), u_coarse.clone(), None if u_fine is None else u_fine.clone())
+                if self.torso:
+                    self.s_in += (kp_d.clone(),)
                 self.graph, self.s_out = self._capture_graph(*self.s_in)
-            for dst, src in zip(self.s_in, (planes, cameras, u_coarse, u_fine)):
+            for dst, src in zip(self.s_in, (planes, cameras, u_coarse, u_fine, kp_d)):
                 if dst is not None and src.data_ptr() != dst.data_ptr():
                     dst.copy_(src, non_blocking=True)
             self.graph.replay()
             out = self.s_out
         else:
-            out = self._body(planes, cameras, u_coarse, u_fine)
+            out = self._body(planes, cameras, u_coarse, u_fine, kp_d)
         if self.exchange == 'allgather':
             if capi.PROF is not None:                                   # profiling pass: serial, so the region time is the collective's own
                 gathered = torch.empty((self.world * self.batch,) + tuple(out.shape[1:]), dtype=out.dtype, device=self.device)
@@ -229,7 +349,7 @@ class FrameEngine:
                     self.dist.all_gather_into_tensor(gathered, out.contiguous())
                 return gathered
             return self._gather_async(out)
-        if self.exchange == 'p2p' and self._clip is not None and frame_index is not None:
+        if (self.exchange == 'p2p' or self.world == 1) and self._clip is not None and frame_index is not None:      # world 1: the clip is local
             with capi.region('exchange'):
                 self._push(out, frame_index)
         return out
@@ -353,30 +473,35 @@ class FrameEngine:
 
     @torch.no_grad()
     def step_host(self, h_planes: torch.Tensor, h_cameras: torch.Tensor, h_u: torch.Tensor, h_out: torch.Tensor,
-                  h_u_fine: Optional[torch.Tensor] = None) -> None:
+                  h_u_fine: Optional[torch.Tensor] = None, h_kp_d: Optional[torch.Tensor] = None) -> None:
         """Same step, from PINNED HOST tensors to a pinned host output (frames of THIS rank), fully asynchronous: the call
         enqueues H2D (copy-in stream) -> step (current stream) -> D2H (copy-out stream) and returns; with two staging slots the
-        copy of step i+1 runs under the compute of step i.  Call `sync_host()` before reading `h_out`."""
+        copy of step i+1 runs under the compute of step i.  Call `sync_host()` before reading `h_out`.  h_kp_d: the torso head's kp_d."""
+        self._check_kp_d(h_kp_d)
         hp = self._host_pipeline()
         k = hp['k'] & 1
         hp['k'] += 1
         cur = torch.cuda.current_stream()
         hosts = (h_planes, h_cameras, h_u) + ((h_u_fine,) if h_u_fine is not None else ())
+        if self.torso:
+            hosts = hosts[:3] + (h_u_fine, h_kp_d)                     # prepare()'s torso tuple: u_fine may be None
         if hp['stage'][k] is None:
-            hp['stage'][k] = tuple(torch.empty_like(h, device=self.device) for h in hosts)
+            hp['stage'][k] = tuple(None if h is None else torch.empty_like(h, device=self.device) for h in hosts)
             hp['out'][k] = torch.empty((self.batch,) + self.frame_shape(), dtype=self.frame_dtype(), device=self.device)
             for dst, src in zip(hp['stage'][k], hosts):
-                dst.copy_(src)                                         # warm-up / capture run on REAL inputs (uninitialised cameras give NaN depths)
+                if dst is not None:
+                    dst.copy_(src)                                     # warm-up / capture run on REAL inputs (uninitialised cameras give NaN depths)
             self.prepare([hp['stage'][k]])                             # the step reads the staging slot in place (no device-side input copy)
             hp['in_free'][k].record(cur); hp['out_free'][k].record(cur)
         stage = hp['stage'][k]
         with torch.cuda.stream(hp['copy_in']):
             hp['copy_in'].wait_event(hp['in_free'][k])                 # the step that last read this slot is done
             for dst, src in zip(stage, hosts):
-                dst.copy_(src, non_blocking=True)
+                if dst is not None:
+                    dst.copy_(src, non_blocking=True)
             hp['in_ready'][k].record(hp['copy_in'])
         cur.wait_event(hp['in_ready'][k])
-        out = self.step(*stage)
+        out = self.step(*stage[:4], kp_d=stage[4]) if self.torso else self.step(*stage)
         self.wait_gather()
         hp['in_free'][k].record(cur)
         cur.wait_event(hp['out_free'][k])

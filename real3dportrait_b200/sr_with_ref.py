@@ -95,6 +95,16 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
                                           'ap4': sr_tc.pack_plain(ap[4], 128, split=True)})
         return self._plain_cache
 
+    def prepare_styles(self, wsel: torch.Tensor) -> Dict:
+        """Folded + packed weights of block0/1 and head_torso_block for styles wsel [Nw,3,512].  Assign the result to
+        `static_prepared_warp` when the styles are constant (Real3D passes ws == 1): forward() then stops preparing them per call."""
+        sp = self._split
+        prep = {'main': sr_tc.Prepared(self, wsel, sp)}
+        if self.fuse_mode != 'v1':
+            prep.update({'ht0': sr_tc.pack_for(self.head_torso_block.conv0, wsel[:, 0], sp), 'ht1': sr_tc.pack_for(self.head_torso_block.conv1, wsel[:, 1], sp),
+                         'htrgb': self.head_torso_block.torgb.folded_weight(wsel[:, 2])})
+        return prep
+
     def _load_from_state_dict(self, *a, **k):
         # runs for THIS module whenever it or any parent (RenderHead, FrameEngine.load_params) loads a state_dict: every cache that was
         # derived from the parameters is dropped (packed fp16 conv weights, per-clip constants, prepared styles)
@@ -129,14 +139,30 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
 
     # ---- per-clip constants (SURVEY.md §8f #2) -------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def begin_clip(self, ref_torso_rgb: torch.Tensor, ref_bg_rgb: torch.Tensor) -> None:
+    def begin_clip(self, ref_torso_rgb: torch.Tensor, ref_bg_rgb: torch.Tensor, batch: Optional[int] = None, in_place: bool = False) -> bool:
         """Hoist what the reference recomputes for every frame although it only depends on the clip's reference images
         (sr_with_ref.py:77-90): the two antialiased 512->256 resizes and bg_encoder(ref_bg) (96.9 GFLOP/frame).  ref_* [1,3,512,512].
-        Until end_clip(), forward() ignores its ref_torso_rgb / ref_bg_rgb arguments and uses these."""
+        Until end_clip(), forward() ignores its ref_torso_rgb / ref_bg_rgb arguments and uses these.
+        batch: also keep the [batch,3,256,256] broadcasts of the two resized images, read by every call with that batch instead of
+        copies made per call.  in_place: when a clip with the same mode and batch is already begun, write the new constants into its
+        tensors (CUDA graphs captured against them then render the new clip).  Returns True when the constants were refilled in place."""
         assert ref_torso_rgb.shape[0] == 1 and ref_bg_rgb.shape[0] == 1, 'one reference image per clip'
         plain, sp = self._plain(), self._split
         t256, b256 = self._aa_down2(ref_torso_rgb), self._aa_down2(ref_bg_rgb)
-        self._clip_cache = {'ref_torso_256': t256, 'ref_bg_256': b256, 'x_bg': self._bg_features(b256, plain, sp), 'split': sp}
+        cc = {'ref_torso_256': t256, 'ref_bg_256': b256, 'x_bg': self._bg_features(b256, plain, sp), 'split': sp, 'batch': None}
+        if batch is not None:
+            cc['batch'] = (t256.expand(batch, -1, -1, -1).contiguous(), b256.expand(batch, -1, -1, -1).contiguous())
+        old = self._clip_cache
+        if in_place and old is not None and old['split'] == sp and (old['batch'] is None) == (batch is None) and \
+                (batch is None or old['batch'][0].shape[0] == batch):
+            for k in ('ref_torso_256', 'ref_bg_256', 'x_bg'):
+                old[k].copy_(cc[k])
+            if batch is not None:
+                for dst, src in zip(old['batch'], cc['batch']):
+                    dst.copy_(src)
+            return True
+        self._clip_cache = cc
+        return False
 
     def end_clip(self) -> None:
         self._clip_cache = None
@@ -165,13 +191,26 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
     # ---- forward -------------------------------------------------------------------------------------------------------------
     def forward(self, rgb, x, ws, ref_torso_rgb, ref_bg_rgb, weights_img, segmap, kp_s, kp_d, target_torso_mask=None, **block_kwargs):
         """rgb [N,3,h,w], x [N,32,h,w], ws [N,>=1,512], ref_torso_rgb/ref_bg_rgb [N,3,512,512], weights_img [N,1,h,w], segmap [N,6,512,512],
-        kp_s/kp_d [N,68,3] -> (rgb [N,3,512,512], facev2v_ret)   (sr_with_ref.py:67-162)."""
+        kp_s/kp_d [N,68,3] -> (rgb [N,3,512,512], facev2v_ret)   (sr_with_ref.py:67-162).
+        Optional, as for the plain head (tensor-core path): x_nhwc = the renderer's channels-last features [N,h,w,C] with rgb_from_x=True
+        (rgb == x[:, :3]) and wsum = its channels-last weights [N,h*w,1] - the inputs are then read in place by one launch;
+        out_clamp: the image leaves the last epilogue clamped to [-1,1]; out_uint8: it leaves as uint8 HWC frames [N,512,512,3]."""
+        st = self.forward_pre(rgb, x, ws, ref_torso_rgb, ref_bg_rgb, weights_img, segmap, kp_s, kp_d, target_torso_mask, **block_kwargs)
+        rgb_torso, facev2v_ret = self.run_torso(st)
+        return self.forward_post(st, rgb_torso, facev2v_ret), facev2v_ret
+
+    def forward_pre(self, rgb, x, ws, ref_torso_rgb, ref_bg_rgb, weights_img, segmap, kp_s, kp_d, target_torso_mask=None, **block_kwargs) -> Dict:
+        """First half of forward(), up to the torso_model call: input preparation, block0 and the warper's inputs.  Returns the state that
+        run_torso() and forward_post() take; every tensor in it is written on the current stream (a CUDA graph may capture this half)."""
         if getattr(self, 'torso_model', None) is None:
             raise RuntimeError('SuperresolutionHybrid8XDC_Warp needs its torso_model child (the reference WarpBasedTorsoModelMediaPipe); '
                                'pass torso_model=... to the constructor')
         if block_kwargs.get('noise_mode', 'none') != 'none':
             raise NotImplementedError("only noise_mode='none' is on the inference path")
-        L = capi.lib()
+        x_nhwc, wsum = block_kwargs.pop('x_nhwc', None), block_kwargs.pop('wsum', None)
+        rgb_from_x = bool(block_kwargs.pop('rgb_from_x', False))
+        if x_nhwc is not None and not (rgb_from_x and wsum is not None):
+            raise NotImplementedError('x_nhwc is the lean hand-off from the renderer: it needs rgb_from_x=True and wsum (the channels-last weights)')
         N = rgb.shape[0]
         if ref_torso_rgb.shape[-1] != 512 or ref_bg_rgb.shape[-1] != 512:
             raise NotImplementedError('reference images must be 512x512 (antialiased 1/2 resize is the only down-scaling built)')
@@ -184,25 +223,34 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         with capi.region('sr_prep'):
             if prep is None:
                 shared = N == 1 or getattr(self, 'assume_shared_styles', False)
-                wsel = ws3[:1] if shared else ws3
-                prep = {'main': sr_tc.Prepared(self, wsel, sp)}
-                if self.fuse_mode != 'v1':
-                    prep.update({'ht0': sr_tc.pack_for(self.head_torso_block.conv0, wsel[:, 0], sp), 'ht1': sr_tc.pack_for(self.head_torso_block.conv1, wsel[:, 1], sp),
-                                 'htrgb': self.head_torso_block.torgb.folded_weight(wsel[:, 2])})
+                prep = self.prepare_styles(ws3[:1] if shared else ws3)
             plain = self._plain()
-            x0 = sr_tc.to_nhwc_f16(x, self.input_resolution, sp)
-            rgb0 = self._resize(rgb, self.input_resolution) if rgb.shape[-1] != self.input_resolution else capi.f32(rgb)
-            rgb_256 = self._resize(rgb0, 256)
-            weights_256 = self._resize(weights_img.detach(), 256)
+            R = self.input_resolution
+            if x_nhwc is not None:                                       # one launch, bit-identical to the three below
+                xn = capi.f32(x_nhwc)
+                _, h, w, Cc = xn.shape
+                x0 = torch.empty(N, R, R, (Cc + 63) // 64 * 64 * wide, device=xn.device, dtype=torch.float16)
+                rgb0 = torch.empty(N, 3, R, R, device=xn.device)
+                rgb_256 = torch.empty(N, 3, 256, 256, device=xn.device)
+                weights_256 = torch.empty(N, 1, 256, 256, device=xn.device)
+                capi.check(capi.lib().r3dp_sr_warp_input(capi.ptr(xn), capi.ptr(capi.f32(wsum)), N, Cc, h, w, R, capi.ptr(x0, torch.float16), capi.ptr(rgb0),
+                                                         capi.ptr(rgb_256), capi.ptr(weights_256), int(sp), capi.stream()))
+            else:
+                x0 = sr_tc.to_nhwc_f16(x, R, sp)
+                rgb0 = self._resize(rgb, R) if rgb.shape[-1] != R else capi.f32(rgb)
+                rgb_256 = self._resize(rgb0, 256)
+                weights_256 = self._resize(weights_img.detach(), 256)
             cc = self._clip_cache
             if cc is not None and cc['split'] != sp:                    # begun in another sr_mode: run uncached
                 cc = None
             if cc is None:
                 ref_torso_256, ref_bg_256 = self._aa_down2(ref_torso_rgb), self._aa_down2(ref_bg_rgb)
+            elif cc['batch'] is not None and cc['batch'][0].shape[0] == N:  # per-clip constants, broadcast over the batch once per clip
+                ref_torso_256, ref_bg_256 = cc['batch']
             else:                                                        # per-clip constants, one frame broadcast over the batch (0.8 MB copies)
                 ref_torso_256, ref_bg_256 = cc['ref_torso_256'].expand(N, -1, -1, -1).contiguous(), cc['ref_bg_256'].expand(N, -1, -1, -1).contiguous()
         main, Nw = prep['main'], prep['main'].Nw
-        b0, b1, hb = self.block0, self.block1, getattr(self, 'head_torso_block', None)
+        b0 = self.block0
         # block0: 128^2 -> 256^2 head features + head rgb
         a0 = sr_tc.layer(x0, b0.conv0, main.wp[0], 2, sp)
         xh = torch.empty(N, 256, 256, 256 * wide, device=x.device, dtype=torch.float16)
@@ -211,13 +259,29 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
             capi.check(sr_tc._fn('layer_torgb', sp)(capi.ptr(a0, torch.float16), capi.ptr(main.wp[1], torch.float16), capi.ptr(capi.f32(b0.conv1.bias)),
                                                 capi.ptr(main.wrgb0), capi.ptr(capi.f32(b0.torgb.bias)), capi.ptr(rgb0), N, Nw, 256, 256, 256, 256,
                                                 capi.ptr(xh, torch.float16), capi.ptr(rgb_h), capi.stream()))
-        # torso warper: the caller's PyTorch module (opaque child, sr_with_ref.py:84-87)
+        return {'N': N, 'split': sp, 'prep': prep, 'plain': plain, 'cc': cc, 'device': x.device, 'xh': xh, 'rgb_h': rgb_h, 'ref_bg_256': ref_bg_256,
+                'weights_256': weights_256, 'out_clamp': bool(block_kwargs.pop('out_clamp', False)), 'out_uint8': bool(block_kwargs.pop('out_uint8', False)),
+                'torso_args': (ref_torso_256, segmap, kp_s, kp_d, rgb_256, weights_256), 'target_torso_mask': target_torso_mask}
+
+    def run_torso(self, st: Dict):
+        """The torso warper: the caller's PyTorch module (opaque child, sr_with_ref.py:84-87) -> (rgb_torso, facev2v_ret)."""
+        ref_torso_256, segmap, kp_s, kp_d, rgb_256, weights_256 = st['torso_args']
         with capi.region('torso_model'):
-            rgb_torso, facev2v_ret = self.torso_model(ref_torso_256, segmap, kp_s, kp_d, rgb_256.detach(), weights_256.detach(), cal_loss=True,
-                                                      target_torso_mask=target_torso_mask)
+            return self.torso_model(ref_torso_256, segmap, kp_s, kp_d, rgb_256.detach(), weights_256.detach(), cal_loss=True,
+                                    target_torso_mask=st['target_torso_mask'])
+
+    def forward_post(self, st: Dict, rgb_torso: torch.Tensor, facev2v_ret: Dict) -> torch.Tensor:
+        """Second half of forward(), after the torso_model call: torso encoder, background features, head / torso / background fusion
+        and block1 -> the image (fp32 [N,3,512,512], or uint8 [N,512,512,3] when forward_pre() got out_uint8)."""
+        L = capi.lib()
+        N, sp, prep, plain, cc, dev = st['N'], st['split'], st['prep'], st['plain'], st['cc'], st['device']
+        wide = 2 if sp else 1
+        xh, rgb_h, weights_256 = st['xh'], st['rgb_h'], st['weights_256']
+        main, Nw = prep['main'], prep['main'].Nw
+        b1, hb = self.block1, getattr(self, 'head_torso_block', None)
         x_torso = self._conv(sr_tc.to_nhwc_f16(facev2v_ret['deformed_torso_hid'], 256, sp), plain['te'], 0, sp)       # 1x1, 64 -> 256
         if cc is None:
-            x_bg = self._bg_features(ref_bg_256, plain, sp)
+            x_bg = self._bg_features(st['ref_bg_256'], plain, sp)
         else:
             x_bg = cc['x_bg']                                            # [1,256,256,256 (x2 split)] fp16, read by every frame of the batch
         thr = float(self.hparams['htbsr_head_threshold'])
@@ -225,7 +289,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
             # head/torso fusion v1 (sr_with_ref.py:96-98): plain alpha blend of the rgb images AND of the feature maps; no fusing convs, no head_torso_block
             alpha = weights_256
             rgb_p2 = self._blend(rgb_h, rgb_torso, alpha)
-            xp = torch.empty(N, 256, 256, 256 * wide, device=x.device, dtype=torch.float16)
+            xp = torch.empty(N, 256, 256, 256 * wide, device=dev, dtype=torch.float16)
             capi.check((L.r3dp_sr_tcx_alpha_mix if sp else L.r3dp_sr_alpha_mix)(capi.ptr(xh, torch.float16), xh.shape[-1], capi.ptr(x_torso, torch.float16), x_torso.shape[-1], capi.ptr(alpha), 256,
                                            N, 256, 256, capi.ptr(xp, torch.float16), capi.stream()))
         else:
@@ -235,7 +299,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
                 inp7 = torch.cat([rgb_h.clamp(-1, 1) / 2 + 0.5, weights_256, capi.f32(rgb_torso).clamp(-1, 1) / 2 + 0.5], dim=1)
                 t = sr_tc.to_nhwc_f16(inp7, 256, split=True)
                 t = self._conv(self._conv(self._conv(t, plain['ap0'], 2, split=True), plain['ap2'], 2, split=True), plain['ap4'], 0, split=True)
-                alpha = torch.empty(N, 1, 256, 256, device=x.device)
+                alpha = torch.empty(N, 1, 256, 256, device=dev)
                 capi.check(L.r3dp_sr_alpha_gate(capi.ptr(t, torch.float16), t.shape[-1], t.shape[-1] // 2, capi.ptr(weights_256), N, 256, 256, capi.ptr(alpha),
                                                 capi.stream()))
                 if not self.training:                              # :141-143: batch-wide 5 % quantile of the mask values above 0.05 (a host-side scalar, as in the reference)
@@ -248,8 +312,8 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
             rgb_p = self._blend(rgb_h, rgb_torso, alpha)
             xf = self._conv(self._conv(self._alpha_cat(xh, 256, x_torso, 256, alpha, sp), plain['fh0'], 2, sp), plain['fh2'], 0, sp)
             c0 = sr_tc.layer(xf, hb.conv0, prep['ht0'], 1, sp)
-            xp = torch.empty(N, 256, 256, 256 * wide, device=x.device, dtype=torch.float16)
-            rgb_p2 = torch.empty(N, 3, 256, 256, device=x.device)
+            xp = torch.empty(N, 256, 256, 256 * wide, device=dev, dtype=torch.float16)
+            rgb_p2 = torch.empty(N, 3, 256, 256, device=dev)
             with capi.region('sr_conv'):
                 capi.check(sr_tc._fn('layer_torgb_noup', sp)(capi.ptr(c0, torch.float16), capi.ptr(prep['ht1'], torch.float16), capi.ptr(capi.f32(hb.conv1.bias)),
                                                          capi.ptr(prep['htrgb']), capi.ptr(capi.f32(hb.torgb.bias)), capi.ptr(rgb_p), N, Nw, 256, 256, 256, 256,
@@ -257,17 +321,19 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         # person / background fusion, sr_with_ref.py:115-124
         occ = capi.f32(facev2v_ret['occlusion_2'])
         torso_occ = occ if occ.shape[-1] == 256 else self._resize(occ, 256)
-        person = torch.empty(N, 1, 256, 256, device=x.device)
+        person = torch.empty(N, 1, 256, 256, device=dev)
         capi.check(L.r3dp_sr_person_occlusion(capi.ptr(alpha), capi.ptr(torso_occ), thr, N, 256, 256,
                                               capi.ptr(person), capi.stream()))
-        rgb_f = self._blend(rgb_p2, ref_bg_256, person)
+        rgb_f = self._blend(rgb_p2, st['ref_bg_256'], person)
         xg = self._alpha_cat(xp, 256, x_bg, 256, person, sp)
         xg = self._conv(self._conv(self._conv(xg, plain['ff0'], 2, sp), plain['ff2'], 2, sp), plain['ff4'], 0, sp)
-        # block1: 256^2 -> 512^2
+        # block1: 256^2 -> 512^2; with out_uint8 the last epilogue writes the video frames (real3d_infer.py:515-519)
         a2 = sr_tc.layer(xg, b1.conv0, main.wp[2], 2, sp)
-        out = torch.empty(N, 3, 512, 512, device=x.device)
+        u8 = st['out_uint8']
+        out = torch.empty(N, 512, 512, 3, device=dev, dtype=torch.uint8) if u8 else torch.empty(N, 3, 512, 512, device=dev)
         with capi.region('sr_conv'):
             capi.check((L.r3dp_sr_tcx_last_layer if sp else L.r3dp_sr_tc_last_layer_ex)(
                 capi.ptr(a2, torch.float16), capi.ptr(main.wp[3], torch.float16), capi.ptr(capi.f32(b1.conv1.bias)), capi.ptr(main.wrgb1),
-                capi.ptr(capi.f32(b1.torgb.bias)), capi.ptr(rgb_f), N, Nw, 128, 512, 512, capi.ptr(out), None, 0, capi.stream()))
-        return out, facev2v_ret
+                capi.ptr(capi.f32(b1.torgb.bias)), capi.ptr(rgb_f), N, Nw, 128, 512, 512, None if u8 else capi.ptr(out),
+                capi.ptr(out, torch.uint8) if u8 else None, int(st['out_clamp'] or u8), capi.stream()))
+        return out

@@ -52,29 +52,65 @@ class RenderHead(torch.nn.Module):
             'box_warp': hp.get('box_warp', 1.0), 'white_back': False,
         }
 
-    @torch.no_grad()
-    def synthesis(self, planes, camera: torch.Tensor, ret: Optional[Dict] = None, cond: Optional[Dict] = None, **render_overrides) -> Dict[str, torch.Tensor]:
-        """planes [N,3,C,H,W], camera [N,25] -> ret dict with the reference's keys (secc_img2plane.py:134-136)."""
-        if ret is None:
-            ret = {}
+    def _render(self, planes, camera: torch.Tensor, render_overrides: Dict):
         cam2world = camera[:, :16].reshape(-1, 4, 4)
         intrinsics = camera[:, 16:25].reshape(-1, 3, 3)
+        ray_o, ray_d = self.ray_sampler(cam2world, intrinsics, self.neural_rendering_resolution)
+        opts = dict(self.rendering_kwargs, **render_overrides)
+        return self.renderer(planes, self.decoder, ray_o, ray_d, opts)
+
+    def _lean(self) -> bool:
+        return self.superresolution.sr_mode in ('tc', 'tc_exact') and not self.hparams.get('mask_invalid_rays', False)
+
+    def _lean_sr_inputs(self, feat: torch.Tensor):
+        """The renderer's channels-last output as the SR's lean inputs: (rgb view, feature view, x_nhwc, ones_ws) - no NCHW copies, and
+        ones_ws is allocated once per batch size."""
         res = self.neural_rendering_resolution
-        ray_o, ray_d = self.ray_sampler(cam2world, intrinsics, res)
-        N = ray_o.shape[0]
+        N = feat.shape[0]
+        x_nhwc = feat.view(N, res, res, feat.shape[-1])
+        if getattr(self, '_ones_ws', None) is None or self._ones_ws.shape[0] != N or self._ones_ws.device != feat.device:
+            self._ones_ws = torch.ones(N, 14, self.hparams['w_dim'], device=feat.device)
+        return x_nhwc[..., :3].permute(0, 3, 1, 2), x_nhwc.permute(0, 3, 1, 2), x_nhwc, self._ones_ws
+
+    def _torso_pre_from(self, feat, wsum, cond: Dict, out_uint8: bool) -> Dict:
+        rgb, x, x_nhwc, ones_ws = self._lean_sr_inputs(feat)
+        res = self.neural_rendering_resolution
+        return self.superresolution.forward_pre(rgb, x, ones_ws, cond['ref_torso_img'], cond['bg_img'], wsum.view(feat.shape[0], 1, res, res), cond['segmap'],
+                                                cond['kp_s'], cond['kp_d'], cond.get('target_torso_mask'), noise_mode='none', x_nhwc=x_nhwc, wsum=wsum,
+                                                rgb_from_x=True, out_clamp=True, out_uint8=out_uint8)
+
+    @torch.no_grad()
+    def torso_pre(self, planes, camera: torch.Tensor, cond: Dict, out_uint8: bool = False, **render_overrides) -> Dict:
+        """Lean torso step up to the torso_model call: render, then the first half of the torso SR head (forward_pre) on the renderer's
+        channels-last output.  Continue with superresolution.run_torso(state) and superresolution.forward_post(state, ...) -> the image,
+        clamped to [-1,1] (uint8 HWC frames with out_uint8)."""
+        feat, _, wsum, _ = self._render(planes, camera, render_overrides)
+        return self._torso_pre_from(feat, wsum, cond, out_uint8)
+
+    @torch.no_grad()
+    def synthesis(self, planes, camera: torch.Tensor, ret: Optional[Dict] = None, cond: Optional[Dict] = None, **render_overrides) -> Dict[str, torch.Tensor]:
+        """planes [N,3,C,H,W], camera [N,25] -> ret dict with the reference's keys (secc_img2plane.py:134-136).
+        lean=True (tensor-core SR, no mask_invalid_rays): the frame-loop fast path of FrameEngine; only ret['image'] (plus ret['is_ray_valid']
+        for the plain head) is filled, clamped to [-1,1], or as uint8 HWC frames [N,512,512,3] with out_uint8=True."""
+        if ret is None:
+            ret = {}
+        res = self.neural_rendering_resolution
         lean = bool(render_overrides.pop('lean', False))
         out_uint8 = bool(render_overrides.pop('out_uint8', False))
-        opts = dict(self.rendering_kwargs, **render_overrides)
-        feat, depth, wsum, valid = self.renderer(planes, self.decoder, ray_o, ray_d, opts)
-        if lean and not self.torso and self.superresolution.sr_mode in ('tc', 'tc_exact') and not self.hparams.get('mask_invalid_rays', False):
+        feat, depth, wsum, valid = self._render(planes, camera, render_overrides)
+        N = feat.shape[0]
+        if lean and self._lean():
             # frame-loop fast path (FrameEngine): only ret['image'] is wanted, so the NCHW copies of the feature / weight images, the
-            # clamped raw image and the per-call ones_ws are not materialised; the SR reads the renderer's channels-last output directly
-            x_nhwc = feat.view(N, res, res, feat.shape[-1])
-            if getattr(self, '_ones_ws', None) is None or self._ones_ws.shape[0] != N or self._ones_ws.device != feat.device:
-                self._ones_ws = torch.ones(N, 14, self.hparams['w_dim'], device=feat.device)
-            # the clamp (and, if asked, the uint8 HWC conversion of real3d_infer.py:519) happen in the last SR epilogue
-            sr_image = self.superresolution(x_nhwc[..., :3].permute(0, 3, 1, 2), x_nhwc.permute(0, 3, 1, 2), self._ones_ws, noise_mode='none',
-                                            x_nhwc=x_nhwc, out_clamp=True, out_uint8=out_uint8, rgb_from_x=True)
+            # clamped raw image and the per-call ones_ws are not materialised; the SR reads the renderer's channels-last output directly.
+            # The clamp (and, if asked, the uint8 HWC conversion of real3d_infer.py:519) happen in the last SR epilogue
+            if self.torso:
+                sr = self.superresolution
+                st = self._torso_pre_from(feat, wsum, cond, out_uint8)
+                rgb_torso, facev2v_ret = sr.run_torso(st)
+                ret['image'] = sr.forward_post(st, rgb_torso, facev2v_ret)
+                return ret
+            rgb, x, x_nhwc, ones_ws = self._lean_sr_inputs(feat)
+            sr_image = self.superresolution(rgb, x, ones_ws, noise_mode='none', x_nhwc=x_nhwc, out_clamp=True, out_uint8=out_uint8, rgb_from_x=True)
             ret.update({'image': sr_image, 'is_ray_valid': valid})
             return ret
         if out_uint8:

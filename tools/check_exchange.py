@@ -4,7 +4,8 @@
 
 Every rank renders `steps` batches of its own frames; with exchange='p2p' the frames are pushed by the copy engine into the clip on rank 0
 (CUDA IPC mapping), with exchange='allgather' NCCL gathers them.  Rank 0 then compares the assembled clip with the frames every rank kept
-locally (sent through an independent NCCL gather at the end) - bit for bit - and prints the per-step cost of both exchanges."""
+locally (sent through an independent NCCL gather at the end) - bit for bit - and prints the per-step cost of both exchanges.
+With --torso the engines run the torso head (synthetic.StubTorsoModel as the warper, the clip constants of begin_clip(), kp_d per frame)."""
 import os
 import sys
 
@@ -20,17 +21,27 @@ def main():
     torch.cuda.set_device(local)
     dev = torch.device('cuda', local)
     dist.init_process_group('nccl', device_id=dev)
+    torso = '--torso' in sys.argv[1:]
     B, steps = 4, 6
     planes = ren.planes_to_channels_last(syn.make_planes(B * 2, seed=10 + rank).to(dev)).data
     cams = syn.make_cameras(B * 2, seed=20 + rank).to(dev)
     u = syn.make_jitter(B * 2, 4096, 48, 0, seed=30 + rank)[0].to(dev)
     res = [(ren.PlanesCL(planes[i * B:(i + 1) * B]), cams[i * B:(i + 1) * B], u[i * B:(i + 1) * B]) for i in range(2)]
+    kw, kp_d = {}, [None, None]
+    if torso:
+        kp = (torch.rand(B * 2, 68, 3, generator=torch.Generator().manual_seed(40 + rank)) * 2 - 1).to(dev)
+        kp_d = [kp[i * B:(i + 1) * B] for i in range(2)]
+        res = [r + (None, kp_d[i]) for i, r in enumerate(res)]
+        kw = {'torso_model': syn.StubTorsoModel()}
+        consts = syn.make_warp_inputs(1, seed=7)
     ok = True
     for u8 in (True, False):
         for mode in ('p2p', 'allgather'):
-            eng = engine.FrameEngine(batch=B, sr_mode='tc', device=dev, world=world, rank=rank, dist=dist, hp={'num_samples_fine': 0}, out_uint8=u8,
-                                     exchange=mode)
-            eng.load_params(syn.make_decoder_params(seed=4), syn.make_sr_params(seed=5))
+            hp = dict(syn.WARP_HPARAMS, num_samples_fine=0) if torso else {'num_samples_fine': 0}
+            eng = engine.FrameEngine(batch=B, sr_mode='tc', device=dev, world=world, rank=rank, dist=dist, hp=hp, out_uint8=u8, exchange=mode, **kw)
+            eng.load_params(syn.make_decoder_params(seed=4), syn.make_sr_warp_params(seed=6) if torso else syn.make_sr_params(seed=5))
+            if torso:
+                eng.begin_clip(*(consts[k].to(dev) for k in ('ref_torso_rgb', 'ref_bg_rgb', 'segmap', 'kp_s')))
             eng.prepare(res)
             clip = eng.open_clip(steps * B) if mode == 'p2p' else None
             local_frames, gathered = [], []
@@ -38,7 +49,7 @@ def main():
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             for s in range(steps):
-                out = eng.step(*res[s % 2], frame_index=s * B)
+                out = eng.step(*res[s % 2][:3], frame_index=s * B, **({'kp_d': kp_d[s % 2]} if torso else {}))
                 if mode == 'allgather':
                     eng.wait_gather()
                     gathered.append(out.clone())

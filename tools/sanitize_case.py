@@ -2,7 +2,9 @@
     compute-sanitizer --tool memcheck python tools/sanitize_case.py
 Covers: streaming render kernel (single pass), two-pass tensor-core render kernel, tri-grid variant, tensor-core SR (all four conv launches,
 FIR, edge) with fp16 and with split operands, uint8 epilogue, stand-alone sampler, the torso head (`warp`: alpha-cat / blend kernels, plain convs,
-SynthesisBlockNoUp tail, per-clip cache) and large_sr (`large`: residual epilogue, plain ToRGB), both in 'tc' and 'tc_exact'."""
+SynthesisBlockNoUp tail, per-clip cache) and large_sr (`large`: residual epilogue, plain ToRGB), both in 'tc' and 'tc_exact'.
+`torso_engine`: the torso head's one-launch input kernel (64^2 and 128^2 sources, both split values) and one FrameEngine step of the torso
+head with uint8 frames per warper setting (split graphs, whole graph)."""
 import os
 import sys
 
@@ -70,6 +72,30 @@ def main():
             m.end_clip()
         torch.cuda.synchronize()
         print('warp', mode, float(img.abs().mean()), float(img_c.abs().mean()))
+    if what in ('all', 'torso_engine'):
+        from real3dportrait_b200 import _capi as capi, engine
+        for res in (64, 128):
+            for split in (0, 1):
+                N, C = 1, 32
+                x = torch.randn(N, res, res, C, generator=g).to(dev)
+                w = torch.rand(N, res * res, 1, generator=g).to(dev)
+                y = torch.empty(N, 128, 128, 64 * (1 + split), device=dev, dtype=torch.float16)
+                rgb0, rgb256, w256 = torch.empty(N, 3, 128, 128, device=dev), torch.empty(N, 3, 256, 256, device=dev), torch.empty(N, 1, 256, 256, device=dev)
+                capi.check(capi.lib().r3dp_sr_warp_input(capi.ptr(x), capi.ptr(w), N, C, res, res, 128, capi.ptr(y, torch.float16), capi.ptr(rgb0),
+                                                         capi.ptr(rgb256), capi.ptr(w256), split, capi.stream()))
+                torch.cuda.synchronize()
+                print('warp_input', res, split, float(rgb256.abs().mean()), float(w256.mean()))
+        inp = {k: v.to(dev) for k, v in syn.make_warp_inputs(1, seed=7).items()}
+        for in_graph in (False, True):
+            eng = engine.FrameEngine(batch=1, sr_mode='tc', hp=dict(syn.WARP_HPARAMS, num_samples_fine=0), torso_model=syn.StubTorsoModel(),
+                                     out_uint8=True, warper_in_graph=in_graph)
+            eng.load_params(syn.make_decoder_params(seed=4), syn.make_sr_warp_params(seed=6))
+            eng.begin_clip(inp['ref_torso_rgb'], inp['ref_bg_rgb'], inp['segmap'], inp['kp_s'])
+            planes, cam = syn.make_planes(1, seed=3).to(dev), syn.make_cameras(1, seed=4).to(dev)
+            u_c, _ = syn.make_jitter(1, 4096, 48, 0, seed=5)
+            out = eng.step(planes, cam, u_c.to(dev), kp_d=inp['kp_d'])
+            torch.cuda.synchronize()
+            print('torso_engine', in_graph, eng.graph is not None, float(out.float().mean()))
     for mode in (('tc', 'tc_exact') if what in ('all', 'large') else ()):
         sr = r3.SuperresolutionHybrid8XDC(channels=32, img_resolution=512, sr_num_fp16_res=0, sr_antialias=True, large_sr=True, sr_mode=mode,
                                           resblocks_in_large_sr=1)
