@@ -208,7 +208,8 @@ int r3dp_sr_torgb_fp32(const float* x, const float* wf_rgb, const float* bias, c
  *                          r3dp_sr_tc_scratch_bytes(N,O,H,W)
  * r3dp_sr_tc_torgb         ToRGB + upsampled skip of a non-final block -> img fp32 NCHW [N,3,H,W]
  * r3dp_sr_tc_last_layer    last conv (I -> 128) fused with ToRGB + skip: only the image is written (fp32 NCHW [N,3,H,W]);
- *                          wrgb [Nw,3,128], brgb [3], img_prev [N,3,H/2,W/2]. */
+ *                          wrgb [Nw,3,128], brgb [3], img_prev [N,3,H/2,W/2]; img_prev may be NULL (no skip: the image is
+ *                          ToRGB + brgb alone, the block1(x, None, ws) of weight_fuse=False, sr_with_ref.py:161). */
 int r3dp_sr_tc_pack_weights(const float* wf, int Nw, int O, int I, void* packed_f16, r3dp_stream_t stream);
 int r3dp_sr_tc_input(const float* x, int N, int C, int h, int w, int size, void* y_f16, r3dp_stream_t stream);
 size_t r3dp_sr_tc_scratch_bytes(int N, int O, int H, int W);
@@ -236,7 +237,8 @@ int r3dp_sr_tc_last_layer(const void* x_f16, const void* wp_f16, const float* bi
 /* The same with the caller loop's output conversion fused into the epilogue (inference/real3d_infer.py:515-519):
  *   clamp != 0       img_out clamped to [-1, 1] (imgs.clamp(-1,1))
  *   img_out_u8       non-NULL: write uint8 HWC video frames [N,H,W,3] = uint8(int((clamp(x) + 1) / 2 * 255)) INSTEAD of the fp32 image
- *                    (4x fewer bytes to gather / copy to the host); img_out may then be NULL. */
+ *                    (4x fewer bytes to gather / copy to the host); img_out may then be NULL.
+ * img_prev may be NULL (no skip), as for r3dp_sr_tc_last_layer; so may it for r3dp_sr_tcx_last_layer. */
 int r3dp_sr_tc_last_layer_ex(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
                              const float* img_prev, int N, int Nw, int I, int H, int W, float* img_out, uint8_t* img_out_u8, int clamp,
                              r3dp_stream_t stream);
@@ -272,7 +274,8 @@ int r3dp_sr_tcx_conv(const void* x_f16, const void* wp_f16, const float* bias, i
  * r3dp_sr_tcx_layer_torgb_noup    SynthesisBlockNoUp tail; ToRGB over the fp32 activation
  * r3dp_sr_tcx_alpha_cat_ex        out [N,H,W,2*(Ca+Cb)] = split of cat[xa*alpha, xb*(1-alpha)]; stride_a / stride_b are the physical pixel strides
  * r3dp_sr_tcx_alpha_mix           out [N,H,W,2*C] = split of xa*alpha + xb*(1-alpha); strides as above
- * r3dp_sr_tcx_torgb_ex            x [N,H,W,2*C]: the dot product runs over hi + lo in fp32 */
+ * r3dp_sr_tcx_torgb_ex            x [N,H,W,2*C]: the dot product runs over hi + lo in fp32
+ * r3dp_sr_tcx_cat3                out [N,H,W,2*(Ca+Cb+Cc)] = [hi | lo] layout of cat[xa, xb, xc]: each operand's hi and lo halves are copied unchanged */
 int r3dp_sr_tcx_conv_res(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
                          int act, const void* residual_f16, void* y_f16, r3dp_stream_t stream);
 int r3dp_sr_tcx_layer_torgb_noup(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
@@ -284,6 +287,8 @@ int r3dp_sr_tcx_alpha_mix(const void* xa_f16, int stride_a, const void* xb_f16, 
                           void* out_f16, r3dp_stream_t stream);
 int r3dp_sr_tcx_torgb_ex(const void* x_f16, const float* wrgb, const float* brgb, const float* img_prev, int same_res, int N, int Nw, int C,
                          int H, int W, float* img_out, r3dp_stream_t stream);
+int r3dp_sr_tcx_cat3(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, const void* xc_f16, int Cc, int stride_c,
+                     int xc_shared, int N, int H, int W, void* out_f16, r3dp_stream_t stream);
 
 /* Measurement hooks (bench.py): time every tensor-core conv launch with a CUDA-event pair on its launching stream. */
 int r3dp_sr_tc_prof(int enable);
@@ -325,6 +330,10 @@ int r3dp_sr_alpha_cat(const void* xa_f16, int Ca, int stride_a, const void* xb_f
 /* xb_shared != 0: xb holds ONE frame [1,H,W,Cb] read by every frame of the batch (per-clip constant features, e.g. bg_encoder(ref_bg)). */
 int r3dp_sr_alpha_cat_ex(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, int xb_shared, const float* alpha,
                          int N, int H, int W, void* out_f16, r3dp_stream_t stream);
+/* weight_fuse=False (sr_with_ref.py:159): out [N,H,W,Ca+Cb+Cc] = cat[xa, xb, xc] on fp16 NHWC, unweighted (a bit-exact copy); pixel strides
+ * stride_a/b/c in elements; xc_shared != 0: xc holds ONE frame [1,H,W,Cc] read by every frame of the batch (the per-clip bg_encoder(ref_bg)). */
+int r3dp_sr_cat3(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, const void* xc_f16, int Cc, int stride_c,
+                 int xc_shared, int N, int H, int W, void* out_f16, r3dp_stream_t stream);
 int r3dp_sr_blend(const float* a, const float* b, const float* alpha, int N, int C, int H, int W, float* out, r3dp_stream_t stream);
 int r3dp_sr_person_occlusion(const float* head_alpha, const float* torso_occlusion, float threshold, int N, int H, int W, float* out,
                              r3dp_stream_t stream);

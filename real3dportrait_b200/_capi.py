@@ -100,6 +100,8 @@ _SIGNATURES = {
     'r3dp_sr_tc_layer_torgb_noup': (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     'r3dp_sr_alpha_cat': (_I, [_P, _I, _I, _P, _I, _I, _P, _I, _I, _I, _P, _P]),
     'r3dp_sr_alpha_cat_ex': (_I, [_P, _I, _I, _P, _I, _I, _I, _P, _I, _I, _I, _P, _P]),
+    'r3dp_sr_cat3': (_I, [_P, _I, _I, _P, _I, _I, _P, _I, _I, _I, _I, _I, _I, _P, _P]),
+    'r3dp_sr_tcx_cat3': (_I, [_P, _I, _I, _P, _I, _I, _P, _I, _I, _I, _I, _I, _I, _P, _P]),
     'r3dp_sr_blend': (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P]),
     'r3dp_sr_person_occlusion': (_I, [_P, _P, _F, _I, _I, _I, _P, _P]),
     'r3dp_sr_resize_aa_down2': (_I, [_P, _I, _I, _I, _I, _P, _P]),

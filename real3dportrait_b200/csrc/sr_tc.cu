@@ -1430,28 +1430,40 @@ extern "C" int r3dp_sr_tcx_layer_torgb_noup(const void* x_f16, const void* wp_f1
 // out[n,y,x,:] = [ xa[n,y,x,0:Ca] * alpha[n,y,x] , xb[n,y,x,0:Cb] * (1 - alpha[n,y,x]) ]   (sr_with_ref.py:111,122: alpha-cat fusion), fp16 NHWC
 // SPLIT: xa / xb hold [hi | lo] halves (lo at half their pixel stride); hi + lo is scaled in fp32 and the output is the [hi | lo] layout of the
 // (Ca + Cb)-channel result: out [N,H,W, 2 (Ca + Cb)], lo at channel Ca + Cb.
+// alpha == NULL: the plain concat [xa, xb, xc] (sr_with_ref.py:159, weight_fuse=False); the 8-channel vectors (both halves when SPLIT) are
+// copied unchanged.  The LAST operand (xb, or xc when Cc > 0) may hold one frame shared by the batch (hw_last > 0).
 template <bool SPLIT>
 __global__ void alpha_cat_kernel(const __half* __restrict__ xa, int Ca, int sa, const __half* __restrict__ xb, int Cb, int sb,
-                                 long long hw_b, const float* __restrict__ alpha, long long npix, __half* __restrict__ out) {
-    const int cv = (Ca + Cb) / 8;
+                                 const __half* __restrict__ xc, int Cc, int sc, long long hw_last, const float* __restrict__ alpha, long long npix,
+                                 __half* __restrict__ out) {
+    const int Ct = Ca + Cb + Cc, cv = Ct / 8;
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= npix * cv) return;
-    const long long pix = idx / cv; const int c8 = (int)(idx - pix * cv);
-    const float al = alpha[pix];
-    const bool first = c8 * 8 < Ca;
-    const long long pb = hw_b > 0 ? pix % hw_b : pix;                    // xb holds one frame shared by the batch
-    const __half* src = first ? xa + pix * sa + c8 * 8 : xb + pb * sb + (c8 * 8 - Ca);
+    const long long pix = idx / cv; const int c8 = (int)(idx - pix * cv), c = c8 * 8;
+    const bool first = c < Ca;
+    const long long p_last = hw_last > 0 ? pix % hw_last : pix;             // the last operand holds one frame shared by the batch
+    const __half* src; int s;
+    if (first) { src = xa + pix * sa + c; s = sa; }
+    else if (c < Ca + Cb) { src = xb + (Cc > 0 ? pix : p_last) * sb + (c - Ca); s = sb; }
+    else { src = xc + p_last * sc + (c - Ca - Cb); s = sc; }
     const uint4 raw = __ldg(reinterpret_cast<const uint4*>(src));
+    __half* dst = out + pix * (SPLIT ? 2 : 1) * Ct + c;
+    if (!alpha) {
+        *reinterpret_cast<uint4*>(dst) = raw;
+        if (SPLIT) *reinterpret_cast<uint4*>(dst + Ct) = __ldg(reinterpret_cast<const uint4*>(src + s / 2));
+        return;
+    }
+    const float al = alpha[pix];
     const float m = first ? al : 1.0f - al;
     const __half2* h = reinterpret_cast<const __half2*>(&raw);
     uint4 pk; __half2* ph = reinterpret_cast<__half2*>(&pk);
     if (!SPLIT) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) { const float2 f = __half22float2(h[j]); ph[j] = __floats2half2_rn(f.x * m, f.y * m); }
-        *reinterpret_cast<uint4*>(out + idx * 8) = pk;
+        *reinterpret_cast<uint4*>(dst) = pk;
         return;
     }
-    const uint4 rawl = __ldg(reinterpret_cast<const uint4*>(src + (first ? sa : sb) / 2));
+    const uint4 rawl = __ldg(reinterpret_cast<const uint4*>(src + s / 2));
     const __half2* hl = reinterpret_cast<const __half2*>(&rawl);
     uint4 pl; __half2* pq = reinterpret_cast<__half2*>(&pl);
 #pragma unroll
@@ -1462,31 +1474,45 @@ __global__ void alpha_cat_kernel(const __half* __restrict__ xa, int Ca, int sa, 
         const float2 hf = __half22float2(ph[j]);
         pq[j] = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
     }
-    __half* dst = out + pix * 2 * (Ca + Cb) + c8 * 8;
     *reinterpret_cast<uint4*>(dst) = pk;
-    *reinterpret_cast<uint4*>(dst + Ca + Cb) = pl;
+    *reinterpret_cast<uint4*>(dst + Ct) = pl;
 }
-static int alpha_cat_impl(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, int xb_shared,
-                          const float* alpha, int N, int H, int W, void* out_f16, int split, r3dp_stream_t stream) {
-    R3DP_REQUIRE(xa_f16 && xb_f16 && alpha && out_f16, "sr_alpha_cat: null pointer");
+// Cc == 0: two operands (alpha-cat); alpha == NULL: unweighted concat.  last_shared: the last operand holds one frame [1,H,W,C].
+static int alpha_cat_impl(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, const void* xc_f16, int Cc,
+                          int stride_c, int last_shared, const float* alpha, int N, int H, int W, void* out_f16, int split, r3dp_stream_t stream) {
+    const char* what = alpha ? "sr_alpha_cat" : "sr_cat3";
+    R3DP_REQUIRE(xa_f16 && xb_f16 && (xc_f16 || Cc == 0) && out_f16, "%s: null pointer", what);
+    R3DP_REQUIRE(!alpha || Cc == 0, "%s: alpha weights two operands", what);
     const int wide = split ? 2 : 1;
-    R3DP_REQUIRE(N > 0 && H > 0 && W > 0 && Ca % 8 == 0 && Cb % 8 == 0 && stride_a >= wide * Ca && stride_b >= wide * Cb &&
-                 stride_a % (8 * wide) == 0 && stride_b % (8 * wide) == 0, "sr_alpha_cat: bad shape");
-    const long long npix = (long long)N * H * W, total = npix * ((Ca + Cb) / 8);
+    R3DP_REQUIRE(N > 0 && H > 0 && W > 0 && Ca % 8 == 0 && Cb % 8 == 0 && Cc % 8 == 0 && Cc >= 0 && stride_a >= wide * Ca && stride_b >= wide * Cb &&
+                 stride_a % (8 * wide) == 0 && stride_b % (8 * wide) == 0 && (Cc == 0 || (stride_c >= wide * Cc && stride_c % (8 * wide) == 0)),
+                 "%s: bad shape", what);
+    const long long npix = (long long)N * H * W, total = npix * ((Ca + Cb + Cc) / 8);
     auto kern = split ? alpha_cat_kernel<true> : alpha_cat_kernel<false>;
     kern<<<(unsigned)((total + 255) / 256), 256, 0, as_stream(stream)>>>(reinterpret_cast<const __half*>(xa_f16), Ca, stride_a,
-        reinterpret_cast<const __half*>(xb_f16), Cb, stride_b, xb_shared ? (long long)H * W : 0ll, alpha, npix, reinterpret_cast<__half*>(out_f16));
+        reinterpret_cast<const __half*>(xb_f16), Cb, stride_b, reinterpret_cast<const __half*>(xc_f16), Cc, stride_c,
+        last_shared ? (long long)H * W : 0ll, alpha, npix, reinterpret_cast<__half*>(out_f16));
     R3DP_LAUNCH_CHECK();
     count_launches(1);
     return 0;
 }
 extern "C" int r3dp_sr_alpha_cat_ex(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, int xb_shared,
                                     const float* alpha, int N, int H, int W, void* out_f16, r3dp_stream_t stream) {
-    return alpha_cat_impl(xa_f16, Ca, stride_a, xb_f16, Cb, stride_b, xb_shared, alpha, N, H, W, out_f16, 0, stream);
+    R3DP_REQUIRE(alpha, "sr_alpha_cat: null pointer");
+    return alpha_cat_impl(xa_f16, Ca, stride_a, xb_f16, Cb, stride_b, nullptr, 0, 0, xb_shared, alpha, N, H, W, out_f16, 0, stream);
 }
 extern "C" int r3dp_sr_tcx_alpha_cat_ex(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, int xb_shared,
                                         const float* alpha, int N, int H, int W, void* out_f16, r3dp_stream_t stream) {
-    return alpha_cat_impl(xa_f16, Ca, stride_a, xb_f16, Cb, stride_b, xb_shared, alpha, N, H, W, out_f16, 1, stream);
+    R3DP_REQUIRE(alpha, "sr_alpha_cat: null pointer");
+    return alpha_cat_impl(xa_f16, Ca, stride_a, xb_f16, Cb, stride_b, nullptr, 0, 0, xb_shared, alpha, N, H, W, out_f16, 1, stream);
+}
+extern "C" int r3dp_sr_cat3(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, const void* xc_f16, int Cc,
+                            int stride_c, int xc_shared, int N, int H, int W, void* out_f16, r3dp_stream_t stream) {
+    return alpha_cat_impl(xa_f16, Ca, stride_a, xb_f16, Cb, stride_b, xc_f16, Cc, stride_c, xc_shared, nullptr, N, H, W, out_f16, 0, stream);
+}
+extern "C" int r3dp_sr_tcx_cat3(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, const void* xc_f16, int Cc,
+                                int stride_c, int xc_shared, int N, int H, int W, void* out_f16, r3dp_stream_t stream) {
+    return alpha_cat_impl(xa_f16, Ca, stride_a, xb_f16, Cb, stride_b, xc_f16, Cc, stride_c, xc_shared, nullptr, N, H, W, out_f16, 1, stream);
 }
 extern "C" int r3dp_sr_alpha_cat(const void* xa_f16, int Ca, int stride_a, const void* xb_f16, int Cb, int stride_b, const float* alpha, int N,
                                  int H, int W, void* out_f16, r3dp_stream_t stream) {

@@ -102,7 +102,8 @@ def _frames_of(planes) -> int:
 class _TorsoGraphs:
     """One torso step as two CUDA graphs around an eager torso_model call: graph A (render, SR prep, block0, the warper's inputs), the
     warper on the current stream, its three outputs copied into graph B's static inputs (the caching allocator does not keep their
-    addresses), graph B (the rest of the head)."""
+    addresses), graph B (the rest of the head).  Under weight_fuse=False graph B reads neither rgb_torso nor occlusion_2; they are copied
+    all the same (two small copies) so that every configuration keeps one step layout."""
 
     def __init__(self, sr, a, st, b_in, b):
         self.sr, self.a, self.st, self.b_in, self.b = sr, a, st, b_in, b

@@ -5,8 +5,9 @@ Same constructor arguments, child-module names (`block0/1`, `torso_encoder`, `bg
 `fuse_head_torso_convs`, `head_torso_block`, `fuse_fg_bg_convs`, `torso_model`) and `forward` signature/return as the reference, so
 released checkpoints load with strict=True.  The conv stack (782 GFLOP/frame, SURVEY.md §8d) runs on the tensor-core kernels of
 csrc/sr_tc.cu; the torso warper `torso_model` (WarpBasedTorsoModelMediaPipe, SURVEY.md §2 #11: out of scope) stays the caller's
-PyTorch module and is called as an opaque child exactly where the reference calls it.  Supported configuration = the released one
-(egs/os_avatar/real3d_orig/secc_img2plane_torso_orig.yaml:26-30): torso_model_version v2, htbsr_head_weight_fuse_mode v2."""
+PyTorch module and is called as an opaque child exactly where the reference calls it.  Every configuration of the reference class is built:
+torso_model_version v1 | v2, weight_fuse True (htbsr_head_weight_fuse_mode v1 | v2 | v3) | False.  The released one
+(egs/os_avatar/real3d_orig/secc_img2plane_torso_orig.yaml:26-30) is torso_model_version v2, htbsr_head_weight_fuse_mode v2."""
 from __future__ import annotations
 
 from typing import Dict, Optional
@@ -48,23 +49,26 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         hp = dict(hp or {})
         self.hparams = {'torso_model_version': hp.get('torso_model_version', 'v2'), 'htbsr_head_weight_fuse_mode': hp.get('htbsr_head_weight_fuse_mode', 'v2'),
                         'htbsr_head_threshold': float(hp.get('htbsr_head_threshold', 0.9)), 'weight_fuse': hp.get('weight_fuse', True)}
-        self.fuse_mode = self.hparams['htbsr_head_weight_fuse_mode']
-        if self.hparams['torso_model_version'] != 'v2' or self.fuse_mode not in ('v1', 'v2', 'v3') or not self.hparams['weight_fuse']:
-            raise NotImplementedError('built: torso_model_version=v2 with htbsr_head_weight_fuse_mode v1 | v2 (the released Real3D torso config) | v3, weight_fuse=True')
+        self.weight_fuse = bool(self.hparams['weight_fuse'])
+        # weight_fuse=False concatenates the head, torso and background features unweighted and ignores the fuse mode (sr_with_ref.py:36,158-161)
+        self.fuse_mode = self.hparams['htbsr_head_weight_fuse_mode'] if self.weight_fuse else None
+        if self.hparams['torso_model_version'] not in ('v1', 'v2') or (self.weight_fuse and self.fuse_mode not in ('v1', 'v2', 'v3')):
+            raise NotImplementedError('built: torso_model_version v1 | v2 with weight_fuse=False or htbsr_head_weight_fuse_mode v1 | v2 | v3')
         if torso_model is not None:
-            self.torso_model = torso_model                      # the reference's WarpBasedTorsoModelMediaPipe('standard'), supplied by the caller
+            self.torso_model = torso_model                      # the reference's WarpBasedTorsoModelMediaPipe('standard') (model.py for v1, model2.py for v2)
         nn = torch.nn
         self.torso_encoder = nn.Sequential(nn.Conv2d(64, 256, 1, 1, padding=0))
         self.bg_encoder = nn.Sequential(nn.Conv2d(3, 64, 3, 1, padding=1), nn.LeakyReLU(), nn.Conv2d(64, 256, 3, 1, padding=1), nn.LeakyReLU(),
                                         nn.Conv2d(256, 256, 3, 1, padding=1))
-        if self.fuse_mode != 'v1':                              # the reference builds these children for every mode but v1 (sr_with_ref.py:36-55)
+        if self.fuse_mode in ('v2', 'v3'):                      # the reference builds these children for every weighted mode but v1 (sr_with_ref.py:36-55)
             self.head_torso_alpha_predictor = nn.Sequential(nn.Conv2d(7, 32, 3, 1, padding=1), nn.LeakyReLU(), nn.Conv2d(32, 32, 3, 1, padding=1),
                                                             nn.LeakyReLU(), nn.Conv2d(32, 1, 3, 1, padding=1), nn.Sigmoid())   # used by v3 only
             self.fuse_head_torso_convs = nn.Sequential(nn.Conv2d(512, 256, 3, 1, padding=1), nn.LeakyReLU(), nn.Conv2d(256, 256, 3, 1, padding=1))
             bk = {k: v for k, v in block_kwargs.items() if k not in ('sr_mode', 'channel_base', 'channel_max')}
             self.head_torso_block = SynthesisBlockNoUp(256, 256, w_dim=512, resolution=256, img_channels=3, is_last=False, use_fp16=False,
                                                        conv_clamp=None, **bk)
-        self.fuse_fg_bg_convs = nn.Sequential(nn.Conv2d(512, 64, 1, 1, padding=0), nn.LeakyReLU(), nn.Conv2d(64, 256, 3, 1, padding=1),
+        self.fuse_in_dim = 512 if self.weight_fuse else 768      # weight_fuse=False: cat[x, x_torso, x_bg] (sr_with_ref.py:57-58)
+        self.fuse_fg_bg_convs = nn.Sequential(nn.Conv2d(self.fuse_in_dim, 64, 1, 1, padding=0), nn.LeakyReLU(), nn.Conv2d(64, 256, 3, 1, padding=1),
                                               nn.LeakyReLU(), nn.Conv2d(256, 256, 3, 1, padding=1))
         self._plain_cache = None
         self._clip_cache = None
@@ -84,9 +88,9 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
                 'split': sp,
                 'te': _pack_plain(te[0], 64, split=sp), 'bg0': _pack_plain(bg[0], 64, split=sp), 'bg2': _pack_plain(bg[2], 128, split=sp),
                 'bg4': _pack_plain(bg[4], 256, split=sp),
-                'ff0': _pack_plain(ff[0], 512, split=sp), 'ff2': _pack_plain(ff[2], 128, split=sp), 'ff4': _pack_plain(ff[4], 256, split=sp),
+                'ff0': _pack_plain(ff[0], self.fuse_in_dim, split=sp), 'ff2': _pack_plain(ff[2], 128, split=sp), 'ff4': _pack_plain(ff[4], 256, split=sp),
             }
-            if self.fuse_mode != 'v1':
+            if self.fuse_mode in ('v2', 'v3'):
                 fh = self.fuse_head_torso_convs
                 self._plain_cache.update({'fh0': _pack_plain(fh[0], 512, split=sp), 'fh2': _pack_plain(fh[2], 256, split=sp)})
             if self.fuse_mode == 'v3':                             # the mask predictor runs with split fp16 operands (its output is thresholded)
@@ -100,7 +104,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         `static_prepared_warp` when the styles are constant (Real3D passes ws == 1): forward() then stops preparing them per call."""
         sp = self._split
         prep = {'main': sr_tc.Prepared(self, wsel, sp)}
-        if self.fuse_mode != 'v1':
+        if self.fuse_mode in ('v2', 'v3'):
             prep.update({'ht0': sr_tc.pack_for(self.head_torso_block.conv0, wsel[:, 0], sp), 'ht1': sr_tc.pack_for(self.head_torso_block.conv1, wsel[:, 1], sp),
                          'htrgb': self.head_torso_block.torgb.folded_weight(wsel[:, 2])})
         return prep
@@ -135,6 +139,18 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         fn = capi.lib().r3dp_sr_tcx_alpha_cat_ex if split else capi.lib().r3dp_sr_alpha_cat_ex
         capi.check(fn(capi.ptr(xa16, torch.float16), Ca, xa16.shape[-1], capi.ptr(xb16, torch.float16), Cb, xb16.shape[-1],
                       int(xb16.shape[0] == 1 and N > 1), capi.ptr(alpha), N, H, W, capi.ptr(out, torch.float16), capi.stream()))
+        return out
+
+    @staticmethod
+    def _cat3(xa16, xb16, xc16, split: bool = False) -> torch.Tensor:
+        """cat[xa, xb, xc] of three 256-channel NHWC fp16 tensors, unweighted; xc may hold ONE frame shared by the whole batch (per-clip constant
+        features).  split: [hi | lo] inputs, output = the [hi | lo] layout of the 768-channel result."""
+        N, H, W, _ = xa16.shape
+        out = torch.empty(N, H, W, 768 * (2 if split else 1), device=xa16.device, dtype=torch.float16)
+        fn = capi.lib().r3dp_sr_tcx_cat3 if split else capi.lib().r3dp_sr_cat3
+        capi.check(fn(capi.ptr(xa16, torch.float16), 256, xa16.shape[-1], capi.ptr(xb16, torch.float16), 256, xb16.shape[-1],
+                      capi.ptr(xc16, torch.float16), 256, xc16.shape[-1], int(xc16.shape[0] == 1 and N > 1), N, H, W, capi.ptr(out, torch.float16),
+                      capi.stream()))
         return out
 
     # ---- per-clip constants (SURVEY.md §8f #2) -------------------------------------------------------------------------------------------
@@ -264,26 +280,33 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
                 'torso_args': (ref_torso_256, segmap, kp_s, kp_d, rgb_256, weights_256), 'target_torso_mask': target_torso_mask}
 
     def run_torso(self, st: Dict):
-        """The torso warper: the caller's PyTorch module (opaque child, sr_with_ref.py:84-87) -> (rgb_torso, facev2v_ret)."""
+        """The torso warper: the caller's PyTorch module (opaque child, sr_with_ref.py:84-87) -> (rgb_torso, facev2v_ret).
+        torso_model_version v1 (model.py) takes no head weights image; v2 (model2.py) does."""
         ref_torso_256, segmap, kp_s, kp_d, rgb_256, weights_256 = st['torso_args']
         with capi.region('torso_model'):
+            if self.hparams['torso_model_version'] == 'v1':
+                return self.torso_model(ref_torso_256, segmap, kp_s, kp_d, rgb_256.detach(), cal_loss=True, target_torso_mask=st['target_torso_mask'])
             return self.torso_model(ref_torso_256, segmap, kp_s, kp_d, rgb_256.detach(), weights_256.detach(), cal_loss=True,
                                     target_torso_mask=st['target_torso_mask'])
 
     def forward_post(self, st: Dict, rgb_torso: torch.Tensor, facev2v_ret: Dict) -> torch.Tensor:
         """Second half of forward(), after the torso_model call: torso encoder, background features, head / torso / background fusion
-        and block1 -> the image (fp32 [N,3,512,512], or uint8 [N,512,512,3] when forward_pre() got out_uint8)."""
+        and block1 -> the image (fp32 [N,3,512,512], or uint8 [N,512,512,3] when forward_pre() got out_uint8).  weight_fuse=False reads neither
+        rgb_torso nor facev2v_ret['occlusion_2']."""
         L = capi.lib()
         N, sp, prep, plain, cc, dev = st['N'], st['split'], st['prep'], st['plain'], st['cc'], st['device']
         wide = 2 if sp else 1
         xh, rgb_h, weights_256 = st['xh'], st['rgb_h'], st['weights_256']
-        main, Nw = prep['main'], prep['main'].Nw
-        b1, hb = self.block1, getattr(self, 'head_torso_block', None)
+        Nw = prep['main'].Nw
+        hb = getattr(self, 'head_torso_block', None)
         x_torso = self._conv(sr_tc.to_nhwc_f16(facev2v_ret['deformed_torso_hid'], 256, sp), plain['te'], 0, sp)       # 1x1, 64 -> 256
         if cc is None:
             x_bg = self._bg_features(st['ref_bg_256'], plain, sp)
         else:
             x_bg = cc['x_bg']                                            # [1,256,256,256 (x2 split)] fp16, read by every frame of the batch
+        if not self.weight_fuse:
+            # sr_with_ref.py:159-161: cat[x, x_torso, x_bg] unweighted, and block1 without a skip image
+            return self._fg_bg_block1(st, self._cat3(xh, x_torso, x_bg, sp), None)
         thr = float(self.hparams['htbsr_head_threshold'])
         if self.fuse_mode == 'v1':
             # head/torso fusion v1 (sr_with_ref.py:96-98): plain alpha blend of the rgb images AND of the feature maps; no fusing convs, no head_torso_block
@@ -325,7 +348,14 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         capi.check(L.r3dp_sr_person_occlusion(capi.ptr(alpha), capi.ptr(torso_occ), thr, N, 256, 256,
                                               capi.ptr(person), capi.stream()))
         rgb_f = self._blend(rgb_p2, st['ref_bg_256'], person)
-        xg = self._alpha_cat(xp, 256, x_bg, 256, person, sp)
+        return self._fg_bg_block1(st, self._alpha_cat(xp, 256, x_bg, 256, person, sp), rgb_f)
+
+    def _fg_bg_block1(self, st: Dict, xg: torch.Tensor, rgb_f: Optional[torch.Tensor]) -> torch.Tensor:
+        """fuse_fg_bg_convs and block1 on the fused features xg; rgb_f = block1's skip image (None: no skip, the image is ToRGB alone)."""
+        L = capi.lib()
+        N, sp, plain, dev = st['N'], st['split'], st['plain'], st['device']
+        main, Nw = st['prep']['main'], st['prep']['main'].Nw
+        b1 = self.block1
         xg = self._conv(self._conv(self._conv(xg, plain['ff0'], 2, sp), plain['ff2'], 2, sp), plain['ff4'], 0, sp)
         # block1: 256^2 -> 512^2; with out_uint8 the last epilogue writes the video frames (real3d_infer.py:515-519)
         a2 = sr_tc.layer(xg, b1.conv0, main.wp[2], 2, sp)

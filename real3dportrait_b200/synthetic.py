@@ -140,9 +140,25 @@ class StubTorsoModel(torch.nn.Module):
         return rgb_torso, {'deformed_torso_hid': hid, 'occlusion_2': occ}
 
 
-def make_sr_warp_params(seed: int = 6, fuse_mode: str = 'v2') -> Dict[str, torch.Tensor]:
+class StubTorsoModelV1(StubTorsoModel):
+    """The same stand-in with the forward signature of torso_model_version 'v1' (modules/real3d/facev2v_warp/model.py:216), which takes no head
+    weights image; the weights channel of its hidden features is zero.  `calls` counts the forward calls.  Called with the v2 argument list it
+    raises TypeError (cal_loss given twice)."""
+
+    def __init__(self):
+        super().__init__()
+        self.calls = 0
+
+    def forward(self, torso_src_img, segmap, kp_s, kp_d, tgt_head_img, cal_loss=False, target_torso_mask=None):
+        self.calls += 1
+        return super().forward(torso_src_img, segmap, kp_s, kp_d, tgt_head_img, torch.zeros_like(tgt_head_img[:, :1]), cal_loss, target_torso_mask)
+
+
+def make_sr_warp_params(seed: int = 6, fuse_mode: str = 'v2', weight_fuse: bool = True) -> Dict[str, torch.Tensor]:
     """state_dict of SuperresolutionHybrid8XDC_Warp WITHOUT its torso_model child (sr_with_ref.py:16-66).  The same random values for every fuse mode;
-    mode 'v1' has no head_torso_alpha_predictor / fuse_head_torso_convs / head_torso_block children (sr_with_ref.py:36-55), so their keys are dropped."""
+    mode 'v1' has no head_torso_alpha_predictor / fuse_head_torso_convs / head_torso_block children (sr_with_ref.py:36-55), so their keys are dropped.
+    weight_fuse=False has none of them either, whatever the mode, and fuse_fg_bg_convs.0 takes 768 inputs: that weight and bias are drawn from a
+    generator of their own (seed + 300), so every other key keeps its weight_fuse=True value."""
     p = make_sr_params(seed=seed)
     g = torch.Generator().manual_seed(seed + 100)
     f = p['block0.resample_filter']
@@ -172,8 +188,11 @@ def make_sr_warp_params(seed: int = 6, fuse_mode: str = 'v2') -> Dict[str, torch
     p[pre + 'bias'] = 0.1 * torch.randn(3, generator=g)
     p[pre + 'affine.weight'] = torch.randn(256, 512, generator=g)
     p[pre + 'affine.bias'] = 1.0 + 0.1 * torch.randn(256, generator=g)
-    if fuse_mode == 'v1':
+    if fuse_mode == 'v1' or not weight_fuse:
         p = {k: v for k, v in p.items() if not k.startswith(('head_torso_alpha_predictor.', 'fuse_head_torso_convs.', 'head_torso_block.'))}
+    if not weight_fuse:
+        g = torch.Generator().manual_seed(seed + 300)          # conv() draws from g
+        conv('fuse_fg_bg_convs.0', 64, 768, 1)
     return p
 
 

@@ -1,7 +1,7 @@
 """BASELINE configs[4] in both tensor-core SR modes: 48 + 48 samples/ray -> SuperresolutionHybrid8XDC_Warp (fuse mode v2, stub torso warper),
 per-clip constants cached with begin_clip(), one CUDA graph per resident batch.
 
-    python tools/bench_torso.py [--modes tc tc_exact] [--batch 4] [--steps 16] [--warmup 3] [--reps 3]
+    python tools/bench_torso.py [--modes tc tc_exact] [--batch 4] [--steps 16] [--warmup 3] [--reps 3] [--no-weight-fuse]
 
 The modes are timed alternately, --reps times each; the JSON line carries every rep and the median frames/s per mode, with the card's name,
 power limit and the SM clock sampled during the timed runs (a power-capped card lowers its clocks under this load).  The timing loop and the
@@ -12,7 +12,9 @@ graph pool are bench.py's, so the numbers are comparable with its roofline.extra
 
 --engine times configs[4] as a clip through FrameEngine(torso_model=...) in 'tc': --frames uint8 frames, sharded over the ranks, pushed into
 the clip on rank 0 (exchange='p2p'), with the warper run eagerly between two graphs and with the warper inside one graph, alternating with
-the GraphPool loop above (one GPU per rank, fp32 frames, no clip).  Each reports the median of --reps clips; frames/s counts the whole clip."""
+the GraphPool loop above (one GPU per rank, fp32 frames, no clip).  Each reports the median of --reps clips; frames/s counts the whole clip.
+
+--no-weight-fuse times the head's weight_fuse=False configuration instead of fuse mode v2 (sr_with_ref.py:158-161)."""
 import argparse
 import importlib.util
 import json
@@ -46,6 +48,10 @@ def _card(dev):
     return props.name, power
 
 
+def _fuse(args) -> str:
+    return 'fuse v2' if args.weight_fuse else 'weight_fuse=False'
+
+
 def engine_main(args):
     """configs[4] as a clip through FrameEngine(torso_model=stub): uint8 frames, p2p clip exchange, both warper settings, alternating with
     the GraphPool loop of main()."""
@@ -72,8 +78,8 @@ def engine_main(args):
     resident = [(ren.PlanesCL(planes_cl[sl(i)]), cams[sl(i)], u_c[sl(i)], u_f[sl(i).start * 4096:sl(i).stop * 4096], kp_d[sl(i)]) for i in range(nb)]
     inp = {k: v.to(dev) for k, v in syn.make_warp_inputs(1, seed=7).items()}
     consts = (inp['ref_torso_rgb'], inp['ref_bg_rgb'], inp['segmap'], inp['kp_s'])
-    dec, srp = syn.make_decoder_params(seed=4), syn.make_sr_warp_params(seed=6)
-    hp = dict(syn.WARP_HPARAMS, num_samples_fine=48)
+    dec, srp = syn.make_decoder_params(seed=4), syn.make_sr_warp_params(seed=6, weight_fuse=args.weight_fuse)
+    hp = dict(syn.WARP_HPARAMS, num_samples_fine=48, weight_fuse=args.weight_fuse)
 
     runs = {}
     for name, in_graph in (('engine_split_graphs', False), ('engine_whole_graph', True)):
@@ -126,7 +132,7 @@ def engine_main(args):
     clocks = sampler.summary()
     name_, power = _card(dev)
     if rank == 0:
-        out = {'config': 'configs[4] clip: 48+48 samples/ray + SuperresolutionHybrid8XDC_Warp (fuse v2, stub torso warper), tc, uint8 frames, p2p clip',
+        out = {'config': f'configs[4] clip: 48+48 samples/ray + SuperresolutionHybrid8XDC_Warp ({_fuse(args)}, stub torso warper), tc, uint8 frames, p2p clip',
                'frames': fpr * world, 'gpus': world, 'batch': B, 'reps': args.reps, 'device': name_, 'power_limit': power, 'clocks': clocks,
                'graphpool_note': 'GraphPool: the same frames per GPU without clip, exchange or uint8 frames', 'runs': {}}
         for name, v in ms.items():
@@ -147,6 +153,7 @@ def main():
     ap.add_argument('--steps', type=int, default=16)
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--reps', type=int, default=3)
+    ap.add_argument('--no-weight-fuse', dest='weight_fuse', action='store_false', help='the weight_fuse=False head instead of fuse mode v2')
     args = ap.parse_args()
     if args.engine:
         return engine_main(args)
@@ -165,11 +172,11 @@ def main():
     cond_static = {'ref_torso_img': inp['ref_torso_rgb'].expand(B, -1, -1, -1).contiguous(), 'bg_img': inp['ref_bg_rgb'].expand(B, -1, -1, -1).contiguous(),
                    'segmap': inp['segmap'].expand(B, -1, -1, -1).contiguous(), 'kp_s': inp['kp_s'].expand(B, -1, -1).contiguous()}
     sd = {'decoder.' + k: v for k, v in syn.make_decoder_params(seed=4).items()}
-    sd.update({'superresolution.' + k: v for k, v in syn.make_sr_warp_params(seed=6).items()})
+    sd.update({'superresolution.' + k: v for k, v in syn.make_sr_warp_params(seed=6, weight_fuse=args.weight_fuse).items()})
 
     pools = {}
     for mode in args.modes:
-        head = r3.RenderHead(hp=dict(syn.WARP_HPARAMS, num_samples_fine=48), torso_model=syn.StubTorsoModel(), sr_mode=mode)
+        head = r3.RenderHead(hp=dict(syn.WARP_HPARAMS, num_samples_fine=48, weight_fuse=args.weight_fuse), torso_model=syn.StubTorsoModel(), sr_mode=mode)
         head.load_state_dict(sd, strict=True)
         head = head.to(dev).eval()
         head.superresolution.assume_shared_styles = True
@@ -197,7 +204,7 @@ def main():
                                timeout=20).stdout.strip()
     except Exception as e:                                                    # noqa: BLE001
         power = f'unavailable ({type(e).__name__})'
-    out = {'config': "configs[4]: 48+48 samples/ray + SuperresolutionHybrid8XDC_Warp (fuse v2, stub torso warper), begin_clip() cache, CUDA graphs",
+    out = {'config': f"configs[4]: 48+48 samples/ray + SuperresolutionHybrid8XDC_Warp ({_fuse(args)}, stub torso warper), begin_clip() cache, CUDA graphs",
            'batch': B, 'steps': args.steps, 'reps': args.reps, 'device': props.name, 'power_limit': power, 'clocks': clocks, 'modes': {}}
     for mode, v in ms.items():
         med = statistics.median(v)

@@ -5,7 +5,9 @@
 Every rank renders `steps` batches of its own frames; with exchange='p2p' the frames are pushed by the copy engine into the clip on rank 0
 (CUDA IPC mapping), with exchange='allgather' NCCL gathers them.  Rank 0 then compares the assembled clip with the frames every rank kept
 locally (sent through an independent NCCL gather at the end) - bit for bit - and prints the per-step cost of both exchanges.
-With --torso the engines run the torso head (synthetic.StubTorsoModel as the warper, the clip constants of begin_clip(), kp_d per frame)."""
+With --torso the engines run the torso head (synthetic.StubTorsoModel as the warper, the clip constants of begin_clip(), kp_d per frame);
+--no-weight-fuse runs its weight_fuse=False configuration and --torso-v1 its torso_model_version 'v1' (synthetic.StubTorsoModelV1); either implies
+--torso."""
 import os
 import sys
 
@@ -21,7 +23,12 @@ def main():
     torch.cuda.set_device(local)
     dev = torch.device('cuda', local)
     dist.init_process_group('nccl', device_id=dev)
-    torso = '--torso' in sys.argv[1:]
+    cfg = {}
+    if '--no-weight-fuse' in sys.argv[1:]:
+        cfg['weight_fuse'] = False
+    if '--torso-v1' in sys.argv[1:]:
+        cfg['torso_model_version'] = 'v1'
+    torso = '--torso' in sys.argv[1:] or bool(cfg)
     B, steps = 4, 6
     planes = ren.planes_to_channels_last(syn.make_planes(B * 2, seed=10 + rank).to(dev)).data
     cams = syn.make_cameras(B * 2, seed=20 + rank).to(dev)
@@ -32,14 +39,14 @@ def main():
         kp = (torch.rand(B * 2, 68, 3, generator=torch.Generator().manual_seed(40 + rank)) * 2 - 1).to(dev)
         kp_d = [kp[i * B:(i + 1) * B] for i in range(2)]
         res = [r + (None, kp_d[i]) for i, r in enumerate(res)]
-        kw = {'torso_model': syn.StubTorsoModel()}
+        kw = {'torso_model': syn.StubTorsoModelV1() if 'torso_model_version' in cfg else syn.StubTorsoModel()}
         consts = syn.make_warp_inputs(1, seed=7)
     ok = True
     for u8 in (True, False):
         for mode in ('p2p', 'allgather'):
-            hp = dict(syn.WARP_HPARAMS, num_samples_fine=0) if torso else {'num_samples_fine': 0}
+            hp = dict(syn.WARP_HPARAMS, num_samples_fine=0, **cfg) if torso else {'num_samples_fine': 0}
             eng = engine.FrameEngine(batch=B, sr_mode='tc', device=dev, world=world, rank=rank, dist=dist, hp=hp, out_uint8=u8, exchange=mode, **kw)
-            eng.load_params(syn.make_decoder_params(seed=4), syn.make_sr_warp_params(seed=6) if torso else syn.make_sr_params(seed=5))
+            eng.load_params(syn.make_decoder_params(seed=4), syn.make_sr_warp_params(seed=6, weight_fuse=cfg.get('weight_fuse', True)) if torso else syn.make_sr_params(seed=5))
             if torso:
                 eng.begin_clip(*(consts[k].to(dev) for k in ('ref_torso_rgb', 'ref_bg_rgb', 'segmap', 'kp_s')))
             eng.prepare(res)

@@ -4,7 +4,9 @@ Covers: streaming render kernel (single pass), two-pass tensor-core render kerne
 FIR, edge) with fp16 and with split operands, uint8 epilogue, stand-alone sampler, the torso head (`warp`: alpha-cat / blend kernels, plain convs,
 SynthesisBlockNoUp tail, per-clip cache) and large_sr (`large`: residual epilogue, plain ToRGB), both in 'tc' and 'tc_exact'.
 `torso_engine`: the torso head's one-launch input kernel (64^2 and 128^2 sources, both split values) and one FrameEngine step of the torso
-head with uint8 frames per warper setting (split graphs, whole graph)."""
+head with uint8 frames per warper setting (split graphs, whole graph).
+`torso_nofuse`: the unweighted three-way concat (shared and per-frame third operand, both split values) and one FrameEngine step at batch 2 of
+the weight_fuse=False head (block1 without a skip image) per sr_mode, with uint8 frames."""
 import os
 import sys
 
@@ -96,6 +98,30 @@ def main():
             out = eng.step(planes, cam, u_c.to(dev), kp_d=inp['kp_d'])
             torch.cuda.synchronize()
             print('torso_engine', in_graph, eng.graph is not None, float(out.float().mean()))
+    if what in ('all', 'torso_nofuse'):
+        from real3dportrait_b200 import _capi as capi, engine
+        for split in (0, 1):
+            wide = 1 + split
+            N, H, W = 2, 3, 5
+            xs = [torch.randn(n, H, W, 256 * wide, generator=g).half().to(dev) for n in (N, N, N, 1)]
+            out = torch.empty(N, H, W, 768 * wide, device=dev, dtype=torch.float16)
+            fn = capi.lib().r3dp_sr_tcx_cat3 if split else capi.lib().r3dp_sr_cat3
+            for xc in (xs[2], xs[3]):
+                capi.check(fn(capi.ptr(xs[0], torch.float16), 256, 256 * wide, capi.ptr(xs[1], torch.float16), 256, 256 * wide, capi.ptr(xc, torch.float16),
+                              256, 256 * wide, int(xc.shape[0] == 1), N, H, W, capi.ptr(out, torch.float16), capi.stream()))
+                torch.cuda.synchronize()
+                print('cat3', split, xc.shape[0], float(out.float().abs().mean()))
+        inp = {k: v.to(dev) for k, v in syn.make_warp_inputs(1, seed=7).items()}
+        for mode in ('tc', 'tc_exact'):
+            eng = engine.FrameEngine(batch=2, sr_mode=mode, hp=dict(syn.WARP_HPARAMS, num_samples_fine=0, weight_fuse=False), torso_model=syn.StubTorsoModel(),
+                                     out_uint8=True)
+            eng.load_params(syn.make_decoder_params(seed=4), syn.make_sr_warp_params(seed=6, weight_fuse=False))
+            eng.begin_clip(inp['ref_torso_rgb'], inp['ref_bg_rgb'], inp['segmap'], inp['kp_s'])
+            planes, cam = syn.make_planes(2, seed=3).to(dev), syn.make_cameras(2, seed=4).to(dev)
+            u_c, _ = syn.make_jitter(2, 4096, 48, 0, seed=5)
+            out = eng.step(planes, cam, u_c.to(dev), kp_d=inp['kp_d'].expand(2, -1, -1).contiguous())
+            torch.cuda.synchronize()
+            print('torso_nofuse', mode, eng.graph is not None, float(out.float().mean()))
     for mode in (('tc', 'tc_exact') if what in ('all', 'large') else ()):
         sr = r3.SuperresolutionHybrid8XDC(channels=32, img_resolution=512, sr_num_fp16_res=0, sr_antialias=True, large_sr=True, sr_mode=mode,
                                           resblocks_in_large_sr=1)
