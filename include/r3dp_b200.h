@@ -348,6 +348,33 @@ int r3dp_sr_resize_aa_down2(const float* x, int N, int C, int h_out, int w_out, 
 int r3dp_sr_warp_input(const float* x_nhwc, const float* wsum, int N, int C, int h, int w, int size, void* y_f16, float* rgb0, float* rgb_256,
                        float* w_256, int split, r3dp_stream_t stream);
 
+/* Stage 2 of the torso warper: Generator (modules/real3d/facev2v_warp/network2.py:248-301) + occlusion_2_predictor (model2.py:212-219,
+ * 260-263).  Activations NHWC fp16 ([hi | lo] halves when split != 0, as in the r3dp_sr_tcx_* family), weights folded on the host.
+ * r3dp_tw_gather3d          Generator.get_deformed_feature (network2.py:298-301): F.grid_sample(fs, grid, trilinear, padding_mode='border',
+ *                           align_corners=True).view(N, C*D, H, W).  fs NDHWC fp32 [N,D,H,W,C] ([1,D,H,W,C] read by every image when fs_shared != 0), grid [N,D,H,W,3] -> y [N,H,W,C*D] fp16,
+ *                           channel c*D + d
+ * r3dp_tw_conv              nn.Conv2d k=1|3 (+ folded SpectralNorm / BatchNorm) with act max(v, slope*v) and an optional residual added after
+ *                           it (ResBlock2D, layers.py:104-105): in_conv, mid_conv, res.*; W % 64 == 0, O = 128 | 256, weights as r3dp_sr_tc_conv
+ * r3dp_tw_conv_up_nearest   UpBlock2D (layers.py:77-88): nn.Upsample(x2, nearest) + 3x3 conv (+ folded BatchNorm) + act, x [N,H,W,Ipad] ->
+ *                           y [N,2H,2W,O]; weights = 4 output-parity sets of composed 2x2 taps packed by r3dp_sr_tc_pack_weights with Nw = 4
+ * r3dp_tw_affine_relu       relu(scale[c] * x + shift[c]): eval BatchNorm + ReLU at the head of a pre-activation ResBlock2D (layers.py:100)
+ * r3dp_tw_narrow_conv       KxK conv to CO = 1 | 3 | 32 channels on CUDA cores in fp32 (Generator.out_conv, the occlusion_2_predictor convs):
+ *                           input xa (NHWC fp16, pixel stride sa, ca channels, split remainder at lo_a > 0) or xf (NHWC fp32), plus optionally the
+ *                           bilinear (align_corners=False) resize of ex [N,1,eh,ew] to HxW as the last channel (model2.py:262's concat);
+ *                           wk [K*K][cin][CO] fp32, act 0 linear / 1 ReLU / 2 sigmoid, out fp32 NCHW (nchw != 0) or NHWC
+ * r3dp_tw_hid_to_nchw       NHWC fp16 (pixel stride cs, split remainder at lo > 0) -> [N,C,H,W] fp32: ret['deformed_torso_hid'] (model2.py:261) */
+int r3dp_tw_gather3d(const float* fs_ndhwc, int fs_shared, const float* grid, int N, int C, int D, int H, int W, void* y_f16, int split,
+                     r3dp_stream_t stream);
+int r3dp_tw_conv(const void* x_f16, const void* wp_f16, const float* bias, int N, int I, int O, int H, int W, int ksize, float slope,
+                 const void* residual_f16, void* y_f16, int split, r3dp_stream_t stream);
+int r3dp_tw_conv_up_nearest(const void* x_f16, const void* wp_f16, const float* bias, int N, int I, int O, int H, int W, float slope, void* y_f16,
+                            int split, r3dp_stream_t stream);
+int r3dp_tw_affine_relu(const void* x_f16, const float* scale, const float* shift, int N, int H, int W, int C, int split, void* y_f16,
+                        r3dp_stream_t stream);
+int r3dp_tw_narrow_conv(const void* xa_f16, int sa, int ca, int lo_a, const float* xf, int sf, int cf, const float* ex, int eh, int ew,
+                        const float* wk, const float* bias, int N, int H, int W, int K, int CO, int act, int nchw, float* out, r3dp_stream_t stream);
+int r3dp_tw_hid_to_nchw(const void* x_f16, int N, int C, int H, int W, int cs, int lo, float* y, r3dp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

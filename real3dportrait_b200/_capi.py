@@ -111,6 +111,12 @@ _SIGNATURES = {
     'r3dp_sr_tc_prof_read': (_I, [C.POINTER(C.c_float), C.POINTER(_I)]),
     'r3dp_sr_tc_last_layer': (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
     'r3dp_sr_tc_last_layer_ex': (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _P]),
+    'r3dp_tw_gather3d': (_I, [_P, _I, _P, _I, _I, _I, _I, _I, _P, _I, _P]),
+    'r3dp_tw_conv': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P, _P, _I, _P]),
+    'r3dp_tw_conv_up_nearest': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P, _I, _P]),
+    'r3dp_tw_affine_relu': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
+    'r3dp_tw_narrow_conv': (_I, [_P, _I, _I, _I, _P, _I, _I, _P, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
+    'r3dp_tw_hid_to_nchw': (_I, [_P, _I, _I, _I, _I, _I, _I, _P, _P]),
 }
 
 

@@ -929,7 +929,8 @@ static int run_conv2(const void* x, int N, int H, int W, int Cp, const void* wp,
     if (make_map_4d_box(&tmB, wp, Cphys, (uint64_t)O, (uint64_t)n_taps, (uint64_t)Nw, BN)) return 1;
     if (a.split) { a.acc_scale = 1.0f / kSplitWeightScale; a.lo_off = a.out_C; a.out_C *= 2; }
     else { a.acc_scale = 1.0f; a.lo_off = 0; }
-    a.k_chunks = Cp / BK; a.tiles_x = W / BM; a.n_blocks = O / BN; a.n_images = N; a.w_shared = (Nw == 1);
+    // W = 64 (the torso warper's 64^2 maps): one tile per row whose right half reads TMA zero fill and stores nothing (the stores check out_W)
+    a.k_chunks = Cp / BK; a.tiles_x = (W + BM - 1) / BM; a.n_blocks = O / BN; a.n_images = N; a.w_shared = (Nw == 1);
     { static int mixv = -1; if (mixv < 0) { const char* e = getenv("R3DP_TC_MIX"); mixv = (e && e[0] == '0') ? 0 : 1; } a.phase_mix = mixv; }      // A/B knob
     if (a.act_gain == 0.f) { a.act_slope = 0.2f; a.act_gain = 1.4142135623730951f; }      // default: bias_act lrelu
     R3DP_REQUIRE(a.n_blocks >= 1 && a.n_blocks <= 2, "conv_tc3: 128 or 256 output channels");
@@ -1357,11 +1358,10 @@ extern "C" int r3dp_sr_tcx_layer_up_composed(const void* x_f16, const void* wpc_
 // Plain nn.Conv2d (k = 1 or 3, stride 1, "same" padding) [+ activation] on the tensor-core path: x [N][H][W][Ip] fp16, weights packed by
 // r3dp_sr_tc_pack_weights from the [1][O][I][k][k] fp32 tensor (k = 1: the value sits in tap 4), y [N][H][W][O] fp16.
 // act: 0 = linear, 1 = lrelu(0.2)*sqrt2 (bias_act), 2 = nn.LeakyReLU() (slope 0.01).
-static int conv_res_impl(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
-                         int act, const void* residual_f16, void* y_f16, int split, r3dp_stream_t stream) {
-    R3DP_REQUIRE(x_f16 && wp_f16 && bias && y_f16, "sr_tc_conv: null pointer");
-    R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && W % BM == 0 && O % BN == 0 && O <= 256 && (ksize == 1 || ksize == 3) && act >= 0 && act <= 3,
-                 "sr_tc_conv: bad shape / options");
+// the launch behind r3dp_sr_tc_conv(_res) / r3dp_sr_tcx_conv(_res) and r3dp_tw_conv (shapes checked by the callers):
+// act = max(v, v * slope) * gain, residual added after it
+static int conv_plain_launch(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
+                             float slope, float gain, const void* residual_f16, void* y_f16, int split, r3dp_stream_t stream) {
     const int Ip = (I + 63) / 64 * 64;
     Conv2Args a = {};
     Taps t = {};
@@ -1371,11 +1371,19 @@ static int conv_res_impl(const void* x_f16, const void* wp_f16, const float* bia
     fill_taps2(a.ph[0].taps, t);
     a.ph[0].rows = H;
     a.mode = kStoreAct; a.out = reinterpret_cast<__half*>(y_f16); a.out_H = H; a.out_W = W; a.out_C = O; a.oy_mul = a.ox_mul = 1; a.bias = bias;
-    a.act_slope = act == 0 ? 1.0f : (act == 1 ? 0.2f : (act == 2 ? 0.01f : 0.0f));      // max(v, v*slope): slope 0 = ReLU
-    a.act_gain = act == 1 ? 1.4142135623730951f : 1.0f;
+    a.act_slope = slope; a.act_gain = gain;
     a.residual = reinterpret_cast<const __half*>(residual_f16);
     a.split = split;
     return run_conv2(x_f16, N, H, W, Ip, wp_f16, Nw, O, a, H, as_stream(stream));
+}
+static int conv_res_impl(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
+                         int act, const void* residual_f16, void* y_f16, int split, r3dp_stream_t stream) {
+    R3DP_REQUIRE(x_f16 && wp_f16 && bias && y_f16, "sr_tc_conv: null pointer");
+    R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && W % BM == 0 && O % BN == 0 && O <= 256 && (ksize == 1 || ksize == 3) && act >= 0 && act <= 3,
+                 "sr_tc_conv: bad shape / options");
+    const float slope = act == 0 ? 1.0f : (act == 1 ? 0.2f : (act == 2 ? 0.01f : 0.0f));       // max(v, v*slope): slope 0 = ReLU
+    return conv_plain_launch(x_f16, wp_f16, bias, N, Nw, I, O, H, W, ksize, slope, act == 1 ? 1.4142135623730951f : 1.0f, residual_f16, y_f16, split,
+                             stream);
 }
 extern "C" int r3dp_sr_tc_conv_res(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
                                    int act, const void* residual_f16, void* y_f16, r3dp_stream_t stream) {
@@ -1664,6 +1672,48 @@ extern "C" int r3dp_sr_alpha_gate(const void* logits_f16, int stride, int lo_off
     R3DP_LAUNCH_CHECK();
     count_launches(1);
     return 0;
+}
+
+// ---- stage 2 of the torso warper (facev2v_warp/network2.py:248-301, Generator) on conv_tc3 -------------------------------------------
+// Launch options only: the kernel is the one above.  W a multiple of 64 (64-wide maps use half of each 128-pixel tile), O = 128 | 256 (the
+// 64-cout up.1 is packed with zero filters up to 128), act = max(v, v * slope) (1 linear, 0.2 nn.LeakyReLU(0.2), 0 ReLU), gain 1.
+static int tw_conv_impl(const void* x_f16, const void* wp_f16, const float* bias, int N, int I, int O, int H, int W, int ksize, float slope,
+                        const void* residual_f16, void* y_f16, int split, r3dp_stream_t stream) {
+    R3DP_REQUIRE(x_f16 && wp_f16 && bias && y_f16, "tw_conv: null pointer");
+    R3DP_REQUIRE(N > 0 && H > 0 && W % 64 == 0 && W > 0 && (O == 128 || O == 256) && (ksize == 1 || ksize == 3) && slope >= 0.f && slope <= 1.f,
+                 "tw_conv: bad shape / options");
+    return conv_plain_launch(x_f16, wp_f16, bias, N, 1, I, O, H, W, ksize, slope, 1.0f, residual_f16, y_f16, split, stream);
+}
+extern "C" int r3dp_tw_conv(const void* x_f16, const void* wp_f16, const float* bias, int N, int I, int O, int H, int W, int ksize, float slope,
+                            const void* residual_f16, void* y_f16, int split, r3dp_stream_t stream) {
+    return tw_conv_impl(x_f16, wp_f16, bias, N, I, O, H, W, ksize, slope, residual_f16, y_f16, split, stream);
+}
+
+// nn.Upsample(scale 2, nearest) + 3x3 conv as four output-parity phases of 2x2 taps on the low-resolution input (16 tap GEMMs per input
+// pixel instead of 36).  Weights: 4 phase sets packed as [4][9][O][Ip] (r3dp_sr_tc_pack_weights with Nw = 4), set p*2+q holds the composed
+// taps of output parity (p, q) at (dy+1)*3 + (dx+1), dy in {-1, 0} for p = 0 and {0, +1} for p = 1 (the same per axis for q, dx).
+static int tw_conv_up_nearest_impl(const void* x_f16, const void* wp_f16, const float* bias, int N, int I, int O, int H, int W, float slope,
+                                   void* y_f16, int split, r3dp_stream_t stream) {
+    R3DP_REQUIRE(x_f16 && wp_f16 && bias && y_f16, "tw_conv_up_nearest: null pointer");
+    R3DP_REQUIRE(N > 0 && H > 0 && W % 64 == 0 && W > 0 && (O == 128 || O == 256) && slope >= 0.f && slope <= 1.f, "tw_conv_up_nearest: bad shape / options");
+    Conv2Args a = {};
+    a.n_phases = 4;
+    for (int p = 0; p < 2; ++p)
+        for (int q = 0; q < 2; ++q) {
+            Taps t = {};
+            for (int dy = p - 1; dy <= p; ++dy)
+                for (int dx = q - 1; dx <= q; ++dx) { const int i = t.n++; t.dy[i] = dy; t.dx[i] = dx; t.widx[i] = (p * 2 + q) * 9 + (dy + 1) * 3 + (dx + 1); }
+            Phase2& P = a.ph[p * 2 + q];
+            fill_taps2(P.taps, t);
+            P.rows = H; P.oy_off = p; P.ox_off = q;
+        }
+    a.mode = kStoreAct; a.out = reinterpret_cast<__half*>(y_f16); a.out_H = 2 * H; a.out_W = 2 * W; a.out_C = O; a.oy_mul = a.ox_mul = 2;
+    a.bias = bias; a.act_slope = slope; a.act_gain = 1.0f; a.split = split;
+    return run_conv2(x_f16, N, H, W, (I + 63) / 64 * 64, wp_f16, 1, O, a, H, as_stream(stream), 36);
+}
+extern "C" int r3dp_tw_conv_up_nearest(const void* x_f16, const void* wp_f16, const float* bias, int N, int I, int O, int H, int W, float slope,
+                                       void* y_f16, int split, r3dp_stream_t stream) {
+    return tw_conv_up_nearest_impl(x_f16, wp_f16, bias, N, I, O, H, W, slope, y_f16, split, stream);
 }
 
 // Timing of the tensor-core conv launches: r3dp_sr_tc_prof(1) starts recording a CUDA-event pair around every conv_tc3 launch,

@@ -121,17 +121,22 @@ class FrameEngine:
     the folded fp16 weights are prepared once per parameter load; use_graph: replay the step as CUDA graphs.
     torso_model: run the torso head with this warper (WarpBasedTorsoModelMediaPipe or a module with its forward signature);
     warper_in_graph: capture the warper inside the step's single graph (only for capturable warpers; the default runs it eagerly
-    between two graphs)."""
+    between two graphs).  torso_stage2='cuda': the warper's stage 2 on this library's kernels, its appearance features cached per clip by
+    begin_clip() (SuperresolutionHybrid8XDC_Warp.set_torso_stage2)."""
 
     def __init__(self, batch: int = 4, sr_mode: str = 'fp32', device=None, world: int = 1, rank: int = 0, dist=None, hp: Optional[dict] = None,
                  static_styles: bool = True, use_graph: bool = True, out_uint8: bool = False, exchange: str = 'allgather',
-                 torso_model: Optional[torch.nn.Module] = None, warper_in_graph: bool = False):
+                 torso_model: Optional[torch.nn.Module] = None, warper_in_graph: bool = False, torso_stage2: str = 'torch'):
         assert exchange in ('allgather', 'p2p', 'none')
         self.batch, self.world, self.rank, self.dist = batch, world, rank, dist
         self.device = device if device is not None else torch.device('cuda', torch.cuda.current_device())
         self.head = RenderHead(hp=hp, sr_mode=sr_mode, torso_model=torso_model).to(self.device).eval()
         self.static_styles, self.use_graph = static_styles, use_graph
         self.torso, self.warper_in_graph = self.head.torso, bool(warper_in_graph)
+        if torso_stage2 != 'torch':
+            if not self.torso:
+                raise ValueError('torso_stage2 is an option of the torso head: FrameEngine(torso_model=...)')
+            self.head.superresolution.set_torso_stage2(torso_stage2)
         self.out_uint8 = bool(out_uint8)
         if self.out_uint8 and self.head.superresolution.sr_mode not in ('tc', 'tc_exact'):     # the head's effective mode: a torso head maps 'fp32' to 'tc'
             raise NotImplementedError('uint8 frames are written by the tensor-core SR epilogue (sr_mode="tc")')
@@ -184,7 +189,7 @@ class FrameEngine:
         if not (ref_torso_img.shape[0] == bg_img.shape[0] == segmap.shape[0] == kp_s.shape[0] == 1):
             raise ValueError('one set of clip constants: ref_torso_img, bg_img, segmap and kp_s have batch size 1')
         B = self.batch
-        if not self.head.superresolution.begin_clip(ref_torso_img, bg_img, batch=B, in_place=True):
+        if not self.head.superresolution.begin_clip(ref_torso_img, bg_img, batch=B, in_place=True, segmap=segmap.to(self.device)):
             self.graph, self.inplace = None, {}                       # new constant buffers: graphs captured earlier read the old ones
         bc = {'segmap': segmap.expand(B, -1, -1, -1), 'kp_s': kp_s.expand(B, -1, -1)}
         if self._consts is None:

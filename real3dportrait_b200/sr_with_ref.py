@@ -41,7 +41,7 @@ _pack_plain = sr_tc.pack_plain
 
 class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
     def __init__(self, channels, img_resolution, sr_num_fp16_res, sr_antialias, hp: Optional[dict] = None, torso_model: Optional[torch.nn.Module] = None,
-                 **block_kwargs):
+                 torso_stage2: str = 'torch', **block_kwargs):
         block_kwargs.setdefault('sr_mode', 'tc')
         super().__init__(channels, img_resolution, sr_num_fp16_res, sr_antialias, **block_kwargs)
         if self.sr_mode not in ('tc', 'tc_exact'):
@@ -73,6 +73,32 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         self._plain_cache = None
         self._clip_cache = None
         self.static_prepared_warp = None
+        self._stage2_cache = None
+        self._warper = None
+        self.set_torso_stage2(torso_stage2)
+
+    def set_torso_stage2(self, mode: str) -> None:
+        """'torch': the caller's torso_model(...) call (the reference's path).  'cuda': the warper's stage 2 (Generator + occlusion_2_predictor)
+        on this library's kernels, stage 1 restated in torso_warp.py around the caller's appearance_extractor and motion_field_estimator;
+        built for torso_model_version v2 (model2.py) only."""
+        if mode not in ('torch', 'cuda'):
+            raise ValueError(f"torso_stage2 is 'torch' or 'cuda', got {mode!r}")
+        if mode == 'cuda' and self.hparams['torso_model_version'] != 'v2':
+            raise NotImplementedError("torso_stage2='cuda' is built for torso_model_version v2 (facev2v_warp/model2.py) only")
+        self.torso_stage2 = mode
+        self._stage2_cache = None
+
+    def _stage2_weights(self):
+        """Folded + packed stage-2 weights, rebuilt when the mode, the device or any of the warper's parameters / buffers changed (a
+        load_state_dict of the head or of torso_model alone, an optimizer step, .to(device)).  The per-clip appearance cache is not re-keyed:
+        it holds until the next begin_clip(), like the head's other clip constants."""
+        from . import torso_warp
+        sp, tm = self._split, self.torso_model
+        mods = (tm.deform_based_generator, tm.occlusion_2_predictor)
+        key = (sp, tuple((t.data_ptr(), t._version) for m in mods for t in list(m.parameters()) + list(m.buffers())))
+        if self._stage2_cache is None or self._stage2_cache[0] != key:
+            self._stage2_cache = (key, torso_warp.Stage2Weights(*mods, sp))
+        return self._stage2_cache[1]
 
     @property
     def _split(self) -> bool:
@@ -115,6 +141,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         self._plain_cache = None
         self._clip_cache = None
         self.static_prepared_warp = None
+        self._stage2_cache = None
         return super()._load_from_state_dict(*a, **k)
 
     @staticmethod
@@ -155,24 +182,34 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
 
     # ---- per-clip constants (SURVEY.md §8f #2) -------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def begin_clip(self, ref_torso_rgb: torch.Tensor, ref_bg_rgb: torch.Tensor, batch: Optional[int] = None, in_place: bool = False) -> bool:
+    def begin_clip(self, ref_torso_rgb: torch.Tensor, ref_bg_rgb: torch.Tensor, batch: Optional[int] = None, in_place: bool = False,
+                   segmap: Optional[torch.Tensor] = None) -> bool:
         """Hoist what the reference recomputes for every frame although it only depends on the clip's reference images
         (sr_with_ref.py:77-90): the two antialiased 512->256 resizes and bg_encoder(ref_bg) (96.9 GFLOP/frame).  ref_* [1,3,512,512].
         Until end_clip(), forward() ignores its ref_torso_rgb / ref_bg_rgb arguments and uses these.
         batch: also keep the [batch,3,256,256] broadcasts of the two resized images, read by every call with that batch instead of
         copies made per call.  in_place: when a clip with the same mode and batch is already begun, write the new constants into its
-        tensors (CUDA graphs captured against them then render the new clip).  Returns True when the constants were refilled in place."""
+        tensors (CUDA graphs captured against them then render the new clip).  Returns True when the constants were refilled in place.
+        segmap [1,6,512,512] with torso_stage2='cuda': also keep the warper's per-clip part (torso_warp.appearance: appearance_extractor of
+        the reference torso image, the dilated torso mask, the 64^2 segmap, the volume in NDHWC); forward() then ignores its segmap argument."""
         assert ref_torso_rgb.shape[0] == 1 and ref_bg_rgb.shape[0] == 1, 'one reference image per clip'
         plain, sp = self._plain(), self._split
         t256, b256 = self._aa_down2(ref_torso_rgb), self._aa_down2(ref_bg_rgb)
-        cc = {'ref_torso_256': t256, 'ref_bg_256': b256, 'x_bg': self._bg_features(b256, plain, sp), 'split': sp, 'batch': None}
+        cc = {'ref_torso_256': t256, 'ref_bg_256': b256, 'x_bg': self._bg_features(b256, plain, sp), 'split': sp, 'batch': None, 'torso_app': None}
+        if segmap is not None and self.torso_stage2 == 'cuda':
+            from . import torso_warp
+            assert segmap.shape[0] == 1, 'one segmap per clip'
+            cc['torso_app'] = torso_warp.appearance(self.torso_model, t256, segmap)
         if batch is not None:
             cc['batch'] = (t256.expand(batch, -1, -1, -1).contiguous(), b256.expand(batch, -1, -1, -1).contiguous())
         old = self._clip_cache
         if in_place and old is not None and old['split'] == sp and (old['batch'] is None) == (batch is None) and \
-                (batch is None or old['batch'][0].shape[0] == batch):
+                (batch is None or old['batch'][0].shape[0] == batch) and (old['torso_app'] is None) == (cc['torso_app'] is None):
             for k in ('ref_torso_256', 'ref_bg_256', 'x_bg'):
                 old[k].copy_(cc[k])
+            if cc['torso_app'] is not None:                         # a graph that captured the warper reads these tensors by address
+                for k, v in cc['torso_app'].items():
+                    old['torso_app'][k].copy_(v)
             if batch is not None:
                 for dst, src in zip(old['batch'], cc['batch']):
                     dst.copy_(src)
@@ -283,6 +320,14 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         """The torso warper: the caller's PyTorch module (opaque child, sr_with_ref.py:84-87) -> (rgb_torso, facev2v_ret).
         torso_model_version v1 (model.py) takes no head weights image; v2 (model2.py) does."""
         ref_torso_256, segmap, kp_s, kp_d, rgb_256, weights_256 = st['torso_args']
+        if self.torso_stage2 == 'cuda':
+            from . import torso_warp
+            if self._warper is None or self._warper.tm is not self.torso_model:
+                self._warper = torso_warp.TorsoWarper(self.torso_model)
+            cc = st['cc']
+            with capi.region('torso_model'):
+                return self._warper(self._stage2_weights(), ref_torso_256, segmap, kp_s, kp_d, rgb_256.detach(), weights_256.detach(),
+                                    app=cc.get('torso_app') if cc is not None else None)
         with capi.region('torso_model'):
             if self.hparams['torso_model_version'] == 'v1':
                 return self.torso_model(ref_torso_256, segmap, kp_s, kp_d, rgb_256.detach(), cal_loss=True, target_torso_mask=st['target_torso_mask'])
