@@ -112,7 +112,7 @@ int r3dp_decode(const float* feat, int N, int K, int P, int C, const r3dp_mlp_t*
  * Kernels: single-pass renders (S_imp == 0) run the warp-specialised streaming kernel (render_stream.cu: gather, wgmma decoder and
  * ray march of consecutive 128-sample tiles overlap inside one persistent CTA per SM); importance renders run the CTA-per-ray-tile
  * kernel (render.cu).  Decoder arithmetic: the OSGDecoder GEMMs run on wgmma with every fp32 operand split into two fp16 halves (three
- * partial products, fp32 accumulation in TMEM) - fp32-grade results (rgb within 2e-6 of the CUDA-core decoder); two-pass shapes whose
+ * partial products, fp32 accumulation in TMEM) - fp32-grade results (rgb within 5e-6 of float64, tests/test_gpu_render_conformance.py); two-pass shapes whose
  * tiles do not fit use the fp32 CUDA-core decoder.  The prepared decoder operands live in the caller's `workspace`, so calls with
  * different decoders may run concurrently on different streams (each with its own workspace).
  * A/B knobs (read once per process): R3DP_RENDER=tile, R3DP_RS_D=4|8|16, R3DP_MLP=tc|smem|const (const keeps process-wide state). */
@@ -147,6 +147,9 @@ typedef struct r3dp_render_args {
     void* workspace; size_t workspace_bytes;
 } r3dp_render_args_t;
 int r3dp_render_ex(const r3dp_render_args_t* args, r3dp_stream_t stream);
+/* The kernel r3dp_render_ex runs for `args` under the current options: 0 = streaming kernel, 1 = CTA-per-ray-tile kernel with the
+ * tensor-core decoder, 2 = CTA-per-ray-tile kernel with the CUDA-core decoder; -1 if `args` or its decoder is NULL.  Launches nothing. */
+int r3dp_render_path(const r3dp_render_args_t* args);
 
 int r3dp_render(const float* planes_cl, int N, int C, int H, int W,
                 const float* ray_o, const float* ray_d, const float* camera, int M, int res,

@@ -60,6 +60,7 @@ _SIGNATURES = {
     'r3dp_render_workspace_bytes': (_Z, [_I, _I]),
     'r3dp_render': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _I, _I, _I, _I, _F, _I, _P, _P, _M, _P, _P, _P, _P, _P, _Z, _P]),
     'r3dp_render_ex': (_I, [C.POINTER(RenderArgs), _P]),
+    'r3dp_render_path': (_I, [C.POINTER(RenderArgs)]),
     'r3dp_ray_march': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
     'r3dp_sr_styles': (_I, [_P, _P, _P, _I, _I, _I, _F, _P, _P]),
     'r3dp_sr_fold_weights': (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P]),

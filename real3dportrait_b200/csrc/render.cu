@@ -555,17 +555,41 @@ static int launch_render_v(const RenderArgs& a, cudaStream_t st) {
     return 0;
 }
 template <int R>
-static int launch_render(const RenderArgs& a, cudaStream_t st) {
-    // tensor-core decoder when the tile fits, else the smem-weights CUDA-core decoder; both keep the decoder in per-call storage
-    const bool grid_single = a.p0.depth > 1 && a.S_imp == 0;      // tri-grid descriptors (27 floats) do not fit the single-pass [nsamp][16] layout
-    if (mlp_variant() == 2 && !grid_single && render_tc_fits(R, a.S, a.S_imp)) return launch_render_tc<R>(a, st);
-    return launch_render_v<R>(a, st);
+static int launch_render(const RenderArgs& a, bool tc, cudaStream_t st) {
+    return tc ? launch_render_tc<R>(a, st) : launch_render_v<R>(a, st);
 }
 
 int g_render_variant = -1;                         // R3DP_RENDER = stream (default for single-pass renders) | tile: A/B knob
 static int render_variant() {
     if (g_render_variant < 0) { const char* e = getenv("R3DP_RENDER"); g_render_variant = (e && e[0] == 't') ? 1 : 0; }
     return g_render_variant;
+}
+
+static int tile_rays(int ST) { return ST <= 48 ? 8 : ST <= 96 ? 4 : ST <= 192 ? 2 : 1; }     // rays per CTA of the tile kernel
+
+// The kernel a render runs (r3dp_render_ex dispatches on this, r3dp_render_path reports it): 0 = streaming kernel, 1 = tile kernel with the
+// tensor-core decoder, 2 = tile kernel with the smem-weights CUDA-core decoder (tiles that do not fit the wgmma layout); both tile decoders
+// keep the decoder in per-call storage
+static int render_path(const RenderArgs& a) {
+    if (render_variant() == 0 && mlp_variant() == 2 && render_stream_fits(a)) return 0;
+    const bool grid_single = a.p0.depth > 1 && a.S_imp == 0;      // tri-grid descriptors (27 floats) do not fit the single-pass [nsamp][16] layout
+    return mlp_variant() == 2 && !grid_single && render_tc_fits(tile_rays(a.S + a.S_imp), a.S, a.S_imp) ? 1 : 2;
+}
+
+// the fields of the kernel arguments that follow from the caller's argument block alone (not from the workspace)
+static RenderArgs render_args(const r3dp_render_args_t* g) {
+    RenderArgs a = {};
+    a.p0.base = g->planes; a.p0.frame_stride = g->layout.frame_stride; a.p0.plane_stride = g->layout.plane_stride;
+    a.p0.row_stride = g->layout.row_stride; a.p0.texel_stride = g->layout.texel_stride; a.p0.depth = g->layout.depth; a.p0.slice_stride = g->layout.slice_stride;
+    if (g->planes2) {
+        a.p1.base = g->planes2; a.p1.frame_stride = g->layout2.frame_stride; a.p1.plane_stride = g->layout2.plane_stride;
+        a.p1.row_stride = g->layout2.row_stride; a.p1.texel_stride = g->layout2.texel_stride; a.p1.depth = g->layout2.depth; a.p1.slice_stride = g->layout2.slice_stride;
+    }
+    a.N = g->N; a.H = g->H; a.W = g->W; a.ray_o = g->ray_o; a.ray_d = g->ray_d; a.camera = g->camera; a.M = g->M; a.res = g->res;
+    a.S = g->S; a.S_imp = g->S_imp; a.box_warp = g->box_warp; a.white_back = g->white_back; a.u_coarse = g->u_coarse; a.u_fine = g->u_fine;
+    a.mlp = *g->mlp;
+    a.rgb = g->rgb; a.depth = g->depth; a.wsum = g->weights_sum; a.valid = g->is_ray_valid;
+    return a;
 }
 
 }  // namespace r3dp
@@ -649,33 +673,31 @@ extern "C" int r3dp_render_ex(const r3dp_render_args_t* g, r3dp_stream_t stream)
     ray_limits_kernel<<<(total + 255) / 256, 256, 0, st>>>(g->ray_o, g->ray_d, g->camera, res, N, M, g->box_warp, limits, g->is_ray_valid, ws);
     R3DP_LAUNCH_CHECK();
 
-    RenderArgs a = {};
-    a.p0.base = g->planes; a.p0.frame_stride = g->layout.frame_stride; a.p0.plane_stride = g->layout.plane_stride;
-    a.p0.row_stride = g->layout.row_stride; a.p0.texel_stride = g->layout.texel_stride; a.p0.depth = g->layout.depth; a.p0.slice_stride = g->layout.slice_stride;
-    if (g->planes2) {
-        a.p1.base = g->planes2; a.p1.frame_stride = g->layout2.frame_stride; a.p1.plane_stride = g->layout2.plane_stride;
-        a.p1.row_stride = g->layout2.row_stride; a.p1.texel_stride = g->layout2.texel_stride; a.p1.depth = g->layout2.depth; a.p1.slice_stride = g->layout2.slice_stride;
-    }
-    a.N = N; a.H = H; a.W = W; a.ray_o = g->ray_o; a.ray_d = g->ray_d; a.camera = g->camera; a.M = M; a.res = res;
-    a.S = S; a.S_imp = S_imp; a.box_warp = g->box_warp; a.white_back = g->white_back; a.u_coarse = g->u_coarse; a.u_fine = g->u_fine;
-    a.mlp = *g->mlp; a.image = reinterpret_cast<const MlpTcImage*>(wsb + kWsImageOff);
-    a.rgb = g->rgb; a.depth = g->depth; a.wsum = g->weights_sum; a.limits = limits; a.valid = g->is_ray_valid; a.ws = ws;
+    RenderArgs a = render_args(g);
+    a.image = reinterpret_cast<const MlpTcImage*>(wsb + kWsImageOff); a.limits = limits; a.ws = ws;
     a.lookahead = render_lookahead();
     int rc;
-    if (render_variant() == 0 && mlp_variant() == 2 && render_stream_fits(a)) {
+    const int path = render_path(a);
+    if (path == 0) {
         rc = launch_render_stream(a, st);
     } else {
-        const int R = ST <= 48 ? 8 : ST <= 96 ? 4 : ST <= 192 ? 2 : 1;
+        const int R = tile_rays(ST);
         const bool image = res > 0 && res * res == M && (res % R) == 0;
         a.tile_cols = image ? res : 0;
         a.tiles_per_frame = (M + R - 1) / R;
-        rc = R == 8 ? launch_render<8>(a, st) : R == 4 ? launch_render<4>(a, st) : R == 2 ? launch_render<2>(a, st) : launch_render<1>(a, st);
+        const bool tc = path == 1;
+        rc = R == 8 ? launch_render<8>(a, tc, st) : R == 4 ? launch_render<4>(a, tc, st) : R == 2 ? launch_render<2>(a, tc, st) : launch_render<1>(a, tc, st);
     }
     if (rc) return rc;
     count_launches(4);
     depth_clamp_kernel<<<(total + 255) / 256, 256, 0, st>>>(g->depth, total, ws);
     R3DP_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int r3dp_render_path(const r3dp_render_args_t* g) {
+    if (g == nullptr || g->mlp == nullptr) { set_error("render_path: null argument block or decoder"); return -1; }
+    return render_path(render_args(g));
 }
 
 extern "C" int r3dp_render(const float* planes_cl, int N, int C, int H, int W, const float* ray_o, const float* ray_d,
