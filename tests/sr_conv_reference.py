@@ -1,5 +1,6 @@
 """Float64 references and element-wise error bounds for the tensor-core SR convolutions (csrc/sr_tc.cu), for
-tests/test_gpu_sr_conv_conformance.py.  Test infrastructure: it does not import the library, so it also runs on a machine without a GPU.
+tests/test_gpu_sr_conv_conformance.py, and for the exact-fp32 SR path (csrc/sr_fp32.cu, last section below), for
+tests/test_gpu_sr_fp32_conformance.py.  Test infrastructure: it does not import the library, so it also runs on a machine without a GPU.
 
 Operands.  Every reference is computed from the operands the kernel actually reads, converted exactly to float64: the fp16 activations
 (hi + lo for split [hi | lo] tensors), the packed weights read back and unpacked ((hi + lo) / 2^10 for split weights), and the fp32
@@ -31,7 +32,31 @@ the element, so beta S bounds the accumulation error whatever the summation orde
 beta is the accumulation term: fp32 sums of fp16 x fp16 products (exact in fp32) in the tensor cores' order, plus for split operands
 the dropped lo x lo product (<= 2^-22 |x| |w| per term).  It is set from the worst (|got - ref| - alpha |ref| - extra) / S measured over
 every case of the conformance suite, with headroom (see BETA).  The split mode's worst ratio is ten times the fp16 mode's: its K loop is
-three times longer (hi x hi + lo x hi + hi x lo) and the worst case has 256 input channels, 6912 products per output."""
+three times longer (hi x hi + lo x hi + hi x lo) and the worst case has 256 input channels, 6912 products per output.
+
+The exact-fp32 path (csrc/sr_fp32.cu, sr_mode='fp32'; tests/test_gpu_sr_fp32_conformance.py).  Operands are fp32 and NCHW, and every
+product is an fma on fp32 operands, so the conv output is an fp32 sum whose roundings all lie in beta S.  What remains, with
+u = 2^-24 and the library built without --use_fast_math (sqrtf and divisions correctly rounded):
+
+  * SR layer epilogue (bias + lrelu(0.2) * sqrt2):  three roundings, the bias add, the x 0.2f of negative values and the
+    x 1.4142135623730951f, each <= u relative and multiplicative, so they compose to a relative error of the stored value.  The
+    constants are not the reference's: 0.2f = 0.2 (1 + 1.5e-8) and the fp32 sqrt2 = sqrt2 (1 - 1.7e-8).  3u + 3.2e-8 = 2.1e-7 <= 2^-22:
+    ALPHA_FP32_LAYER = 2^-22, against the float64 reference with the exact 0.2 and sqrt2.
+  * up=2: the kernel writes the (2H+1) x (2W+1) transposed-conv grid to fp32 scratch and runs the FIR over it.  Each grid value carries
+    its final rounding 2^-24 |grid|; the FIR's positive taps and the gain-Lipschitz activation carry it to the output as
+    extra = gain * FIR(2^-24 |grid|), the fp32 analogue of the `tc` up-path term.  The FIR's own partial sums are bounded by S.
+  * ToRGB: bias and the upsampled skip image are summands of the same fp32 sum: alpha = 2^-24 on the result, as for the fp32 images above.
+  * styles = (w . fl(A fl(1 / sqrtf(w_dim))) + a) * post, post the fp32 value the kernel is given: every term's relative error (the fp32
+    gain and the scaled affine weight, <= 2.5u) and the partial sums lie in beta S with S = post (|w| @ |A|^T / sqrt(w_dim) + |a|); the
+    final x post rounds once: alpha = 2^-24.
+  * fold:  v = fl(W s) (u), q = sum of the len = k^2 I squares v^2 (positive terms: <= gamma_len relative in any order, plus 2u from the
+    rounding of v), fl(q + 1e-8f) (u), d = 1 / sqrtf (2u), out = fl(v d) (u).  rsqrt halves the relative error of q, so
+    |out - ref| <= (5.5u + gamma_len / 2) |ref|; fold_alpha rounds 5.5u up to 6u to cover the second-order terms.  1e-8f differs from
+    1e-8 by 6e-17, far below u q.  Without demodulation only fl(W s) remains: u.  fold_error carries an error of the styles on.
+
+BETA['fp32'] covers the accumulation of the conv and ToRGB sums and of the styles.  It is measured like the others and is also no larger
+than the deterministic bound gamma_K = K u / (1 - K u) of recursive summation at the suite's largest K = 9 * 256, so the bar is never
+looser than what can be proved."""
 import math
 
 import torch
@@ -43,13 +68,18 @@ SQRT2 = math.sqrt(2.0)
 ALPHA_F16 = 2.0 ** -11
 ALPHA_SPLIT = 2.0 ** -22
 ALPHA_F32 = 2.0 ** -24
+ALPHA_FP32_LAYER = 2.0 ** -22                # the fp32 SR layer epilogue: bias add, x 0.2f, x fp32 sqrt2 (module docstring)
+U_F32 = 2.0 ** -24                           # unit roundoff of fp32
 FLOOR_F16 = 2.0 ** -25                       # half the spacing of fp16 subnormals
 SPLIT_WEIGHT_SCALE = 1024.0                  # split weights are stored x 2^10 so that their lo halves stay normal fp16 numbers
 #: accumulation term per mode.  Worst ratio measured over the conformance suite on one H100 80GB HBM3 (SXM, 700 W power limit):
 #: tc 2.12e-7 (torgb_ex, 256 channels; the worst conv output 1.76e-7, layer_torgb 128 -> 256), tcx 2.27e-6 (layer up=1, 256 -> 128).
 #: beta = 2^-21 = 4.77e-7 (2.2x) and 2^-18 = 3.81e-6 (1.7x).  The kernels are deterministic and every H100 runs the same SASS in the
 #: same summation order, so the headroom only has to cover new cases, not run-to-run noise.
-BETA = {'tc': 2.0 ** -21, 'tcx': 2.0 ** -18}
+#: fp32 (tests/test_gpu_sr_fp32_conformance.py), on one H100 80GB HBM3 (SXM, 400 W power limit): 4.27e-7 (the up=2 scratch grid,
+#: 256 -> 128 at 256^2; the worst layer output 3.57e-7, up=1 128 -> 128 at 512^2; ToRGB 2.50e-7; styles 3.42e-8).  beta = 2^-20 =
+#: 9.54e-7 (2.2x), far below gamma_K = 1.37e-4 at K = 9 * 256.
+BETA = {'tc': 2.0 ** -21, 'tcx': 2.0 ** -18, 'fp32': 2.0 ** -20}
 #: epilogue activations of conv_tc3_kernel: code -> (slope, gain).  0 linear, 1 bias_act lrelu * sqrt2, 2 nn.LeakyReLU(0.01), 3 ReLU
 ACT = {0: (1.0, 1.0), 1: (0.2, SQRT2), 2: (0.01, 1.0), 3: (0.0, 1.0)}
 #: the FIR [1,3,3,1] x gain 4 per axis, as composed into the up weights
@@ -174,6 +204,56 @@ def conv_up_composed(x: torch.Tensor, G: torch.Tensor) -> torch.Tensor:
 def torgb(a: torch.Tensor, wrgb: torch.Tensor) -> torch.Tensor:
     """Per-sample 1x1 ToRGB without bias: a [N,C,H,W], wrgb [N,3,C] -> [N,3,H,W]."""
     return torch.einsum('nchw,nkc->nkhw', a, wrgb)
+
+
+def styles(w: torch.Tensor, A: torch.Tensor, a: torch.Tensor, post: float = 1.0) -> torch.Tensor:
+    """affine(w) * post: w [N,w_dim], A [Cin,w_dim], a [Cin] -> [N,Cin]."""
+    return orc.affine_styles(w, A, a) * post
+
+
+def styles_abs(w: torch.Tensor, A: torch.Tensor, a: torch.Tensor, post: float = 1.0) -> torch.Tensor:
+    """S of styles(): |post| (|w| @ |A|^T / sqrt(w_dim) + |a|)."""
+    return orc.affine_styles(w.abs(), A.abs(), a.abs()) * abs(post)
+
+
+def fold(W: torch.Tensor, s: torch.Tensor, demod: bool) -> torch.Tensor:
+    """Modulated (+ demodulated) weights: W [O,I,k,k], s [N,I] -> [N,O,I,k,k]."""
+    return orc.fold_weight(W, s, demod)
+
+
+def fold_abs(W: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """|W| |s|, the magnitude of every modulated weight before demodulation."""
+    return orc.fold_weight(W.abs(), s.abs(), False)
+
+
+def gamma(k: int) -> float:
+    """gamma_k = k u / (1 - k u): the relative bound of k fp32 roundings, e.g. of a recursive sum of k terms."""
+    return k * U_F32 / (1 - k * U_F32)
+
+
+def fold_alpha(length: int, demod: bool) -> float:
+    """Relative error of r3dp_sr_fold_weights for exact styles; length = k^2 I (module docstring)."""
+    return 6 * U_F32 + gamma(length) / 2 if demod else U_F32
+
+
+def fold_error(W: torch.Tensor, s: torch.Tensor, ds: torch.Tensor, demod: bool):
+    """(ref, E): ref = fold(W, s) and an element-wise bound E on |fold_kernel(W, s') - ref| for any styles s' with |s' - s| <= ds.
+    W [O,I,k,k], s and ds [N,I], float64.  With v = W s, D = |W| ds and eta = fold_alpha: the kernel's result is W s' d' (1 + eta') with
+    |eta'| <= eta and d' = rsqrt(||W s'||^2 + 1e-8) per output channel.  sqrt(||W s'||^2 + 1e-8) lies within ||D|| of
+    sqrt(||W s||^2 + 1e-8) = 1 / d (triangle inequality), so d / (1 + r) <= d' <= d / (1 - r) with r = ||D|| d, and
+        |W s' d' (1 + eta') - W s d| <= D d g + |ref| (g - 1),   g = (1 + eta) / (1 - r).
+    Without demodulation: |fl(W s') - W s| <= D (1 + eta) + eta |ref|.  ds = 0 gives eta |ref|."""
+    ref = fold(W, s, demod)
+    D = fold_abs(W, ds)
+    eta = fold_alpha(W[0].numel(), demod)
+    if not demod:
+        return ref, D * (1 + eta) + eta * ref.abs()
+    dims = [2, 3, 4]
+    q = fold(W, s, False).square().sum(dim=dims, keepdim=True) + 1e-8
+    r = D.square().sum(dim=dims, keepdim=True).sqrt() / q.sqrt()
+    assert float(r.max()) < 0.5, 'styles error too large for the first-order fold bound'
+    g = (1 + eta) / (1 - r)
+    return ref, D * q.rsqrt() * g + ref.abs() * (g - 1)
 
 
 def to_uint8(img: torch.Tensor) -> torch.Tensor:
