@@ -46,6 +46,10 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         super().__init__(channels, img_resolution, sr_num_fp16_res, sr_antialias, **block_kwargs)
         if self.sr_mode not in ('tc', 'tc_exact'):
             raise NotImplementedError('the torso head is built on the tensor-core path only (sr_mode="tc" | "tc_exact")')
+        if not sr_antialias:
+            # sr_with_ref.py:79-82 would down-sample the 512^2 reference images with plain bilinear; _aa_down2 is the antialiased filter
+            # (the head's other resizes are up-samplings, where antialias changes nothing)
+            raise NotImplementedError('the torso head is built with sr_antialias=True only (its 512 -> 256 resizes are antialiased)')
         hp = dict(hp or {})
         self.hparams = {'torso_model_version': hp.get('torso_model_version', 'v2'), 'htbsr_head_weight_fuse_mode': hp.get('htbsr_head_weight_fuse_mode', 'v2'),
                         'htbsr_head_threshold': float(hp.get('htbsr_head_threshold', 0.9)), 'weight_fuse': hp.get('weight_fuse', True)}
