@@ -378,6 +378,35 @@ int r3dp_tw_narrow_conv(const void* xa_f16, int sa, int ca, int lo_a, const floa
                         const float* wk, const float* bias, int N, int H, int W, int K, int CO, int act, int nchw, float* out, r3dp_stream_t stream);
 int r3dp_tw_hid_to_nchw(const void* x_f16, int N, int C, int H, int W, int cs, int lo, float* y, r3dp_stream_t stream);
 
+/* The torso warper's motion-field estimator (modules/real3d/facev2v_warp/network2.py:162-244, MotionFieldEstimator('standard')).
+ * Activations NDHWC fp16 with voxel stride xs / ys halves; split != 0: the fp16 remainder of each value sits `lo` halves after it in the same
+ * voxel ([hi | lo]) and the weights are [hi | lo] of w * 2^10, as in the r3dp_sr_tcx_* family.
+ * r3dp_mf_conv3d       3-D conv on wgmma (stride 1, zero padding): box taps kd x kh x kw (odd) centred, or with up != 0 the 4 output-parity
+ *                      phases of nn.Upsample((1,2,2), nearest) + 3x3x3 conv as kd x 2 x 2 taps on the low-resolution input (layers.py:77-93).
+ *                      M space = the input grid N x D x H x W; x channels [0, cin) (cin % 32 == 0); wp [nph][taps][cop][cin (x2 split)] fp16,
+ *                      bias [cop]; y = relu? (conv + bias) (+ res, same layout as y) stored at channels [yc0, yc0 + cout) of voxels of ys
+ *                      halves (up: output grid D x 2H x 2W), fp16 or fp32 (out_f32, no residual)
+ * r3dp_mf_input        create_heatmap_representations + create_sparse_motions + create_deformed_source_image (func_utils.py:130-191, Rs = Rd = I):
+ *                      fc [N or 1,D,H,W,4] fp32 (the compressed source), kp_s / kp_d [N,K,3] -> channel k*5 + j of y, zeros up to cpad
+ * r3dp_mf_pool         AvgPool3d((1,2,2)) (layers.py:58-74); H, W: the pooled size
+ * r3dp_mf_head_input   interpolate(cat[rgb, weights], 1/2, bilinear) = the 2x2 mean, [N,3|1,2H,2W] fp32 -> NHWC channels 0..3, zeros up to cpad
+ * r3dp_mf_head_bcast   interpolate(head features, 1/2, bilinear) repeated over depth (network2.py:221-224) into channels [yc0, yc0 + C) of y
+ * r3dp_mf_deform       softmax over the K+1 fp32 logits (voxel stride ls) and deformation [N,D,H,W,3] = sum_k mask_k * sparse_motion_k
+ * r3dp_mf_occlusion    occlusion_conv / occlusion_conv2 (7x7, C*D -> 1, sigmoid) on x.view(N, C*D, H, W): wk [D][49][C][2] fp32, bias [2] */
+int r3dp_mf_conv3d(const void* x_f16, int xs, int xlo, int cin, const void* wp_f16, const float* bias, const void* res_f16, int N, int D, int H,
+                   int W, int kd, int kh, int kw, int up, int cout, int cop, int relu, void* y, int ys, int yc0, int ylo, int out_f32, int split,
+                   r3dp_stream_t stream);
+int r3dp_mf_input(const float* fc, int fc_shared, const float* kp_s, const float* kp_d, int N, int K, int D, int H, int W, int cpad, void* y_f16,
+                  int ys, int ylo, int split, r3dp_stream_t stream);
+int r3dp_mf_pool(const void* x_f16, int N, int D, int H, int W, int C, int xs, int xlo, void* y_f16, int ys, int ylo, int split, r3dp_stream_t stream);
+int r3dp_mf_head_input(const float* rgb, const float* wts, int N, int H, int W, int cpad, void* y_f16, int ys, int ylo, int split, r3dp_stream_t stream);
+int r3dp_mf_head_bcast(const void* x_f16, int N, int D, int H, int W, int C, int xs, int xlo, void* y_f16, int ys, int yc0, int ylo, int split,
+                       r3dp_stream_t stream);
+int r3dp_mf_deform(const float* logits, int ls, const float* kp_s, const float* kp_d, int N, int K, int D, int H, int W, float* deformation,
+                   r3dp_stream_t stream);
+int r3dp_mf_occlusion(const void* x_f16, int N, int D, int H, int W, int C, int xs, int xlo, int split, const float* wk, const float* bias, float* occ,
+                      float* occ2, r3dp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

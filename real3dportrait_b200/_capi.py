@@ -118,6 +118,13 @@ _SIGNATURES = {
     'r3dp_tw_affine_relu': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
     'r3dp_tw_narrow_conv': (_I, [_P, _I, _I, _I, _P, _I, _I, _P, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     'r3dp_tw_hid_to_nchw': (_I, [_P, _I, _I, _I, _I, _I, _I, _P, _P]),
+    'r3dp_mf_conv3d': (_I, [_P, _I, _I, _I, _P, _P, _P] + [_I] * 11 + [_P] + [_I] * 5 + [_P]),
+    'r3dp_mf_input': (_I, [_P, _I, _P, _P] + [_I] * 6 + [_P, _I, _I, _I, _P]),
+    'r3dp_mf_pool': (_I, [_P] + [_I] * 7 + [_P, _I, _I, _I, _P]),
+    'r3dp_mf_head_input': (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _I, _I, _P]),
+    'r3dp_mf_head_bcast': (_I, [_P] + [_I] * 7 + [_P, _I, _I, _I, _I, _P]),
+    'r3dp_mf_deform': (_I, [_P, _I, _P, _P] + [_I] * 5 + [_P, _P]),
+    'r3dp_mf_occlusion': (_I, [_P] + [_I] * 8 + [_P, _P, _P, _P, _P]),
 }
 
 

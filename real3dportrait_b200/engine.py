@@ -122,11 +122,13 @@ class FrameEngine:
     torso_model: run the torso head with this warper (WarpBasedTorsoModelMediaPipe or a module with its forward signature);
     warper_in_graph: capture the warper inside the step's single graph (only for capturable warpers; the default runs it eagerly
     between two graphs).  torso_stage2='cuda': the warper's stage 2 on this library's kernels, its appearance features cached per clip by
-    begin_clip() (SuperresolutionHybrid8XDC_Warp.set_torso_stage2)."""
+    begin_clip() (SuperresolutionHybrid8XDC_Warp.set_torso_stage2).  torso_motion='cuda' (needs torso_stage2='cuda'): the warper's
+    motion-field estimator on this library's 3-D convolutions too (SuperresolutionHybrid8XDC_Warp.set_torso_motion)."""
 
     def __init__(self, batch: int = 4, sr_mode: str = 'fp32', device=None, world: int = 1, rank: int = 0, dist=None, hp: Optional[dict] = None,
                  static_styles: bool = True, use_graph: bool = True, out_uint8: bool = False, exchange: str = 'allgather',
-                 torso_model: Optional[torch.nn.Module] = None, warper_in_graph: bool = False, torso_stage2: str = 'torch'):
+                 torso_model: Optional[torch.nn.Module] = None, warper_in_graph: bool = False, torso_stage2: str = 'torch',
+                 torso_motion: str = 'torch'):
         assert exchange in ('allgather', 'p2p', 'none')
         self.batch, self.world, self.rank, self.dist = batch, world, rank, dist
         self.device = device if device is not None else torch.device('cuda', torch.cuda.current_device())
@@ -137,6 +139,10 @@ class FrameEngine:
             if not self.torso:
                 raise ValueError('torso_stage2 is an option of the torso head: FrameEngine(torso_model=...)')
             self.head.superresolution.set_torso_stage2(torso_stage2)
+        if torso_motion != 'torch':
+            if not self.torso:
+                raise ValueError('torso_motion is an option of the torso head: FrameEngine(torso_model=...)')
+            self.head.superresolution.set_torso_motion(torso_motion)
         self.out_uint8 = bool(out_uint8)
         if self.out_uint8 and self.head.superresolution.sr_mode not in ('tc', 'tc_exact'):     # the head's effective mode: a torso head maps 'fp32' to 'tc'
             raise NotImplementedError('uint8 frames are written by the tensor-core SR epilogue (sr_mode="tc")')

@@ -41,7 +41,7 @@ _pack_plain = sr_tc.pack_plain
 
 class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
     def __init__(self, channels, img_resolution, sr_num_fp16_res, sr_antialias, hp: Optional[dict] = None, torso_model: Optional[torch.nn.Module] = None,
-                 torso_stage2: str = 'torch', **block_kwargs):
+                 torso_stage2: str = 'torch', torso_motion: str = 'torch', **block_kwargs):
         block_kwargs.setdefault('sr_mode', 'tc')
         super().__init__(channels, img_resolution, sr_num_fp16_res, sr_antialias, **block_kwargs)
         if self.sr_mode not in ('tc', 'tc_exact'):
@@ -79,7 +79,10 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         self.static_prepared_warp = None
         self._stage2_cache = None
         self._warper = None
+        self._motion_cache = None
+        self.torso_motion = 'torch'
         self.set_torso_stage2(torso_stage2)
+        self.set_torso_motion(torso_motion)
 
     def set_torso_stage2(self, mode: str) -> None:
         """'torch': the caller's torso_model(...) call (the reference's path).  'cuda': the warper's stage 2 (Generator + occlusion_2_predictor)
@@ -89,8 +92,41 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
             raise ValueError(f"torso_stage2 is 'torch' or 'cuda', got {mode!r}")
         if mode == 'cuda' and self.hparams['torso_model_version'] != 'v2':
             raise NotImplementedError("torso_stage2='cuda' is built for torso_model_version v2 (facev2v_warp/model2.py) only")
+        if mode == 'torch' and getattr(self, 'torso_motion', 'torch') == 'cuda':
+            raise ValueError("torso_motion='cuda' needs torso_stage2='cuda': call set_torso_motion('torch') first")
         self.torso_stage2 = mode
         self._stage2_cache = None
+
+    def set_torso_motion(self, mode: str) -> None:
+        """'torch': the warper calls the caller's motion_field_estimator.  'cuda': the estimator (network2.py:162-244) runs on this library's
+        3-D convolutions (torso_warp.motion), its compressed source volume cached per clip by begin_clip(segmap=...).  Needs torso_stage2='cuda'
+        (the restated stage 1 is where the call is replaced) and MotionFieldEstimator('standard') with torso_kp_num 4 or 9."""
+        if mode not in ('torch', 'cuda'):
+            raise ValueError(f"torso_motion is 'torch' or 'cuda', got {mode!r}")
+        if mode == 'cuda':
+            if self.hparams['torso_model_version'] != 'v2':
+                raise NotImplementedError("torso_motion='cuda' is built for torso_model_version v2 (facev2v_warp/model2.py) only")
+            if self.torso_stage2 != 'cuda':
+                raise ValueError("torso_motion='cuda' needs torso_stage2='cuda'")
+            tm = getattr(self, 'torso_model', None)
+            if tm is not None:
+                from . import torso_warp
+                err = torso_warp.estimator_shape_error(tm.motion_field_estimator)
+                if err is not None:
+                    raise NotImplementedError(f"torso_motion='cuda' is built for MotionFieldEstimator('standard'): {err}")
+        self.torso_motion = mode
+        self._motion_cache = None
+
+    def _motion_weights(self):
+        """Folded + packed estimator weights (torso_warp.MotionWeights), keyed like _stage2_weights(); None unless torso_motion='cuda'."""
+        if self.torso_motion != 'cuda':
+            return None
+        from . import torso_warp
+        mfe = self.torso_model.motion_field_estimator
+        key = (self._split, tuple((t.data_ptr(), t._version) for t in list(mfe.parameters()) + list(mfe.buffers())))
+        if self._motion_cache is None or self._motion_cache[0] != key:
+            self._motion_cache = (key, torso_warp.MotionWeights(mfe, self._split))
+        return self._motion_cache[1]
 
     def _stage2_weights(self):
         """Folded + packed stage-2 weights, rebuilt when the mode, the device or any of the warper's parameters / buffers changed (a
@@ -146,6 +182,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         self._clip_cache = None
         self.static_prepared_warp = None
         self._stage2_cache = None
+        self._motion_cache = None
         return super()._load_from_state_dict(*a, **k)
 
     @staticmethod
@@ -195,7 +232,8 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         copies made per call.  in_place: when a clip with the same mode and batch is already begun, write the new constants into its
         tensors (CUDA graphs captured against them then render the new clip).  Returns True when the constants were refilled in place.
         segmap [1,6,512,512] with torso_stage2='cuda': also keep the warper's per-clip part (torso_warp.appearance: appearance_extractor of
-        the reference torso image, the dilated torso mask, the 64^2 segmap, the volume in NDHWC); forward() then ignores its segmap argument."""
+        the reference torso image, the dilated torso mask, the 64^2 segmap, the volume in NDHWC; with torso_motion='cuda' the estimator's
+        compressed source volume too); forward() then ignores its segmap argument."""
         assert ref_torso_rgb.shape[0] == 1 and ref_bg_rgb.shape[0] == 1, 'one reference image per clip'
         plain, sp = self._plain(), self._split
         t256, b256 = self._aa_down2(ref_torso_rgb), self._aa_down2(ref_bg_rgb)
@@ -203,12 +241,13 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         if segmap is not None and self.torso_stage2 == 'cuda':
             from . import torso_warp
             assert segmap.shape[0] == 1, 'one segmap per clip'
-            cc['torso_app'] = torso_warp.appearance(self.torso_model, t256, segmap)
+            cc['torso_app'] = torso_warp.appearance(self.torso_model, t256, segmap, self._motion_weights())
         if batch is not None:
             cc['batch'] = (t256.expand(batch, -1, -1, -1).contiguous(), b256.expand(batch, -1, -1, -1).contiguous())
         old = self._clip_cache
         if in_place and old is not None and old['split'] == sp and (old['batch'] is None) == (batch is None) and \
-                (batch is None or old['batch'][0].shape[0] == batch) and (old['torso_app'] is None) == (cc['torso_app'] is None):
+                (batch is None or old['batch'][0].shape[0] == batch) and (old['torso_app'] is None) == (cc['torso_app'] is None) and \
+                (cc['torso_app'] is None or old['torso_app'].keys() == cc['torso_app'].keys()):
             for k in ('ref_torso_256', 'ref_bg_256', 'x_bg'):
                 old[k].copy_(cc[k])
             if cc['torso_app'] is not None:                         # a graph that captured the warper reads these tensors by address
@@ -331,7 +370,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
             cc = st['cc']
             with capi.region('torso_model'):
                 return self._warper(self._stage2_weights(), ref_torso_256, segmap, kp_s, kp_d, rgb_256.detach(), weights_256.detach(),
-                                    app=cc.get('torso_app') if cc is not None else None)
+                                    app=cc.get('torso_app') if cc is not None else None, motion_wts=self._motion_weights())
         with capi.region('torso_model'):
             if self.hparams['torso_model_version'] == 'v1':
                 return self.torso_model(ref_torso_256, segmap, kp_s, kp_d, rgb_256.detach(), cal_loss=True, target_torso_mask=st['target_torso_mask'])

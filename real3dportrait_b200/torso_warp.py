@@ -2,7 +2,8 @@
 this library's kernels: the deformation-based Generator (network2.py:248-301) and the occlusion_2_predictor (model2.py:212-219, 260-263).
 
 Stage 1 (model2.py:222-258) is restated here and calls the caller's `appearance_extractor` and `motion_field_estimator` children, which stay
-PyTorch.  Stage 2 reads its weights from the caller's `deform_based_generator` and `occlusion_2_predictor`: eval spectral norm and eval
+PyTorch; with torso_motion='cuda' the motion_field_estimator runs on the 3-D convolutions of csrc/conv3d_tc.cu instead (MotionWeights,
+motion()).  Stage 2 reads its weights from the caller's `deform_based_generator` and `occlusion_2_predictor`: eval spectral norm and eval
 BatchNorm are folded on the host in float64, then packed once (Stage2Weights, cached by the SR head until its parameters are reloaded).
 
 Layout of stage 2 (N images; tc: fp16 NHWC activations, tc_exact: [hi | lo] halves):
@@ -46,11 +47,11 @@ def bn_affine(bn: torch.nn.Module):
 
 
 def fold_cna(block) -> tuple:
-    """ConvBlock2D 'CNA' (conv -> BN -> act): (W [O,I,k,k], b [O]) float64 with the BN folded in."""
+    """ConvBlock2D / ConvBlock3D 'CNA' (conv -> BN -> act): (W [O,I,k,k(,k)], b [O]) float64 with the BN folded in."""
     conv, bn = block.layers[0], block.layers[1]
     w, b = sn_weight(conv), conv.bias.detach().double()
     s, t = bn_affine(bn)
-    return w * s[:, None, None, None], b * s + t
+    return w * s.reshape(-1, *[1] * (w.dim() - 1)), b * s + t
 
 
 def compose_nearest_up(w: torch.Tensor) -> torch.Tensor:
@@ -162,6 +163,196 @@ def stage2(wts: Stage2Weights, fs_ndhwc: torch.Tensor, deformation: torch.Tensor
     return rgb, hid, occ2
 
 
+def compose_nearest_up3d(w: torch.Tensor) -> torch.Tensor:
+    """3x3x3 weights [O,I,3,3,3] of a conv applied after nn.Upsample((1,2,2), nearest) -> [4,O,I,3,2,2]: depth untouched, phase p*2+q holds
+    the 2x2 (H, W) taps of output parity (p, q) on the low-resolution input; tap (iy, ix) reads input offset (p + iy - 1, q + ix - 1)."""
+    O, I = w.shape[:2]
+    g = compose_nearest_up(w.reshape(O, I * 3, 3, 3)).reshape(4, O, I, 3, 3, 3)      # [.., kz, dy+1, dx+1]
+    out = w.new_zeros(4, O, I, 3, 2, 2)
+    for p in range(2):
+        for q in range(2):
+            out[p * 2 + q] = g[p * 2 + q][..., p:p + 2, q:q + 2]
+    return out
+
+
+# ---- the motion-field estimator (network2.py:162-244) on the 3-D convolutions of csrc/conv3d_tc.cu -------------------------------------
+MOTION_D, MOTION_HW = 16, 64
+
+
+def pack_conv3d(w: torch.Tensor, b: torch.Tensor, cin: int, split: bool, cin_map=None, cout_tile: Optional[int] = None):
+    """Folded float64 weights [nph,O,I,kd,kh,kw] -> (packed fp16 [nph, taps, cop, cin (x2 split: [hi | lo] of w * 2^10)], bias [cop] fp32,
+    O, cop).  cin: the channels the conv reads (a multiple of 32); cin_map: the physical input channel of each of the I logical channels."""
+    nph, O, I = w.shape[:3]
+    taps = w.shape[3] * w.shape[4] * w.shape[5]
+    tile = cout_tile or (16 if O <= 16 else 32 if O <= 32 else 64 if O <= 64 else 128)
+    cop = (O + tile - 1) // tile * tile
+    idx = torch.as_tensor(list(range(I)) if cin_map is None else cin_map, dtype=torch.long, device=w.device)
+    wt = torch.zeros(nph, taps, cop, cin, dtype=torch.float64, device=w.device)
+    wt[:, :, :O].index_copy_(3, idx, w.permute(0, 3, 4, 5, 1, 2).reshape(nph, taps, O, I))
+    if split:
+        s = wt * 1024.0
+        hi = s.half()
+        packed = torch.cat([hi, (s - hi.double()).half()], dim=-1)
+    else:
+        packed = wt.half()
+    bias = torch.zeros(cop, dtype=torch.float32, device=w.device)
+    bias[:O] = b.float()
+    return packed.contiguous(), bias, O, cop
+
+
+def estimator_shape_error(mfe: torch.nn.Module) -> Optional[str]:
+    """Why `mfe` is not the estimator the kernels restate (MotionFieldEstimator('standard', 34, K in {4, 9}), predict_multiref_occ), or None."""
+    try:
+        if not getattr(mfe, 'predict_multiref_occ', False):
+            return 'predict_multiref_occ=False'
+        down = [blk.layers[0].layers[0] for blk in mfe.down]
+        up = [blk.layers[1].layers[0] for blk in mfe.up]
+        c0 = down[0].in_channels
+        if c0 % 5 or c0 // 5 - 1 not in (4, 9):
+            return f'{c0} input channels (torso_kp_num 4 or 9 are built)'
+        if [c.out_channels for c in down] != [64, 128, 256, 512, 1024] or [c.out_channels for c in up] != [512, 256, 128, 64, 32]:
+            return "model_scale other than 'standard'"
+        if mfe.compress.out_channels != 4 or mfe.tgt_head_fuser.in_channels != c0 + 64 or mfe.mask_conv.out_channels != c0 // 5:
+            return 'unexpected estimator layers'
+    except AttributeError as e:
+        return f'not a MotionFieldEstimator ({e})'
+    return None
+
+
+class MotionWeights:
+    """Folded and packed weights of the motion-field estimator for one sr_mode (split = tc_exact).  Every BatchNorm is eval-mode and folds
+    into the conv before it (fold_cna); the tgt-head encoder's pre-activation ResBlock2D keeps BN1 as an affine + ReLU (r3dp_tw_affine_relu)."""
+
+    def __init__(self, mfe: torch.nn.Module, split: bool):
+        err = estimator_shape_error(mfe)
+        if err is not None:
+            raise NotImplementedError(f"torso_motion='cuda' is built for MotionFieldEstimator('standard'): {err}")
+        self.split = bool(split)
+        dev = next(mfe.parameters()).device
+        d = lambda t: t.detach().double()                                               # noqa: E731
+        c0 = mfe.down[0].layers[0].layers[0].in_channels
+        self.K = c0 // 5 - 1
+        self.c0, self.P0 = c0, (c0 + 31) // 32 * 32                        # input channels, padded to the 32-channel K step
+        self.CF = self.P0 + 64                                             # fuser input: [input c0 | pad | up output 32 | head features 32]
+        self.compress = (d(mfe.compress.weight)[:, :, 0, 0, 0], d(mfe.compress.bias))
+        self.down = []
+        cin = self.P0
+        for blk in mfe.down:
+            w, b = fold_cna(blk.layers[0])
+            self.down.append(pack_conv3d(w[None], b, cin, split))
+            cin = w.shape[0]
+        self.up = []
+        for blk in mfe.up:
+            w, b = fold_cna(blk.layers[1])
+            self.up.append(pack_conv3d(compose_nearest_up3d(w), b, cin, split))
+            cin = w.shape[0]
+        enc = mfe.tgt_head_encoder
+        w, b = fold_cna(enc[0])
+        self.enc0 = pack_conv3d(w[None, :, :, None], b, 32, split)
+        self.res = []
+        for rb in list(enc)[1:]:
+            nac1, nac2 = rb.layers[0].layers, rb.layers[1].layers                   # NAC: BN, ReLU, conv
+            s1, t1 = bn_affine(nac1[0])
+            s2, t2 = bn_affine(nac2[0])
+            w1, b1 = sn_weight(nac1[2]), d(nac1[2].bias)
+            w2, b2 = sn_weight(nac2[2]), d(nac2[2].bias)
+            self.res.append((s1.float().to(dev), t1.float().to(dev),
+                             pack_conv3d((w1 * s2[:, None, None, None])[None, :, :, None], b1 * s2 + t2, 32, split),
+                             pack_conv3d(w2[None, :, :, None], b2, 32, split)))
+        fu = mfe.tgt_head_fuser
+        fmap = list(range(c0)) + [self.P0 + i for i in range(64)]
+        self.fuser = pack_conv3d(d(fu.weight)[None], d(fu.bias), self.CF, split, cin_map=fmap)
+        mc = mfe.mask_conv
+        self.mask = pack_conv3d(d(mc.weight)[None], d(mc.bias), 32, split)
+        D = MOTION_D
+        occ = [d(c.weight)[0].reshape(32, D, 7, 7).permute(1, 2, 3, 0) for c in (mfe.occlusion_conv, mfe.occlusion_conv2)]
+        self.occ_w = torch.stack(occ, dim=-1).reshape(D, 49, 32, 2).float().contiguous().to(dev)
+        self.occ_b = torch.cat([d(mfe.occlusion_conv.bias), d(mfe.occlusion_conv2.bias)]).float().contiguous().to(dev)
+
+
+def compress_volume(wts: MotionWeights, motion_inp: torch.Tensor) -> torch.Tensor:
+    """compress(motion_inp): the 1x1x1 conv 34 -> 4 in float64, as the NDHWC fp32 volume [N,D,H,W,4] the input kernel samples."""
+    wc, bc = wts.compress
+    x = torch.einsum('oi,nidhw->ndhwo', wc.to(motion_inp.device), motion_inp.double()) + bc.to(motion_inp.device)
+    return x.float().contiguous()
+
+
+def motion(wts: MotionWeights, fc: torch.Tensor, kp_s: torch.Tensor, kp_d: torch.Tensor, rgb_256: torch.Tensor, weights_256: torch.Tensor):
+    """MotionFieldEstimator.forward with Rs = Rd = I -> (deformation [N,D,64,64,3], occlusion, occlusion_2 [N,1,64,64]) fp32.
+    fc [N or 1,D,64,64,4] fp32: the compressed source volume (compress_volume; one volume for the batch is read by every image),
+    kp_s / kp_d [N,K,3], rgb_256 [N,3,256,256], weights_256 [N,1,256,256]."""
+    L, sp, st = capi.lib(), wts.split, capi.stream()
+    wide = 2 if sp else 1
+    N, K = kp_s.shape[:2]
+    if K != wts.K:
+        raise ValueError(f'{K} keypoints for an estimator built for {wts.K}')
+    D, S = MOTION_D, MOTION_HW
+    fc, kp_s, kp_d = capi.f32(fc), capi.f32(kp_s), capi.f32(kp_d)
+    dev = kp_s.device
+    f16 = torch.float16
+    P0, CF = wts.P0, wts.CF
+
+    def conv(x, xs, xlo, cin, packed, dims, taps, relu, y, ys, yc0, ylo, up=0, res=None, out_f32=0):
+        wp, bias, O, cop = packed
+        n, dd, h, w = dims
+        capi.check(L.r3dp_mf_conv3d(capi.ptr(x, f16), xs, xlo, cin, capi.ptr(wp, f16), capi.ptr(bias), capi.ptr(res, f16), n, dd, h, w, *taps, up, O, cop,
+                                    relu, capi.ptr(y, torch.float32 if out_f32 else f16), ys, yc0, ylo, out_f32, int(sp), st))
+
+    with capi.region('torso_motion'):
+        xf = torch.empty(N, D, S, S, CF * wide, device=dev, dtype=f16)                 # the fuser input; its first P0 channels feed the down path
+        capi.check(L.r3dp_mf_input(capi.ptr(fc), int(fc.shape[0] == 1 and N > 1), capi.ptr(kp_s), capi.ptr(kp_d), N, K, D, S, S, P0,
+                                   capi.ptr(xf, f16), CF * wide, CF, int(sp), st))
+        x, xs, xlo, cin, hw = xf, CF * wide, CF, P0, S
+        for packed in wts.down:
+            O = packed[2]
+            y = torch.empty(N, D, hw, hw, O * wide, device=dev, dtype=f16)
+            conv(x, xs, xlo, cin, packed, (N, D, hw, hw), (3, 3, 3), 1, y, O * wide, 0, O)
+            hw //= 2
+            x = torch.empty(N, D, hw, hw, O * wide, device=dev, dtype=f16)
+            capi.check(L.r3dp_mf_pool(capi.ptr(y, f16), N, D, hw, hw, O, O * wide, O, capi.ptr(x, f16), O * wide, O, int(sp), st))
+            xs, xlo, cin = O * wide, O, O
+        for i, packed in enumerate(wts.up):
+            O = packed[2]
+            if i + 1 < len(wts.up):
+                y, ys, yc0, ylo = torch.empty(N, D, 2 * hw, 2 * hw, O * wide, device=dev, dtype=f16), O * wide, 0, O
+            else:                                                                          # the last up block writes its slice of the fuser input
+                y, ys, yc0, ylo = xf, CF * wide, P0, CF
+            conv(x, xs, xlo, cin, packed, (N, D, hw, hw), (3, 2, 2), 1, y, ys, yc0, ylo, up=1)
+            x, xs, xlo, cin, hw = y, O * wide, O, O, 2 * hw
+        # tgt-head encoder at 128^2 (D = 1), then its 2x2 mean broadcast over depth into the fuser input
+        if tuple(rgb_256.shape) != (N, 3, 4 * S, 4 * S) or tuple(weights_256.shape) != (N, 1, 4 * S, 4 * S):
+            raise ValueError(f'rgb_256 / weights_256 must be [N,3|1,{4 * S},{4 * S}], got {tuple(rgb_256.shape)} / {tuple(weights_256.shape)}')
+        H2 = 2 * S
+        e = torch.empty(N, 1, H2, H2, 32 * wide, device=dev, dtype=f16)
+        capi.check(L.r3dp_mf_head_input(capi.ptr(capi.f32(rgb_256)), capi.ptr(capi.f32(weights_256)), N, H2, H2, 32, capi.ptr(e, f16), 32 * wide, 32,
+                                        int(sp), st))
+        dims2 = (N, 1, H2, H2)
+        x = torch.empty_like(e)
+        conv(e, 32 * wide, 32, 32, wts.enc0, dims2, (1, 7, 7), 1, x, 32 * wide, 0, 32)
+        for s1, t1, c1, c2 in wts.res:
+            a = torch.empty_like(x)
+            capi.check(L.r3dp_tw_affine_relu(capi.ptr(x, f16), capi.ptr(s1), capi.ptr(t1), N, H2, H2, 32, int(sp), capi.ptr(a, f16), st))
+            t = torch.empty_like(x)
+            conv(a, 32 * wide, 32, 32, c1, dims2, (1, 3, 3), 1, t, 32 * wide, 0, 32)
+            xn = torch.empty_like(x)
+            conv(t, 32 * wide, 32, 32, c2, dims2, (1, 3, 3), 0, xn, 32 * wide, 0, 32, res=x)
+            x = xn
+        capi.check(L.r3dp_mf_head_bcast(capi.ptr(x, f16), N, D, S, S, 32, 32 * wide, 32, capi.ptr(xf, f16), CF * wide, P0 + 32, CF, int(sp), st))
+        # fuser (7^3, no activation), mask logits (fp32), softmax + deformation, the occlusion pair
+        fx = torch.empty(N, D, S, S, 32 * wide, device=dev, dtype=f16)
+        conv(xf, CF * wide, CF, CF, wts.fuser, (N, D, S, S), (7, 7, 7), 0, fx, 32 * wide, 0, 32)
+        ls = (K + 2) // 2 * 2                                                           # K+1 logits per voxel, an even stride
+        logits = torch.empty(N, D, S, S, ls, device=dev)
+        conv(fx, 32 * wide, 32, 32, wts.mask, (N, D, S, S), (7, 7, 7), 0, logits, ls, 0, 0, out_f32=1)
+        deformation = torch.empty(N, D, S, S, 3, device=dev)
+        capi.check(L.r3dp_mf_deform(capi.ptr(logits), ls, capi.ptr(kp_s), capi.ptr(kp_d), N, K, D, S, S, capi.ptr(deformation), st))
+        occ = torch.empty(N, 1, S, S, device=dev)
+        occ2 = torch.empty(N, 1, S, S, device=dev)
+        capi.check(L.r3dp_mf_occlusion(capi.ptr(fx, f16), N, D, S, S, 32, 32 * wide, 32, int(sp), capi.ptr(wts.occ_w), capi.ptr(wts.occ_b), capi.ptr(occ),
+                                       capi.ptr(occ2), st))
+    return deformation, occ, occ2
+
+
 def hid_to_nchw(hid16: torch.Tensor, C: int, split: bool) -> torch.Tensor:
     """NHWC fp16 hid ([hi | lo] when split) -> [N,C,H,W] fp32."""
     N, H, W, cs = hid16.shape
@@ -185,9 +376,10 @@ def dilate(m: torch.Tensor, ksize: int) -> torch.Tensor:
 
 
 @torch.no_grad()
-def appearance(tm, torso_src_img: torch.Tensor, segmap: torch.Tensor) -> Dict[str, torch.Tensor]:
+def appearance(tm, torso_src_img: torch.Tensor, segmap: torch.Tensor, motion_wts: Optional['MotionWeights'] = None) -> Dict[str, torch.Tensor]:
     """What stage 1 derives from the reference torso image and the segmap alone (the per-clip part): the masked appearance volume
-    [N,32,16,64,64], the 64^2 torso segmap, the dilated torso mask, the motion estimator's appearance input, and the volume in NDHWC."""
+    [N,32,16,64,64], the 64^2 torso segmap, the dilated torso mask, the motion estimator's appearance input, and the volume in NDHWC.
+    motion_wts: also 'fc', the estimator's compressed source volume [N,16,64,64,4] fp32 (compress_volume)."""
     hp = _hp(tm)
     src = torso_src_img
     if hp.get('torso_inp_mode', 'rgb') == 'rgb_alpha':
@@ -199,22 +391,30 @@ def appearance(tm, torso_src_img: torch.Tensor, segmap: torch.Tensor) -> Dict[st
     if hp.get('mul_torso_mask', True):
         feats = feats * mask.unsqueeze(1)
     motion_inp = torch.cat([feats, seg64.unsqueeze(2).repeat([1, 1, feats.shape[2], 1, 1])], dim=1)
-    return {'feats': feats, 'seg64': seg64, 'mask': mask, 'motion_inp': motion_inp, 'fs_ndhwc': feats.permute(0, 2, 3, 4, 1).contiguous()}
+    out = {'feats': feats, 'seg64': seg64, 'mask': mask, 'motion_inp': motion_inp, 'fs_ndhwc': feats.permute(0, 2, 3, 4, 1).contiguous()}
+    if motion_wts is not None:
+        out['fc'] = compress_volume(motion_wts, motion_inp)
+    return out
 
 
 class TorsoWarper:
     """WarpBasedTorsoModelMediaPipe.forward (model2.py:222-287, eval) around the caller's module `tm`, stage 2 on the kernels.
-    `app`: the output of appearance() for this clip (per-clip cache), or None to compute it per call."""
+    `app`: the output of appearance() for this clip (per-clip cache), or None to compute it per call.  `motion_wts`: run the
+    motion_field_estimator on the kernels (motion()) instead of calling the caller's module."""
 
     def __init__(self, tm: torch.nn.Module):
         self.tm = tm
         self._eye = None
 
     @torch.no_grad()
-    def __call__(self, wts: Stage2Weights, torso_src_img, segmap, kp_s, kp_d, tgt_head_img, tgt_head_weights, app: Optional[Dict] = None):
+    def __call__(self, wts: Stage2Weights, torso_src_img, segmap, kp_s, kp_d, tgt_head_img, tgt_head_weights, app: Optional[Dict] = None,
+                 motion_wts: Optional[MotionWeights] = None):
         tm, hp = self.tm, _hp(self.tm)
         if app is None:
-            app = appearance(tm, torso_src_img, segmap)
+            app = appearance(tm, torso_src_img, segmap, motion_wts)
+        elif motion_wts is not None and 'fc' not in app:
+            # a clip begun before torso_motion='cuda' was set: its cached volume lacks the compressed source; add it to the cache once
+            app['fc'] = compress_volume(motion_wts, app['motion_inp'])
         B = kp_s.shape[0]
         motion_inp = app['motion_inp']
         if motion_inp.shape[0] != B:
@@ -225,7 +425,10 @@ class TorsoWarper:
         kp_s, kp_d = kp_s[:, KP_IDX[kp_num], :], kp_d[:, KP_IDX[kp_num], :]
         if self._eye is None or self._eye.shape[0] != B or self._eye.device != kp_s.device:
             self._eye = torch.eye(3, 3, device=kp_s.device).unsqueeze(0).repeat([B, 1, 1])          # Rs = Rd = I, made once
-        deformation, occlusion, occlusion_2 = tm.motion_field_estimator(motion_inp, kp_s, kp_d, self._eye, self._eye, tgt_head_img, tgt_head_weights)
+        if motion_wts is not None:
+            deformation, occlusion, occlusion_2 = motion(motion_wts, app['fc'], kp_s, kp_d, tgt_head_img, tgt_head_weights)
+        else:
+            deformation, occlusion, occlusion_2 = tm.motion_field_estimator(motion_inp, kp_s, kp_d, self._eye, self._eye, tgt_head_img, tgt_head_weights)
         # the reference's gradient-scaling blend (model2.py:251-257); kept so the values are the reference's bits
         deformation = deformation * 0.1 + deformation.detach() * 0.9
         occlusion = occlusion * 0.1 + occlusion.detach() * 0.9
