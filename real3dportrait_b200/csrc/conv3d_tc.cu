@@ -43,16 +43,6 @@ struct Conv3dArgs {
 // byte offset of 16-byte chunk j of row r in a K-major tile of 64-byte rows, 64-byte swizzle (cute Swizzle<2,4,3>)
 __device__ __forceinline__ uint32_t sw64(int r, int j) { return (uint32_t)(r * 64 + ((j ^ ((r >> 1) & 3)) << 4)); }
 
-// K-major, 64-byte-swizzled operand tile (cute::GMMA::GmmaDescriptor, layout SWIZZLE_64B = 2): 8-row groups 512 B apart
-__device__ __forceinline__ uint64_t gmma_desc_sw64(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3ffff) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(512 >> 4) << 32;
-    d |= (uint64_t)2 << 62;
-    return d;
-}
-
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool ok) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(ok ? 16 : 0) : "memory");
 }

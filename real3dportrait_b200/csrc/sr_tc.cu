@@ -59,7 +59,8 @@ struct ConvArgs {
 // The design cuts the operand fill traffic and the per-tile overheads:
 //   * an input ROW STRIP {64 ch, 130 px} is loaded once per 64-channel chunk and serves all horizontal taps (the wgmma smem
 //     descriptor starts 128 B x shift later; the 128-byte swizzle is a function of the ABSOLUTE smem address, so the descriptor's
-//     base_offset stays 0) and the R output rows that touch it vertically;
+//     base_offset stays 0) and the R output rows that touch it vertically; launches with at most 32 real input channels use {32 ch, 130 px}
+//     strips and {32 ch, 128 couts} taps in the 64-byte swizzle instead (Cfg3<32>), so no MMA runs on the zero-padded channels;
 //   * every weight tile {64 ch, 128 couts} of a tap is used by R MMA groups before it is released;
 //   * persistent CTAs;
 //   * the four output-parity phases of a transposed conv are units of ONE launch;
@@ -67,7 +68,7 @@ struct ConvArgs {
 //     256-channel layer stay in registers (block0's ToRGB is fused like the last layer's).
 // Two mbarrier rings (A strips, B taps) are filled by one TMA lane in exactly the order the consumer warpgroups use them.
 // =====================================================================================================================
-constexpr int A2_ROWS = 130, A2_BYTES = A2_ROWS * 128, A2_SLOT = 17408;       // 17 x 1024: every slot keeps the swizzle alignment
+constexpr int A2_ROWS = 130, A2_SLOT = 17408;                                // 17 x 1024: every slot keeps the swizzle alignment
 struct Taps2 {
     int n, ngroups;                 // taps sorted by (dy, dx); group = taps sharing dy
     int dyi[9], shift[9], widx[9];  // group index, horizontal shift (dx + 1, in pixels: strips start at x0 - 1), weight tap index
@@ -156,27 +157,36 @@ __device__ __forceinline__ void store_half32(__half* dst, const float* f) {
 constexpr int kConvRows = 2;                                                 // output rows per tile
 constexpr int kThreads3 = 384;                                               // TMA warpgroup + 2 consumer warpgroups
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;                       // 128 x 40 + 256 x 232 <= 64 K registers
-constexpr int B3_BYTES = BN * BK * 2;                                        // 128 couts x 64 ch fp16 = 16 KB
+// KC = channels per K chunk: 64 (128-byte rows, SWIZZLE_128B), or 32 for launches with at most 32 real input channels (64-byte rows,
+// SWIZZLE_64B: the boxes read the first 32 channels of each 64-channel pixel, so no MMA runs on the zero padding).
+template <int KC>
 struct Cfg3 {
     // ring depths: what the 227 KB of shared memory leave.  A 3x3 chunk needs kConvRows + 2 = 4 strips and 3 x 3 taps, so 6-deep rings let
-    // the producer fill the next chunk while the current one drains.
-    static constexpr int NA = 6, NB = 6;
+    // the producer fill the next chunk while the current one drains; the half-size slots of KC = 32 allow 8 strips and 16 taps.
+    static constexpr int ROW = KC * 2;                                       // bytes per pixel row of a strip / per cout row of a tap
+    static constexpr int A_BYTES = A2_ROWS * ROW, A_SLOT = KC == BK ? A2_SLOT : (A_BYTES + 1023) / 1024 * 1024;
+    static constexpr int B_BYTES = BN * ROW;
+    static constexpr int NA = KC == BK ? 6 : 8, NB = KC == BK ? 6 : 16;
     static constexpr int TAIL = 8192;                                        // barriers, bias, ToRGB weights
     static constexpr int STAGE = 8 * 8 * BN * 2;                             // fp16 store staging: 8 consumer warps x 8 px x 128 couts
-    static constexpr int SMEM = NA * A2_SLOT + NB * B3_BYTES + 1024 + TAIL + STAGE;
+    static constexpr int SMEM = NA * A_SLOT + NB * B_BYTES + 1024 + TAIL + STAGE;
+    static_assert(KC == BK || KC == 32, "conv_tc3: 64- or 32-channel chunks");
+    static_assert(SMEM <= 227 * 1024, "conv_tc3: shared memory over the sm_90 per-block limit");
+    static_assert(2 * (NA + NB) * 8 <= 512, "conv_tc3: ring barriers overlap the bias");
 };
-static_assert(Cfg3::SMEM <= 227 * 1024, "conv_tc3: shared memory over the sm_90 per-block limit");
+template <int KC>
+__device__ __forceinline__ uint64_t conv_desc(uint32_t saddr) { return KC == BK ? gmma_desc_sw128(saddr) : gmma_desc_sw64(saddr); }
 
-template <bool SPLIT>
+template <bool SPLIT, int KC>
 __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                const __grid_constant__ CUtensorMap tmB, const Conv2Args a) {
-    using C = Cfg3;
+    using C = Cfg3<KC>;
     constexpr int R = kConvRows;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = align_smem_1024(smem_raw);
     uint8_t* a_ring = smem;
-    uint8_t* b_ring = smem + C::NA * A2_SLOT;
-    uint8_t* tail = b_ring + C::NB * B3_BYTES;
+    uint8_t* b_ring = smem + C::NA * C::A_SLOT;
+    uint8_t* tail = b_ring + C::NB * C::B_BYTES;
     uint64_t* a_full = reinterpret_cast<uint64_t*>(tail);
     uint64_t* a_empty = a_full + C::NA;
     uint64_t* b_full = a_empty + C::NA;
@@ -230,19 +240,20 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
                     for (int kq = 0; kq < K3; ++kq) {
                         const int kc = kq < 2 * a.k_chunks ? kq : kq - 2 * a.k_chunks;    // activation chunk: hi, lo (at k_chunks + c), hi again
                         const int kb = kq < a.k_chunks ? kq : kq - a.k_chunks;            // weight chunk: hi, hi, lo (at k_chunks + c)
+                        // chunk c starts at channel 64 c for both widths: KC = 32 has one chunk per half (channels [0, 32) of hi, and of lo at 64)
                         for (int d = 0; d < DY; ++d) {
                             const int s_lo = d == 0 ? 0 : R - 1 + d, s_hi = R - 1 + d;
                             for (int s = s_lo; s <= s_hi; ++s, ++aq) {
                                 const int slot = aq % C::NA;
                                 mbar_wait(&a_empty[slot], ((aq / C::NA) & 1) ^ 1);
-                                mbar_expect_tx(&a_full[slot], A2_BYTES);
-                                tma_load_4d(a_ring + slot * A2_SLOT, &tmA, &a_full[slot], kc * BK, col0 - 1, row0 + tp.dy_min + s, n);
+                                mbar_expect_tx(&a_full[slot], C::A_BYTES);
+                                tma_load_4d(a_ring + slot * C::A_SLOT, &tmA, &a_full[slot], kc * BK, col0 - 1, row0 + tp.dy_min + s, n);
                             }
                             for (int t = tp.gstart[d]; t < tp.gstart[d + 1]; ++t, ++bq) {
                                 const int slot = bq % C::NB;
                                 mbar_wait(&b_empty[slot], ((bq / C::NB) & 1) ^ 1);
-                                mbar_expect_tx(&b_full[slot], B3_BYTES);
-                                tma_load_4d(b_ring + slot * B3_BYTES, &tmB, &b_full[slot], kb * BK, nblk * BN, tp.widx[t], wn);
+                                mbar_expect_tx(&b_full[slot], C::B_BYTES);
+                                tma_load_4d(b_ring + slot * C::B_BYTES, &tmB, &b_full[slot], kb * BK, nblk * BN, tp.widx[t], wn);
                             }
                         }
                     }
@@ -334,15 +345,15 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
                         for (int t = tp.gstart[d]; t < tp.gstart[d + 1]; ++t, ++bq) {
                             const int bslot = bq % C::NB;
                             mbar_wait(&b_full[bslot], (bq / C::NB) & 1);
-                            const uint64_t db = gmma_desc_sw128(smem_u32(b_ring + bslot * B3_BYTES));
+                            const uint64_t db = conv_desc<KC>(smem_u32(b_ring + bslot * C::B_BYTES));
                             const int sh = tp.shift[t];
                             const uint32_t first = (uint32_t)(kc | t);
                             uint64_t da[R];
 #pragma unroll
-                            for (int j = 0; j < R; ++j) da[j] = gmma_desc_sw128(smem_u32(a_ring + ((a_base + j + d) % C::NA) * A2_SLOT) + 128 * (64 * wg + sh));
+                            for (int j = 0; j < R; ++j) da[j] = conv_desc<KC>(smem_u32(a_ring + ((a_base + j + d) % C::NA) * C::A_SLOT) + C::ROW * (64 * wg + sh));
                             wg_fence();
 #pragma unroll
-                            for (int k = 0; k < BK / 16; ++k) {
+                            for (int k = 0; k < KC / 16; ++k) {
 #pragma unroll
                                 for (int j = 0; j < R; ++j) wgmma_m64n128k16(acc[j], da[j] + (uint64_t)(2 * k), db + (uint64_t)(2 * k), first | (uint32_t)k);
                             }
@@ -838,24 +849,24 @@ static EncodeTiledFn encode_fn() {
 }
 
 // fp16 tensor [d3][d2][d1][d0] (d0 innermost, dense), box {64, box1, 1, 1}, 128-byte swizzle, zero fill outside
-static int make_map_4d_box(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t d3, uint32_t box1);
-static int make_map_4d(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t d3, uint32_t box1) {
-    return make_map_4d_box(m, ptr, d0, d1, d2, d3, box1);
-}
-static int make_map_4d_box(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t d3, uint32_t box1) {
+// box0 = 64 channels: 128-byte swizzle; box0 = 32: 64-byte swizzle (the KC = 32 conv operands)
+static int make_map_4d_box(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t d3, uint32_t box1, uint32_t box0 = 64) {
     EncodeTiledFn fn = encode_fn();
     R3DP_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled is not available from the driver");
     cuuint64_t dims[4] = {d0, d1, d2, d3};
     cuuint64_t strides[3] = {d0 * 2, d0 * d1 * 2, d0 * d1 * d2 * 2};
-    cuuint32_t box[4] = {64, box1, 1, 1};
+    cuuint32_t box[4] = {box0, box1, 1, 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                    box0 == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     R3DP_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with CUresult %d (dims %llu x %llu x %llu x %llu)", (int)r,
                  (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2, (unsigned long long)d3);
     return 0;
 }
 
+// 128-byte L2 promotion: a box row is 128 B (one 64-channel group) of a pixel that is 2 or 4 such groups wide, and the other groups are read by
+// work items far away in the schedule; 256-byte promotion fetched the neighbouring group from DRAM too, and it was evicted before its use.
 static int make_map_fir(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t d3, uint32_t box_rows) {
     EncodeTiledFn fn = encode_fn();
     R3DP_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled is not available from the driver");
@@ -864,15 +875,15 @@ static int make_map_fir(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d
     cuuint32_t box[4] = {64, (cuuint32_t)FIR_BW, box_rows, 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     R3DP_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (FIR) failed with CUresult %d", (int)r);
     return 0;
 }
 
-static int launch_conv2(const void* x, int N, int H, int W, int Cp, const void* wp, int Nw, int O, const ConvArgs& a1, cudaStream_t st);
-static int launch_upconv2(const void* x, int N, int H, int W, int Cp, const void* wp, int Nw, int O, __half* yb, const float* bias, int split, cudaStream_t st);
-static int launch_conv(const void* x, int N, int H, int W, int Cp, const void* wp, int Nw, int O, ConvArgs a, cudaStream_t st) {
-    return launch_conv2(x, N, H, W, Cp, wp, Nw, O, a, st);
+static int launch_conv2(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int O, const ConvArgs& a1, cudaStream_t st);
+static int launch_upconv2(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int O, __half* yb, const float* bias, int split, cudaStream_t st);
+static int launch_conv(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int O, ConvArgs a, cudaStream_t st) {
+    return launch_conv2(x, N, H, W, I, wp, Nw, O, a, st);
 }
 
 // ---- optional in-library timing of the conv launches (bench.py's roofline): CUDA events on the launching stream around each launch --------
@@ -886,15 +897,15 @@ static void prof_mark(cudaStream_t st) {
 
 static unsigned long long* g_debug_buf = nullptr;
 static int g_debug_launch = 0;
-template <bool SPLIT>
+template <bool SPLIT, int KC>
 static int launch_conv3_s(const CUtensorMap& tmA, const CUtensorMap& tmB, Conv2Args a, int max_rows, cudaStream_t st) {
-    R3DP_CUDA(cudaFuncSetAttribute(conv_tc3_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg3::SMEM));
+    R3DP_CUDA(cudaFuncSetAttribute(conv_tc3_kernel<SPLIT, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg3<KC>::SMEM));
     a.debug = g_debug_buf ? g_debug_buf + 24 * (g_debug_launch++ % 32) : nullptr;
     a.row_groups = (max_rows + kConvRows - 1) / kConvRows;
     a.total_units = a.n_images * a.n_phases * a.row_groups * a.tiles_x;
     const int grid = a.total_units < sm_count() ? a.total_units : sm_count();
     prof_mark(st);
-    conv_tc3_kernel<SPLIT><<<grid, kThreads3, Cfg3::SMEM, st>>>(tmA, tmB, a);
+    conv_tc3_kernel<SPLIT, KC><<<grid, kThreads3, Cfg3<KC>::SMEM, st>>>(tmA, tmB, a);
     R3DP_LAUNCH_CHECK();
     prof_mark(st);
     count_launches(1);
@@ -922,11 +933,14 @@ static void fill_taps2(Taps2& t2, const Taps& t) {
     t2.gstart[t2.ngroups] = n;
 }
 
-static int run_conv2(const void* x, int N, int H, int W, int Cp, const void* wp, int Nw, int O, Conv2Args& a, int max_rows, cudaStream_t st, int n_taps = 9) {
+// I = the real input channels; x and wp hold them padded to Cp = I rounded up to 64.  I <= 32 runs the 32-channel K chunks (KC = 32).
+static int run_conv2(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int O, Conv2Args& a, int max_rows, cudaStream_t st, int n_taps = 9) {
     CUtensorMap tmA, tmB;
+    const int Cp = (I + 63) / 64 * 64;
+    const bool kc32 = I <= 32;
     const uint64_t Cphys = (uint64_t)Cp * (a.split ? 2 : 1);                      // split: [hi | lo] halves of Cp channels each
-    if (make_map_4d_box(&tmA, x, Cphys, (uint64_t)W, (uint64_t)H, (uint64_t)N, A2_ROWS)) return 1;
-    if (make_map_4d_box(&tmB, wp, Cphys, (uint64_t)O, (uint64_t)n_taps, (uint64_t)Nw, BN)) return 1;
+    if (make_map_4d_box(&tmA, x, Cphys, (uint64_t)W, (uint64_t)H, (uint64_t)N, A2_ROWS, kc32 ? 32 : BK)) return 1;
+    if (make_map_4d_box(&tmB, wp, Cphys, (uint64_t)O, (uint64_t)n_taps, (uint64_t)Nw, BN, kc32 ? 32 : BK)) return 1;
     if (a.split) { a.acc_scale = 1.0f / kSplitWeightScale; a.lo_off = a.out_C; a.out_C *= 2; }
     else { a.acc_scale = 1.0f; a.lo_off = 0; }
     // W = 64 (the torso warper's 64^2 maps): one tile per row whose right half reads TMA zero fill and stores nothing (the stores check out_W)
@@ -934,11 +948,12 @@ static int run_conv2(const void* x, int N, int H, int W, int Cp, const void* wp,
     { static int mixv = -1; if (mixv < 0) { const char* e = getenv("R3DP_TC_MIX"); mixv = (e && e[0] == '0') ? 0 : 1; } a.phase_mix = mixv; }      // A/B knob
     if (a.act_gain == 0.f) { a.act_slope = 0.2f; a.act_gain = 1.4142135623730951f; }      // default: bias_act lrelu
     R3DP_REQUIRE(a.n_blocks >= 1 && a.n_blocks <= 2, "conv_tc3: 128 or 256 output channels");
-    return a.split ? launch_conv3_s<true>(tmA, tmB, a, max_rows, st) : launch_conv3_s<false>(tmA, tmB, a, max_rows, st);
+    if (kc32) return a.split ? launch_conv3_s<true, 32>(tmA, tmB, a, max_rows, st) : launch_conv3_s<false, 32>(tmA, tmB, a, max_rows, st);
+    return a.split ? launch_conv3_s<true, BK>(tmA, tmB, a, max_rows, st) : launch_conv3_s<false, BK>(tmA, tmB, a, max_rows, st);
 }
 
 // v1-style single-phase description -> v2 launch
-static int launch_conv2(const void* x, int N, int H, int W, int Cp, const void* wp, int Nw, int O, const ConvArgs& a1, cudaStream_t st) {
+static int launch_conv2(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int O, const ConvArgs& a1, cudaStream_t st) {
     Conv2Args a = {};
     a.n_phases = 1;
     fill_taps2(a.ph[0].taps, a1.taps);
@@ -946,11 +961,11 @@ static int launch_conv2(const void* x, int N, int H, int W, int Cp, const void* 
     a.mode = a1.mode; a.out = a1.out; a.out_H = a1.out_H; a.out_W = a1.out_W; a.out_C = a1.out_C; a.oy_mul = a1.oy_mul; a.ox_mul = a1.ox_mul;
     a.bias = a1.bias; a.wrgb = a1.wrgb; a.brgb = a1.brgb; a.img_prev = a1.img_prev; a.img_out = a1.img_out; a.img_H = a1.out_H; a.img_W = a1.out_W;
     a.out_clamp = a1.out_clamp; a.img_out_u8 = a1.img_out_u8; a.split = a1.split;
-    return run_conv2(x, N, H, W, Cp, wp, Nw, O, a, a1.rows, st);
+    return run_conv2(x, N, H, W, I, wp, Nw, O, a, a1.rows, st);
 }
 
 // all four output-parity phases of the stride-2 transposed conv in ONE persistent launch (raw fp16 result on the (2H+1)x(2W+1) grid)
-static int launch_upconv2(const void* x, int N, int H, int W, int Cp, const void* wp, int Nw, int O, __half* yb, const float* bias, int split, cudaStream_t st) {
+static int launch_upconv2(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int O, __half* yb, const float* bias, int split, cudaStream_t st) {
     Conv2Args a = {};
     a.n_phases = 4; a.split = split;
     for (int pa = 0; pa < 2; ++pa)
@@ -963,7 +978,7 @@ static int launch_upconv2(const void* x, int N, int H, int W, int Cp, const void
             P.rows = pa ? H : H + 1; P.oy_off = pa; P.ox_off = pb;
         }
     a.mode = kStoreRaw; a.out = yb; a.out_H = 2 * H + 1; a.out_W = 2 * W + 1; a.out_C = O; a.oy_mul = a.ox_mul = 2; a.bias = bias;
-    return run_conv2(x, N, H, W, Cp, wp, Nw, O, a, H + 1, st);
+    return run_conv2(x, N, H, W, I, wp, Nw, O, a, H + 1, st);
 }
 
 }  // namespace tc
@@ -1018,11 +1033,11 @@ static int layer_impl(const void* x_f16, const void* wp_f16, const float* bias, 
         for (int t = 0; t < 9; ++t) { a.taps.dy[t] = t / 3 - 1; a.taps.dx[t] = t % 3 - 1; a.taps.widx[t] = t; }
         a.tiles_x = W / BM; a.rows = H; a.mode = kStoreAct;
         a.out = reinterpret_cast<__half*>(y_f16); a.out_H = H; a.out_W = W; a.out_C = O; a.oy_mul = a.ox_mul = 1;
-        return launch_conv(x_f16, N, H, W, Ip, wp_f16, Nw, O, a, st);
+        return launch_conv(x_f16, N, H, W, I, wp_f16, Nw, O, a, st);
     }
     R3DP_REQUIRE(scratch, "sr_tc_layer: up=2 needs scratch");
     __half* yb = reinterpret_cast<__half*>(scratch);
-    if (launch_upconv2(x_f16, N, H, W, Ip, wp_f16, Nw, O, yb, bias, split, st)) return 1;
+    if (launch_upconv2(x_f16, N, H, W, I, wp_f16, Nw, O, yb, bias, split, st)) return 1;
     {
         R3DP_REQUIRE(Ip <= 256, "sr_tc_layer: up=2 supports at most 256 input channels");
         const int erows = split ? kEdgeRowsSplit : kEdgeRows;
@@ -1076,14 +1091,13 @@ static int last_layer_impl(const void* x_f16, const void* wp_f16, const float* b
                            r3dp_stream_t stream) {
     R3DP_REQUIRE(x_f16 && wp_f16 && bias && wrgb && brgb && (img_out || img_out_u8), "sr_tc_last_layer: null pointer");
     R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && W % BM == 0 && H % 2 == 0, "sr_tc_last_layer: bad shape");
-    const int Ip = (I + 63) / 64 * 64;
     ConvArgs a = {};
     a.bias = bias; a.wrgb = wrgb; a.brgb = brgb; a.img_prev = img_prev; a.img_out = img_out; a.img_out_u8 = img_out_u8; a.out_clamp = clamp || img_out_u8;
     a.split = split;
     a.taps.n = 9;
     for (int t = 0; t < 9; ++t) { a.taps.dy[t] = t / 3 - 1; a.taps.dx[t] = t % 3 - 1; a.taps.widx[t] = t; }
     a.tiles_x = W / BM; a.rows = H; a.mode = kToRgbFinal; a.out_H = H; a.out_W = W; a.out_C = BN; a.oy_mul = a.ox_mul = 1;
-    return launch_conv(x_f16, N, H, W, Ip, wp_f16, Nw, BN, a, as_stream(stream));
+    return launch_conv(x_f16, N, H, W, I, wp_f16, Nw, BN, a, as_stream(stream));
 }
 extern "C" int r3dp_sr_tc_last_layer_ex(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
                                         const float* img_prev, int N, int Nw, int I, int H, int W, float* img_out, uint8_t* img_out_u8, int clamp,
@@ -1133,7 +1147,6 @@ static int layer_torgb_impl(const void* x_f16, const void* wp_f16, const float* 
                             r3dp_stream_t stream) {
     R3DP_REQUIRE(x_f16 && wp_f16 && bias && wrgb && brgb && y_f16 && img_out, "sr_tc_layer_torgb: null pointer");
     R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && W % BM == 0 && O % BN == 0 && O <= 256 && H % 2 == 0, "sr_tc_layer_torgb: bad shape");
-    const int Ip = (I + 63) / 64 * 64;
     Conv2Args a = {};
     Taps t = {};
     t.n = 9;
@@ -1143,7 +1156,7 @@ static int layer_torgb_impl(const void* x_f16, const void* wp_f16, const float* 
     a.ph[0].rows = H; a.ph[0].oy_off = 0; a.ph[0].ox_off = 0;
     a.mode = kActRgb; a.out = reinterpret_cast<__half*>(y_f16); a.out_H = H; a.out_W = W; a.out_C = O; a.oy_mul = a.ox_mul = 1;
     a.bias = bias; a.wrgb = wrgb; a.brgb = brgb; a.img_prev = img_prev; a.img_out = img_out; a.img_H = H; a.img_W = W; a.split = split;
-    return run_conv2(x_f16, N, H, W, Ip, wp_f16, Nw, O, a, H, as_stream(stream));
+    return run_conv2(x_f16, N, H, W, I, wp_f16, Nw, O, a, H, as_stream(stream));
 }
 extern "C" int r3dp_sr_tc_layer_torgb(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
                                       const float* img_prev, int N, int Nw, int I, int O, int H, int W, void* y_f16, float* img_out,
@@ -1331,7 +1344,6 @@ static int layer_up_composed_impl(const void* x_f16, const void* wpc_f16, const 
                                   int W, void* y_f16, int split, r3dp_stream_t stream) {
     R3DP_REQUIRE(x_f16 && wpc_f16 && bias && y_f16, "sr_tc_layer_up_composed: null pointer");
     R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && W % BM == 0 && O % BN == 0 && O <= 256, "sr_tc_layer_up_composed: bad shape");
-    const int Ip = (I + 63) / 64 * 64;
     Conv2Args a = {};
     a.n_phases = 4;
     for (int ph = 0; ph < 4; ++ph) {
@@ -1343,7 +1355,7 @@ static int layer_up_composed_impl(const void* x_f16, const void* wpc_f16, const 
     }
     a.mode = kStoreAct; a.out = reinterpret_cast<__half*>(y_f16); a.out_H = 2 * H; a.out_W = 2 * W; a.out_C = O; a.oy_mul = a.ox_mul = 2;
     a.bias = bias; a.split = split;
-    return run_conv2(x_f16, N, H, W, Ip, wpc_f16, Nw, O, a, H, as_stream(stream), 36);
+    return run_conv2(x_f16, N, H, W, I, wpc_f16, Nw, O, a, H, as_stream(stream), 36);
 }
 extern "C" int r3dp_sr_tc_layer_up_composed(const void* x_f16, const void* wpc_f16, const float* bias, int N, int Nw, int I, int O, int H,
                                             int W, void* y_f16, r3dp_stream_t stream) {
@@ -1362,7 +1374,6 @@ extern "C" int r3dp_sr_tcx_layer_up_composed(const void* x_f16, const void* wpc_
 // act = max(v, v * slope) * gain, residual added after it
 static int conv_plain_launch(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
                              float slope, float gain, const void* residual_f16, void* y_f16, int split, r3dp_stream_t stream) {
-    const int Ip = (I + 63) / 64 * 64;
     Conv2Args a = {};
     Taps t = {};
     if (ksize == 3) { t.n = 9; for (int i = 0; i < 9; ++i) { t.dy[i] = i / 3 - 1; t.dx[i] = i % 3 - 1; t.widx[i] = i; } }
@@ -1374,7 +1385,7 @@ static int conv_plain_launch(const void* x_f16, const void* wp_f16, const float*
     a.act_slope = slope; a.act_gain = gain;
     a.residual = reinterpret_cast<const __half*>(residual_f16);
     a.split = split;
-    return run_conv2(x_f16, N, H, W, Ip, wp_f16, Nw, O, a, H, as_stream(stream));
+    return run_conv2(x_f16, N, H, W, I, wp_f16, Nw, O, a, H, as_stream(stream));
 }
 static int conv_res_impl(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
                          int act, const void* residual_f16, void* y_f16, int split, r3dp_stream_t stream) {
@@ -1411,7 +1422,6 @@ static int layer_torgb_noup_impl(const void* x_f16, const void* wp_f16, const fl
                                  r3dp_stream_t stream) {
     R3DP_REQUIRE(x_f16 && wp_f16 && bias && wrgb && brgb && y_f16 && img_out, "sr_tc_layer_torgb_noup: null pointer");
     R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && W % BM == 0 && O % BN == 0 && O <= 256, "sr_tc_layer_torgb_noup: bad shape");
-    const int Ip = (I + 63) / 64 * 64;
     Conv2Args a = {};
     Taps t = {};
     t.n = 9;
@@ -1422,7 +1432,7 @@ static int layer_torgb_noup_impl(const void* x_f16, const void* wp_f16, const fl
     a.mode = kActRgb; a.out = reinterpret_cast<__half*>(y_f16); a.out_H = H; a.out_W = W; a.out_C = O; a.oy_mul = a.ox_mul = 1;
     a.bias = bias; a.wrgb = wrgb; a.brgb = brgb; a.img_prev = img_prev; a.img_out = img_out; a.img_H = H; a.img_W = W; a.skip_same_res = 1;
     a.split = split;
-    return run_conv2(x_f16, N, H, W, Ip, wp_f16, Nw, O, a, H, as_stream(stream));
+    return run_conv2(x_f16, N, H, W, I, wp_f16, Nw, O, a, H, as_stream(stream));
 }
 extern "C" int r3dp_sr_tc_layer_torgb_noup(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
                                            const float* img_prev, int N, int Nw, int I, int O, int H, int W, void* y_f16, float* img_out,
@@ -1709,7 +1719,7 @@ static int tw_conv_up_nearest_impl(const void* x_f16, const void* wp_f16, const 
         }
     a.mode = kStoreAct; a.out = reinterpret_cast<__half*>(y_f16); a.out_H = 2 * H; a.out_W = 2 * W; a.out_C = O; a.oy_mul = a.ox_mul = 2;
     a.bias = bias; a.act_slope = slope; a.act_gain = 1.0f; a.split = split;
-    return run_conv2(x_f16, N, H, W, (I + 63) / 64 * 64, wp_f16, 1, O, a, H, as_stream(stream), 36);
+    return run_conv2(x_f16, N, H, W, I, wp_f16, 1, O, a, H, as_stream(stream), 36);
 }
 extern "C" int r3dp_tw_conv_up_nearest(const void* x_f16, const void* wp_f16, const float* bias, int N, int I, int O, int H, int W, float slope,
                                        void* y_f16, int split, r3dp_stream_t stream) {

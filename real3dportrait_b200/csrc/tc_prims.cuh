@@ -111,5 +111,15 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) {
     d |= (uint64_t)1 << 62;                      // SWIZZLE_128B
     return d;
 }
+// K-major, 64-byte-swizzled operand tile (layout SWIZZLE_64B = 2): rows of 64 B, 8-row groups 512 B apart.  Like the 128-byte form, the
+// swizzle is a function of the absolute address (512-byte aligned atoms): a start address 64 B x r or 32 B x k further selects row r / k-step k.
+__device__ __forceinline__ uint64_t gmma_desc_sw64(uint32_t saddr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((saddr & 0x3ffff) >> 4);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(512 >> 4) << 32;
+    d |= (uint64_t)2 << 62;
+    return d;
+}
 }  // namespace tc
 }  // namespace r3dp

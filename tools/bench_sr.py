@@ -6,7 +6,7 @@ The SR runs layer by layer through the library's C entry points, in the order sr
 (static) styles, so that every intermediate can be kept.  Kernel times are the device durations of torch.profiler's CUDA activity
 records, median over the iterations: the transposed conv, its edge column and its FIR pass are launched by one library call, so CUDA
 events around the calls could not split them.  The whole SR is also timed with CUDA events (median), in a run without the profiler.
-Per conv launch the script prints the MMA GFLOP issued for the valid output rows (input channels padded to 64, three products per
+Per conv launch the script prints the MMA GFLOP issued for the valid output rows (input channels padded to 64, 32 for block0.conv0, three products per
 multiply-add in tc_exact) and the TFLOP/s this gives.
 
 --dump DIR writes every layer's output of the last iteration as DIR/<mode>/<name>.npy.  R3DP_LIB selects the library file, so two
@@ -29,8 +29,8 @@ CONV_LAUNCHES = ('block0.conv0', 'block0.conv1+torgb', 'block1.conv0', 'block1.c
 
 
 def conv_gflop(B, split):
-    """MMA GFLOP of the four conv launches for the valid output rows (Cin padded to 64 as issued)."""
-    f = [4 * 9 * 128 * 128 * 256 * 64,                     # block0.conv0: 4 output parities x 9 FIR-composed taps on the 128^2 grid, Cin 32 -> 64
+    """MMA GFLOP of the four conv launches for the valid output rows (Cin padded to 64 as issued; block0.conv0 runs 32-channel K chunks)."""
+    f = [4 * 9 * 128 * 128 * 256 * 32,                     # block0.conv0: 4 output parities x 9 FIR-composed taps on the 128^2 grid, Cin 32
          9 * 256 * 256 * 256 * 256,                        # block0.conv1
          (6 * 257 + 3 * 256) * 256 * 128 * 256,            # block1.conv0: 4 + 2 taps on 257 rows, 2 + 1 taps on 256 rows, 256 columns
          9 * 512 * 512 * 128 * 128]                        # block1.conv1
