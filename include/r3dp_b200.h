@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define R3DP_ABI_VERSION 2
+#define R3DP_ABI_VERSION 3
 
 typedef void* r3dp_stream_t; /* cudaStream_t */
 
@@ -47,10 +47,6 @@ const char* r3dp_last_error(void);
 int r3dp_device_info(int* sm_count, int* cc_major, int* cc_minor);
 /* Running total of CUDA kernels this library has launched in the process (bench.py's `gpu_launches`). */
 unsigned long long r3dp_launch_count(void);
-/* A/B switches for profiling runs (same meaning as the R3DP_* environment variables, settable at run time):
- *   "render": 0 = streaming kernel for single-pass renders (default), 1 = CTA-per-ray-tile kernel;  "rs_d": 4 | 8 | 16 samples per ray and tile;
- *   "rs_prefetch": frames of planes the fused render streams DRAM -> L2 ahead of its gather (default 2, 0 = off) */
-int r3dp_set_option(const char* key, int value);
 /* Frame exchange of a sharded clip (inference/real3d_infer.py:515-521 collects the frames of a clip on one device): copy-engine peer copy of
  * `bytes` from `src` on device `src_device` to `dst` on device `dst_device` (e.g. a CUDA-IPC mapping of rank 0's clip buffer), enqueued on
  * `stream` (a stream of the CALLING device); no SM is used and nothing is synchronised. */
@@ -109,13 +105,13 @@ int r3dp_decode(const float* feat, int N, int K, int P, int C, const r3dp_mlp_t*
  * (uint8 0/1).  Batch-global quirks are reproduced per call: invalid rays inherit min/max of the valid ray starts
  * (renderer.py:123-126) and depth is clamped to the call-wide [min,max] sample depth (ray_marcher.py:50).
  * workspace: r3dp_render_workspace_bytes(N, M) bytes of scratch.
- * Kernels: single-pass renders (S_imp == 0) run the warp-specialised streaming kernel (render_stream.cu: gather, wgmma decoder and
- * ray march of consecutive 128-sample tiles overlap inside one persistent CTA per SM); importance renders run the CTA-per-ray-tile
- * kernel (render.cu).  Decoder arithmetic: the OSGDecoder GEMMs run on wgmma with every fp32 operand split into two fp16 halves (three
- * partial products, fp32 accumulation in TMEM) - fp32-grade results (rgb within 5e-6 of float64, tests/test_gpu_render_conformance.py); two-pass shapes whose
- * tiles do not fit use the fp32 CUDA-core decoder.  The prepared decoder operands live in the caller's `workspace`, so calls with
- * different decoders may run concurrently on different streams (each with its own workspace).
- * A/B knobs (read once per process): R3DP_RENDER=tile, R3DP_RS_D=4|8|16, R3DP_MLP=tc|smem|const (const keeps process-wide state). */
+ * Kernels, chosen from the arguments alone: single-pass renders (S_imp == 0) run the warp-specialised streaming kernel (render_stream.cu:
+ * gather, wgmma decoder and ray march of consecutive 128-sample tiles overlap inside one persistent CTA per SM); importance renders
+ * (S_imp > 0) run the CTA-per-ray-tile kernel (render.cu), with the wgmma decoder when each pass of a tile fits two 128-sample tiles
+ * and the fp32 CUDA-core decoder otherwise.  The wgmma decoder splits every fp32 operand into two fp16 halves (three partial products,
+ * fp32 accumulation in registers) - fp32-grade results (rgb within 5e-6 of float64, tests/test_gpu_render_conformance.py).  The prepared
+ * decoder operands live in the caller's `workspace`, so calls with different decoders may run concurrently on different streams (each
+ * with its own workspace). */
 size_t r3dp_render_workspace_bytes(int N, int M);
 
 /* Channels-last plane addressing, strides in floats: the C = 32 features of texel (plane p, row y, col x) of frame n start at
@@ -133,7 +129,7 @@ typedef struct r3dp_plane_layout {
     int depth, slice_stride;
 } r3dp_plane_layout_t;
 
-/* r3dp_render with explicit plane layouts and an optional SECOND plane set sampled at the same points and added to the first
+/* The render's arguments: explicit plane layouts and an optional SECOND plane set sampled at the same points and added to the first
  * (bilinear sampling is linear): `planes = cano_planes + secc_planes` (secc_img2plane.py:73-81) without the 75 MB/frame add. */
 typedef struct r3dp_render_args {
     const float* planes;  r3dp_plane_layout_t layout;
@@ -147,16 +143,9 @@ typedef struct r3dp_render_args {
     void* workspace; size_t workspace_bytes;
 } r3dp_render_args_t;
 int r3dp_render_ex(const r3dp_render_args_t* args, r3dp_stream_t stream);
-/* The kernel r3dp_render_ex runs for `args` under the current options: 0 = streaming kernel, 1 = CTA-per-ray-tile kernel with the
- * tensor-core decoder, 2 = CTA-per-ray-tile kernel with the CUDA-core decoder; -1 if `args` or its decoder is NULL.  Launches nothing. */
+/* The kernel r3dp_render_ex runs for `args`: 0 = streaming kernel, 1 = CTA-per-ray-tile kernel with the tensor-core decoder,
+ * 2 = CTA-per-ray-tile kernel with the CUDA-core decoder; -1 if `args` or its decoder is NULL.  Launches nothing. */
 int r3dp_render_path(const r3dp_render_args_t* args);
-
-int r3dp_render(const float* planes_cl, int N, int C, int H, int W,
-                const float* ray_o, const float* ray_d, const float* camera, int M, int res,
-                int S, int S_imp, float box_warp, int white_back,
-                const float* u_coarse, const float* u_fine, const r3dp_mlp_t* mlp,
-                float* rgb, float* depth, float* weights_sum, uint8_t* is_ray_valid,
-                void* workspace, size_t workspace_bytes, r3dp_stream_t stream);
 
 /* MipRayMarcher2.run_forward (ray_marcher.py:25-57) stand-alone: colors [N,M,S,C], sigmas [N,M,S,1],
  * depths [N,M,S,1] -> rgb [N,M,C], depth [N,M,1], weights [N,M,S-1,1].  workspace: 16 bytes. */

@@ -47,7 +47,6 @@ _SIGNATURES = {
     'r3dp_last_error': (C.c_char_p, []),
     'r3dp_device_info': (_I, [C.POINTER(_I)] * 3),
     'r3dp_launch_count': (C.c_ulonglong, []),
-    'r3dp_set_option': (_I, [C.c_char_p, _I]),
     'r3dp_peer_copy': (_I, [_P, _I, _P, _I, _Z, _P]),
     'r3dp_gen_rays': (_I, [_P, _P, _I, _I, _P, _P, _P]),
     'r3dp_planes_to_channels_last': (_I, [_P, _I, _I, _I, _I, _P, _P]),
@@ -58,7 +57,6 @@ _SIGNATURES = {
     'r3dp_run_model': (_I, [_P, _I, _I, _I, _I, _P, _I, _F, _M, _P, _P, _P]),
     'r3dp_decode': (_I, [_P, _I, _I, _I, _I, _M, _P, _P, _P]),
     'r3dp_render_workspace_bytes': (_Z, [_I, _I]),
-    'r3dp_render': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _I, _I, _I, _I, _F, _I, _P, _P, _M, _P, _P, _P, _P, _P, _Z, _P]),
     'r3dp_render_ex': (_I, [C.POINTER(RenderArgs), _P]),
     'r3dp_render_path': (_I, [C.POINTER(RenderArgs)]),
     'r3dp_ray_march': (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
@@ -146,7 +144,7 @@ def lib() -> C.CDLL:
         for name, (restype, argtypes) in _SIGNATURES.items():
             fn = getattr(L, name)          # AttributeError here = header and library out of sync
             fn.restype, fn.argtypes = restype, argtypes
-        if L.r3dp_abi_version() != 2:
+        if L.r3dp_abi_version() != 3:
             raise RuntimeError('libr3dp_b200.so ABI version mismatch')
         _lib = L
     return _lib

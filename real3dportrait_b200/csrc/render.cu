@@ -1,11 +1,10 @@
-// Fused volumetric renderer: ImportanceRenderer.forward with 'auto' limits (renderer.py:118-167) as three launches
+// Fused volumetric renderer: ImportanceRenderer.forward with 'auto' limits (renderer.py:118-167) as three launches after the set-up launch
 //   1. ray_limits_kernel   rays (given or generated from cameras) -> (t0,t1,valid) + call-wide min/max of valid t0
-//   2. render_kernel       depths -> tri-plane gather -> OSG decoder -> ray march [-> importance pass -> merge -> march]
+//   2. render_stream_kernel (single-pass renders, render_stream.cu) or render_kernel (two-pass importance renders):
+//                          depths -> tri-plane gather -> OSG decoder -> ray march [-> importance pass -> merge -> march]
 //   3. depth_clamp_kernel  NaN->inf, clamp depth to the call-wide [min,max] sample depth (ray_marcher.py:49-50)
 // plus gen_rays (RaySampler.forward) and a stand-alone ray marcher.
 #include "render_shared.cuh"
-#include <stdlib.h>
-#include <string>
 
 namespace r3dp {
 
@@ -35,9 +34,7 @@ __global__ void mlp_to_tc_kernel(const r3dp_mlp_t m, MlpTcImage* dst, RenderWs* 
     for (int i = tid; i < 48; i += nt) dst->b2[i] = i < kOut ? m.b2[i] : 0.f;
 }
 constexpr int kTcThreads = 256;                          // 2 warpgroups: warpgroup g takes rows [64 g, 64 g + 64) of every 128-sample tile
-constexpr int kTcMaxTiles = 3;                           // 128-sample tiles per pass
-constexpr int kTcA1Bytes = 51200;                        // 3 x 16 KB A1 tiles; later the [R*ST][33] fp32 decoded rows (<= 384 x 132 B)
-constexpr int kTcA2Bytes = 32768;                        // two 16 KB atoms; before the decode: tap descriptors [nsamp][16]; after: march scratch
+constexpr int kTcA2Bytes = 32768;                        // the two 16 KB A1 tiles of a pass; after layer 1, the two A2 atoms
 __device__ __forceinline__ void init_ws(RenderWs* ws) {
     ws->t0_min = 0xffffffffu; ws->t0_max = 0u; ws->d_min = 0xffffffffu; ws->d_max = 0u; ws->n_valid = 0u;
 }
@@ -104,15 +101,15 @@ __device__ __forceinline__ int ray_of(const RenderArgs& a, int tile, int r) {
     return tile * R + r;
 }
 
-// TC = false: decoder weights staged in smem, CUDA-core decoder, two samples per thread (odd shapes that do not fit the tensor-core tiles)
-// (the round-1 constant-bank decoder variants - process-wide state - were removed in round 2; git history keeps them)
-// TC = decoder on wgmma (single-pass renders with R*S <= 384; 256 threads, 2 CTAs/SM); see the MlpTcImage comment
+// Two-pass (importance) renders; single-pass renders run the streaming kernel of render_stream.cu.
+// TC = false: decoder weights staged in smem, CUDA-core decoder, two samples per thread (passes that do not fit the tensor-core tiles)
+// TC = decoder on wgmma (passes of R*max(S, S_imp) <= 256 samples; 256 threads, 2 CTAs/SM); see the MlpTcImage comment
 constexpr int kPfCtas = 32;                            // CTAs of a frame that issue its L2 prefetches
 template <int R, bool TC>
 __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_kernel(const RenderArgs a) {
     extern __shared__ __align__(16) float smem[];
     constexpr int kRenderThreads = TC ? kTcThreads : r3dp::kRenderThreads;     // shadows the namespace constant inside this kernel
-    const int ST = a.S + a.S_imp;                         // samples per ray after the optional importance pass
+    const int ST = a.S + a.S_imp;                         // samples per ray after the importance pass
     MlpSmem& mlp = *reinterpret_cast<MlpSmem*>(smem);
     float* rows = smem + sizeof(MlpSmem) / 4;               // [R*ST][kRow]   features -> (sigma, colours)
     float* dep = rows + R * ST * kRow;                     // [R*ST]          sample depths
@@ -120,34 +117,19 @@ __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_ke
     float* cdf = wts + R * ST;                             // [R*ST]          importance cdf
     float* rayf = cdf + R * ST;                            // [R][8]          ox oy oz dx dy dz t0 t1
     int* ord = reinterpret_cast<int*>(rayf + R * 8);       // [R*ST]          depth order of the merged samples
-    // TC layout (1024-aligned): [A1 tiles | decoded rows] [A2 atoms | tap descriptors | march scratch] [W image + biases] dep rayf
-    uint8_t* a1 = nullptr; uint8_t* a2 = nullptr; uint8_t* wimg = nullptr; float* dsc = nullptr; float* b1s = nullptr; float* b2s = nullptr;
-    // TC, two passes (importance sampling): the decoded rows of pass 1 must survive pass 2, so they get their own region (and hold the
-    // tap descriptors of the samples in flight, like the CUDA-core variants); A2 reuses the (by then consumed) A1 tiles instead:
-    //   [A1 tiles (2) = A2 atoms] [W image + biases] rows dep wts cdf rayf ord
-    const bool two_pass = TC && a.S_imp > 0;
+    // TC layout (1024-aligned): [A1 tiles (2) = A2 atoms] [W image + biases] rows dep wts cdf rayf ord
+    // The decoded rows of pass 1 must survive pass 2, so they get their own region (and hold the tap descriptors of the samples in flight,
+    // like the CUDA-core decoder); A2 reuses the (by then consumed) A1 tiles.
+    uint8_t* a1 = nullptr; uint8_t* a2 = nullptr; uint8_t* wimg = nullptr; float* b1s = nullptr; float* b2s = nullptr;
     if (TC) {
         a1 = tc::align_smem_1024(reinterpret_cast<uint8_t*>(smem));
-        if (!two_pass) {
-            a2 = a1 + kTcA1Bytes;
-            wimg = a2 + kTcA2Bytes;
-            rows = reinterpret_cast<float*>(a1);
-            dsc = reinterpret_cast<float*>(a2);                               // [nsamp][16]  (<= 24 KB)
-            wts = reinterpret_cast<float*>(a2 + 24576);                       // [R*ST]  march scratch (the atoms are dead by then)
-            cdf = wts + R * ST;
-            b1s = reinterpret_cast<float*>(wimg + 20480); b2s = b1s + kHidden;
-            dep = b2s + 48;
-            rayf = dep + R * ST;
-            ord = nullptr;
-        } else {
-            a2 = a1;
-            wimg = a1 + kTcA2Bytes;
-            b1s = reinterpret_cast<float*>(wimg + 20480); b2s = b1s + kHidden;
-            rows = b2s + 48;
-            dep = rows + R * ST * kRow; wts = dep + R * ST; cdf = wts + R * ST;
-            rayf = cdf + R * ST;
-            ord = reinterpret_cast<int*>(rayf + R * 8);
-        }
+        a2 = a1;
+        wimg = a1 + kTcA2Bytes;
+        b1s = reinterpret_cast<float*>(wimg + 20480); b2s = b1s + kHidden;
+        rows = b2s + 48;
+        dep = rows + R * ST * kRow; wts = dep + R * ST; cdf = wts + R * ST;
+        rayf = cdf + R * ST;
+        ord = reinterpret_cast<int*>(rayf + R * 8);
     }
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -222,8 +204,8 @@ __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_ke
             const float x = __fadd_rn(rf[0], __fmul_rn(d, rf[3]));
             const float y = __fadd_rn(rf[1], __fmul_rn(d, rf[4]));
             const float z = __fadd_rn(rf[2], __fmul_rn(d, rf[5]));
-            float* row = (TC && !two_pass) ? dsc + q * 16 : rows + (size_t)(r * ST + k) * kRow;
-            sample_desc(a.p0, a.H, a.W, pscale * x, pscale * y, pscale * z, row);       // 15 floats (tri-planes) | 27 (tri-grids: rows only)
+            float* row = rows + (size_t)(r * ST + k) * kRow;
+            sample_desc(a.p0, a.H, a.W, pscale * x, pscale * y, pscale * z, row);       // 15 floats (tri-planes) | 27 (tri-grids)
         }
         __syncthreads();
         // (2) gather: each warp takes 4 samples per iteration, 8 lanes x float4 per sample; the row's descriptor is read by all 8
@@ -233,9 +215,9 @@ __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_ke
             const int q = q4 + sub;
             if (q < nsamp) {
                 const int r = q / kn, k = k0 + (q - r * kn);
-                float* row = (TC && !two_pass) ? dsc + q * 16 : rows + (size_t)(r * ST + k) * kRow;
+                float* row = rows + (size_t)(r * ST + k) * kRow;
                 float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (a.p0.depth > 1) {                                    // tri-grids (never with the [nsamp][16] descriptor layout: see r3dp_render_ex)
+                if (a.p0.depth > 1) {                                    // tri-grids
                     float dg[27];
 #pragma unroll
                     for (int e = 0; e < 27; ++e) dg[e] = row[e];
@@ -291,7 +273,7 @@ __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_ke
             float h[32], hn[32];                                               // layer-1 accumulators of the current and the next tile
             tc::wg_fence();
             layer1(0, h);
-            if (two_pass && nt > 1) layer1(1, hn);                              // A2 overlays the A1 tiles: every layer-1 product is taken first
+            if (nt > 1) layer1(1, hn);                                         // A2 overlays the A1 tiles: every layer-1 product is taken first
             tc::wg_commit();
             tc::wg_wait<0>();
             tc::wg_fence_acc<32>(h); tc::wg_fence_acc<32>(hn);
@@ -323,11 +305,10 @@ __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_ke
                         }
                     }
                 }
-                if (!two_pass && t + 1 < nt) layer1(t + 1, hn);                 // A1 tile t+1 is read before the decoded rows of tile t overlay it
                 tc::wg_commit();
                 tc::wg_wait<0>();
-                tc::wg_fence_acc<24>(o); tc::wg_fence_acc<32>(hn);
-                __syncthreads();                                               // both warpgroups are done reading A2 and A1 tile t+1
+                tc::wg_fence_acc<24>(o);
+                __syncthreads();                                               // both warpgroups are done reading A2
                 // outputs of tile t: bias, sigma raw, colours through the scaled sigmoid
 #pragma unroll
                 for (int i = 0; i < 24; ++i) {
@@ -414,66 +395,62 @@ __global__ void __launch_bounds__(TC ? kTcThreads : kRenderThreads, 2) render_ke
 
     run_pass(0, a.S);
 
-    if (a.S_imp == 0) {
-        for (int r = warp; r < R; r += kWarps) march(r, a.S, nullptr, true, wts + r * ST, cdf + r * ST);
-    } else {
-        const int S = a.S, Ni = a.S_imp;
-        for (int r = warp; r < R; r += kWarps) {
-            float* w = wts + r * ST; float* cd = cdf + r * ST; float* dd = dep + r * ST;
-            march(r, S, nullptr, false, w, cd);                               // coarse weights w[0..S-2]
-            __syncwarp();
-            // renderer.py:245-247: max_pool1d(2,1,pad 1) -> avg_pool1d(2,1) -> +0.01 ; a_i, i = 0..S-2
-            // pdf over p_i = a_{i+1} + 1e-5, i = 0..S-4 ; cdf has S-2 entries (renderer.py:272-276)
-            float total = 0.f;
-            for (int i = 0; i < S - 3; ++i) {          // every lane computes the same serial sums (torch.cumsum order)
-                const int j = i + 1;                                         // index into a
-                const float m0 = fmaxf(w[j - 1], w[j]), m1 = fmaxf(w[j], w[j + 1]);   // 1 <= j <= S-3: no -inf padding reached
-                total += (0.5f * (m0 + m1) + 0.01f) + 1e-5f;
-            }
-            float run = 0.f;
-            if (lane == 0) cd[0] = 0.f;
-            for (int i = 0; i < S - 3; ++i) {
-                const int j = i + 1;
-                const float m0 = fmaxf(w[j - 1], w[j]), m1 = fmaxf(w[j], w[j + 1]);
-                run += __fdiv_rn((0.5f * (m0 + m1) + 0.01f) + 1e-5f, total);
-                if (lane == 0) cd[i + 1] = run;
-            }
-            __syncwarp();
-            const int ncdf = S - 2;
-            const int m_ray = ray_of<R>(a, tile, r);
-            for (int j = lane; j < Ni; j += 32) {
-                float dfine = 0.f;
-                if (m_ray < a.M) {
-                    const float u = a.u_fine[((size_t)n * a.M + m_ray) * Ni + j];
-                    int idx = 0;                                             // searchsorted(cdf, u, right=True)
-                    while (idx < ncdf && cd[idx] <= u) ++idx;
-                    const int lo = max(idx - 1, 0), hi = min(idx, S - 3);
-                    const float c_lo = cd[lo], c_hi = cd[hi];
-                    float den = c_hi - c_lo;
-                    if (den < 1e-5f) den = 1.0f;
-                    const float b_lo = 0.5f * (dd[lo] + dd[lo + 1]), b_hi = 0.5f * (dd[hi] + dd[hi + 1]);
-                    dfine = b_lo + __fdiv_rn(u - c_lo, den) * (b_hi - b_lo);
-                    dmin = fminf(dmin, dfine); dmax = fmaxf(dmax, dfine);
-                }
-                dd[S + j] = dfine;
-            }
+    const int S = a.S, Ni = a.S_imp;
+    for (int r = warp; r < R; r += kWarps) {
+        float* w = wts + r * ST; float* cd = cdf + r * ST; float* dd = dep + r * ST;
+        march(r, S, nullptr, false, w, cd);                                   // coarse weights w[0..S-2]
+        __syncwarp();
+        // renderer.py:245-247: max_pool1d(2,1,pad 1) -> avg_pool1d(2,1) -> +0.01 ; a_i, i = 0..S-2
+        // pdf over p_i = a_{i+1} + 1e-5, i = 0..S-4 ; cdf has S-2 entries (renderer.py:272-276)
+        float total = 0.f;
+        for (int i = 0; i < S - 3; ++i) {              // every lane computes the same serial sums (torch.cumsum order)
+            const int j = i + 1;                                             // index into a
+            const float m0 = fmaxf(w[j - 1], w[j]), m1 = fmaxf(w[j], w[j + 1]);   // 1 <= j <= S-3: no -inf padding reached
+            total += (0.5f * (m0 + m1) + 0.01f) + 1e-5f;
         }
-        __syncthreads();
-        run_pass(S, Ni);
-        // merge: stable rank of every sample among the ray's ST depths (== torch.sort order when depths are distinct)
-        for (int r = warp; r < R; r += kWarps) {
-            const float* dd = dep + r * ST; int* od = ord + r * ST;
-            for (int i = lane; i < ST; i += 32) {
-                // total order (torch.sort puts NaN last, -0 == +0): every sample gets a distinct rank even for NaN depths (degenerate
-                // cameras), so `ord` never holds an unwritten slot
-                const unsigned ki = sort_key(dd[i]);
-                int rank = 0;
-                for (int j = 0; j < ST; ++j) { const unsigned kj = sort_key(dd[j]); rank += (kj < ki) || (kj == ki && j < i); }
-                od[rank] = i;
-            }
-            __syncwarp();
-            march(r, ST, od, true, wts + r * ST, cdf + r * ST);
+        float run = 0.f;
+        if (lane == 0) cd[0] = 0.f;
+        for (int i = 0; i < S - 3; ++i) {
+            const int j = i + 1;
+            const float m0 = fmaxf(w[j - 1], w[j]), m1 = fmaxf(w[j], w[j + 1]);
+            run += __fdiv_rn((0.5f * (m0 + m1) + 0.01f) + 1e-5f, total);
+            if (lane == 0) cd[i + 1] = run;
         }
+        __syncwarp();
+        const int ncdf = S - 2;
+        const int m_ray = ray_of<R>(a, tile, r);
+        for (int j = lane; j < Ni; j += 32) {
+            float dfine = 0.f;
+            if (m_ray < a.M) {
+                const float u = a.u_fine[((size_t)n * a.M + m_ray) * Ni + j];
+                int idx = 0;                                                 // searchsorted(cdf, u, right=True)
+                while (idx < ncdf && cd[idx] <= u) ++idx;
+                const int lo = max(idx - 1, 0), hi = min(idx, S - 3);
+                const float c_lo = cd[lo], c_hi = cd[hi];
+                float den = c_hi - c_lo;
+                if (den < 1e-5f) den = 1.0f;
+                const float b_lo = 0.5f * (dd[lo] + dd[lo + 1]), b_hi = 0.5f * (dd[hi] + dd[hi + 1]);
+                dfine = b_lo + __fdiv_rn(u - c_lo, den) * (b_hi - b_lo);
+                dmin = fminf(dmin, dfine); dmax = fmaxf(dmax, dfine);
+            }
+            dd[S + j] = dfine;
+        }
+    }
+    __syncthreads();
+    run_pass(S, Ni);
+    // merge: stable rank of every sample among the ray's ST depths (== torch.sort order when depths are distinct)
+    for (int r = warp; r < R; r += kWarps) {
+        const float* dd = dep + r * ST; int* od = ord + r * ST;
+        for (int i = lane; i < ST; i += 32) {
+            // total order (torch.sort puts NaN last, -0 == +0): every sample gets a distinct rank even for NaN depths (degenerate
+            // cameras), so `ord` never holds an unwritten slot
+            const unsigned ki = sort_key(dd[i]);
+            int rank = 0;
+            for (int j = 0; j < ST; ++j) { const unsigned kj = sort_key(dd[j]); rank += (kj < ki) || (kj == ki && j < i); }
+            od[rank] = i;
+        }
+        __syncwarp();
+        march(r, ST, od, true, wts + r * ST, cdf + r * ST);
     }
 
     // call-wide min/max of the sample depths (ray_marcher.py:50)
@@ -517,21 +494,12 @@ static size_t render_smem_bytes(int R, int ST) {
     return sizeof(MlpSmem) + (size_t)R * ST * kRow * 4 + 3 * (size_t)R * ST * 4 + (size_t)R * 8 * 4 + (size_t)R * ST * 4;
 }
 
-static int mlp_variant() {                         // R3DP_MLP = tc (default) | smem: decoder variant, for A/B comparison
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("R3DP_MLP"); v = (e && e[0] == 's') ? 0 : 2; }
-    return v;
-}
-
 static size_t render_tc_smem(int R, int S, int S_imp) {
     const int ST = S + S_imp;
-    if (S_imp == 0) return 1024 + kTcA1Bytes + kTcA2Bytes + 20480 + (kHidden + 48) * 4 + (size_t)R * (S + 8) * 4;
     return 1024 + kTcA2Bytes + 20480 + (kHidden + 48) * 4 + (size_t)R * ST * (kRow + 4) * 4 + (size_t)R * 8 * 4;
 }
-// the tensor-core decoder needs its CTA tile to fit the A tiles: three 128-sample tiles for single-pass renders (decoded rows overlay
-// them), two per pass for importance renders; and two CTAs per SM (2 x 113 KB of shared memory)
+// the tensor-core decoder needs each pass of its CTA tile to fit the two 128-sample A tiles, and two CTAs per SM (2 x 113 KB of shared memory)
 static bool render_tc_fits(int R, int S, int S_imp) {
-    if (S_imp == 0) return R * S <= 128 * kTcMaxTiles && R * S * kRow * 4 <= kTcA1Bytes;
     const int per_pass = R * (S > S_imp ? S : S_imp);
     return per_pass <= 256 && render_tc_smem(R, S, S_imp) <= 113 * 1024;
 }
@@ -556,24 +524,18 @@ static int launch_render_v(const RenderArgs& a, cudaStream_t st) {
 }
 template <int R>
 static int launch_render(const RenderArgs& a, bool tc, cudaStream_t st) {
+    R3DP_REQUIRE(a.S_imp > 0, "render: the tile kernel runs two-pass renders only (S_imp = %d)", a.S_imp);
     return tc ? launch_render_tc<R>(a, st) : launch_render_v<R>(a, st);
-}
-
-int g_render_variant = -1;                         // R3DP_RENDER = stream (default for single-pass renders) | tile: A/B knob
-static int render_variant() {
-    if (g_render_variant < 0) { const char* e = getenv("R3DP_RENDER"); g_render_variant = (e && e[0] == 't') ? 1 : 0; }
-    return g_render_variant;
 }
 
 static int tile_rays(int ST) { return ST <= 48 ? 8 : ST <= 96 ? 4 : ST <= 192 ? 2 : 1; }     // rays per CTA of the tile kernel
 
-// The kernel a render runs (r3dp_render_ex dispatches on this, r3dp_render_path reports it): 0 = streaming kernel, 1 = tile kernel with the
-// tensor-core decoder, 2 = tile kernel with the smem-weights CUDA-core decoder (tiles that do not fit the wgmma layout); both tile decoders
-// keep the decoder in per-call storage
+// The kernel a render runs (r3dp_render_ex dispatches on this, r3dp_render_path reports it): 0 = streaming kernel (single-pass renders),
+// 1 = tile kernel with the tensor-core decoder (two-pass renders whose passes fit its tiles), 2 = tile kernel with the smem-weights
+// CUDA-core decoder (the other two-pass renders); both tile decoders keep the decoder in per-call storage
 static int render_path(const RenderArgs& a) {
-    if (render_variant() == 0 && mlp_variant() == 2 && render_stream_fits(a)) return 0;
-    const bool grid_single = a.p0.depth > 1 && a.S_imp == 0;      // tri-grid descriptors (27 floats) do not fit the single-pass [nsamp][16] layout
-    return mlp_variant() == 2 && !grid_single && render_tc_fits(tile_rays(a.S + a.S_imp), a.S, a.S_imp) ? 1 : 2;
+    if (a.S_imp == 0) return 0;
+    return render_tc_fits(tile_rays(a.S + a.S_imp), a.S, a.S_imp) ? 1 : 2;
 }
 
 // the fields of the kernel arguments that follow from the caller's argument block alone (not from the workspace)
@@ -605,16 +567,6 @@ extern "C" int r3dp_gen_rays(const float* cam2world, const float* intrinsics, in
     count_launches(1);
     R3DP_LAUNCH_CHECK();
     return 0;
-}
-
-extern "C" int r3dp_set_option(const char* key, int value) {
-    R3DP_REQUIRE(key != nullptr, "set_option: null key");
-    const std::string k(key);
-    if (k == "render") { R3DP_REQUIRE(value == 0 || value == 1, "set_option: render = 0 (stream) | 1 (tile)"); g_render_variant = value; return 0; }
-    if (k == "rs_d") { R3DP_REQUIRE(value == 4 || value == 8 || value == 16, "set_option: rs_d = 4 | 8 | 16"); g_rs_chunk_log2 = value == 4 ? 2 : (value == 16 ? 4 : 3); return 0; }
-    if (k == "rs_prefetch") { R3DP_REQUIRE(value >= 0 && value <= 64, "set_option: rs_prefetch = frames of L2 look-ahead (0 = off)"); g_rs_prefetch = value; return 0; }
-    R3DP_REQUIRE(false, "set_option: unknown key '%s'", key);
-    return 1;
 }
 
 extern "C" size_t r3dp_render_workspace_bytes(int N, int M) {
@@ -667,15 +619,14 @@ extern "C" int r3dp_render_ex(const r3dp_render_args_t* g, r3dp_stream_t stream)
     char* wsb = reinterpret_cast<char*>(g->workspace);
     RenderWs* ws = reinterpret_cast<RenderWs*>(wsb);
     float2* limits = reinterpret_cast<float2*>(wsb + kWsLimitsOff);
-    if (mlp_variant() == 2) mlp_to_tc_kernel<<<4, 256, 0, st>>>(*g->mlp, reinterpret_cast<MlpTcImage*>(wsb + kWsImageOff), ws);      // + workspace header
-    else init_ws_kernel<<<1, 1, 0, st>>>(ws);
+    mlp_to_tc_kernel<<<4, 256, 0, st>>>(*g->mlp, reinterpret_cast<MlpTcImage*>(wsb + kWsImageOff), ws);      // + workspace header
     const int total = N * M;
     ray_limits_kernel<<<(total + 255) / 256, 256, 0, st>>>(g->ray_o, g->ray_d, g->camera, res, N, M, g->box_warp, limits, g->is_ray_valid, ws);
     R3DP_LAUNCH_CHECK();
 
     RenderArgs a = render_args(g);
     a.image = reinterpret_cast<const MlpTcImage*>(wsb + kWsImageOff); a.limits = limits; a.ws = ws;
-    a.lookahead = render_lookahead();
+    a.lookahead = kRenderLookahead;
     int rc;
     const int path = render_path(a);
     if (path == 0) {
@@ -698,20 +649,6 @@ extern "C" int r3dp_render_ex(const r3dp_render_args_t* g, r3dp_stream_t stream)
 extern "C" int r3dp_render_path(const r3dp_render_args_t* g) {
     if (g == nullptr || g->mlp == nullptr) { set_error("render_path: null argument block or decoder"); return -1; }
     return render_path(render_args(g));
-}
-
-extern "C" int r3dp_render(const float* planes_cl, int N, int C, int H, int W, const float* ray_o, const float* ray_d,
-                           const float* camera, int M, int res, int S, int S_imp, float box_warp, int white_back,
-                           const float* u_coarse, const float* u_fine, const r3dp_mlp_t* mlp, float* rgb, float* depth,
-                           float* weights_sum, uint8_t* is_ray_valid, void* workspace, size_t workspace_bytes,
-                           r3dp_stream_t stream) {
-    r3dp_render_args_t g = {};
-    g.planes = planes_cl; g.N = N; g.C = C; g.H = H; g.W = W;
-    g.layout.frame_stride = 3ll * H * W * C; g.layout.plane_stride = H * W * C; g.layout.row_stride = W * C; g.layout.texel_stride = C;
-    g.ray_o = ray_o; g.ray_d = ray_d; g.camera = camera; g.M = M; g.res = res; g.S = S; g.S_imp = S_imp; g.box_warp = box_warp;
-    g.white_back = white_back; g.u_coarse = u_coarse; g.u_fine = u_fine; g.mlp = mlp; g.rgb = rgb; g.depth = depth;
-    g.weights_sum = weights_sum; g.is_ray_valid = is_ray_valid; g.workspace = workspace; g.workspace_bytes = workspace_bytes;
-    return r3dp_render_ex(&g, stream);
 }
 
 extern "C" int r3dp_ray_march(const float* colors, const float* sigmas, const float* depths, int N, int M, int S, int C,

@@ -1,5 +1,5 @@
 // Structures shared by the two fused-render translation units:
-//   render.cu         entry points, limits / clamp kernels, the CTA-per-ray-tile kernel (two-pass importance renders, odd shapes)
+//   render.cu         entry points, limits / clamp kernels, the CTA-per-ray-tile kernel (two-pass importance renders)
 //   render_stream.cu  the warp-specialised streaming kernel (single-pass renders: gather || wgmma decode || march overlap)
 #pragma once
 #include "render_core.cuh"
@@ -236,11 +236,10 @@ __device__ __forceinline__ unsigned sort_key(float d) {
     return f2ord(d == 0.f ? 0.f : d);
 }
 
+// frames of planes streamed DRAM -> L2 ahead of the gather (RenderArgs::lookahead; 0, 1 and 4 measured, DESIGN.md §4 "Retired switches")
+constexpr int kRenderLookahead = 2;
+
 // render_stream.cu
-extern int g_rs_chunk_log2;      // A/B knob (r3dp_set_option / R3DP_RS_D)
-extern int g_rs_prefetch;        // frames of L2 look-ahead of the streaming kernel (r3dp_set_option / R3DP_RS_PREFETCH)
-bool render_stream_fits(const RenderArgs& a);
 int launch_render_stream(const RenderArgs& a, cudaStream_t st);
-int render_lookahead();
 
 }  // namespace r3dp

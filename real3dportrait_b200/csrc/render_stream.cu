@@ -16,13 +16,12 @@
 //               for the marcher; L2 look-ahead prefetch of the next frames' planes
 // Decoder arithmetic is the split-fp16 scheme of render_shared.cuh (fp32-grade results).
 #include "render_shared.cuh"
-#include <stdlib.h>
 
 namespace r3dp {
-int g_rs_chunk_log2 = -1;
-int g_rs_prefetch = -1;                                           // frames of L2 look-ahead (0 = off); r3dp_set_option("rs_prefetch") / R3DP_RS_PREFETCH
 namespace rs {
 
+constexpr int kLog2D = 3;                                       // D = 8 samples per ray and tile, G = 16 rays per item (DESIGN.md §4.1)
+                                                                // (D = 4 and 16 measured, DESIGN.md §4 "Retired switches")
 constexpr int kGatherWarps = 8;
 // warps 0-3 decode (the warpgroup that issues the MMAs and holds their accumulators), 4-7 march, 8-15 gather.  512 threads leave 128
 // registers per thread, enough for the gather warps to keep all twelve 16-byte loads of a sample in flight
@@ -369,46 +368,24 @@ __global__ void __launch_bounds__(kThreads, 1) render_stream_kernel(const Render
     }
 }
 
-static int chunk_log2() {                          // R3DP_RS_D = 4 | 8 | 16: depth samples per ray and tile (rays per item = 128 / D); A/B knob
-    if (g_rs_chunk_log2 < 0) { const char* e = getenv("R3DP_RS_D"); const int d = e ? atoi(e) : 8; g_rs_chunk_log2 = d == 4 ? 2 : (d == 16 ? 4 : 3); }
-    return g_rs_chunk_log2;
-}
-
-template <int LOG2D, bool GRID>
+template <bool GRID>
 static int launch(RenderArgs a, cudaStream_t st) {
-    constexpr int G = 128 >> LOG2D;
+    constexpr int G = 128 >> kLog2D;
     const bool image = a.res > 0 && a.res * a.res == a.M && (a.res % G) == 0;
     a.tile_cols = image ? a.res : 0;
     const int items_per_frame = (a.M + G - 1) / G;
     const int total = a.N * items_per_frame;
-    R3DP_CUDA(cudaFuncSetAttribute(render_stream_kernel<LOG2D, GRID>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+    R3DP_CUDA(cudaFuncSetAttribute(render_stream_kernel<kLog2D, GRID>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
     const int grid = total < sm_count() ? total : sm_count();
-    render_stream_kernel<LOG2D, GRID><<<grid, kThreads, kSmem, st>>>(a, items_per_frame, total);
+    render_stream_kernel<kLog2D, GRID><<<grid, kThreads, kSmem, st>>>(a, items_per_frame, total);
     R3DP_LAUNCH_CHECK();
     return 0;
 }
 
 }  // namespace rs
 
-bool render_stream_fits(const RenderArgs& a) {
-    if (a.S_imp != 0 || a.S < 2) return false;
-    if (a.p1.base && (a.p1.plane_stride != a.p0.plane_stride || a.p1.row_stride != a.p0.row_stride || a.p1.texel_stride != a.p0.texel_stride ||
-                      a.p1.depth != a.p0.depth || a.p1.slice_stride != a.p0.slice_stride)) return false;
-    return true;
-}
-
-int render_lookahead() {                           // R3DP_RS_PREFETCH = frames of planes streamed into L2 ahead of the gather (default 2, 0 = off)
-    if (g_rs_prefetch < 0) { const char* e = getenv("R3DP_RS_PREFETCH"); g_rs_prefetch = e ? atoi(e) : 2; if (g_rs_prefetch < 0) g_rs_prefetch = 0; }
-    return g_rs_prefetch;
-}
-
 int launch_render_stream(const RenderArgs& a, cudaStream_t st) {
-    if (a.p0.depth > 1) return rs::launch<3, true>(a, st);                      // tri-grids: D = 8 chunks only
-    switch (rs::chunk_log2()) {
-        case 2: return rs::launch<2, false>(a, st);
-        case 4: return rs::launch<4, false>(a, st);
-        default: return rs::launch<3, false>(a, st);
-    }
+    return a.p0.depth > 1 ? rs::launch<true>(a, st) : rs::launch<false>(a, st);
 }
 
 }  // namespace r3dp

@@ -3,7 +3,6 @@
 //   triplane_sample           sample_from_planes (renderer.py:65-75): the HBM-roofline gather, write-dominated
 //   run_model                 ImportanceRenderer.run_model (renderer.py:169-188): gather + OSG decoder
 #include "render_shared.cuh"
-#include <stdlib.h>
 
 namespace r3dp {
 
@@ -88,11 +87,12 @@ __global__ void __launch_bounds__(256, 3) trigrid_sample_kernel(const float* __r
 // 8 lanes x float4 = one 128-byte texel line per tap, ALL twelve 16-byte loads of a point issued before the first use, streaming stores
 // (the output is never re-read here).  The coordinates of the next chunk are requested before this chunk's taps.
 // Earlier forms: descriptors recomputed by all 8 lanes of a point + loads split into dependent groups at 64
-// registers -> 59 % of the HBM peak with 60 % issue-active; MINB = resident CTAs per SM the register allocation targets.
-template <int MINB>
-__global__ void __launch_bounds__(256, MINB) triplane_sample_kernel(const float* __restrict__ planes, int N, int H, int W,
-                                                                    const float* __restrict__ coords, int P, float scale,
-                                                                    float* __restrict__ out) {
+// registers -> 59 % of the HBM peak with 60 % issue-active.  The register allocation targets kSampleCtas resident CTAs per SM (2 and 4 measured,
+// DESIGN.md §4 "Retired switches").
+constexpr int kSampleCtas = 3;
+__global__ void __launch_bounds__(256, kSampleCtas) triplane_sample_kernel(const float* __restrict__ planes, int N, int H, int W,
+                                                                           const float* __restrict__ coords, int P, float scale,
+                                                                           float* __restrict__ out) {
     __shared__ __align__(16) float s_desc[8][32][16];           // per warp: [point][off0 off1 off2 frame | 4 weights x 3 planes]
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, sub = lane >> 3, cq = lane & 7;
     const long long NP = (long long)N * P, n_chunks = (NP + 31) / 32;
@@ -265,18 +265,9 @@ extern "C" int r3dp_triplane_sample(const float* planes_cl, int N, int C, int H,
     R3DP_REQUIRE(C == kC, "triplane_sample: C must be %d (got %d)", kC, C);
     R3DP_REQUIRE(N > 0 && P > 0 && H > 0 && W > 0 && box_warp > 0.f, "triplane_sample: bad shape");
     const long long chunks = ((long long)N * P + 31) / 32;          // one warp-chunk = 32 consecutive points
-    long long need = (chunks + 7) / 8;
-    static int minb = -1;                          // R3DP_SAMPLE_MINB = 2 | 3 | 4 (register/occupancy trade-off: A/B knob)
-    if (minb < 0) { const char* e = getenv("R3DP_SAMPLE_MINB"); minb = e ? atoi(e) : 3; if (minb < 2 || minb > 4) minb = 3; }
-    const long long cap = (long long)sm_count() * minb;
+    const long long need = (chunks + 7) / 8, cap = (long long)sm_count() * kSampleCtas;
     const unsigned blocks = (unsigned)(need < cap ? need : cap);
-    const float sc = 2.0f / box_warp;
-    cudaStream_t st = as_stream(stream);
-    switch (minb) {
-        case 2: triplane_sample_kernel<2><<<blocks, 256, 0, st>>>(planes_cl, N, H, W, coords, P, sc, out); break;
-        case 4: triplane_sample_kernel<4><<<blocks, 256, 0, st>>>(planes_cl, N, H, W, coords, P, sc, out); break;
-        default: triplane_sample_kernel<3><<<blocks, 256, 0, st>>>(planes_cl, N, H, W, coords, P, sc, out); break;
-    }
+    triplane_sample_kernel<<<blocks, 256, 0, as_stream(stream)>>>(planes_cl, N, H, W, coords, P, 2.0f / box_warp, out);
     R3DP_LAUNCH_CHECK();
     return 0;
 }

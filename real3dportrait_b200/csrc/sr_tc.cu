@@ -93,7 +93,6 @@ struct Conv2Args {
     uint8_t* img_out_u8;            // non-null: final image as uint8 HWC frames [N][H][W][3] = int((clamp(x)+1)/2*255) (real3d_infer.py:519) instead of fp32 NCHW
     int split;                      // fp32-grade operands: activations [hi | lo] (2 x Cin_pad channels), weights [hi | lo]; K loop = hi*hi + lo*hi + hi*lo
     int lo_off;                     // split: channel offset of the lo half in the OUTPUT tensor (= logical output channels); out_C is the physical pixel stride
-    int phase_mix;                  // interleave the phases of a multi-phase launch over the units (see decode)
     float acc_scale;                // accumulator scale applied before the bias (split weights are stored x 2^10 so their lo halves stay normal fp16)
     unsigned long long* debug;      // R3DP_TC_DEBUG_TIMING builds: [acc wait, strip wait, tap wait, issue, total, #CTAs] clock sums of the MMA warp
 };
@@ -215,7 +214,7 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
     // Multi-phase launches with an even number of x blocks (the 4/2/2/1-tap phases of a transposed conv at W = 256): phases are interleaved,
     // slot = rg * n_phases + p' with ph = (p' + rg) mod n_phases, so that at any moment the CTAs are spread over all phases (the 1- and
     // 2-tap phases need more operand bandwidth per MMA than the 4-tap phase) and every CTA sees every phase.
-    const bool mix = a.phase_mix && a.n_phases > 1 && (a.tiles_x & 1) == 0;
+    const bool mix = a.n_phases > 1 && (a.tiles_x & 1) == 0;
     auto decode = [&](int unit, int& n, int& ph, int& row0, int& col0) {
         n = unit / units_per_image; int r = unit - n * units_per_image;
         const int xb = r % a.tiles_x; r /= a.tiles_x;
@@ -945,7 +944,6 @@ static int run_conv2(const void* x, int N, int H, int W, int I, const void* wp, 
     else { a.acc_scale = 1.0f; a.lo_off = 0; }
     // W = 64 (the torso warper's 64^2 maps): one tile per row whose right half reads TMA zero fill and stores nothing (the stores check out_W)
     a.k_chunks = Cp / BK; a.tiles_x = (W + BM - 1) / BM; a.n_blocks = O / BN; a.n_images = N; a.w_shared = (Nw == 1);
-    { static int mixv = -1; if (mixv < 0) { const char* e = getenv("R3DP_TC_MIX"); mixv = (e && e[0] == '0') ? 0 : 1; } a.phase_mix = mixv; }      // A/B knob
     if (a.act_gain == 0.f) { a.act_slope = 0.2f; a.act_gain = 1.4142135623730951f; }      // default: bias_act lrelu
     R3DP_REQUIRE(a.n_blocks >= 1 && a.n_blocks <= 2, "conv_tc3: 128 or 256 output channels");
     if (kc32) return a.split ? launch_conv3_s<true, 32>(tmA, tmB, a, max_rows, st) : launch_conv3_s<false, 32>(tmA, tmB, a, max_rows, st);

@@ -1,7 +1,7 @@
 """ImportanceRenderer — host mirror of modules/eg3ds/volumetric_rendering/renderer.py:30-297.
 
 `forward` keeps the reference signature and return tuple; the whole body (box limits, stratified depths, tri-plane
-gather, OSG decoder, ray march, importance resampling, merge) is ONE fused CUDA call (r3dp_render).  Jitter uniforms
+gather, OSG decoder, ray march, importance resampling, merge) is ONE fused CUDA call (r3dp_render_ex).  Jitter uniforms
 are drawn here with torch.rand in the reference's order and shapes ([N,M,S,1] then [N*M,S_imp]; renderer.py:226,281), so
 `torch.manual_seed` reproduces runs exactly as it does for the reference; tests may instead pass them explicitly through
 rendering_options['u_coarse'] / ['u_fine']."""

@@ -18,7 +18,7 @@ def test_library_builds_and_exports_every_declared_symbol():
     missing = [s for s in declared if not hasattr(L, s)]
     assert not missing, missing
     assert set(declared) == set(_capi._SIGNATURES), set(declared) ^ set(_capi._SIGNATURES)
-    assert L.r3dp_abi_version() == 2
+    assert L.r3dp_abi_version() == 3
 
 
 def test_state_dict_layout_matches_reference_checkpoints():

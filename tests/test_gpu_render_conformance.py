@@ -1,8 +1,8 @@
 """The fused render against float64 (tests/render_reference.py) at bars that tell the split-fp16 decoder from plain fp16, on every kernel
 r3dp_render_ex can pick:
-  path 0  the streaming kernel (render_stream.cu; rs_d = 4, 8, 16),
-  path 1  the CTA-per-ray-tile kernel with the wgmma decoder (render.cu, single-pass and two-pass),
-  path 2  the CTA-per-ray-tile kernel with the CUDA-core decoder (tiles the wgmma layout does not fit, tri-grids in single-pass tile renders).
+  path 0  the streaming kernel (render_stream.cu; single-pass renders),
+  path 1  the CTA-per-ray-tile kernel with the wgmma decoder (render.cu; two-pass renders whose passes fit its tiles),
+  path 2  the CTA-per-ray-tile kernel with the CUDA-core decoder (the other two-pass renders).
 Every case asserts the path it is meant to cover (r3dp_render_path), and the module checks that all three were covered.
 
 (a) decoder probe: rays along exactly (0, 0, -1) through a plane set whose planes 1 and 2 are zero give every sample of a ray the same
@@ -13,7 +13,6 @@ Every case asserts the path it is meant to cover (r3dp_render_path), and the mod
 (d) every call: nothing outside the outputs is written and every output element is written (sentinel-filled allocations); frames are
     independent of each other and a repeated render gives the same bits."""
 import ctypes as C
-import os
 
 import pytest
 import torch
@@ -31,29 +30,6 @@ PAD = 1024
 
 
 # ---- calling the renderer ---------------------------------------------------------------------------------------------------------------
-def _env_defaults():
-    """The options the library starts with (R3DP_RENDER / R3DP_RS_D, read as render.cu and render_stream.cu read them)."""
-    rs_d = os.environ.get('R3DP_RS_D', '8')
-    return (1 if os.environ.get('R3DP_RENDER', '').startswith('t') else 0), (int(rs_d) if rs_d in ('4', '16') else 8)
-
-
-class _Opt:
-    """r3dp_set_option for the duration of a `with` block; restores the process defaults afterwards."""
-
-    def __init__(self, render=0, rs_d=8):
-        self.render, self.rs_d = render, rs_d
-
-    def __enter__(self):
-        L = capi.lib()
-        capi.check(L.r3dp_set_option(b'render', self.render)); capi.check(L.r3dp_set_option(b'rs_d', self.rs_d))
-
-    def __exit__(self, *exc):
-        L = capi.lib()
-        render, rs_d = _env_defaults()
-        capi.check(L.r3dp_set_option(b'render', render)); capi.check(L.r3dp_set_option(b'rs_d', rs_d))
-        return False
-
-
 def _canary(n, dtype):
     if dtype == torch.uint8:
         buf = torch.full((n + 2 * PAD,), 0xA5, dtype=torch.uint8, device=DEV)
@@ -130,15 +106,14 @@ def camera_rays(camera, res):
 
 
 # ---- (a) decoder probe --------------------------------------------------------------------------------------------------------------------
-PROBE_PATHS = [  # (id, render option, rs_d, S, S_imp, path)
-    ('stream_d4', 0, 4, 13, 0, 0), ('stream_d8', 0, 8, 13, 0, 0), ('stream_d16', 0, 16, 13, 0, 0),
-    ('tile_tc_single', 1, 8, 13, 0, 1), ('tile_tc_two_pass', 0, 8, 12, 12, 1), ('tile_cuda_core', 0, 8, 33, 15, 2)]
+PROBE_PATHS = [  # (id, S, S_imp, path)
+    ('stream_d8', 13, 0, 0), ('tile_tc_two_pass', 12, 12, 1), ('tile_cuda_core', 33, 15, 2)]
 WORST = {}
 
 
 @pytest.mark.parametrize('scale', [1.0, 8.0, 1e-3])
-@pytest.mark.parametrize('pid,variant,rs_d,S,S_imp,path', PROBE_PATHS, ids=[p[0] for p in PROBE_PATHS])
-def test_decoder_probe_element_bound(pid, variant, rs_d, S, S_imp, path, scale):
+@pytest.mark.parametrize('pid,S,S_imp,path', PROBE_PATHS, ids=[p[0] for p in PROBE_PATHS])
+def test_decoder_probe_element_bound(pid, S, S_imp, path, scale):
     N, M = 1, 4096
     planes = rr.probe_planes(N, 64, 48, scale, seed=3)
     o, d = rr.probe_rays(N, M, seed=5)
@@ -149,8 +124,7 @@ def test_decoder_probe_element_bound(pid, variant, rs_d, S, S_imp, path, scale):
     u_f = torch.rand(N * M, S_imp, generator=g) if S_imp else None
     worst = 0.0
     for name, mlp in rr.decoder_set():
-        with _Opt(variant, rs_d):
-            rgb, _, wsum, valid = render(planes, mlp, S, S_imp, o=o, d=d, res=64, u_c=u_c, u_f=u_f, path=path)
+        rgb, _, wsum, valid = render(planes, mlp, S, S_imp, o=o, d=d, res=64, u_c=u_c, u_f=u_f, path=path)
         assert bool(valid.all()) and float(wsum.min()) > 0.5
         c_got = ((rgb.double() + 1) / 2) / wsum.double()
         cref, _ = rr.decode64(f, mlp)
@@ -181,34 +155,32 @@ def _compare(got, ref, tau_rgb, tag):
     assert e_rgb <= tau_rgb and e_w <= rr.TAU_WSUM and e_d <= rr.TAU_DEPTH, tag
 
 
-# (id, N, M, S, S_imp, H, W, decoder, kwargs, {render option: path})
+# (id, N, M, S, S_imp, H, W, decoder, kwargs, path)
 E2E = [
-    ('ragged_3x100_s7', 3, 100, 7, 0, 20, 36, 'opaque_s4', {}, {0: 0, 1: 1}),
-    ('ragged_imp_24_9', 2, 37, 24, 9, 48, 16, 'opaque_s11', {}, {0: 1}),
-    ('imp_48_48', 2, 64, 48, 48, 32, 32, 'opaque_s4', {}, {0: 1}),
-    ('s4_m5_2x2_box2', 1, 5, 4, 0, 2, 2, 'opaque_s4', {'box': 2.0}, {0: 0, 1: 1}),
-    ('s9_odd_h2_w3', 2, 70, 9, 0, 2, 3, 'opaque_s11', {}, {0: 0, 1: 1}),
-    ('imp_32_16_tiles256', 1, 50, 32, 16, 9, 7, 'opaque_s4', {}, {0: 1}),
-    ('imp_33_15_fallback', 1, 50, 33, 15, 9, 7, 'opaque_s4', {}, {0: 2}),
-    ('imp_st384', 1, 20, 192, 192, 16, 16, 'opaque_s11', {}, {0: 1}),
-    ('single_s384', 1, 9, 384, 0, 16, 16, 'opaque_s4', {'miss': False}, {0: 0, 1: 1}),
-    ('x4_single', 2, 80, 21, 0, 24, 24, 'opaque_s5_x4', {}, {0: 0, 1: 1}),
-    ('x005_imp', 1, 64, 16, 16, 24, 24, 'opaque_s23_x0.05', {}, {0: 1}),
-    ('white_back_imp', 2, 40, 12, 12, 16, 16, 'opaque_s4', {'wb': True}, {0: 1}),
+    ('ragged_3x100_s7', 3, 100, 7, 0, 20, 36, 'opaque_s4', {}, 0),
+    ('ragged_imp_24_9', 2, 37, 24, 9, 48, 16, 'opaque_s11', {}, 1),
+    ('imp_48_48', 2, 64, 48, 48, 32, 32, 'opaque_s4', {}, 1),
+    ('s4_m5_2x2_box2', 1, 5, 4, 0, 2, 2, 'opaque_s4', {'box': 2.0}, 0),
+    ('s9_odd_h2_w3', 2, 70, 9, 0, 2, 3, 'opaque_s11', {}, 0),
+    ('imp_32_16_tiles256', 1, 50, 32, 16, 9, 7, 'opaque_s4', {}, 1),
+    ('imp_33_15_fallback', 1, 50, 33, 15, 9, 7, 'opaque_s4', {}, 2),
+    ('imp_st384', 1, 20, 192, 192, 16, 16, 'opaque_s11', {}, 1),
+    ('single_s384', 1, 9, 384, 0, 16, 16, 'opaque_s4', {'miss': False}, 0),
+    ('x4_single', 2, 80, 21, 0, 24, 24, 'opaque_s5_x4', {}, 0),
+    ('x005_imp', 1, 64, 16, 16, 24, 24, 'opaque_s23_x0.05', {}, 1),
+    ('white_back_imp', 2, 40, 12, 12, 16, 16, 'opaque_s4', {'wb': True}, 1),
 ]
 DECODERS = dict(rr.decoder_set())
 
 
-@pytest.mark.parametrize('cid,N,M,S,S_imp,H,W,dec,kw,paths', E2E, ids=[c[0] for c in E2E])
-def test_render_vs_float64(cid, N, M, S, S_imp, H, W, dec, kw, paths):
+@pytest.mark.parametrize('cid,N,M,S,S_imp,H,W,dec,kw,path', E2E, ids=[c[0] for c in E2E])
+def test_render_vs_float64(cid, N, M, S, S_imp, H, W, dec, kw, path):
     kw = dict(kw)
     planes, o, d, u_c, u_f = _ragged(N, M, S, S_imp, H, W, seed=len(cid) * 31 + S, miss=kw.pop('miss', True))
     mlp = DECODERS[dec]
     ref = rr.render64(planes, mlp, o, d, S=S, S_imp=S_imp, box_warp=kw.get('box', 1.0), white_back=kw.get('wb', False), u_coarse=u_c, u_fine=u_f)
-    for variant, path in paths.items():
-        with _Opt(variant):
-            got = render(planes, mlp, S, S_imp, o=o, d=d, u_c=u_c, u_f=u_f, path=path, **kw)
-        _compare(got, ref, rr.TAU_RGB, f'{cid} path {path}')
+    got = render(planes, mlp, S, S_imp, o=o, d=d, u_c=u_c, u_f=u_f, path=path, **kw)
+    _compare(got, ref, rr.TAU_RGB, f'{cid} path {path}')
 
 
 @pytest.mark.parametrize('S_imp', [0, 12])
@@ -223,17 +195,15 @@ def test_hwpc_view_and_two_plane_sets(S_imp):
     mlp = DECODERS['opaque_s4']
     ref = rr.render64(secc, mlp, o, d, S=S, S_imp=S_imp, u_coarse=u_c, u_fine=u_f, planes2=cano)
     ref1 = rr.render64(secc, mlp, o, d, S=S, S_imp=S_imp, u_coarse=u_c, u_fine=u_f)
-    paths = {0: 0, 1: 1} if S_imp == 0 else {0: 1}
-    for variant, path in paths.items():
-        with _Opt(variant):
-            got = render(secc, mlp, S, S_imp, o=o, d=d, u_c=u_c, u_f=u_f, planes2=cano, path=path)
-            hw = render(secc, mlp, S, S_imp, o=o, d=d, u_c=u_c, u_f=u_f, hwpc=True, path=path)
-        _compare(got, ref, rr.TAU_RGB, f'two sets S_imp={S_imp} path {path}')
-        _compare(hw, ref1, rr.TAU_RGB, f'hwpc S_imp={S_imp} path {path}')
+    path = 0 if S_imp == 0 else 1
+    got = render(secc, mlp, S, S_imp, o=o, d=d, u_c=u_c, u_f=u_f, planes2=cano, path=path)
+    hw = render(secc, mlp, S, S_imp, o=o, d=d, u_c=u_c, u_f=u_f, hwpc=True, path=path)
+    _compare(got, ref, rr.TAU_RGB, f'two sets S_imp={S_imp} path {path}')
+    _compare(hw, ref1, rr.TAU_RGB, f'hwpc S_imp={S_imp} path {path}')
 
 
-@pytest.mark.parametrize('D,S,S_imp,paths', [(2, 11, 0, {0: 0, 1: 2}), (4, 9, 6, {0: 1})])
-def test_trigrids_vs_float64(D, S, S_imp, paths):
+@pytest.mark.parametrize('D,S,S_imp,path', [(2, 11, 0, 0), (4, 9, 6, 1)])
+def test_trigrids_vs_float64(D, S, S_imp, path):
     N, M = 2, 90
     g = torch.Generator().manual_seed(D * 7 + S)
     grids = torch.randn(N, 3, 32 * D, 12, 10, generator=g)
@@ -242,10 +212,8 @@ def test_trigrids_vs_float64(D, S, S_imp, paths):
     u_f = torch.rand(N * M, S_imp, generator=g) if S_imp else None
     mlp = DECODERS['opaque_s11']
     ref = rr.render64(grids, mlp, o, d, S=S, S_imp=S_imp, u_coarse=u_c, u_fine=u_f, trigrid_depth=D)
-    for variant, path in paths.items():
-        with _Opt(variant):
-            got = render(grids, mlp, S, S_imp, o=o, d=d, u_c=u_c, u_f=u_f, depth=D, path=path)
-        _compare(got, ref, rr.TAU_RGB, f'trigrid D={D} S_imp={S_imp} path {path}')
+    got = render(grids, mlp, S, S_imp, o=o, d=d, u_c=u_c, u_f=u_f, depth=D, path=path)
+    _compare(got, ref, rr.TAU_RGB, f'trigrid D={D} S_imp={S_imp} path {path}')
 
 
 @pytest.mark.parametrize('S_imp,dec', [(0, 'opaque_s4'), (0, 'transparent'), (48, 'transparent'),
@@ -259,16 +227,15 @@ def test_baseline_config1_vs_float64(S_imp, dec):
     o, d = camera_rays(cam, 64)
     mlp = DECODERS[dec] if dec != 'transparent' else rr.transparent_decoder()
     ref = rr.render64(planes, mlp, o, d, S=48, S_imp=S_imp, u_coarse=u_c, u_fine=u_f)
-    for variant, path in ({0: 0, 1: 1} if S_imp == 0 else {0: 1}).items():
-        with _Opt(variant):
-            got = render(planes, mlp, 48, S_imp, camera=cam, res=64, u_c=u_c, u_f=u_f, path=path)
-        _compare(got, ref, rr.TAU_RGB, f'baseline S_imp={S_imp} {dec} path {path}')
+    path = 0 if S_imp == 0 else 1
+    got = render(planes, mlp, 48, S_imp, camera=cam, res=64, u_c=u_c, u_f=u_f, path=path)
+    _compare(got, ref, rr.TAU_RGB, f'baseline S_imp={S_imp} {dec} path {path}')
 
 
 @pytest.mark.parametrize('res', [24, 20])
 def test_camera_rays_white_back(res):
-    """In-kernel camera rays, white_back, some rays missing the box; res = 20 is not a multiple of the tile kernel's R = 8 nor of the
-    streaming kernel's G = 16 (non-image ray tiles), res = 24 is a multiple of R."""
+    """In-kernel camera rays, white_back, some rays missing the box; neither res is a multiple of the streaming kernel's G = 16 (non-image
+    ray groups)."""
     N, S = 3, 13
     cam = syn.make_cameras(N, seed=78)
     cam[1, 16] = cam[1, 20] = 1.5                                             # wide FOV: rays miss the box
@@ -279,10 +246,8 @@ def test_camera_rays_white_back(res):
     mlp = DECODERS['opaque_s11']
     ref = rr.render64(planes, mlp, o, d, S=S, white_back=True, u_coarse=u_c)
     assert 0 < int(ref[3].sum()) < ref[3].numel()
-    for variant, path in ((0, 0), (1, 1)):
-        with _Opt(variant):
-            got = render(planes, mlp, S, camera=cam, res=res, wb=True, u_c=u_c, path=path)
-        _compare(got, ref, rr.TAU_RGB, f'camera res={res} path {path}')
+    got = render(planes, mlp, S, camera=cam, res=res, wb=True, u_c=u_c, path=0)
+    _compare(got, ref, rr.TAU_RGB, f'camera res={res}')
 
 
 def test_every_ray_misses():
@@ -296,10 +261,8 @@ def test_every_ray_misses():
     mlp = rr.transparent_decoder()
     ref = rr.render64(planes, mlp, o, d, S=S, u_coarse=u_c)
     assert int(ref[3].sum()) == 0
-    for variant, path in ((0, 0), (1, 1)):
-        with _Opt(variant):
-            got = render(planes, mlp, S, o=o, d=d, u_c=u_c, path=path)
-        _compare(got, ref, rr.TAU_RGB, f'all miss path {path}')
+    got = render(planes, mlp, S, o=o, d=d, u_c=u_c, path=0)
+    _compare(got, ref, rr.TAU_RGB, 'all miss')
 
 
 # ---- (c) stand-alone ops --------------------------------------------------------------------------------------------------------------------
@@ -433,11 +396,11 @@ def test_ray_march_element_bound(opaque):
 
 
 # ---- (d) bit-exact properties ---------------------------------------------------------------------------------------------------------------
-FRAME_CASES = [(0, 13, 0, 0), (1, 13, 0, 1), (0, 12, 12, 1), (0, 33, 15, 2)]      # (render option, S, S_imp, path)
+FRAME_CASES = [(13, 0, 0), (48, 0, 0), (12, 12, 1), (33, 15, 2)]      # (S, S_imp, path)
 
 
-@pytest.mark.parametrize('variant,S,S_imp,path', FRAME_CASES)
-def test_frames_independent_and_repeatable(variant, S, S_imp, path):
+@pytest.mark.parametrize('S,S_imp,path', FRAME_CASES)
+def test_frames_independent_and_repeatable(S, S_imp, path):
     """Frame k of an N = 3 render equals the N = 1 render of frame k, and a repeated render gives the same bits.  Every ray hits the box:
     invalid rays take the call-wide limits (renderer.py:123-126), so with one of them the frames would rightly differ."""
     N, M = 3, 24 * 24
@@ -446,20 +409,19 @@ def test_frames_independent_and_repeatable(variant, S, S_imp, path):
     o[..., 2] = 1.6
     d = torch.nn.functional.normalize(torch.tensor([0.0, 0.0, -1.0]) + 0.02 * torch.randn(N, M, 3, generator=torch.Generator().manual_seed(S)), dim=-1)
     mlp = DECODERS['opaque_s4']
-    with _Opt(variant):
-        full = render(planes, mlp, S, S_imp, o=o, d=d, u_c=u_c, u_f=u_f, path=path)
-        again = render(planes, mlp, S, S_imp, o=o, d=d, u_c=u_c, u_f=u_f, path=path)
-        assert bool(full[3].all())
-        for a, b in zip(full, again):
-            assert torch.equal(a, b)
-        for k in range(N):
-            uf = u_f[k * M:(k + 1) * M] if u_f is not None else None
-            one = render(planes[k:k + 1], mlp, S, S_imp, o=o[k:k + 1], d=d[k:k + 1], u_c=u_c[k:k + 1], u_f=uf, path=path)
-            for a, b in zip(one, full):
-                assert torch.equal(a[0], b[k]), k
+    full = render(planes, mlp, S, S_imp, o=o, d=d, u_c=u_c, u_f=u_f, path=path)
+    again = render(planes, mlp, S, S_imp, o=o, d=d, u_c=u_c, u_f=u_f, path=path)
+    assert bool(full[3].all())
+    for a, b in zip(full, again):
+        assert torch.equal(a, b)
+    for k in range(N):
+        uf = u_f[k * M:(k + 1) * M] if u_f is not None else None
+        one = render(planes[k:k + 1], mlp, S, S_imp, o=o[k:k + 1], d=d[k:k + 1], u_c=u_c[k:k + 1], u_f=uf, path=path)
+        for a, b in zip(one, full):
+            assert torch.equal(a[0], b[k]), k
 
 
 def test_all_paths_covered():
     """The case tables of this module, each of whose renders asserts its path through r3dp_render_path, span all three paths."""
-    paths = {p[-1] for p in PROBE_PATHS} | {p for c in E2E for p in c[-1].values()} | {c[-1] for c in FRAME_CASES}
+    paths = {p[-1] for p in PROBE_PATHS} | {c[-1] for c in E2E} | {c[-1] for c in FRAME_CASES}
     assert paths == {0, 1, 2}, paths

@@ -1,10 +1,11 @@
-"""A/B timing of the fused render kernels on one GPU (BASELINE configs[1]: batch of 4 frames, 64x64 rays x 48 samples, render only).
+"""Timing of the fused render on one GPU (BASELINE configs[1]: batch of 4 frames, 64x64 rays x 48 samples, render only).
 
-    python tools/bench_render.py [--frames 4] [--pool 32] [--iters 30]
+    python tools/bench_render.py [--frames 4] [--pool 32] [--iters 30] [--fine 0 | 48]
 
-Prints one JSON line per variant: CUDA-event time per call of r3dp_render (limits + decoder image + render + clamp kernels) over a pool
-of resident frames larger than L2, for the streaming kernel at D = 4 | 8 | 16, the CTA-per-tile kernel, both plane layouts and the
-two-plane-set (cano + secc) mode.  Also checks that every variant returns the same image as the tile kernel."""
+Prints one JSON line per plane layout: CUDA-event time per call of r3dp_render_ex (limits + decoder image + render + clamp kernels) over
+a pool of resident frames larger than L2, for channels-last planes, the producer's channels_last view ('hwpc') and the two-plane-set
+(cano + secc) mode.  --fine 0 times single-pass renders (the streaming kernel), --fine 48 importance renders (the CTA-per-ray-tile
+kernel).  Also checks that every layout returns the same image as the first.  Comparing two builds: run once per library (R3DP_LIB)."""
 import argparse
 import json
 import os
@@ -36,7 +37,6 @@ def main():
     dec.load_state_dict(syn.make_decoder_params(seed=4), strict=True)
     dec = dec.to(dev).eval()
     R = r3.ImportanceRenderer()
-    L = _capi.lib()
     nb = P // B
     cl = [ren.planes_to_channels_last(planes[i * B:(i + 1) * B]) for i in range(nb)]
     hw = [ren.PlanesCL(c.data.permute(0, 2, 3, 1, 4).contiguous(), 'hwpc') for c in cl]
@@ -64,25 +64,18 @@ def main():
         torch.cuda.synchronize()
         return a.elapsed_time(b) / args.iters
 
-    _capi.check(L.r3dp_set_option(b'render', 1))
-    ref = run(cl, 0)[0].clone()
-    variants = [('tile', 1, 8, cl, 2), ('stream_d8', 0, 8, cl, 2), ('stream_d8_nopf', 0, 8, cl, 0), ('stream_d8_pf1', 0, 8, cl, 1), ('stream_d8_pf4', 0, 8, cl, 4),
-                ('stream_d4', 0, 4, cl, 2), ('stream_d16', 0, 16, cl, 2), ('stream_d8_hwpc', 0, 8, hw, 2), ('stream_d8_two_sets', 0, 8, None, 2)]
-    if args.fine:
-        variants = [('tile', 1, 8, cl, 2), ('tile_nopf', 1, 8, cl, 0), ('tile_hwpc', 1, 8, hw, 2), ('tile_two_sets', 1, 8, None, 2)]
+    variants = [('cl', cl), ('hwpc', hw), ('two_sets', [(h, h) for h in half])]      # two sets: x/2 + x/2, same image, twice the gather
     if args.only:
         variants = [v for v in variants if v[0] in args.only.split(',')]
-    for name, variant, d, pl, pf in variants:
-        _capi.check(L.r3dp_set_option(b'render', variant))
-        _capi.check(L.r3dp_set_option(b'rs_d', d))
-        _capi.check(L.r3dp_set_option(b'rs_prefetch', pf))
-        if pl is None:
-            pl = [(h, h) for h in half]                                    # x/2 + x/2: same image, twice the gather
-        diff = float((run(pl, 0)[0] - ref).abs().max())
+    ref = None
+    for name, pl in variants:
+        out = run(pl, 0)[0]
+        if ref is None:
+            ref, first = out.clone(), name
+        diff = float((out - ref).abs().max())
         ms = timed(pl)
         print(json.dumps({'variant': name, 'ms_per_call': round(ms, 4), 'us_per_frame': round(1e3 * ms / B, 2), 'frames': B,
-                          'samples_per_ray': 48 + args.fine, 'max_abs_diff_vs_tile': diff}))
-    _capi.check(L.r3dp_set_option(b'render', 0)); _capi.check(L.r3dp_set_option(b'rs_d', 8)); _capi.check(L.r3dp_set_option(b'rs_prefetch', 2))
+                          'samples_per_ray': 48 + args.fine, 'max_abs_diff_vs_' + first: diff, 'lib': _capi.LIB_PATH}))
 
 
 if __name__ == '__main__':

@@ -1,5 +1,6 @@
 #!/bin/bash
-# One GPU: full parity suite, render-variant A/B, default bench.   bash tools/gpu_check.sh
+# One GPU: full parity suite, render timings per plane layout (single-pass and importance), sampler, SR accuracy, smoke, default bench.
+#   bash tools/gpu_check.sh
 mkdir -p gpurun_out
 timeout 1200 python -m pytest tests -m gpu -q -rf --timeout 600 2>&1 | tail -30 > gpurun_out/check_pytest.log
 timeout 300 python tools/bench_render.py > gpurun_out/check_render.log 2>&1
