@@ -29,30 +29,6 @@ namespace tc {
 constexpr int BM = 128, BN = 128, BK = 64;
 constexpr float kSplitWeightScale = 1024.0f;       // split-fp16 weights are stored x 2^10: their lo halves (|w| 2^-11) stay normal fp16 numbers
 
-
-struct Taps {
-    int n;
-    int dy[9], dx[9], widx[9];
-};
-enum Mode { kStoreAct = 0, kStoreRaw = 1, kToRgbFinal = 2 };
-struct ConvArgs {
-    Taps taps;
-    int k_chunks;            // Cin_pad / 64
-    int tiles_x, rows;       // grid of M tiles: rows x tiles_x (each tile = 128 consecutive grid columns of one row)
-    int w_shared;            // 1: all samples use weight set 0
-    int mode;
-    // output (fp16 NHWC) for kStoreAct / kStoreRaw: pixel (row*oy_mul+oy_off, col*ox_mul+ox_off) of an out_H x out_W x out_C image
-    __half* out; int out_H, out_W, out_C, oy_mul, oy_off, ox_mul, ox_off;
-    const float* bias;       // [Cout] conv bias (kStoreAct, kToRgbFinal)
-    // kToRgbFinal: img_out[n][3][out_H][out_W] = upsample2d(img_prev[n][3][out_H/2][out_W/2]) + torgb(act) + brgb
-    const float* wrgb;       // [Nw][3][128] folded ToRGB weights (fp32)
-    const float* brgb;       // [3]
-    const float* img_prev;
-    float* img_out;
-    int out_clamp; uint8_t* img_out_u8;
-    int split;               // fp32-grade [hi | lo] operands (see Conv2Args)
-};
-
 // =====================================================================================================================
 // Persistent implicit-GEMM conv design (conv_tc3_kernel): R = kConvRows output rows (R x 128 pixels) x 128 couts per tile.
 //
@@ -69,22 +45,28 @@ struct ConvArgs {
 // Two mbarrier rings (A strips, B taps) are filled by one TMA lane in exactly the order the consumer warpgroups use them.
 // =====================================================================================================================
 constexpr int A2_ROWS = 130, A2_SLOT = 17408;                                // 17 x 1024: every slot keeps the swizzle alignment
-struct Taps2 {
+struct Taps {
     int n, ngroups;                 // taps sorted by (dy, dx); group = taps sharing dy
     int dyi[9], shift[9], widx[9];  // group index, horizontal shift (dx + 1, in pixels: strips start at x0 - 1), weight tap index
     int gstart[4];                  // first tap of each group (+ sentinel)
     int dy_min;
 };
-struct Phase2 {
-    Taps2 taps;
+struct Phase {
+    Taps taps;
     int rows, oy_off, ox_off;       // valid grid rows of this phase; output pixel = (row*oy_mul + oy_off, col*ox_mul + ox_off)
 };
-enum Mode2 { kActRgb = 3 };         // kStoreAct + ToRGB/skip accumulated over the cout blocks (in addition to Mode)
-struct Conv2Args {
-    Phase2 ph[4];
+enum Mode {
+    kStoreAct = 0,                  // bias + activation -> fp16 NHWC
+    kStoreRaw = 1,                  // the raw sums -> fp16 NHWC (the transposed conv's grid, filtered afterwards)
+    kToRgbFinal = 2,                // only the image: img_out = skip(img_prev) + ToRGB(activated sums) + brgb
+    kActRgb = 3                     // kStoreAct + ToRGB/skip accumulated over the cout blocks
+};
+struct ConvArgs {
+    Phase ph[4];
     int n_phases, k_chunks, tiles_x, row_groups, n_blocks, n_images, total_units;
-    int w_shared, mode;
+    int w_shared, mode;             // w_shared: all samples use weight set 0; mode: a Mode
     __half* out; int out_H, out_W, out_C, oy_mul, ox_mul;
+    // bias [n_blocks * 128]; ToRGB: wrgb [Nw][3][n_blocks * 128], brgb [3], img_out [N][3][img_H][img_W], img_prev at half or (skip_same_res) full size
     const float* bias; const float* wrgb; const float* brgb; const float* img_prev; float* img_out; int img_H, img_W;
     float act_slope, act_gain;      // epilogue activation: v < 0 ? v*slope : v, then * gain  (0.2, sqrt2 = bias_act lrelu; 0.01, 1 = nn.LeakyReLU; 1, 1 = linear)
     int skip_same_res;              // ToRGB skip image has the output resolution (SynthesisBlockNoUp) instead of half (FIR-upsampled)
@@ -178,7 +160,7 @@ __device__ __forceinline__ uint64_t conv_desc(uint32_t saddr) { return KC == BK 
 
 template <bool SPLIT, int KC>
 __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                               const __grid_constant__ CUtensorMap tmB, const Conv2Args a) {
+                                                               const __grid_constant__ CUtensorMap tmB, const ConvArgs a) {
     using C = Cfg3<KC>;
     constexpr int R = kConvRows;
     extern __shared__ uint8_t smem_raw[];
@@ -231,7 +213,7 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
             uint32_t aq = 0, bq = 0;                                         // running strip / tap sequence numbers
             for (int unit = blockIdx.x; unit < a.total_units; unit += gridDim.x) {
                 int n, ph, row0, col0; decode(unit, n, ph, row0, col0);
-                const Taps2& tp = a.ph[ph].taps;
+                const Taps& tp = a.ph[ph].taps;
                 const int DY = tp.ngroups;
                 const int wn = a.w_shared ? 0 : n;
                 const int K3 = SPLIT ? 3 * a.k_chunks : a.k_chunks;               // split: [x_hi w_hi | x_lo w_hi | x_hi w_lo] over the channel chunks
@@ -280,8 +262,8 @@ __global__ void __launch_bounds__(kThreads3, 1) conv_tc3_kernel(const __grid_con
         float acc[R][64];
         for (int unit = blockIdx.x; unit < a.total_units; unit += gridDim.x) {
             int n, ph, row0, col0; decode(unit, n, ph, row0, col0);
-            const Phase2& P = a.ph[ph];
-            const Taps2& tp = P.taps;
+            const Phase& P = a.ph[ph];
+            const Taps& tp = P.taps;
             const int DY = tp.ngroups, NS = R + DY - 1;
             const int wn = a.w_shared ? 0 : n;
             if (want_rgb && wn != n_loaded) {
@@ -847,42 +829,18 @@ static EncodeTiledFn encode_fn() {
     return fn;
 }
 
-// fp16 tensor [d3][d2][d1][d0] (d0 innermost, dense), box {64, box1, 1, 1}, 128-byte swizzle, zero fill outside
-// box0 = 64 channels: 128-byte swizzle; box0 = 32: 64-byte swizzle (the KC = 32 conv operands)
-static int make_map_4d_box(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t d3, uint32_t box1, uint32_t box0 = 64) {
+// fp16 tensor [d3][d2][d1][d0] (d0 innermost, dense) read in boxes of box[0..3] elements, zero fill outside
+static int make_map(CUtensorMap* m, const void* ptr, const cuuint64_t (&dims)[4], const cuuint32_t (&box)[4], CUtensorMapSwizzle swizzle,
+                    CUtensorMapL2promotion l2) {
     EncodeTiledFn fn = encode_fn();
     R3DP_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled is not available from the driver");
-    cuuint64_t dims[4] = {d0, d1, d2, d3};
-    cuuint64_t strides[3] = {d0 * 2, d0 * d1 * 2, d0 * d1 * d2 * 2};
-    cuuint32_t box[4] = {box0, box1, 1, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
+    const cuuint64_t strides[3] = {dims[0] * 2, dims[0] * dims[1] * 2, dims[0] * dims[1] * dims[2] * 2};
+    const cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    box0 == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                    swizzle, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     R3DP_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with CUresult %d (dims %llu x %llu x %llu x %llu)", (int)r,
-                 (unsigned long long)d0, (unsigned long long)d1, (unsigned long long)d2, (unsigned long long)d3);
+                 (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3]);
     return 0;
-}
-
-// 128-byte L2 promotion: a box row is 128 B (one 64-channel group) of a pixel that is 2 or 4 such groups wide, and the other groups are read by
-// work items far away in the schedule; 256-byte promotion fetched the neighbouring group from DRAM too, and it was evicted before its use.
-static int make_map_fir(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t d3, uint32_t box_rows) {
-    EncodeTiledFn fn = encode_fn();
-    R3DP_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled is not available from the driver");
-    cuuint64_t dims[4] = {d0, d1, d2, d3};
-    cuuint64_t strides[3] = {d0 * 2, d0 * d1 * 2, d0 * d1 * d2 * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)FIR_BW, box_rows, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    R3DP_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (FIR) failed with CUresult %d", (int)r);
-    return 0;
-}
-
-static int launch_conv2(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int O, const ConvArgs& a1, cudaStream_t st);
-static int launch_upconv2(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int O, __half* yb, const float* bias, int split, cudaStream_t st);
-static int launch_conv(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int O, ConvArgs a, cudaStream_t st) {
-    return launch_conv2(x, N, H, W, I, wp, Nw, O, a, st);
 }
 
 // ---- optional in-library timing of the conv launches (bench.py's roofline): CUDA events on the launching stream around each launch --------
@@ -897,10 +855,9 @@ static void prof_mark(cudaStream_t st) {
 static unsigned long long* g_debug_buf = nullptr;
 static int g_debug_launch = 0;
 template <bool SPLIT, int KC>
-static int launch_conv3_s(const CUtensorMap& tmA, const CUtensorMap& tmB, Conv2Args a, int max_rows, cudaStream_t st) {
+static int launch_conv3_s(const CUtensorMap& tmA, const CUtensorMap& tmB, ConvArgs a, cudaStream_t st) {
     R3DP_CUDA(cudaFuncSetAttribute(conv_tc3_kernel<SPLIT, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg3<KC>::SMEM));
     a.debug = g_debug_buf ? g_debug_buf + 24 * (g_debug_launch++ % 32) : nullptr;
-    a.row_groups = (max_rows + kConvRows - 1) / kConvRows;
     a.total_units = a.n_images * a.n_phases * a.row_groups * a.tiles_x;
     const int grid = a.total_units < sm_count() ? a.total_units : sm_count();
     prof_mark(st);
@@ -911,72 +868,89 @@ static int launch_conv3_s(const CUtensorMap& tmA, const CUtensorMap& tmB, Conv2A
     return 0;
 }
 
-// taps given as (dy, dx, widx) lists -> sorted/grouped Taps2 (dy groups are contiguous for 3x3 and every transposed-conv phase)
-static void fill_taps2(Taps2& t2, const Taps& t) {
-    int order[9], n = t.n;
-    for (int i = 0; i < n; ++i) order[i] = i;
-    for (int i = 0; i < n; ++i)
-        for (int j = i + 1; j < n; ++j) {
-            const int a = order[i], b = order[j];
-            if (t.dy[b] < t.dy[a] || (t.dy[b] == t.dy[a] && t.dx[b] < t.dx[a])) { order[i] = b; order[j] = a; }
+// ---- host side: conv_tc3 launch descriptions -------------------------------------------------------------------------
+// Taps are added in (dy, dx) order, so the taps sharing a dy are contiguous and form one group.  The order within a group is the order of
+// the fp32 accumulation: it decides the output bits.
+static void add_tap(Taps& t, int dy, int dx, int widx) {
+    if (t.n == 0) t.dy_min = dy;
+    if (t.n == 0 || dy - t.dy_min != t.dyi[t.n - 1]) t.gstart[t.ngroups++] = t.n;
+    t.dyi[t.n] = dy - t.dy_min; t.shift[t.n] = dx + 1; t.widx[t.n] = widx;         // strip box starts at x0 - 1
+    t.gstart[t.ngroups] = ++t.n;
+}
+// 3x3 box on weight taps base + (dy + 1) * 3 + (dx + 1)  (base = 9 * phase for the composed up weights)
+static Taps taps_3x3(int base) {
+    Taps t = {};
+    for (int i = 0; i < 9; ++i) add_tap(t, i / 3 - 1, i % 3 - 1, base + i);
+    return t;
+}
+// 1x1 conv: the centre tap of the packed 3x3 weights
+static Taps taps_1x1() {
+    Taps t = {};
+    add_tap(t, 0, 0, 4);
+    return t;
+}
+// output parity (p, q) of the stride-2 transposed conv: the kernel rows ky == p (mod 2), read at dy = -(ky >> 1); the same for columns (4/2/2/1 taps)
+static Taps taps_transposed(int p, int q) {
+    Taps t = {};
+    for (int dy = -1; dy <= 0; ++dy)
+        for (int dx = -1; dx <= 0; ++dx) {
+            const int ky = p - 2 * dy, kx = q - 2 * dx;
+            if (ky < 3 && kx < 3) add_tap(t, dy, dx, ky * 3 + kx);
         }
-    int dy_min = 99;
-    for (int i = 0; i < n; ++i) if (t.dy[i] < dy_min) dy_min = t.dy[i];
-    t2.n = n; t2.dy_min = dy_min; t2.ngroups = 0;
-    int last = -99;
-    for (int i = 0; i < n; ++i) {
-        const int o = order[i];
-        if (t.dy[o] != last) { t2.gstart[t2.ngroups++] = i; last = t.dy[o]; }
-        t2.dyi[i] = t.dy[o] - dy_min; t2.shift[i] = t.dx[o] + 1; t2.widx[i] = t.widx[o];      // strip box starts at x0 - 1
-    }
-    t2.gstart[t2.ngroups] = n;
+    return t;
+}
+// output parity (p, q) of nearest-up x2 + 3x3: taps dy in {p - 1, p}, dx in {q - 1, q} of the composed weight set p * 2 + q
+static Taps taps_up_nearest(int p, int q) {
+    Taps t = {};
+    for (int dy = p - 1; dy <= p; ++dy)
+        for (int dx = q - 1; dx <= q; ++dx) add_tap(t, dy, dx, (p * 2 + q) * 9 + (dy + 1) * 3 + (dx + 1));
+    return t;
 }
 
-// I = the real input channels; x and wp hold them padded to Cp = I rounded up to 64.  I <= 32 runs the 32-channel K chunks (KC = 32).
-static int run_conv2(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int O, Conv2Args& a, int max_rows, cudaStream_t st, int n_taps = 9) {
+// the output y [N][out_H][out_W][O] fp16 NHWC and what the epilogue writes to it; grid pixel (row, col) of a phase lands at
+// (row * mul + oy_off, col * mul + ox_off)
+static void set_output(ConvArgs& a, Mode mode, void* y, int out_H, int out_W, int O, int mul) {
+    a.mode = mode; a.out = reinterpret_cast<__half*>(y); a.out_H = out_H; a.out_W = out_W; a.out_C = O; a.oy_mul = a.ox_mul = mul;
+}
+
+constexpr float kLreluSlope = 0.2f, kLreluGain = 1.4142135623730951f;          // bias_act lrelu: max(v, 0.2 v) * sqrt2
+
+// Runs the launch a describes (phases, output, epilogue).  x [N][H][W][Cp] is the input grid; wp [Nw][w_taps][O][Cp] the packed weights
+// (w_taps = 9, or 36 for four composed phase sets).  I = the real input channels; x and wp hold them padded to Cp = I rounded up to 64.
+// I <= 32 runs the 32-channel K chunks (KC = 32).
+static int run_conv(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int w_taps, int O, ConvArgs a, cudaStream_t st) {
     CUtensorMap tmA, tmB;
     const int Cp = (I + 63) / 64 * 64;
     const bool kc32 = I <= 32;
-    const uint64_t Cphys = (uint64_t)Cp * (a.split ? 2 : 1);                      // split: [hi | lo] halves of Cp channels each
-    if (make_map_4d_box(&tmA, x, Cphys, (uint64_t)W, (uint64_t)H, (uint64_t)N, A2_ROWS, kc32 ? 32 : BK)) return 1;
-    if (make_map_4d_box(&tmB, wp, Cphys, (uint64_t)O, (uint64_t)n_taps, (uint64_t)Nw, BN, kc32 ? 32 : BK)) return 1;
+    const cuuint64_t Cphys = (cuuint64_t)Cp * (a.split ? 2 : 1);                  // split: [hi | lo] halves of Cp channels each
+    const cuuint32_t kc = kc32 ? 32 : BK;
+    const CUtensorMapSwizzle swizzle = kc32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
+    if (make_map(&tmA, x, {Cphys, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N}, {kc, A2_ROWS, 1, 1}, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
+        return 1;
+    if (make_map(&tmB, wp, {Cphys, (cuuint64_t)O, (cuuint64_t)w_taps, (cuuint64_t)Nw}, {kc, BN, 1, 1}, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
+        return 1;
     if (a.split) { a.acc_scale = 1.0f / kSplitWeightScale; a.lo_off = a.out_C; a.out_C *= 2; }
     else { a.acc_scale = 1.0f; a.lo_off = 0; }
     // W = 64 (the torso warper's 64^2 maps): one tile per row whose right half reads TMA zero fill and stores nothing (the stores check out_W)
     a.k_chunks = Cp / BK; a.tiles_x = (W + BM - 1) / BM; a.n_blocks = O / BN; a.n_images = N; a.w_shared = (Nw == 1);
-    if (a.act_gain == 0.f) { a.act_slope = 0.2f; a.act_gain = 1.4142135623730951f; }      // default: bias_act lrelu
+    int max_rows = 0;
+    for (int p = 0; p < a.n_phases; ++p) max_rows = a.ph[p].rows > max_rows ? a.ph[p].rows : max_rows;
+    a.row_groups = (max_rows + kConvRows - 1) / kConvRows;
     R3DP_REQUIRE(a.n_blocks >= 1 && a.n_blocks <= 2, "conv_tc3: 128 or 256 output channels");
-    if (kc32) return a.split ? launch_conv3_s<true, 32>(tmA, tmB, a, max_rows, st) : launch_conv3_s<false, 32>(tmA, tmB, a, max_rows, st);
-    return a.split ? launch_conv3_s<true, BK>(tmA, tmB, a, max_rows, st) : launch_conv3_s<false, BK>(tmA, tmB, a, max_rows, st);
+    if (kc32) return a.split ? launch_conv3_s<true, 32>(tmA, tmB, a, st) : launch_conv3_s<false, 32>(tmA, tmB, a, st);
+    return a.split ? launch_conv3_s<true, BK>(tmA, tmB, a, st) : launch_conv3_s<false, BK>(tmA, tmB, a, st);
 }
 
-// v1-style single-phase description -> v2 launch
-static int launch_conv2(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int O, const ConvArgs& a1, cudaStream_t st) {
-    Conv2Args a = {};
-    a.n_phases = 1;
-    fill_taps2(a.ph[0].taps, a1.taps);
-    a.ph[0].rows = a1.rows; a.ph[0].oy_off = a1.oy_off; a.ph[0].ox_off = a1.ox_off;
-    a.mode = a1.mode; a.out = a1.out; a.out_H = a1.out_H; a.out_W = a1.out_W; a.out_C = a1.out_C; a.oy_mul = a1.oy_mul; a.ox_mul = a1.ox_mul;
-    a.bias = a1.bias; a.wrgb = a1.wrgb; a.brgb = a1.brgb; a.img_prev = a1.img_prev; a.img_out = a1.img_out; a.img_H = a1.out_H; a.img_W = a1.out_W;
-    a.out_clamp = a1.out_clamp; a.img_out_u8 = a1.img_out_u8; a.split = a1.split;
-    return run_conv2(x, N, H, W, I, wp, Nw, O, a, a1.rows, st);
-}
-
-// all four output-parity phases of the stride-2 transposed conv in ONE persistent launch (raw fp16 result on the (2H+1)x(2W+1) grid)
-static int launch_upconv2(const void* x, int N, int H, int W, int I, const void* wp, int Nw, int O, __half* yb, const float* bias, int split, cudaStream_t st) {
-    Conv2Args a = {};
-    a.n_phases = 4; a.split = split;
-    for (int pa = 0; pa < 2; ++pa)
-        for (int pb = 0; pb < 2; ++pb) {
-            Taps t = {};
-            for (int ky = pa; ky < 3; ky += 2)
-                for (int kx = pb; kx < 3; kx += 2) { const int i = t.n++; t.dy[i] = -(ky >> 1); t.dx[i] = -(kx >> 1); t.widx[i] = ky * 3 + kx; }
-            Phase2& P = a.ph[pa * 2 + pb];
-            fill_taps2(P.taps, t);
-            P.rows = pa ? H : H + 1; P.oy_off = pa; P.ox_off = pb;
-        }
-    a.mode = kStoreRaw; a.out = yb; a.out_H = 2 * H + 1; a.out_W = 2 * W + 1; a.out_C = O; a.oy_mul = a.ox_mul = 2; a.bias = bias;
-    return run_conv2(x, N, H, W, I, wp, Nw, O, a, H + 1, st);
+// Plain nn.Conv2d (k = 1 or 3, stride 1, "same" padding) at the input's resolution, y [N][H][W][O] fp16: act = max(v, v * slope) * gain,
+// residual (if any) added after it.  The launch behind the up == 1 SynthesisLayer, r3dp_sr_tc_conv(_res) / r3dp_sr_tcx_conv(_res) and
+// r3dp_tw_conv (shapes checked by the callers).
+static int conv_plain_launch(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
+                             float slope, float gain, const void* residual_f16, void* y_f16, int split, r3dp_stream_t stream) {
+    ConvArgs a = {};
+    a.n_phases = 1; a.ph[0] = {ksize == 3 ? taps_3x3(0) : taps_1x1(), H, 0, 0};
+    set_output(a, kStoreAct, y_f16, H, W, O, 1);
+    a.bias = bias; a.act_slope = slope; a.act_gain = gain; a.residual = reinterpret_cast<const __half*>(residual_f16); a.split = split;
+    return run_conv(x_f16, N, H, W, I, wp_f16, Nw, 9, O, a, as_stream(stream));
 }
 
 }  // namespace tc
@@ -1022,53 +996,43 @@ static int layer_impl(const void* x_f16, const void* wp_f16, const float* bias, 
     R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && I > 0 && H > 0, "sr_tc_layer: bad shape");
     R3DP_REQUIRE(W % BM == 0 && O % BN == 0, "sr_tc_layer: needs W %% 128 == 0 and Cout %% 128 == 0 (got W=%d, Cout=%d)", W, O);
     R3DP_REQUIRE(up == 1 || up == 2, "sr_tc_layer: up must be 1 or 2");
+    if (up == 1) return conv_plain_launch(x_f16, wp_f16, bias, N, Nw, I, O, H, W, 3, kLreluSlope, kLreluGain, nullptr, y_f16, split, stream);
+    R3DP_REQUIRE(scratch, "sr_tc_layer: up=2 needs scratch");
     const int Ip = (I + 63) / 64 * 64;
     cudaStream_t st = as_stream(stream);
-    ConvArgs a = {};
-    a.bias = bias; a.split = split;
-    if (up == 1) {
-        a.taps.n = 9;
-        for (int t = 0; t < 9; ++t) { a.taps.dy[t] = t / 3 - 1; a.taps.dx[t] = t % 3 - 1; a.taps.widx[t] = t; }
-        a.tiles_x = W / BM; a.rows = H; a.mode = kStoreAct;
-        a.out = reinterpret_cast<__half*>(y_f16); a.out_H = H; a.out_W = W; a.out_C = O; a.oy_mul = a.ox_mul = 1;
-        return launch_conv(x_f16, N, H, W, I, wp_f16, Nw, O, a, st);
-    }
-    R3DP_REQUIRE(scratch, "sr_tc_layer: up=2 needs scratch");
     __half* yb = reinterpret_cast<__half*>(scratch);
-    if (launch_upconv2(x_f16, N, H, W, I, wp_f16, Nw, O, yb, bias, split, st)) return 1;
-    {
-        R3DP_REQUIRE(Ip <= 256, "sr_tc_layer: up=2 supports at most 256 input channels");
-        const int erows = split ? kEdgeRowsSplit : kEdgeRows;
-        dim3 grid((2 * H + 1 + erows - 1) / erows, (O + kEdgeCo - 1) / kEdgeCo, N);
-        const size_t esmem = ((size_t)(kEdgeRows / 2 + 2) * Ip + 3 * (size_t)kEdgeCo * (Ip + 8)) * sizeof(__half);
-        if (split) {
-            const size_t ssmem = ((size_t)(kEdgeRowsSplit / 2 + 2) * Ip + 3 * (size_t)kEdgeCo * (Ip + 4)) * sizeof(float);
-            R3DP_CUDA(cudaFuncSetAttribute(upconv_edge_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
-            upconv_edge_split_kernel<<<grid, 256, ssmem, st>>>(reinterpret_cast<const __half*>(x_f16), reinterpret_cast<const __half*>(wp_f16), H, W, Ip, O,
-                                                           Nw == 1, yb);
-        } else {
-        R3DP_CUDA(cudaFuncSetAttribute(upconv_edge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 80 * 1024));
-        upconv_edge_kernel<<<grid, 256, esmem, st>>>(reinterpret_cast<const __half*>(x_f16), reinterpret_cast<const __half*>(wp_f16), H, W, Ip, O,
-                                                 Nw == 1, yb);
-        }
-    }
-    {
-        R3DP_REQUIRE((2 * W) % FIR_TW == 0 && O % 64 == 0, "sr_tc_layer: FIR needs 2W %% 32 == 0 and Cout %% 64 == 0");
-        CUtensorMap tmY, tmY8;
-        if (make_map_fir(&tmY, yb, (uint64_t)O * (split ? 2 : 1), (uint64_t)(2 * W + 1), (uint64_t)(2 * H + 1), (uint64_t)N, FIR_BH)) return 1;
-        if (make_map_fir(&tmY8, yb, (uint64_t)O * (split ? 2 : 1), (uint64_t)(2 * W + 1), (uint64_t)(2 * H + 1), (uint64_t)N, FIR_TH)) return 1;
-        const int total = N * (O / 64) * ((2 * H + FIR_SEG - 1) / FIR_SEG) * (2 * W / FIR_TW);
-        if (split) {
-            const int smem = 4 * FIR_SLOT + 1024 + 64;
-            R3DP_CUDA(cudaFuncSetAttribute(fir_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-            const int grid = total < sm_count() ? total : sm_count();
-            fir_tma_kernel<true><<<grid, 256, smem, st>>>(tmY, tmY8, bias, N, 2 * H, 2 * W, O, reinterpret_cast<__half*>(y_f16));
-        } else {
-            R3DP_CUDA(cudaFuncSetAttribute(fir_tma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FIR_SMEM));
-            const int grid = total < 2 * sm_count() ? total : 2 * sm_count();
-            fir_tma_kernel<false><<<grid, 256, FIR_SMEM, st>>>(tmY, tmY8, bias, N, 2 * H, 2 * W, O, reinterpret_cast<__half*>(y_f16));
-        }
-    }
+    // all four output-parity phases of the stride-2 transposed conv in ONE persistent launch: raw sums on the (2H+1)x(2W+1) grid, whose
+    // bias and activation the FIR pass applies
+    ConvArgs a = {};
+    a.n_phases = 4;
+    for (int p = 0; p < 4; ++p) a.ph[p] = {taps_transposed(p >> 1, p & 1), p < 2 ? H + 1 : H, p >> 1, p & 1};
+    set_output(a, kStoreRaw, yb, 2 * H + 1, 2 * W + 1, O, 2);
+    a.split = split;
+    if (run_conv(x_f16, N, H, W, I, wp_f16, Nw, 9, O, a, st)) return 1;
+    // the grid's last column; the split form stages fp32 operands
+    R3DP_REQUIRE(Ip <= 256, "sr_tc_layer: up=2 supports at most 256 input channels");
+    const int erows = split ? kEdgeRowsSplit : kEdgeRows;
+    const dim3 egrid((2 * H + 1 + erows - 1) / erows, (O + kEdgeCo - 1) / kEdgeCo, N);
+    const size_t esmem = split ? ((size_t)(kEdgeRowsSplit / 2 + 2) * Ip + 3 * (size_t)kEdgeCo * (Ip + 4)) * sizeof(float)
+                               : ((size_t)(kEdgeRows / 2 + 2) * Ip + 3 * (size_t)kEdgeCo * (Ip + 8)) * sizeof(__half);
+    const auto edge = split ? upconv_edge_split_kernel : upconv_edge_kernel;
+    R3DP_CUDA(cudaFuncSetAttribute(edge, cudaFuncAttributeMaxDynamicSharedMemorySize, split ? 128 * 1024 : 80 * 1024));
+    edge<<<egrid, 256, esmem, st>>>(reinterpret_cast<const __half*>(x_f16), reinterpret_cast<const __half*>(wp_f16), H, W, Ip, O, Nw == 1, yb);
+    // the FIR pass.  128-byte L2 promotion: a box row is 128 B (one 64-channel group) of a pixel that is 2 or 4 such groups wide, and the other
+    // groups are read by work items far away in the schedule; 256-byte promotion fetched the neighbouring group from DRAM too, and it was
+    // evicted before its use.
+    R3DP_REQUIRE((2 * W) % FIR_TW == 0 && O % 64 == 0, "sr_tc_layer: FIR needs 2W %% 32 == 0 and Cout %% 64 == 0");
+    CUtensorMap tmY, tmY8;
+    const cuuint64_t ydims[4] = {(cuuint64_t)O * (split ? 2 : 1), (cuuint64_t)(2 * W + 1), (cuuint64_t)(2 * H + 1), (cuuint64_t)N};
+    if (make_map(&tmY, yb, ydims, {64, FIR_BW, FIR_BH, 1}, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B)) return 1;
+    if (make_map(&tmY8, yb, ydims, {64, FIR_BW, FIR_TH, 1}, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B)) return 1;
+    const int total = N * (O / 64) * ((2 * H + FIR_SEG - 1) / FIR_SEG) * (2 * W / FIR_TW);
+    // persistent CTAs, as many as are resident at once: two per SM, one with the split form's twice as large buffers
+    const auto fir = split ? fir_tma_kernel<true> : fir_tma_kernel<false>;
+    const int fsmem = split ? 4 * FIR_SLOT + 1024 + 64 : FIR_SMEM;
+    const int fcap = split ? sm_count() : 2 * sm_count();
+    R3DP_CUDA(cudaFuncSetAttribute(fir, cudaFuncAttributeMaxDynamicSharedMemorySize, fsmem));
+    fir<<<total < fcap ? total : fcap, 256, fsmem, st>>>(tmY, tmY8, bias, N, 2 * H, 2 * W, O, reinterpret_cast<__half*>(y_f16));
     R3DP_LAUNCH_CHECK();
     count_launches(2);
     return 0;
@@ -1090,12 +1054,12 @@ static int last_layer_impl(const void* x_f16, const void* wp_f16, const float* b
     R3DP_REQUIRE(x_f16 && wp_f16 && bias && wrgb && brgb && (img_out || img_out_u8), "sr_tc_last_layer: null pointer");
     R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && W % BM == 0 && H % 2 == 0, "sr_tc_last_layer: bad shape");
     ConvArgs a = {};
-    a.bias = bias; a.wrgb = wrgb; a.brgb = brgb; a.img_prev = img_prev; a.img_out = img_out; a.img_out_u8 = img_out_u8; a.out_clamp = clamp || img_out_u8;
-    a.split = split;
-    a.taps.n = 9;
-    for (int t = 0; t < 9; ++t) { a.taps.dy[t] = t / 3 - 1; a.taps.dx[t] = t % 3 - 1; a.taps.widx[t] = t; }
-    a.tiles_x = W / BM; a.rows = H; a.mode = kToRgbFinal; a.out_H = H; a.out_W = W; a.out_C = BN; a.oy_mul = a.ox_mul = 1;
-    return launch_conv(x_f16, N, H, W, I, wp_f16, Nw, BN, a, as_stream(stream));
+    a.n_phases = 1; a.ph[0] = {taps_3x3(0), H, 0, 0};
+    set_output(a, kToRgbFinal, nullptr, H, W, BN, 1);
+    a.bias = bias; a.act_slope = kLreluSlope; a.act_gain = kLreluGain;
+    a.wrgb = wrgb; a.brgb = brgb; a.img_prev = img_prev; a.img_out = img_out; a.img_H = H; a.img_W = W;
+    a.img_out_u8 = img_out_u8; a.out_clamp = clamp || img_out_u8; a.split = split;
+    return run_conv(x_f16, N, H, W, I, wp_f16, Nw, 9, BN, a, as_stream(stream));
 }
 extern "C" int r3dp_sr_tc_last_layer_ex(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
                                         const float* img_prev, int N, int Nw, int I, int H, int W, float* img_out, uint8_t* img_out_u8, int clamp,
@@ -1145,16 +1109,12 @@ static int layer_torgb_impl(const void* x_f16, const void* wp_f16, const float* 
                             r3dp_stream_t stream) {
     R3DP_REQUIRE(x_f16 && wp_f16 && bias && wrgb && brgb && y_f16 && img_out, "sr_tc_layer_torgb: null pointer");
     R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && W % BM == 0 && O % BN == 0 && O <= 256 && H % 2 == 0, "sr_tc_layer_torgb: bad shape");
-    Conv2Args a = {};
-    Taps t = {};
-    t.n = 9;
-    for (int i = 0; i < 9; ++i) { t.dy[i] = i / 3 - 1; t.dx[i] = i % 3 - 1; t.widx[i] = i; }
-    a.n_phases = 1;
-    fill_taps2(a.ph[0].taps, t);
-    a.ph[0].rows = H; a.ph[0].oy_off = 0; a.ph[0].ox_off = 0;
-    a.mode = kActRgb; a.out = reinterpret_cast<__half*>(y_f16); a.out_H = H; a.out_W = W; a.out_C = O; a.oy_mul = a.ox_mul = 1;
-    a.bias = bias; a.wrgb = wrgb; a.brgb = brgb; a.img_prev = img_prev; a.img_out = img_out; a.img_H = H; a.img_W = W; a.split = split;
-    return run_conv2(x_f16, N, H, W, I, wp_f16, Nw, O, a, H, as_stream(stream));
+    ConvArgs a = {};
+    a.n_phases = 1; a.ph[0] = {taps_3x3(0), H, 0, 0};
+    set_output(a, kActRgb, y_f16, H, W, O, 1);
+    a.bias = bias; a.act_slope = kLreluSlope; a.act_gain = kLreluGain;
+    a.wrgb = wrgb; a.brgb = brgb; a.img_prev = img_prev; a.img_out = img_out; a.img_H = H; a.img_W = W; a.split = split;
+    return run_conv(x_f16, N, H, W, I, wp_f16, Nw, 9, O, a, as_stream(stream));
 }
 extern "C" int r3dp_sr_tc_layer_torgb(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
                                       const float* img_prev, int N, int Nw, int I, int O, int H, int W, void* y_f16, float* img_out,
@@ -1342,18 +1302,12 @@ static int layer_up_composed_impl(const void* x_f16, const void* wpc_f16, const 
                                   int W, void* y_f16, int split, r3dp_stream_t stream) {
     R3DP_REQUIRE(x_f16 && wpc_f16 && bias && y_f16, "sr_tc_layer_up_composed: null pointer");
     R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && W % BM == 0 && O % BN == 0 && O <= 256, "sr_tc_layer_up_composed: bad shape");
-    Conv2Args a = {};
+    ConvArgs a = {};
     a.n_phases = 4;
-    for (int ph = 0; ph < 4; ++ph) {
-        Taps t = {};
-        t.n = 9;
-        for (int i = 0; i < 9; ++i) { t.dy[i] = i / 3 - 1; t.dx[i] = i % 3 - 1; t.widx[i] = ph * 9 + i; }
-        fill_taps2(a.ph[ph].taps, t);
-        a.ph[ph].rows = H; a.ph[ph].oy_off = ph >> 1; a.ph[ph].ox_off = ph & 1;
-    }
-    a.mode = kStoreAct; a.out = reinterpret_cast<__half*>(y_f16); a.out_H = 2 * H; a.out_W = 2 * W; a.out_C = O; a.oy_mul = a.ox_mul = 2;
-    a.bias = bias; a.split = split;
-    return run_conv2(x_f16, N, H, W, I, wpc_f16, Nw, O, a, H, as_stream(stream), 36);
+    for (int p = 0; p < 4; ++p) a.ph[p] = {taps_3x3(9 * p), H, p >> 1, p & 1};
+    set_output(a, kStoreAct, y_f16, 2 * H, 2 * W, O, 2);
+    a.bias = bias; a.act_slope = kLreluSlope; a.act_gain = kLreluGain; a.split = split;
+    return run_conv(x_f16, N, H, W, I, wpc_f16, Nw, 36, O, a, as_stream(stream));
 }
 extern "C" int r3dp_sr_tc_layer_up_composed(const void* x_f16, const void* wpc_f16, const float* bias, int N, int Nw, int I, int O, int H,
                                             int W, void* y_f16, r3dp_stream_t stream) {
@@ -1368,31 +1322,13 @@ extern "C" int r3dp_sr_tcx_layer_up_composed(const void* x_f16, const void* wpc_
 // Plain nn.Conv2d (k = 1 or 3, stride 1, "same" padding) [+ activation] on the tensor-core path: x [N][H][W][Ip] fp16, weights packed by
 // r3dp_sr_tc_pack_weights from the [1][O][I][k][k] fp32 tensor (k = 1: the value sits in tap 4), y [N][H][W][O] fp16.
 // act: 0 = linear, 1 = lrelu(0.2)*sqrt2 (bias_act), 2 = nn.LeakyReLU() (slope 0.01).
-// the launch behind r3dp_sr_tc_conv(_res) / r3dp_sr_tcx_conv(_res) and r3dp_tw_conv (shapes checked by the callers):
-// act = max(v, v * slope) * gain, residual added after it
-static int conv_plain_launch(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
-                             float slope, float gain, const void* residual_f16, void* y_f16, int split, r3dp_stream_t stream) {
-    Conv2Args a = {};
-    Taps t = {};
-    if (ksize == 3) { t.n = 9; for (int i = 0; i < 9; ++i) { t.dy[i] = i / 3 - 1; t.dx[i] = i % 3 - 1; t.widx[i] = i; } }
-    else { t.n = 1; t.dy[0] = 0; t.dx[0] = 0; t.widx[0] = 4; }
-    a.n_phases = 1;
-    fill_taps2(a.ph[0].taps, t);
-    a.ph[0].rows = H;
-    a.mode = kStoreAct; a.out = reinterpret_cast<__half*>(y_f16); a.out_H = H; a.out_W = W; a.out_C = O; a.oy_mul = a.ox_mul = 1; a.bias = bias;
-    a.act_slope = slope; a.act_gain = gain;
-    a.residual = reinterpret_cast<const __half*>(residual_f16);
-    a.split = split;
-    return run_conv2(x_f16, N, H, W, I, wp_f16, Nw, O, a, H, as_stream(stream));
-}
 static int conv_res_impl(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
                          int act, const void* residual_f16, void* y_f16, int split, r3dp_stream_t stream) {
     R3DP_REQUIRE(x_f16 && wp_f16 && bias && y_f16, "sr_tc_conv: null pointer");
     R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && W % BM == 0 && O % BN == 0 && O <= 256 && (ksize == 1 || ksize == 3) && act >= 0 && act <= 3,
                  "sr_tc_conv: bad shape / options");
-    const float slope = act == 0 ? 1.0f : (act == 1 ? 0.2f : (act == 2 ? 0.01f : 0.0f));       // max(v, v*slope): slope 0 = ReLU
-    return conv_plain_launch(x_f16, wp_f16, bias, N, Nw, I, O, H, W, ksize, slope, act == 1 ? 1.4142135623730951f : 1.0f, residual_f16, y_f16, split,
-                             stream);
+    const float slope = act == 0 ? 1.0f : (act == 1 ? kLreluSlope : (act == 2 ? 0.01f : 0.0f));       // max(v, v*slope): slope 0 = ReLU
+    return conv_plain_launch(x_f16, wp_f16, bias, N, Nw, I, O, H, W, ksize, slope, act == 1 ? kLreluGain : 1.0f, residual_f16, y_f16, split, stream);
 }
 extern "C" int r3dp_sr_tc_conv_res(const void* x_f16, const void* wp_f16, const float* bias, int N, int Nw, int I, int O, int H, int W, int ksize,
                                    int act, const void* residual_f16, void* y_f16, r3dp_stream_t stream) {
@@ -1420,17 +1356,13 @@ static int layer_torgb_noup_impl(const void* x_f16, const void* wp_f16, const fl
                                  r3dp_stream_t stream) {
     R3DP_REQUIRE(x_f16 && wp_f16 && bias && wrgb && brgb && y_f16 && img_out, "sr_tc_layer_torgb_noup: null pointer");
     R3DP_REQUIRE(N > 0 && (Nw == N || Nw == 1) && W % BM == 0 && O % BN == 0 && O <= 256, "sr_tc_layer_torgb_noup: bad shape");
-    Conv2Args a = {};
-    Taps t = {};
-    t.n = 9;
-    for (int i = 0; i < 9; ++i) { t.dy[i] = i / 3 - 1; t.dx[i] = i % 3 - 1; t.widx[i] = i; }
-    a.n_phases = 1;
-    fill_taps2(a.ph[0].taps, t);
-    a.ph[0].rows = H;
-    a.mode = kActRgb; a.out = reinterpret_cast<__half*>(y_f16); a.out_H = H; a.out_W = W; a.out_C = O; a.oy_mul = a.ox_mul = 1;
-    a.bias = bias; a.wrgb = wrgb; a.brgb = brgb; a.img_prev = img_prev; a.img_out = img_out; a.img_H = H; a.img_W = W; a.skip_same_res = 1;
+    ConvArgs a = {};
+    a.n_phases = 1; a.ph[0] = {taps_3x3(0), H, 0, 0};
+    set_output(a, kActRgb, y_f16, H, W, O, 1);
+    a.bias = bias; a.act_slope = kLreluSlope; a.act_gain = kLreluGain;
+    a.wrgb = wrgb; a.brgb = brgb; a.img_prev = img_prev; a.img_out = img_out; a.img_H = H; a.img_W = W; a.skip_same_res = 1;
     a.split = split;
-    return run_conv2(x_f16, N, H, W, I, wp_f16, Nw, O, a, H, as_stream(stream));
+    return run_conv(x_f16, N, H, W, I, wp_f16, Nw, 9, O, a, as_stream(stream));
 }
 extern "C" int r3dp_sr_tc_layer_torgb_noup(const void* x_f16, const void* wp_f16, const float* bias, const float* wrgb, const float* brgb,
                                            const float* img_prev, int N, int Nw, int I, int O, int H, int W, void* y_f16, float* img_out,
@@ -1704,20 +1636,12 @@ static int tw_conv_up_nearest_impl(const void* x_f16, const void* wp_f16, const 
                                    void* y_f16, int split, r3dp_stream_t stream) {
     R3DP_REQUIRE(x_f16 && wp_f16 && bias && y_f16, "tw_conv_up_nearest: null pointer");
     R3DP_REQUIRE(N > 0 && H > 0 && W % 64 == 0 && W > 0 && (O == 128 || O == 256) && slope >= 0.f && slope <= 1.f, "tw_conv_up_nearest: bad shape / options");
-    Conv2Args a = {};
+    ConvArgs a = {};
     a.n_phases = 4;
-    for (int p = 0; p < 2; ++p)
-        for (int q = 0; q < 2; ++q) {
-            Taps t = {};
-            for (int dy = p - 1; dy <= p; ++dy)
-                for (int dx = q - 1; dx <= q; ++dx) { const int i = t.n++; t.dy[i] = dy; t.dx[i] = dx; t.widx[i] = (p * 2 + q) * 9 + (dy + 1) * 3 + (dx + 1); }
-            Phase2& P = a.ph[p * 2 + q];
-            fill_taps2(P.taps, t);
-            P.rows = H; P.oy_off = p; P.ox_off = q;
-        }
-    a.mode = kStoreAct; a.out = reinterpret_cast<__half*>(y_f16); a.out_H = 2 * H; a.out_W = 2 * W; a.out_C = O; a.oy_mul = a.ox_mul = 2;
+    for (int p = 0; p < 4; ++p) a.ph[p] = {taps_up_nearest(p >> 1, p & 1), H, p >> 1, p & 1};
+    set_output(a, kStoreAct, y_f16, 2 * H, 2 * W, O, 2);
     a.bias = bias; a.act_slope = slope; a.act_gain = 1.0f; a.split = split;
-    return run_conv2(x_f16, N, H, W, I, wp_f16, 1, O, a, H, as_stream(stream), 36);
+    return run_conv(x_f16, N, H, W, I, wp_f16, 1, 36, O, a, as_stream(stream));
 }
 extern "C" int r3dp_tw_conv_up_nearest(const void* x_f16, const void* wp_f16, const float* bias, int N, int I, int O, int H, int W, float slope,
                                        void* y_f16, int split, r3dp_stream_t stream) {
