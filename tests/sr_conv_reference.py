@@ -31,8 +31,8 @@ the element, so beta S bounds the accumulation error whatever the summation orde
 
 beta is the accumulation term: fp32 sums of fp16 x fp16 products (exact in fp32) in the tensor cores' order, plus for split operands
 the dropped lo x lo product (<= 2^-22 |x| |w| per term).  It is set from the worst (|got - ref| - alpha |ref| - extra) / S measured over
-every case of the conformance suite, with headroom (see BETA).  The split mode's worst ratio is ten times the fp16 mode's: its K loop is
-three times longer (hi x hi + lo x hi + hi x lo) and the worst case has 256 input channels, 6912 products per output.
+every case of the conformance suite, with headroom (see BETA).  The split mode's worst ratio is eight to ten times the fp16 mode's: its K
+loop is three times longer (hi x hi + lo x hi + hi x lo) and the worst case has 512 input channels, 3 x 4608 = 13824 products per output.
 
 The exact-fp32 path (csrc/sr_fp32.cu, sr_mode='fp32'; tests/test_gpu_sr_fp32_conformance.py).  Operands are fp32 and NCHW, and every
 product is an fma on fp32 operands, so the conv output is an fp32 sum whose roundings all lie in beta S.  What remains, with
@@ -73,9 +73,12 @@ U_F32 = 2.0 ** -24                           # unit roundoff of fp32
 FLOOR_F16 = 2.0 ** -25                       # half the spacing of fp16 subnormals
 SPLIT_WEIGHT_SCALE = 1024.0                  # split weights are stored x 2^10 so that their lo halves stay normal fp16 numbers
 #: accumulation term per mode.  Worst ratio measured over the conformance suite on one H100 80GB HBM3 (SXM, 700 W power limit):
-#: tc 2.12e-7 (torgb_ex, 256 channels; the worst conv output 1.76e-7, layer_torgb 128 -> 256), tcx 2.27e-6 (layer up=1, 256 -> 128).
-#: beta = 2^-21 = 4.77e-7 (2.2x) and 2^-18 = 3.81e-6 (1.7x).  The kernels are deterministic and every H100 runs the same SASS in the
-#: same summation order, so the headroom only has to cover new cases, not run-to-run noise.
+#: tc 4.25e-7 and tcx 3.45e-6, both the torso head's fuse_head_torso_convs[0] (3x3, 512 -> 256 at 256^2, N = 4): K = 9 x 512 = 4608
+#: products per output, twice the longest K of any other row, and 1.3x to 1.5x the ratios of the 256-channel launches at the same shape
+#: (tc 2.90e-7, tcx 2.62e-6).  The small-shape rows alone: tc 1.75e-7 (layer_torgb 128 -> 256), tcx 2.27e-6 (layer up=1, 256 -> 128);
+#: the rows with I <= 33 input channels 7.2e-8 and 1.0e-6.  beta = 2^-21 = 4.77e-7 (1.12x) and 2^-18 = 3.81e-6 (1.10x), far below the
+#: deterministic bound of fp32 summation, gamma_K = 2.7e-4 at K = 4608.  The kernels are deterministic and every H100 runs the same SASS
+#: in the same summation order, so the headroom only has to cover new cases, not run-to-run noise.
 #: fp32 (tests/test_gpu_sr_fp32_conformance.py), on one H100 80GB HBM3 (SXM, 400 W power limit): 4.27e-7 (the up=2 scratch grid,
 #: 256 -> 128 at 256^2; the worst layer output 3.57e-7, up=1 128 -> 128 at 512^2; ToRGB 2.50e-7; styles 3.42e-8).  beta = 2^-20 =
 #: 9.54e-7 (2.2x), far below gamma_K = 1.37e-4 at K = 9 * 256.

@@ -6,12 +6,19 @@
   The case list covers, per entry point and mode: N = 1 and 3, shared and per-sample weights, odd H where the entry point allows it,
   W = 128 / 256 / 384 (384: an odd number of 128-pixel tiles, which turns the phase interleave of multi-phase launches off) and
   O = 128 / 256, plus one launch of more than 2 x 132 units, so that persistent CTAs run units of several images.
-* Bit-exact properties: image k of an N = 3 per-sample launch equals the N = 1 launch of image k; Nw = 1 equals Nw = N with the
-  weights replicated; a launch repeated gives the same bits; nothing outside the logical output is written (canaries, the lo halves
-  and the uint8 frames included) and every fp16 / fp32 element of it is.
+  PRODUCTION adds every launch of the benchmarked step at its exact shape (up to 4096 units, about 31 per CTA; W = 512, tiles_x = 4; the
+  2048-item FIR pass), PER_SAMPLE the Nw = N variants of block1's two layers; KC32 adds I = 3 / 16 / 32 (the 32-channel K chunks) to
+  every single-phase family and I = 33.  Each launch is compared one image at a time, which bounds the float64 memory.
+* test_benchmarked_launches_have_rows records every conv_tc3 call of one eager step of bench.py's engines and fails, naming the launch,
+  when one has no row here (or, for r3dp_tw_conv*, in tests/test_gpu_torso_warper_layers.py), or when a PRODUCTION row is not launched.
+* Bit-exact properties: image k of an N = 3 per-sample launch equals the N = 1 launch of image k (and the last image of every N = 4
+  launch its N = 1 launch); Nw = 1 equals Nw = N with the weights replicated; a launch repeated gives the same bits; nothing outside the
+  logical output is written (canaries, the lo halves and the uint8 frames included) and every fp16 / fp32 element of it is.
 * The input and packing kernels: weight packing exactly, the composed up weights against the float64 composition, and every input
   resize against float64 bilinear interpolation and bit for bit against each other."""
+import ctypes
 import math
+import re
 
 import pytest
 import torch
@@ -238,11 +245,71 @@ CASES = [
     ('torgb', 1, 1, 128, 0, 6, 384, {'skip': True, 'same_res': 1}),
     ('torgb', 3, 1, 96, 0, 4, 128, {'same_res': 1}),
 ]
+#: every conv_tc3 launch of the benchmarked step (bench.py at batch 4, static styles: one shared weight set), at its exact shape and options;
+#: test_benchmarked_launches_have_rows keeps this list equal to what the step launches
+PRODUCTION = [
+    # SR, FrameEngine in 'tc' and 'tc_exact', and the torso head's block0 / block1
+    ('composed', 4, 1, 32, 256, 128, 128, {}),                     # block0.conv0: 1024 units
+    ('layer_torgb', 4, 1, 256, 256, 256, 256, {'skip': True}),     # block0.conv1 + torgb
+    ('layer2', 4, 1, 256, 128, 256, 256, {}),                      # block1.conv0: transposed conv, 2048 FIR work items, 513-row edge column
+    ('last', 4, 1, 128, 128, 512, 512, {'skip': True, 'clamp': 1}),   # block1.conv1 + torgb: tiles_x = 4, 4096 units (the engine's clamped frames)
+    ('last', 4, 1, 128, 128, 512, 512, {'skip': True}),            # the same, unclamped (RenderHead.synthesis of the torso head)
+    # torso head, fuse mode v2, per step at 256^2
+    ('conv_res', 4, 1, 64, 256, 256, 256, {'ksize': 1, 'act': 0}),        # torso_encoder
+    ('conv_res', 4, 1, 512, 256, 256, 256, {'act': 2}),                    # fuse_head_torso_convs[0]
+    ('conv_res', 4, 1, 256, 256, 256, 256, {'act': 0}),                    # fuse_head_torso_convs[2], fuse_fg_bg_convs[4], bg_encoder[4]
+    ('layer1', 4, 1, 256, 256, 256, 256, {}),                              # head_torso_block.conv0
+    ('noup', 4, 1, 256, 256, 256, 256, {'skip': True}),                    # head_torso_block.conv1 + torgb
+    ('conv_res', 4, 1, 512, 128, 256, 256, {'ksize': 1, 'act': 2}),        # fuse_fg_bg_convs[0] (64 couts padded to 128)
+    ('conv_res', 4, 1, 128, 256, 256, 256, {'act': 2}),                    # fuse_fg_bg_convs[2], bg_encoder[2]
+    ('conv_res', 4, 1, 64, 128, 256, 256, {'act': 2}),                     # bg_encoder[0] (uncached step)
+    # torso head, per clip (begin_clip): bg_encoder on the reference background
+    ('conv_res', 1, 1, 64, 128, 256, 256, {'act': 2}),
+    ('conv_res', 1, 1, 128, 256, 256, 256, {'act': 2}),
+    ('conv_res', 1, 1, 256, 256, 256, 256, {'act': 0}),
+]
+#: block1's two layers with per-sample weights: weight-tap addressing per image at tiles_x = 4 and in the 2048-item FIR pass
+PER_SAMPLE = [
+    ('layer2', 4, 4, 256, 128, 256, 256, {}),
+    ('last', 4, 4, 128, 128, 512, 512, {'skip': True, 'clamp': 1}),
+]
+#: I <= 32 runs the 32-channel K chunks (a 16-slot weight-tap ring, 64-byte swizzle) on every single-phase family; I = 33 is the smallest
+#: launch on 64-channel chunks with padding
+KC32 = [
+    ('layer1', 3, 3, 3, 128, 6, 128, {}),
+    ('layer1', 1, 1, 16, 256, 7, 384, {}),
+    ('layer1', 2, 1, 32, 256, 96, 256, {}),                        # 384 units
+    ('conv_res', 3, 3, 32, 128, 5, 256, {'res': True}),
+    ('conv_res', 1, 1, 3, 256, 7, 128, {'act': 3, 'res': True}),
+    ('conv_res', 2, 1, 16, 128, 6, 384, {'ksize': 1, 'act': 2}),
+    ('conv_res', 3, 3, 32, 256, 4, 128, {'ksize': 1, 'act': 0, 'res': True}),
+    ('layer_torgb', 3, 3, 32, 256, 8, 256, {'skip': True}),
+    ('layer_torgb', 1, 1, 3, 128, 6, 128, {'skip': True}),
+    ('layer_torgb', 2, 1, 16, 128, 4, 384, {}),
+    ('noup', 3, 1, 16, 256, 6, 256, {'skip': True}),
+    ('noup', 1, 1, 32, 128, 7, 384, {}),
+    ('noup', 2, 2, 3, 128, 5, 128, {'skip': True}),
+    ('last', 3, 3, 32, 128, 8, 256, {'skip': True}),
+    ('last', 1, 1, 16, 128, 6, 128, {'clamp': 1}),
+    ('last', 3, 1, 3, 128, 4, 128, {'u8': True, 'skip': True}),
+    ('last', 1, 1, 32, 128, 2, 384, {'u8': True}),
+    ('layer1', 2, 2, 33, 128, 7, 256, {}),                         # 64-channel chunks, 31 of them padding
+]
+CASES += PRODUCTION + PER_SAMPLE + KC32
 
 
 def _case_id(c):
     fam, N, Nw, I, O, H, W, opt = c
     return f'{fam}-N{N}w{Nw}-I{I}-O{O}-{H}x{W}' + ''.join(f'-{k}{int(v)}' for k, v in sorted(opt.items()))
+
+
+def _check_images(P, out, mode, tag):
+    """The bound on every output of a launch, one image at a time: the float64 reference of a whole N = 4 launch at 512^2 would take over
+    10 GB at once."""
+    for k in range(P['N']):
+        one = {name: t[k:k + 1] for name, t in out.items()}
+        for name, ref, S, alpha, extra in _reference(_slice(P, k)):
+            scr.check_bound(_got(P, one, name), ref, S, alpha, scr.BETA[mode], extra, f'{tag} image {k} {name}')
 
 
 @pytest.mark.parametrize('mode', MODES)
@@ -255,16 +322,17 @@ def test_conv_vs_float64(case, mode):
     if P['u8']:
         P_f32 = dict(P, u8=False, clamp=1)                            # the same launch with a clamped fp32 image
         out = _run(P_f32)
-        for name, ref, S, alpha, extra in _reference(P_f32):
-            scr.check_bound(_got(P_f32, out, name), ref, S, alpha, scr.BETA[mode], extra, f'{tag} {name}')
+        _check_images(P_f32, out, mode, tag)
         u8 = _run(P, canary=True)['u8']
         assert torch.equal(u8, scr.to_uint8(out['img'])), f'{tag}: uint8 frames differ from the conversion of the fp32 image'
         return
     out = _run(P, canary=True)
-    for name, ref, S, alpha, extra in _reference(P):
-        scr.check_bound(_got(P, out, name), ref, S, alpha, scr.BETA[mode], extra, f'{tag} {name}')
+    _check_images(P, out, mode, tag)
     if split and 'y' in out:
         _check_split_layout(out['y'])
+    if case in PRODUCTION or case in PER_SAMPLE:                      # the last image is computed by the CTAs' last units
+        k = N - 1
+        _assert_same_bits(_run(_slice(P, k)), {name: t[k:k + 1] for name, t in out.items()}, f'{tag}: image {k} vs its N=1 launch')
 
 
 # ---- bit-exact properties ----------------------------------------------------------------------------------------------------------------
@@ -278,6 +346,7 @@ BITS = {
     'conv_res': (64, 128, 96, 256, {'act': 2, 'res': True}),
     'noup': (64, 256, 96, 256, {'skip': True}),
     'torgb': (128, 0, 8, 256, {'skip': True}),
+    'last-kc32': (32, 128, 96, 256, {'skip': True}),                # the 32-channel K chunks: 288 units, fp32 image and uint8 frames
 }
 
 
@@ -306,11 +375,11 @@ def _assert_same_bits(a, b, what):
 
 
 @pytest.mark.parametrize('mode', MODES)
-@pytest.mark.parametrize('fam', list(BITS))
-def test_conv_bits_slicing_shared_determinism_canaries(fam, mode):
-    I, O, H, W, opt = BITS[fam]
-    split = mode == 'tcx'
-    P = _operands(fam, split, 3, 3, I, O, H, W, seed=2000 + list(BITS).index(fam), **opt)
+@pytest.mark.parametrize('key', list(BITS))
+def test_conv_bits_slicing_shared_determinism_canaries(key, mode):
+    I, O, H, W, opt = BITS[key]
+    split, fam = mode == 'tcx', key.split('-')[0]
+    P = _operands(fam, split, 3, 3, I, O, H, W, seed=2000 + list(BITS).index(key), **opt)
     full = _run(P, canary=True)
     _assert_same_bits(full, _run(P, canary=True), f'{fam} {mode}: repeated launch')
     for k in range(3):
@@ -322,6 +391,120 @@ def test_conv_bits_slicing_shared_determinism_canaries(fam, mode):
         _assert_same_bits(_run(Q, canary=True), _run(Q, canary=True), f'{fam} {mode}: repeated uint8 launch')
     if split and 'y' in full:
         _check_split_layout(full['y'])
+
+
+# ---- the launches of the benchmarked step ------------------------------------------------------------------------------------------------
+#: the C entry points that launch conv_tc3
+CONV_ENTRY = re.compile(r'r3dp_sr_tcx?_(layer|layer_up_composed|layer_torgb|layer_torgb_noup|conv|conv_res|last_layer|last_layer_ex)$|r3dp_tw_conv')
+
+
+class _Recorder:
+    """Stands in for the library object: records the arguments of every conv_tc3 entry point and passes every call on unchanged."""
+
+    def __init__(self, lib):
+        self.lib, self.calls = lib, []
+
+    def __getattr__(self, name):
+        fn = getattr(self.lib, name)
+        if not CONV_ENTRY.match(name):
+            return fn
+
+        def call(*args):
+            self.calls.append((name, args))
+            return fn(*args)
+        return call
+
+
+def _given(p):
+    """A pointer argument is not NULL (capi.ptr(None) is a NULL c_void_p; callers also pass None)."""
+    return (p.value if isinstance(p, ctypes.c_void_p) else p) is not None
+
+
+def _f32(v):
+    return ctypes.c_float(v).value
+
+
+def _row_of_call(name, a):
+    """(table, row) of one recorded launch: a CASES row of this module, or for the torso warper's r3dp_tw_conv* a CONV_CASES / UP_CASES row
+    of tests/test_gpu_torso_warper_layers.py."""
+    if name == 'r3dp_tw_conv':
+        return 'CONV_CASES', (a[3], a[6], a[7], a[4], a[5], a[8], _f32(a[9]), _given(a[10]))
+    if name == 'r3dp_tw_conv_up_nearest':
+        return 'UP_CASES', (a[3], a[6], a[7], a[4], a[5], _f32(a[8]))
+    op, opt = name.split('_', 3)[3], {}
+    if op in ('layer', 'layer_up_composed'):
+        fam = 'composed' if op == 'layer_up_composed' else ('layer1' if a[9] == 1 else 'layer2')
+        N, Nw, I, O, H, W = a[3:9]
+    elif op in ('layer_torgb', 'layer_torgb_noup'):
+        fam = 'layer_torgb' if op == 'layer_torgb' else 'noup'
+        N, Nw, I, O, H, W = a[6:12]
+        opt['skip'] = _given(a[5])
+    elif op in ('conv', 'conv_res'):
+        fam = 'conv_res'
+        N, Nw, I, O, H, W, opt['ksize'], opt['act'] = a[3:11]
+        opt['res'] = op == 'conv_res' and _given(a[11])
+    else:                                                             # last_layer(_ex): 128 couts, the image only
+        fam, O = 'last', 128
+        N, Nw, I, H, W = a[6:11]
+        opt['skip'] = _given(a[5])
+        if op == 'last_layer_ex' or name.startswith('r3dp_sr_tcx_'):
+            opt['u8'], opt['clamp'] = _given(a[12]), a[13]
+    return 'CASES', (fam, N, Nw, I, O, H, W, {k: v for k, v in opt.items() if v != DEFAULT_OPT[k]})
+
+
+#: the options of a CASES row that _operands() defaults
+DEFAULT_OPT = {'ksize': 3, 'act': 1, 'skip': False, 'res': False, 'clamp': 0, 'u8': False, 'same_res': 0}
+
+
+def _signature(table, row):
+    """What decides a launch: the row with every option at its default made explicit (a uint8 launch clamps)."""
+    if table == 'CONV_CASES':
+        return row[:6] + (_f32(row[6]), bool(row[7]))
+    if table == 'UP_CASES':
+        return row[:5] + (_f32(row[5]),)
+    fam, N, Nw, I, O, H, W, opt = row
+    o = dict(DEFAULT_OPT, **opt)
+    return (fam, N, Nw, I, O, H, W, o['ksize'], o['act'], bool(o['skip']), bool(o['res']), int(bool(o['clamp'] or o['u8'])), bool(o['u8']),
+            o['same_res'])
+
+
+def test_benchmarked_launches_have_rows(monkeypatch):
+    """Every conv_tc3 launch of the benchmarked step has a float64 row of the same shape and options: bench.py's FrameEngine(batch=4) in 'tc'
+    and in 'tc_exact', and its configs[4], the torso head (stub warper, fuse mode v2) through RenderHead.synthesis without the clip's
+    constants and through the engine after begin_clip().  One eager step of each, recorded at the C entry points."""
+    import test_gpu_torso_warper_layers as twl
+    from real3dportrait_b200 import engine, synthetic as syn
+    rec = _Recorder(capi.lib())
+    monkeypatch.setattr(capi, '_lib', rec)
+    B = 4
+    planes, cams = syn.make_planes(B, seed=80).to(DEV), syn.make_cameras(B, seed=81).to(DEV)
+    u_c, u_f = (u.to(DEV) for u in syn.make_jitter(B, 64 * 64, 48, 48, seed=82))
+    mlp = syn.make_decoder_params(seed=4)
+    for mode in ('tc', 'tc_exact'):
+        eng = engine.FrameEngine(batch=B, sr_mode=mode, use_graph=False, hp={'num_samples_fine': 0})
+        eng.load_params(mlp, syn.make_sr_params(seed=5))
+        eng.step(planes, cams, u_c)
+    eng = engine.FrameEngine(batch=B, sr_mode='tc', use_graph=False, hp=dict(syn.WARP_HPARAMS, num_samples_fine=48), torso_model=syn.StubTorsoModel())
+    eng.load_params(mlp, syn.make_sr_warp_params(seed=6))
+    inp = {k: v.to(DEV) for k, v in syn.make_warp_inputs(1, seed=7).items()}
+    kp_d = (torch.rand(B, 68, 3, generator=torch.Generator().manual_seed(9)) * 2 - 1).to(DEV)
+    cond = {'ref_torso_img': inp['ref_torso_rgb'].expand(B, -1, -1, -1).contiguous(), 'bg_img': inp['ref_bg_rgb'].expand(B, -1, -1, -1).contiguous(),
+            'segmap': inp['segmap'].expand(B, -1, -1, -1).contiguous(), 'kp_s': inp['kp_s'].expand(B, -1, -1).contiguous(), 'kp_d': kp_d}
+    eng.head.synthesis(planes, cams, cond=cond, u_coarse=u_c, u_fine=u_f)
+    eng.begin_clip(inp['ref_torso_rgb'], inp['ref_bg_rgb'], inp['segmap'], inp['kp_s'])
+    eng.step(planes, cams, u_c, u_f, kp_d=kp_d)
+    torch.cuda.synchronize()
+    tables = {'CASES': CASES, 'CONV_CASES': twl.CONV_CASES, 'UP_CASES': twl.UP_CASES}
+    have = {(t, _signature(t, row)) for t, rows in tables.items() for row in rows}
+    launches = {}
+    for name, args in rec.calls:
+        t, row = _row_of_call(name, args)
+        launches.setdefault((t, _signature(t, row)), (name, t, row))
+    assert {row[0] for _, t, row in launches.values()} >= {'composed', 'layer_torgb', 'layer2', 'last', 'conv_res', 'layer1', 'noup'}
+    missing = [f'{name}: {row} (in {t})' for key, (name, t, row) in launches.items() if key not in have]
+    assert not missing, 'launches of the benchmarked step without a float64 row:\n' + '\n'.join(missing)
+    stale = [row for row in PRODUCTION if ('CASES', _signature('CASES', row)) not in launches]
+    assert not stale, f'PRODUCTION rows the benchmarked step no longer launches: {stale}'
 
 
 # ---- packing kernels ---------------------------------------------------------------------------------------------------------------------

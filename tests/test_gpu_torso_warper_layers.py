@@ -62,6 +62,7 @@ CONV_CASES = [
     (3, 64, 64, 256, 256, 3, 1.0, True),
     (3, 32, 128, 128, 128, 3, 0.0, True),
     (3, 16, 256, 64, 128, 3, 0.2, False),
+    (3, 64, 64, 32, 128, 3, 0.2, False),          # I <= 32: the 32-channel K chunks at W = 64 (one tile per row, its right half TMA zero fill)
 ]
 
 
