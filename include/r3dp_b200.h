@@ -396,6 +396,42 @@ int r3dp_mf_deform(const float* logits, int ls, const float* kp_s, const float* 
 int r3dp_mf_occlusion(const void* x_f16, int N, int D, int H, int W, int C, int xs, int xlo, int split, const float* wk, const float* bias, float* occ,
                       float* occ2, r3dp_stream_t stream);
 
+/* ------------------------------------------------ SECC -> plane backbone: SegFormerSECC2PlaneBackbone('b0') ---
+ * (modules/real3d/segformer.py:673-733; called per frame by cal_secc_plane, modules/real3d/secc_img2plane.py:64-81).  Token tensors are
+ * row-major [N, h*w, C] (row = the NHWC pixel h*W + w).  The GEMMs (q, kv, proj, fc1, fc2, patch embeds 2-4, the spatial reduction, the folded
+ * head maps and the last conv) run on r3dp_mf_conv3d with 1x1x1 or 1x3x3 taps; to_plane_cnn.0/2/4 on r3dp_sr_tc_conv (act 2) where W % 128 == 0.
+ * r3dp_sp_prenet          prenet 1x1 (Conv2dLayer, networks_stylegan2.py:139-183, weight gain folded into w [3,cin]): x [N,cin,H,W] -> y [N,3,H,W];
+ *                         used once per clip on the cano/src channels to make the constant image
+ * r3dp_sp_embed           prenet + patch_embed1.proj (7x7 stride 4 pad 3, segformer.py:206-232) -> y fp32 [N, ceil(H/4)*ceil(W/4), 32], before its
+ *                         LayerNorm.  Prenet output = (base ? base[1,3,H,W] : bpre[3]) + w [3,cin] . x[N,cin,H,W]; wpe [32,3,7,7], bpe [32]
+ * r3dp_sp_layernorm       v = x + t (t may be NULL); xo = v if non-NULL (xo may be x: the in-place residual add of Block.forward, segformer.py:236-239);
+ *                         u = LayerNorm(v)(g, b, eps) (segformer.py:118,216,411) -> yf fp32 [R,C] and/or yh fp16 with row stride yhs; C % 32 == 0, <= 256
+ * r3dp_sp_patches         y fp16 [N*Ho*Wo, k*k*C], column (ky*k + kx)*C + c = x[n, oy*s - p + ky, ox*s - p + kx, c] (zero outside): GEMM rows of
+ *                         the 3x3/2 patch embeds (segformer.py:286-291) and of Attention.sr (k = s = sr_ratio, segformer.py:126-128); C % 8 == 0
+ * r3dp_sp_attention       Attention.forward's core (segformer.py:130-150) for head_dim 32: q fp16 [N,Tq, >= heads*32] (row stride qs), kv fp16
+ *                         [N,Tk, >= 2*heads*32] (k in channels [0, 32 heads), v after it), Tk <= 256 -> o fp16 (row stride os), channel head*32 + d;
+ *                         fp32 scores and an exact full-row softmax
+ * r3dp_sp_dwconv_gelu     Mlp's DWConv 3x3 + bias then nn.GELU (erf) (segformer.py:82-84,459-468): x, y fp16 NHWC [N,H,W,C], w [C,9], b [C]
+ * r3dp_sp_head_fuse       SegFormerHead.forward (segformer.py:525-537) after the fold: y fp16 NHWC [N,h1,h1,256] = ReLU(sum_i resize_i(g_i) + bias),
+ *                         g_i fp32 NHWC [N,h_i,h_i,256] = G_i c_i, resize = bilinear align_corners=False to h1 x h1
+ * r3dp_sp_leaky           nn.LeakyReLU(slope) in place on n fp16 values (to_plane_cnn.1/3/5 where the conv ran on r3dp_mf_conv3d)
+ * r3dp_sp_upsample2_flip  nn.UpsamplingBilinear2d(x2) (align_corners=True) of x fp16 NHWC [N,h,w,C] written twice, mirrored: yr [N,2h,2w,C] rows
+ *                         mirrored, yrc rows and columns mirrored.  A 3x3 zero-padded conv of a mirrored image with mirrored taps is the mirrored
+ *                         conv, so the last conv run on these writes the flipped planes of segformer.py:722-730 directly. */
+int r3dp_sp_prenet(const float* x, int N, int cin, int H, int W, const float* w, const float* b, float* y, r3dp_stream_t stream);
+int r3dp_sp_embed(const float* x, int N, int cin, int H, int W, const float* wpre, const float* base, const float* bpre, const float* wpe,
+                  const float* bpe, float* y, r3dp_stream_t stream);
+int r3dp_sp_layernorm(const float* x, const float* t, int R, int C, const float* g, const float* b, float eps, float* xo, float* yf, void* yh_f16,
+                      int yhs, r3dp_stream_t stream);
+int r3dp_sp_patches(const void* x_f16, int N, int H, int W, int C, int k, int s, int p, void* y_f16, r3dp_stream_t stream);
+int r3dp_sp_attention(const void* q_f16, int qs, const void* kv_f16, int kvs, int N, int Tq, int Tk, int heads, float scale, void* o_f16, int os,
+                      r3dp_stream_t stream);
+int r3dp_sp_dwconv_gelu(const void* x_f16, int N, int H, int W, int C, const float* w, const float* b, void* y_f16, r3dp_stream_t stream);
+int r3dp_sp_head_fuse(const float* g1, int h1, const float* g2, int h2, const float* g3, int h3, const float* g4, int h4, int N, const float* bias,
+                      void* y_f16, r3dp_stream_t stream);
+int r3dp_sp_leaky(void* x_f16, long long n, float slope, r3dp_stream_t stream);
+int r3dp_sp_upsample2_flip(const void* x_f16, int N, int h, int w, int C, void* yr_f16, void* yrc_f16, r3dp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -11,7 +11,9 @@ from .decoder import FullyConnectedLayer, OSGDecoder
 from .superresolution import SuperresolutionHybrid8XDC, SynthesisBlock, SynthesisLayer, ToRGBLayer
 from .sr_with_ref import SuperresolutionHybrid8XDC_Warp, SynthesisBlockNoUp
 from .synthesis import RenderHead
+from .secc2plane import SegFormerSECC2PlaneBackbone, canonical_planes_cl
 
 __all__ = ['RaySampler', 'ImportanceRenderer', 'PlanesCL', 'generate_planes', 'planes_to_channels_last',
            'sample_from_planes', 'sample_from_trigrids', 'grids_to_channels_last', 'producer_view', 'MipRayMarcher2', 'FullyConnectedLayer', 'OSGDecoder', 'SuperresolutionHybrid8XDC',
-           'SynthesisBlock', 'SynthesisLayer', 'ToRGBLayer', 'SuperresolutionHybrid8XDC_Warp', 'SynthesisBlockNoUp', 'RenderHead']
+           'SynthesisBlock', 'SynthesisLayer', 'ToRGBLayer', 'SuperresolutionHybrid8XDC_Warp', 'SynthesisBlockNoUp', 'RenderHead',
+           'SegFormerSECC2PlaneBackbone', 'canonical_planes_cl']

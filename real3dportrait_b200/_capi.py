@@ -123,6 +123,15 @@ _SIGNATURES = {
     'r3dp_mf_head_bcast': (_I, [_P] + [_I] * 7 + [_P, _I, _I, _I, _I, _P]),
     'r3dp_mf_deform': (_I, [_P, _I, _P, _P] + [_I] * 5 + [_P, _P]),
     'r3dp_mf_occlusion': (_I, [_P] + [_I] * 8 + [_P, _P, _P, _P, _P]),
+    'r3dp_sp_prenet': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P]),
+    'r3dp_sp_embed': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
+    'r3dp_sp_layernorm': (_I, [_P, _P, _I, _I, _P, _P, _F, _P, _P, _P, _I, _P]),
+    'r3dp_sp_patches': (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
+    'r3dp_sp_attention': (_I, [_P, _I, _P, _I, _I, _I, _I, _I, _F, _P, _I, _P]),
+    'r3dp_sp_dwconv_gelu': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P]),
+    'r3dp_sp_head_fuse': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _I, _P, _P, _P]),
+    'r3dp_sp_leaky': (_I, [_P, C.c_longlong, _F, _P]),
+    'r3dp_sp_upsample2_flip': (_I, [_P, _I, _I, _I, _I, _P, _P, _P]),
 }
 
 

@@ -123,13 +123,19 @@ class FrameEngine:
     warper_in_graph: capture the warper inside the step's single graph (only for capturable warpers; the default runs it eagerly
     between two graphs).  torso_stage2='cuda': the warper's stage 2 on this library's kernels, its appearance features cached per clip by
     begin_clip() (SuperresolutionHybrid8XDC_Warp.set_torso_stage2).  torso_motion='cuda' (needs torso_stage2='cuda'): the warper's
-    motion-field estimator on this library's 3-D convolutions too (SuperresolutionHybrid8XDC_Warp.set_torso_motion)."""
+    motion-field estimator on this library's 3-D convolutions too (SuperresolutionHybrid8XDC_Warp.set_torso_motion).
+    secc2plane: a SegFormerSECC2PlaneBackbone; the engine then runs it inside the step (captured in the step's graph, graph A of the torso
+    split): begin_planes(cano_planes, cond_cano, cond_src) once per clip, then step(None, cameras, ..., cond_tgt=drv_secc) renders
+    cano_planes + backbone(cat[cano, src, tgt]) (secc_img2plane.py:64-81) without materialising either plane set; prepare() tuples and
+    step_host() take the driving SECC image [B,3,H,W] in the planes slot."""
 
     def __init__(self, batch: int = 4, sr_mode: str = 'fp32', device=None, world: int = 1, rank: int = 0, dist=None, hp: Optional[dict] = None,
                  static_styles: bool = True, use_graph: bool = True, out_uint8: bool = False, exchange: str = 'allgather',
                  torso_model: Optional[torch.nn.Module] = None, warper_in_graph: bool = False, torso_stage2: str = 'torch',
-                 torso_motion: str = 'torch'):
+                 torso_motion: str = 'torch', secc2plane: Optional[torch.nn.Module] = None):
         assert exchange in ('allgather', 'p2p', 'none')
+        if secc2plane is not None and (hp or {}).get('phase1_plane_fusion_mode', 'add') != 'add':
+            raise NotImplementedError('secc2plane: only phase1_plane_fusion_mode="add" (cano + secc, secc_img2plane.py:76-77) is built')
         self.batch, self.world, self.rank, self.dist = batch, world, rank, dist
         self.device = device if device is not None else torch.device('cuda', torch.cuda.current_device())
         self.head = RenderHead(hp=hp, sr_mode=sr_mode, torso_model=torso_model).to(self.device).eval()
@@ -143,6 +149,8 @@ class FrameEngine:
             if not self.torso:
                 raise ValueError('torso_motion is an option of the torso head: FrameEngine(torso_model=...)')
             self.head.superresolution.set_torso_motion(torso_motion)
+        self.secc = secc2plane.to(self.device).eval() if secc2plane is not None else None
+        self._cano_cl = None              # secc2plane: the clip's canonical planes, 'hwpc' [1,H,W,3,C] (begin_planes)
         self.out_uint8 = bool(out_uint8)
         if self.out_uint8 and self.head.superresolution.sr_mode not in ('tc', 'tc_exact'):     # the head's effective mode: a torso head maps 'fp32' to 'tc'
             raise NotImplementedError('uint8 frames are written by the tensor-core SR epilogue (sr_mode="tc")')
@@ -205,6 +213,29 @@ class FrameEngine:
                 self._consts[k].copy_(v)
         self._consts.update({'ref_torso_img': ref_torso_img, 'bg_img': bg_img})
 
+    @torch.no_grad()
+    def begin_planes(self, cano_planes: torch.Tensor, cond_cano: torch.Tensor, cond_src: Optional[torch.Tensor] = None) -> None:
+        """secc2plane engines: the clip's canonical planes [1,3,32,256,256] and the backbone's per-clip SECC images [1,3,H,W] (cond_src only in
+        'cano_src_tgt').  A later begin_planes() refills the same buffers in place, so graphs captured for an earlier clip render the new one."""
+        if self.secc is None:
+            raise ValueError('begin_planes() needs FrameEngine(secc2plane=...)')
+        from .secc2plane import canonical_planes_cl
+        cl = canonical_planes_cl(cano_planes.to(self.device))
+        if self._cano_cl is not None and self._cano_cl.data.shape == cl.data.shape:
+            self._cano_cl.data.copy_(cl.data)
+        else:
+            self._cano_cl = cl
+            self.graph, self.inplace = None, {}
+        self.secc.begin_clip(cond_cano.to(self.device), None if cond_src is None else cond_src.to(self.device))
+
+    def _planes(self, planes):
+        """The render's plane sets: with secc2plane, `planes` is the driving SECC image and the backbone runs here (inside the capture)."""
+        if self.secc is None:
+            return planes
+        if self._cano_cl is None:
+            raise RuntimeError('secc2plane: call begin_planes(cano_planes, cond_cano, cond_src) before the first step')
+        return (self._cano_cl, self.secc.planes_cl(planes))
+
     def end_clip(self) -> None:
         """Release the clip's constants, and the graphs that read them."""
         if self.torso:
@@ -236,7 +267,7 @@ class FrameEngine:
     @torch.no_grad()
     def _body(self, planes, cameras, u_coarse, u_fine=None, kp_d=None) -> torch.Tensor:
         cond = self._cond(kp_d) if self.torso else None
-        return self.head.synthesis(planes, cameras, cond=cond, lean=True, out_uint8=self.out_uint8, **self._over(u_coarse, u_fine))['image']
+        return self.head.synthesis(self._planes(planes), cameras, cond=cond, lean=True, out_uint8=self.out_uint8, **self._over(u_coarse, u_fine))['image']
 
     def _capture_graph(self, planes, cameras, u_coarse, u_fine=None, kp_d=None):
         if self.torso and not self.warper_in_graph:
@@ -260,7 +291,7 @@ class FrameEngine:
     def _capture_split(self, planes, cameras, u_coarse, u_fine, kp_d):
         """Torso step as graph A -> eager warper -> graph B (see _TorsoGraphs); returns (graphs, output buffer)."""
         sr, over = self.head.superresolution, self._over(u_coarse, u_fine)
-        pre = lambda: self.head.torso_pre(planes, cameras, self._cond(kp_d), self.out_uint8, **over)   # noqa: E731
+        pre = lambda: self.head.torso_pre(self._planes(planes), cameras, self._cond(kp_d), self.out_uint8, **over)   # noqa: E731
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side), torch.no_grad():
@@ -324,12 +355,19 @@ class FrameEngine:
 
     @torch.no_grad()
     def step(self, planes, cameras: torch.Tensor, u_coarse: Optional[torch.Tensor] = None, u_fine: Optional[torch.Tensor] = None,
-             frame_index: Optional[int] = None, *, kp_d: Optional[torch.Tensor] = None) -> torch.Tensor:
+             frame_index: Optional[int] = None, *, kp_d: Optional[torch.Tensor] = None, cond_tgt: Optional[torch.Tensor] = None) -> torch.Tensor:
         """planes [B,3,32,256,256] | PlanesCL | (cano, secc); cameras [B,25]; u_coarse [B,4096,S,1], u_fine [B*4096,S_imp] (drawn here if None)
         -> this rank's frames: fp32 [B,3,512,512] in [-1,1] or uint8 [B,512,512,3]; with exchange='allgather' the gathered
         [world*B,...] (rank-major); with exchange='p2p' the frames are additionally pushed into the open clip at `frame_index`.
         kp_d [B,68,3]: the frames' driving key points, the torso head's only per-frame condition (torso engines only).
+        cond_tgt [B,3,H,W]: the driving SECC image, in place of planes (pass None), for FrameEngine(secc2plane=...).
         The returned tensor is reused by the next step."""
+        if self.secc is not None:
+            if planes is not None or cond_tgt is None:
+                raise ValueError('secc2plane engine: step(None, cameras, ..., cond_tgt=drv_secc)')
+            planes = cond_tgt
+        elif cond_tgt is not None:
+            raise ValueError('cond_tgt needs FrameEngine(secc2plane=...)')
         self._check_kp_d(kp_d)
         drawn = u_coarse is None or (u_fine is None and self._needs_fine())
         u_coarse, u_fine = self._draw(cameras.shape[0], cameras.device, u_coarse, u_fine)
@@ -513,7 +551,8 @@ class FrameEngine:
                     dst.copy_(src, non_blocking=True)
             hp['in_ready'][k].record(hp['copy_in'])
         cur.wait_event(hp['in_ready'][k])
-        out = self.step(*stage[:4], kp_d=stage[4]) if self.torso else self.step(*stage)
+        p0, tgt = (None, {'cond_tgt': stage[0]}) if self.secc is not None else (stage[0], {})      # secc2plane: h_planes is the driving SECC image
+        out = self.step(p0, *stage[1:4], kp_d=stage[4], **tgt) if self.torso else self.step(p0, *stage[1:], **tgt)
         self.wait_gather()
         hp['in_free'][k].record(cur)
         cur.wait_event(hp['out_free'][k])
