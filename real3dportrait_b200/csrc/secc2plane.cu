@@ -364,11 +364,9 @@ extern "C" int r3dp_sp_attention(const void* q_f16, int qs, const void* kv_f16, 
     R3DP_REQUIRE(N > 0 && Tq > 0 && Tk > 0 && Tk <= kMaxKeys && heads > 0 && qs >= C && kvs >= 2 * C && os >= C && qs % 2 == 0 && os % 2 == 0,
                  "sp_attention: bad shape (head_dim 32, at most 256 keys)");
     const int smem = 2 * Tk * kHd * (int)sizeof(float);
-    static bool smem_set = false;                                 // once per process (the attribute is per function, not per launch)
-    if (!smem_set) {
-        R3DP_CUDA(cudaFuncSetAttribute(sp_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kMaxKeys * kHd * (int)sizeof(float)));
-        smem_set = true;
-    }
+    // the limit belongs to the current device's function, so it is set on every call (as every other launcher does): a process that drives
+    // a second GPU would otherwise launch there with the 48 KB default and be refused at Tk > 192
+    R3DP_CUDA(cudaFuncSetAttribute(sp_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kMaxKeys * kHd * (int)sizeof(float)));
     const dim3 grid(blocks(Tq, 128), heads, N);
     sp_attention_kernel<<<grid, 128, smem, as_stream(stream)>>>(reinterpret_cast<const __half*>(q_f16), qs, reinterpret_cast<const __half*>(kv_f16), kvs,
                                                                 Tq, Tk, C, scale, reinterpret_cast<__half*>(o_f16), os);

@@ -4,6 +4,7 @@ fixture the reference's own class wrote (tests/golden/secc2plane_small.npz).
 
 Also here: the seeded synthetic parameters and inputs the fixture and the tests share, and the shims that let the reference's segformer.py
 import without timm / mmcv (tests/golden/make_golden_secc2plane.py)."""
+import ctypes
 import math
 import sys
 import types
@@ -142,6 +143,86 @@ def forward(sd, x):
 
 def to64(sd, device='cpu'):
     return {k: (v.to(device, torch.float64) if v.is_floating_point() else v.to(device)) for k, v in sd.items()}
+
+
+# ---- the library's launch sequence, restated from the architecture ----------------------------------------------------------------------
+EMB = 256
+
+
+def launch_signature(fn, args):
+    """(entry point, non-pointer arguments) with every float argument rounded to fp32, as the C side receives it."""
+    return fn, tuple(ctypes.c_float(a).value if isinstance(a, float) else a for a in args)
+
+
+def cop_of(cout):
+    """Packed couts of an r3dp_mf_conv3d launch: cout rounded up to its cout tile (16, 32, 64 or 128)."""
+    bn = 16 if cout <= 16 else 32 if cout <= 32 else 64 if cout <= 64 else 128
+    return -(-cout // bn) * bn
+
+
+def launch_plan(H, B, cin=9):
+    """Every kernel launch of SegFormerSECC2PlaneBackbone.forward on [B, cin, H, H], as (tag, C entry point, the non-pointer arguments in C
+    order), written from the architecture above (MiT-b0 stages, SegFormerHead, to_plane_cnn) rather than from the module's code.  The
+    per-launch tests build their tables from it, and a test that records the module's calls holds it to what the module launches."""
+    plan = []
+
+    def add(tag, fn, *args):
+        plan.append((tag, fn, tuple(args)))
+
+    def gemm(tag, R, K, O, f32):
+        add(tag, 'r3dp_mf_conv3d', K, 0, K, 1, 1, 1, R, 1, 1, 1, 0, O, cop_of(O), 0, O, 0, 0, int(f32), 0)
+
+    def ln(tag, R, C, eps):
+        add(tag, 'r3dp_sp_layernorm', R, C, eps, C)
+
+    def patches(tag, h, C, k, s, p):
+        add(tag, 'r3dp_sp_patches', B, h, h, C, k, s, p)
+        return (h + 2 * p - k) // s + 1
+
+    h = (H - 1) // 4 + 1
+    add('embed', 'r3dp_sp_embed', B, cin, H, H)
+    levels = []
+    for s in range(4):
+        C, st = EMBED[s], f's{s + 1}'
+        if s > 0:
+            h = patches(st + '.pe_patches', h, EMBED[s - 1], 3, 2, 1)
+            gemm(st + '.pe', B * h * h, 9 * EMBED[s - 1], C, True)
+        R = B * h * h
+        ln(st + '.pe_norm', R, C, 1e-5)
+        ln(st + '.norm1', R, C, 1e-6)
+        for bi in range(2):
+            gemm(st + '.q', R, C, C, False)
+            if SR[s] > 1:
+                hk = patches(st + '.sr_patches', h, C, SR[s], SR[s], 0)
+                gemm(st + '.sr', B * hk * hk, SR[s] ** 2 * C, C, True)
+                ln(st + '.sr_norm', B * hk * hk, C, 1e-5)
+                gemm(st + '.kv', B * hk * hk, C, 2 * C, False)
+                tk = hk * hk
+            else:
+                gemm(st + '.kv', R, C, 2 * C, False)
+                tk = h * h
+            add(st + '.attention', 'r3dp_sp_attention', C, 2 * C, B, h * h, tk, HEADS[s], 32 ** -0.5, C)
+            gemm(st + '.proj', R, C, C, True)
+            ln(st + '.norm2', R, C, 1e-6)
+            gemm(st + '.fc1', R, C, 4 * C, False)
+            add(st + '.dwconv', 'r3dp_sp_dwconv_gelu', B, h, h, 4 * C)
+            gemm(st + '.fc2', R, 4 * C, C, True)
+            ln(st + ('.norm1' if bi == 0 else '.norm'), R, C, 1e-6)
+        levels.append(h)
+    for i, hh in enumerate(levels):
+        gemm(f'G{i + 1}', B * hh * hh, EMBED[i], EMB, True)
+    h1 = levels[0]
+    add('head_fuse', 'r3dp_sp_head_fuse', levels[0], levels[1], levels[2], levels[3], B)
+    for i in (0, 2, 4):
+        if h1 % 128 == 0:
+            add(f'to_plane_cnn.{i}', 'r3dp_sr_tc_conv', B, 1, EMB, EMB, h1, h1, 3, 2)
+        else:
+            add(f'to_plane_cnn.{i}', 'r3dp_mf_conv3d', EMB, 0, EMB, B, 1, h1, h1, 1, 3, 3, 0, EMB, EMB, 0, EMB, 0, 0, 0, 0)
+            add(f'to_plane_cnn.{i + 1}', 'r3dp_sp_leaky', B * h1 * h1 * EMB, 0.01)
+    add('upsample', 'r3dp_sp_upsample2_flip', B, h1, h1, EMB)
+    for O, c0 in ((64, 0), (32, 64)):
+        add(f'to_plane_cnn.7[{c0}:{c0 + O}]', 'r3dp_mf_conv3d', EMB, 0, EMB, B, 1, 2 * h1, 2 * h1, 1, 3, 3, 0, O, cop_of(O), 0, 96, c0, 0, 1, 0)
+    return plan
 
 
 # ---- shims for importing the reference's segformer.py without timm / mmcv --------------------------------------------------------------

@@ -7,8 +7,8 @@
   W = 128 / 256 / 384 (384: an odd number of 128-pixel tiles, which turns the phase interleave of multi-phase launches off) and
   O = 128 / 256, plus one launch of more than 2 x 132 units, so that persistent CTAs run units of several images.
   PRODUCTION adds every launch of the benchmarked step at its exact shape (up to 4096 units, about 31 per CTA; W = 512, tiles_x = 4; the
-  2048-item FIR pass), PER_SAMPLE the Nw = N variants of block1's two layers; KC32 adds I = 3 / 16 / 32 (the 32-channel K chunks) to
-  every single-phase family and I = 33.  Each launch is compared one image at a time, which bounds the float64 memory.
+  2048-item FIR pass) and the SECC->plane backbone's to_plane convs (SECC_PRODUCTION), PER_SAMPLE the Nw = N variants of block1's two
+  layers; KC32 adds I = 3 / 16 / 32 (the 32-channel K chunks) to every single-phase family and I = 33.  Each launch is compared one image at a time, which bounds the float64 memory.
 * test_benchmarked_launches_have_rows records every conv_tc3 call of one eager step of bench.py's engines and fails, naming the launch,
   when one has no row here (or, for r3dp_tw_conv*, in tests/test_gpu_torso_warper_layers.py), or when a PRODUCTION row is not launched.
 * Bit-exact properties: image k of an N = 3 per-sample launch equals the N = 1 launch of image k (and the last image of every N = 4
@@ -268,6 +268,13 @@ PRODUCTION = [
     ('conv_res', 1, 1, 128, 256, 256, 256, {'act': 2}),
     ('conv_res', 1, 1, 256, 256, 256, 256, {'act': 0}),
 ]
+#: to_plane_cnn.0/2/4 of the SECC->plane backbone (3x3, 256 -> 256, nn.LeakyReLU(0.01)) at 512^2, forward at B = 4 and 1; the backbone does
+#: not run in the benchmarked step, so test_backbone_launches_have_rows (tests/test_gpu_secc2plane_launches.py) keeps these launched
+SECC_PRODUCTION = [
+    ('conv_res', 4, 1, 256, 256, 128, 128, {'act': 2}),
+    ('conv_res', 1, 1, 256, 256, 128, 128, {'act': 2}),
+]
+PRODUCTION += SECC_PRODUCTION
 #: block1's two layers with per-sample weights: weight-tap addressing per image at tiles_x = 4 and in the 2048-item FIR pass
 PER_SAMPLE = [
     ('layer2', 4, 4, 256, 128, 256, 256, {}),
@@ -503,7 +510,7 @@ def test_benchmarked_launches_have_rows(monkeypatch):
     assert {row[0] for _, t, row in launches.values()} >= {'composed', 'layer_torgb', 'layer2', 'last', 'conv_res', 'layer1', 'noup'}
     missing = [f'{name}: {row} (in {t})' for key, (name, t, row) in launches.items() if key not in have]
     assert not missing, 'launches of the benchmarked step without a float64 row:\n' + '\n'.join(missing)
-    stale = [row for row in PRODUCTION if ('CASES', _signature('CASES', row)) not in launches]
+    stale = [row for row in PRODUCTION if row not in SECC_PRODUCTION and ('CASES', _signature('CASES', row)) not in launches]
     assert not stale, f'PRODUCTION rows the benchmarked step no longer launches: {stale}'
 
 
