@@ -10,7 +10,8 @@
   2048-item FIR pass) and the SECC->plane backbone's to_plane convs (SECC_PRODUCTION), PER_SAMPLE the Nw = N variants of block1's two
   layers; KC32 adds I = 3 / 16 / 32 (the 32-channel K chunks) to every single-phase family and I = 33.  Each launch is compared one image at a time, which bounds the float64 memory.
 * test_benchmarked_launches_have_rows records every conv_tc3 call of one eager step of bench.py's engines and fails, naming the launch,
-  when one has no row here (or, for r3dp_tw_conv*, in tests/test_gpu_torso_warper_layers.py), or when a PRODUCTION row is not launched.
+  when one has no row here, or when a PRODUCTION row is not launched.  (The torso warper's r3dp_tw_conv* launches have their own
+  recorded-launch test, tests/test_gpu_torso_warper_launches.py.)
 * Bit-exact properties: image k of an N = 3 per-sample launch equals the N = 1 launch of image k (and the last image of every N = 4
   launch its N = 1 launch); Nw = 1 equals Nw = N with the weights replicated; a launch repeated gives the same bits; nothing outside the
   logical output is written (canaries, the lo halves and the uint8 frames included) and every fp16 / fp32 element of it is.
@@ -402,7 +403,7 @@ def test_conv_bits_slicing_shared_determinism_canaries(key, mode):
 
 # ---- the launches of the benchmarked step ------------------------------------------------------------------------------------------------
 #: the C entry points that launch conv_tc3
-CONV_ENTRY = re.compile(r'r3dp_sr_tcx?_(layer|layer_up_composed|layer_torgb|layer_torgb_noup|conv|conv_res|last_layer|last_layer_ex)$|r3dp_tw_conv')
+CONV_ENTRY = re.compile(r'r3dp_sr_tcx?_(layer|layer_up_composed|layer_torgb|layer_torgb_noup|conv|conv_res|last_layer|last_layer_ex)$')
 
 
 class _Recorder:
@@ -427,17 +428,8 @@ def _given(p):
     return (p.value if isinstance(p, ctypes.c_void_p) else p) is not None
 
 
-def _f32(v):
-    return ctypes.c_float(v).value
-
-
 def _row_of_call(name, a):
-    """(table, row) of one recorded launch: a CASES row of this module, or for the torso warper's r3dp_tw_conv* a CONV_CASES / UP_CASES row
-    of tests/test_gpu_torso_warper_layers.py."""
-    if name == 'r3dp_tw_conv':
-        return 'CONV_CASES', (a[3], a[6], a[7], a[4], a[5], a[8], _f32(a[9]), _given(a[10]))
-    if name == 'r3dp_tw_conv_up_nearest':
-        return 'UP_CASES', (a[3], a[6], a[7], a[4], a[5], _f32(a[8]))
+    """(table, row) of one recorded launch: a CASES row of this module."""
     op, opt = name.split('_', 3)[3], {}
     if op in ('layer', 'layer_up_composed'):
         fam = 'composed' if op == 'layer_up_composed' else ('layer1' if a[9] == 1 else 'layer2')
@@ -465,10 +457,6 @@ DEFAULT_OPT = {'ksize': 3, 'act': 1, 'skip': False, 'res': False, 'clamp': 0, 'u
 
 def _signature(table, row):
     """What decides a launch: the row with every option at its default made explicit (a uint8 launch clamps)."""
-    if table == 'CONV_CASES':
-        return row[:6] + (_f32(row[6]), bool(row[7]))
-    if table == 'UP_CASES':
-        return row[:5] + (_f32(row[5]),)
     fam, N, Nw, I, O, H, W, opt = row
     o = dict(DEFAULT_OPT, **opt)
     return (fam, N, Nw, I, O, H, W, o['ksize'], o['act'], bool(o['skip']), bool(o['res']), int(bool(o['clamp'] or o['u8'])), bool(o['u8']),
@@ -479,7 +467,6 @@ def test_benchmarked_launches_have_rows(monkeypatch):
     """Every conv_tc3 launch of the benchmarked step has a float64 row of the same shape and options: bench.py's FrameEngine(batch=4) in 'tc'
     and in 'tc_exact', and its configs[4], the torso head (stub warper, fuse mode v2) through RenderHead.synthesis without the clip's
     constants and through the engine after begin_clip().  One eager step of each, recorded at the C entry points."""
-    import test_gpu_torso_warper_layers as twl
     from real3dportrait_b200 import engine, synthetic as syn
     rec = _Recorder(capi.lib())
     monkeypatch.setattr(capi, '_lib', rec)
@@ -501,8 +488,7 @@ def test_benchmarked_launches_have_rows(monkeypatch):
     eng.begin_clip(inp['ref_torso_rgb'], inp['ref_bg_rgb'], inp['segmap'], inp['kp_s'])
     eng.step(planes, cams, u_c, u_f, kp_d=kp_d)
     torch.cuda.synchronize()
-    tables = {'CASES': CASES, 'CONV_CASES': twl.CONV_CASES, 'UP_CASES': twl.UP_CASES}
-    have = {(t, _signature(t, row)) for t, rows in tables.items() for row in rows}
+    have = {('CASES', _signature('CASES', row)) for row in CASES}
     launches = {}
     for name, args in rec.calls:
         t, row = _row_of_call(name, args)

@@ -1,7 +1,8 @@
 """Every stage-2 entry point of the torso warper (r3dp_tw_*) layer by layer against float64 references built from the operands the kernel reads,
 with the element-wise bound of tests/sr_conv_reference.py (|got - ref| <= alpha |ref| + extra + beta S), in 'tc' and 'tc_exact' (split).  Every
 output lives inside a NaN-filled allocation: nothing before or after it is written and every element of it is.  The persistent conv launches
-also show that image k of an N = 3 launch is the N = 1 launch of that image, bit for bit."""
+also show that the last image of an N > 1 launch is the N = 1 launch of that image, bit for bit.  The run_* helpers take a launch's
+arguments; tests/test_gpu_torso_warper_launches.py calls them at every launch of the warper (N = 4 and 1)."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -69,6 +70,12 @@ CONV_CASES = [
 @pytest.mark.parametrize('case', CONV_CASES, ids=lambda c: f'N{c[0]}_{c[1]}x{c[2]}_{c[3]}to{c[4]}_k{c[5]}_s{c[6]}_res{int(c[7])}')
 @pytest.mark.parametrize('split', [False, True], ids=['tc', 'tcx'])
 def test_tw_conv(case, split):
+    run_tw_conv(case, split)
+
+
+def run_tw_conv(case, split):
+    """One r3dp_tw_conv launch (N, H, W, I, O, ksize, slope, residual) against float64, one image at a time; the last image of an N > 1
+    launch equals its N = 1 launch bit for bit."""
     N, H, W, I, O, k, slope, res = case
     g = torch.Generator().manual_seed(H * 7 + W + I + O + k + int(res))
     x16 = _nhwc(torch.randn(N, I, H, W, generator=g).to(DEV), split)
@@ -86,20 +93,23 @@ def test_tw_conv(case, split):
                                            capi.ptr(yy, F16), int(split), capi.stream()))
     run(x16, r16, y, N)
     _check_canary(buf, y, 'tw_conv')
-    x = scr.activations(x16, I, split)
-    w = scr.taps3x3(scr.packed_weights(wp, I, split)).expand(N, -1, -1, -1, -1)
-    v = scr.conv_same(x, w, k) + b.double().view(1, -1, 1, 1)
-    S = scr.conv_same(x.abs(), w.abs(), k) + b.double().abs().view(1, -1, 1, 1)
-    ref, extra = _act(v, slope), scr.FLOOR_F16
-    if res:
-        r = scr.activations(r16, O, split)
-        if not split:                                  # tc rounds the activated value to fp16 before adding the residual
-            extra = extra + scr.ALPHA_F16 * ref.abs() + scr.FLOOR_F16
-        ref, S = ref + r, S + r.abs()
-    scr.check_bound(scr.nhwc(y, split), ref, S, scr.alpha_store(split), scr.BETA['tcx' if split else 'tc'], extra, tag=f'tw_conv {case}')
-    y1 = torch.empty(1, H, W, O * wide, device=DEV, dtype=F16)
-    run(x16[1:2].contiguous(), None if r16 is None else r16[1:2].contiguous(), y1, 1)
-    assert torch.equal(y1[0].view(torch.int16), y[1].view(torch.int16)), 'image 1 of the N=3 launch differs from its N=1 launch'
+    w = scr.taps3x3(scr.packed_weights(wp, I, split))
+    for n in range(N):
+        x = scr.activations(x16[n:n + 1], I, split)
+        v = scr.conv_same(x, w, k) + b.double().view(1, -1, 1, 1)
+        S = scr.conv_same(x.abs(), w.abs(), k) + b.double().abs().view(1, -1, 1, 1)
+        ref, extra = _act(v, slope), scr.FLOOR_F16
+        if res:
+            r = scr.activations(r16[n:n + 1], O, split)
+            if not split:                              # tc rounds the activated value to fp16 before adding the residual
+                extra = extra + scr.ALPHA_F16 * ref.abs() + scr.FLOOR_F16
+            ref, S = ref + r, S + r.abs()
+        scr.check_bound(scr.nhwc(y[n:n + 1], split), ref, S, scr.alpha_store(split), scr.BETA['tcx' if split else 'tc'], extra,
+                        tag=f'tw_conv {case} image {n}')
+    if N > 1:
+        y1 = torch.empty(1, H, W, O * wide, device=DEV, dtype=F16)
+        run(x16[N - 1:].contiguous(), None if r16 is None else r16[N - 1:].contiguous(), y1, 1)
+        assert torch.equal(y1[0].view(torch.int16), y[N - 1].view(torch.int16)), f'the last image of the N={N} launch differs from its N=1 launch'
 
 
 # N, H, W, I, O, slope: up.0 and up.1 of the Generator (the 64 couts of up.1 padded with zero filters to 128) and a linear case
@@ -111,6 +121,12 @@ UP_CASES = [(3, 64, 64, 256, 128, 0.0), (1, 128, 128, 128, 128, 0.0), (3, 32, 64
 def test_tw_conv_up_nearest(case, split):
     """nearest x2 + 3x3 as four parity phases of 2x2 composed taps, against the same taps in float64 (and those taps against
     upsample-then-conv of the unpacked composition in tests/test_cpu_torso_warper.py)."""
+    run_up_nearest(case, split)
+
+
+def run_up_nearest(case, split):
+    """One r3dp_tw_conv_up_nearest launch (N, H, W, I, O, slope) against float64, one image at a time; the last image of an N > 1 launch
+    equals its N = 1 launch bit for bit."""
     N, H, W, I, O, slope = case
     g = torch.Generator().manual_seed(H + W + I + O)
     x16 = _nhwc(torch.randn(N, I, H, W, generator=g).to(DEV), split)
@@ -120,14 +136,23 @@ def test_tw_conv_up_nearest(case, split):
     b = (0.1 * torch.randn(O, generator=g)).to(DEV)
     wide = 2 if split else 1
     buf, y = _canary((N, 2 * H, 2 * W, O * wide), F16)
-    capi.check(capi.lib().r3dp_tw_conv_up_nearest(capi.ptr(x16, F16), capi.ptr(wp, F16), capi.ptr(b), N, I, O, H, W, slope, capi.ptr(y, F16),
-                                                   int(split), capi.stream()))
+
+    def run(xx, yy, n):
+        capi.check(capi.lib().r3dp_tw_conv_up_nearest(capi.ptr(xx, F16), capi.ptr(wp, F16), capi.ptr(b), n, I, O, H, W, slope, capi.ptr(yy, F16),
+                                                       int(split), capi.stream()))
+    run(x16, y, N)
     _check_canary(buf, y, 'tw_conv_up_nearest')
-    x = scr.activations(x16, I, split)
     w4 = scr.taps3x3(scr.packed_weights(wp, I, split))                  # [4,O,I,3,3]
-    ref = _act(twr.conv_up_nearest_phases(x, w4, b.double()), slope)
-    S = twr.conv_up_nearest_phases(x.abs(), w4.abs(), b.double().abs())
-    scr.check_bound(scr.nhwc(y, split), ref, S, scr.alpha_store(split), scr.BETA['tcx' if split else 'tc'], scr.FLOOR_F16, tag=f'up_nearest {case}')
+    for n in range(N):
+        x = scr.activations(x16[n:n + 1], I, split)
+        ref = _act(twr.conv_up_nearest_phases(x, w4, b.double()), slope)
+        S = twr.conv_up_nearest_phases(x.abs(), w4.abs(), b.double().abs())
+        scr.check_bound(scr.nhwc(y[n:n + 1], split), ref, S, scr.alpha_store(split), scr.BETA['tcx' if split else 'tc'], scr.FLOOR_F16,
+                        tag=f'up_nearest {case} image {n}')
+    if N > 1:
+        y1 = torch.empty(1, 2 * H, 2 * W, O * wide, device=DEV, dtype=F16)
+        run(x16[N - 1:].contiguous(), y1, 1)
+        assert torch.equal(y1[0].view(torch.int16), y[N - 1].view(torch.int16)), f'the last image of the N={N} launch differs from its N=1 launch'
 
 
 @pytest.mark.parametrize('split', [False, True], ids=['tc', 'tcx'])
@@ -158,8 +183,14 @@ NARROW_CASES = [
 @pytest.mark.parametrize('case', NARROW_CASES, ids=lambda c: f'k{c[0]}_co{c[1]}_act{c[2]}_{c[3]}_ex{int(c[4])}')
 @pytest.mark.parametrize('split', [False, True], ids=['tc', 'tcx'])
 def test_tw_narrow_conv(case, split):
+    run_narrow_conv(case, split, 3)
+
+
+def run_narrow_conv(case, split, N):
+    """One r3dp_tw_narrow_conv launch (K, CO, act, input kind, resized extra channel, NCHW output) on N images of 256^2 against float64,
+    one image at a time."""
     K, CO, act, kind, with_ex, nchw = case
-    N, H, W = 3, 256, 256
+    H, W = 256, 256
     g = torch.Generator().manual_seed(K + CO + act)
     L = capi.lib()
     if kind == 'f16':
@@ -184,27 +215,30 @@ def test_tw_narrow_conv(case, split):
         capi.check(L.r3dp_tw_narrow_conv(None, 0, 0, 0, capi.ptr(xf), 32, 32, capi.ptr(ex), 64 if with_ex else 0, 64 if with_ex else 0,
                                          capi.ptr(wk), capi.ptr(b), N, H, W, K, CO, act, int(nchw), capi.ptr(y), capi.stream()))
     _check_canary(buf, y, 'narrow_conv')
-    if with_ex:
-        x = torch.cat([x, F.interpolate(ex.double(), size=(H, W), mode='bilinear', align_corners=False)], dim=1)
-    v = F.conv2d(x, w.double(), b.double(), padding=K // 2)
-    S = F.conv2d(x.abs(), w.double().abs(), b.double().abs(), padding=K // 2)
     # fp32 accumulation of K*K*cin products in order: |err| <= K*K*cin * 2^-24 S (gamma_n); the resized channel adds its fp32 interpolation
     beta = K * K * cin * U32 + (8 * U32 if with_ex else 0)
-    if act == 2:                                    # sigmoid is 1/4-Lipschitz; expf / the division add a few ulp of the result
-        ref = torch.sigmoid(v)
-        got, S = y, 0.25 * S
-        alpha = 8 * U32
-    else:
-        ref = torch.relu(v) if act == 1 else v
-        got, alpha = y, U32
-    got = got.double() if nchw else got.double().permute(0, 3, 1, 2)
-    scr.check_bound(got, ref, S, alpha, beta, tag=f'narrow_conv {case}')
+    for n in range(N):
+        xn = x[n:n + 1]
+        if with_ex:
+            xn = torch.cat([xn, F.interpolate(ex[n:n + 1].double(), size=(H, W), mode='bilinear', align_corners=False)], dim=1)
+        v = F.conv2d(xn, w.double(), b.double(), padding=K // 2)
+        S = F.conv2d(xn.abs(), w.double().abs(), b.double().abs(), padding=K // 2)
+        if act == 2:                                # sigmoid is 1/4-Lipschitz; expf / the division add a few ulp of the result
+            ref, S, alpha = torch.sigmoid(v), 0.25 * S, 8 * U32
+        else:
+            ref, alpha = (torch.relu(v) if act == 1 else v), U32
+        got = y[n:n + 1].double() if nchw else y[n:n + 1].double().permute(0, 3, 1, 2)
+        scr.check_bound(got, ref, S, alpha, beta, tag=f'narrow_conv {case} N{N} image {n}')
 
 
 @pytest.mark.parametrize('split', [False, True], ids=['tc', 'tcx'])
 def test_tw_hid_to_nchw(split):
     """hi (+ lo) summed in fp32 and transposed: bit for bit."""
-    N, H, W = 3, 256, 256
+    run_hid_to_nchw(split, 3)
+
+
+def run_hid_to_nchw(split, N):
+    H, W = 256, 256
     hid = sr_tc.to_nhwc_f16(torch.randn(N, 128, H, W, generator=torch.Generator().manual_seed(1)).to(DEV), W, split)
     buf, y = _canary((N, 64, H, W), torch.float32)
     capi.check(capi.lib().r3dp_tw_hid_to_nchw(capi.ptr(hid, F16), N, 64, H, W, hid.shape[-1], 128 if split else 0, capi.ptr(y), capi.stream()))
@@ -216,25 +250,33 @@ def test_tw_hid_to_nchw(split):
 @pytest.mark.parametrize('split', [False, True], ids=['tc', 'tcx'])
 def test_tw_gather3d_canary_and_shared_volume(split):
     """The gather inside NaN guards, N = 3; fs_shared reads one volume for every image and equals the launch on its broadcast copy bit for bit."""
-    fs, deformation, _ = twr.make_stage2_inputs(3, 64, seed=12)
-    fsn = fs[:1].permute(0, 2, 3, 4, 1).contiguous().to(DEV)
+    run_gather3d(split, 3, True)
+
+
+def run_gather3d(split, N, shared):
+    """r3dp_tw_gather3d on N images at 64^2 inside NaN guards against float64, one image at a time.  shared (N > 1): one volume read by every
+    image, bit for bit the launch on its broadcast copy; otherwise each image reads its own volume."""
+    fs, deformation, _ = twr.make_stage2_inputs(N, 64, seed=12)
+    vol = fs[:1] if shared else fs                                     # [1 or N, 32, 16, 64, 64]
+    fsn = vol.permute(0, 2, 3, 4, 1).contiguous().to(DEV)
     deformation = deformation.to(DEV)
     wide = 2 if split else 1
-    buf, y = _canary((3, 64, 64, 512 * wide), F16)
+    buf, y = _canary((N, 64, 64, 512 * wide), F16)
     L = capi.lib()
-    capi.check(L.r3dp_tw_gather3d(capi.ptr(fsn), 1, capi.ptr(deformation), 3, 32, 16, 64, 64, capi.ptr(y, F16), int(split), capi.stream()))
+    capi.check(L.r3dp_tw_gather3d(capi.ptr(fsn), int(shared), capi.ptr(deformation), N, 32, 16, 64, 64, capi.ptr(y, F16), int(split), capi.stream()))
     _check_canary(buf, y, 'gather3d')
-    y_b = torch.empty_like(y)
-    capi.check(L.r3dp_tw_gather3d(capi.ptr(fsn.expand(3, -1, -1, -1, -1).contiguous()), 0, capi.ptr(deformation), 3, 32, 16, 64, 64, capi.ptr(y_b, F16),
-                                  int(split), capi.stream()))
-    assert torch.equal(y.view(torch.int16), y_b.view(torch.int16))
-    ref = F.grid_sample(fs[:1].expand(3, -1, -1, -1, -1).double().to(DEV), deformation.double(), align_corners=True, padding_mode='border')
-    ref = ref.reshape(3, 512, 64, 64)
+    if shared:
+        y_b = torch.empty_like(y)
+        capi.check(L.r3dp_tw_gather3d(capi.ptr(fsn.expand(N, -1, -1, -1, -1).contiguous()), 0, capi.ptr(deformation), N, 32, 16, 64, 64,
+                                      capi.ptr(y_b, F16), int(split), capi.stream()))
+        assert torch.equal(y.view(torch.int16), y_b.view(torch.int16))
     # The kernel unnormalises the coordinates in fp32 (as torch's fp32 grid_sample does): each of the three source coordinates is off by at
     # most delta = 4 ulp of (size - 1) <= 4 * 63 * 2^-24 voxels, which moves the trilinear weights of each axis by delta and the value by at most
     # 2 * delta * max|fs| per axis.  The weighted sum of 8 corners in fp32 adds <= 12 * 2^-24 S; the store rounds as the convs' do.
-    S = F.grid_sample(fs[:1].expand(3, -1, -1, -1, -1).double().abs().to(DEV), deformation.double(), align_corners=True,
-                      padding_mode='border').reshape(3, 512, 64, 64)
     delta = 4 * 63 * U32
-    extra = 3 * 2 * delta * float(fs.abs().max()) + scr.FLOOR_F16
-    scr.check_bound(scr.nhwc(y, split), ref, S, scr.alpha_store(split), 16 * U32, extra, tag='gather3d')
+    for n in range(N):
+        v = vol[0 if shared else n][None].double().to(DEV)
+        ref = F.grid_sample(v, deformation[n:n + 1].double(), align_corners=True, padding_mode='border').reshape(1, 512, 64, 64)
+        S = F.grid_sample(v.abs(), deformation[n:n + 1].double(), align_corners=True, padding_mode='border').reshape(1, 512, 64, 64)
+        extra = 3 * 2 * delta * float(v.abs().max()) + scr.FLOOR_F16
+        scr.check_bound(scr.nhwc(y[n:n + 1], split), ref, S, scr.alpha_store(split), 16 * U32, extra, tag=f'gather3d N{N} shared{int(shared)} image {n}')
