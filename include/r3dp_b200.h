@@ -432,6 +432,25 @@ int r3dp_sp_head_fuse(const float* g1, int h1, const float* g2, int h2, const fl
 int r3dp_sp_leaky(void* x_f16, long long n, float slope, r3dp_stream_t stream);
 int r3dp_sp_upsample2_flip(const void* x_f16, int N, int h, int w, int C, void* yr_f16, void* yrc_f16, r3dp_stream_t stream);
 
+/* ------------------------------------------------ SECC renderer: SECC_Renderer (deep_3drecon/secc_renderer.py) ---
+ * The 3DMM face mesh rasterised at S x S with pytorch3d's rules (blur 0, one face per pixel, perspective-correct barycentrics, no culling
+ * or clipping; DESIGN.md) and shaded with the per-vertex NCC code.  All fp32.
+ * r3dp_secc_vertices  basis [3N, n_id + n_exp] (row 3v + axis, id columns then exp columns, 16-byte aligned), mean [3N] (recentred),
+ *                     id [B, >= n_id] (row stride ids), exp [B, >= n_exp] (row stride exps), euler, trans [B,3] (NULL = zero)
+ *                     -> verts [B,N,4] = (x_ndc, y_ndc, z_view, 0): s = basis . [id|exp] + mean, v = Rz Ry Rx s + t (bfm.py:204-238,260-270),
+ *                     z = cam_dist - v_z, x_ndc = -v_x / (z tan_half), y_ndc = v_y / (z tan_half).  n_id + n_exp <= 256, a multiple of 4.
+ *                     Each basis row is read once per call for all B frames.
+ * r3dp_secc_raster    verts [B,N,4], faces int32 [F,3] (0-based) -> keys [B,S,S] uint64: atomicMin of (bits of pz) << 32 | face over every
+ *                     covered pixel centre (nearest pz, ties to the lower face).  keys must hold ~0 (empty) on entry.
+ * r3dp_secc_resolve   keys -> secc [B,3,S,S] = 2 mask sum_i w_i ncc[v_i] - 1 (-1 where empty) and mask [B,1,S,S] (may be NULL); ncc [N,4]
+ *                     (x, y, z, pad).  drop_face0: face 0 counts as background in image 0 (pix_to_face > 0 on the packed index,
+ *                     mesh_renderer.py:116).  Resets every key to empty. */
+int r3dp_secc_vertices(const float* basis, const float* mean, int N, int n_id, int n_exp, const float* id, int ids, const float* exp, int exps,
+                       const float* euler, const float* trans, int B, float cam_dist, float tan_half, float* verts, r3dp_stream_t stream);
+int r3dp_secc_raster(const float* verts, int N, const int* faces, int F, int B, int S, void* keys, r3dp_stream_t stream);
+int r3dp_secc_resolve(const float* verts, int N, const int* faces, const float* ncc, int B, int S, int drop_face0, void* keys, float* secc,
+                      float* mask, r3dp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

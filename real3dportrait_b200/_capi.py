@@ -132,6 +132,9 @@ _SIGNATURES = {
     'r3dp_sp_head_fuse': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _I, _P, _P, _P]),
     'r3dp_sp_leaky': (_I, [_P, C.c_longlong, _F, _P]),
     'r3dp_sp_upsample2_flip': (_I, [_P, _I, _I, _I, _I, _P, _P, _P]),
+    'r3dp_secc_vertices': (_I, [_P, _P, _I, _I, _I, _P, _I, _P, _I, _P, _P, _I, _F, _F, _P, _P]),
+    'r3dp_secc_raster': (_I, [_P, _I, _P, _I, _I, _I, _P, _P]),
+    'r3dp_secc_resolve': (_I, [_P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P]),
 }
 
 

@@ -127,12 +127,18 @@ class FrameEngine:
     secc2plane: a SegFormerSECC2PlaneBackbone; the engine then runs it inside the step (captured in the step's graph, graph A of the torso
     split): begin_planes(cano_planes, cond_cano, cond_src) once per clip, then step(None, cameras, ..., cond_tgt=drv_secc) renders
     cano_planes + backbone(cat[cano, src, tgt]) (secc_img2plane.py:64-81) without materialising either plane set; prepare() tuples and
-    step_host() take the driving SECC image [B,3,H,W] in the planes slot."""
+    step_host() take the driving SECC image [B,3,H,W] in the planes slot.
+    secc_renderer (with secc2plane): a SECC_Renderer; the engine then renders the SECC images itself from 3DMM coefficients [id | exp] at zero
+    pose (real3d_infer.py:391-405): begin_planes(cano_planes, coeff_src=c [1,144]) renders the clip's two images, and step(None, cameras, ...,
+    coeff=c [B,144]) renders the driving image inside the step (and its graph), in front of the backbone.  Each step is one renderer call, so
+    face 0 is background in the first frame of every step, i.e. every `batch`-th frame of the clip.  The reference renders a clip in 50-frame
+    calls and loses face 0 only in frames 0, 50, 100, ...: the engine's frames differ from it where face 0 wins in the other frames that start a
+    step (one triangle, a few pixels).  prepare() tuples and step_host() then carry the coefficients in the planes slot."""
 
     def __init__(self, batch: int = 4, sr_mode: str = 'fp32', device=None, world: int = 1, rank: int = 0, dist=None, hp: Optional[dict] = None,
                  static_styles: bool = True, use_graph: bool = True, out_uint8: bool = False, exchange: str = 'allgather',
                  torso_model: Optional[torch.nn.Module] = None, warper_in_graph: bool = False, torso_stage2: str = 'torch',
-                 torso_motion: str = 'torch', secc2plane: Optional[torch.nn.Module] = None):
+                 torso_motion: str = 'torch', secc2plane: Optional[torch.nn.Module] = None, secc_renderer: Optional[torch.nn.Module] = None):
         assert exchange in ('allgather', 'p2p', 'none')
         if secc2plane is not None and (hp or {}).get('phase1_plane_fusion_mode', 'add') != 'add':
             raise NotImplementedError('secc2plane: only phase1_plane_fusion_mode="add" (cano + secc, secc_img2plane.py:76-77) is built')
@@ -151,6 +157,9 @@ class FrameEngine:
             self.head.superresolution.set_torso_motion(torso_motion)
         self.secc = secc2plane.to(self.device).eval() if secc2plane is not None else None
         self._cano_cl = None              # secc2plane: the clip's canonical planes, 'hwpc' [1,H,W,3,C] (begin_planes)
+        if secc_renderer is not None and secc2plane is None:
+            raise ValueError('secc_renderer renders the input of the SECC -> plane backbone: FrameEngine(secc2plane=..., secc_renderer=...)')
+        self.secc_r = secc_renderer.to(self.device) if secc_renderer is not None else None
         self.out_uint8 = bool(out_uint8)
         if self.out_uint8 and self.head.superresolution.sr_mode not in ('tc', 'tc_exact'):     # the head's effective mode: a torso head maps 'fp32' to 'tc'
             raise NotImplementedError('uint8 frames are written by the tensor-core SR epilogue (sr_mode="tc")')
@@ -214,11 +223,28 @@ class FrameEngine:
         self._consts.update({'ref_torso_img': ref_torso_img, 'bg_img': bg_img})
 
     @torch.no_grad()
-    def begin_planes(self, cano_planes: torch.Tensor, cond_cano: torch.Tensor, cond_src: Optional[torch.Tensor] = None) -> None:
+    def begin_planes(self, cano_planes: torch.Tensor, cond_cano: Optional[torch.Tensor] = None, cond_src: Optional[torch.Tensor] = None, *,
+                     coeff_src: Optional[torch.Tensor] = None) -> None:
         """secc2plane engines: the clip's canonical planes [1,3,32,256,256] and the backbone's per-clip SECC images [1,3,H,W] (cond_src only in
-        'cano_src_tgt').  A later begin_planes() refills the same buffers in place, so graphs captured for an earlier clip render the new one."""
+        'cano_src_tgt').  With a secc_renderer the images come from the source frame's coefficients coeff_src [1,144] = [id | exp] instead:
+        cond_src = r(id, exp), cond_cano = r(id, 0 exp), zero pose (real3d_infer.py:404-405).  A later begin_planes() refills the same buffers in
+        place, so graphs captured for an earlier clip render the new one."""
         if self.secc is None:
             raise ValueError('begin_planes() needs FrameEngine(secc2plane=...)')
+        if self.secc_r is not None:
+            if coeff_src is None or cond_cano is not None or cond_src is not None:
+                raise ValueError('secc_renderer engine: begin_planes(cano_planes, coeff_src=c [1,144]) (the engine renders cond_cano / cond_src)')
+            c = capi.f32(coeff_src.to(self.device))
+            if c.ndim != 2 or c.shape[0] != 1:
+                raise ValueError(f'begin_planes: coeff_src must be [1,{self.secc_r.n_id + self.secc_r.n_exp}], got {tuple(c.shape)}')
+            cano_c = c.clone()
+            cano_c[:, self.secc_r.n_id:] = 0
+            cond_src = self.secc_r.render(c)[1]
+            cond_cano = self.secc_r.render(cano_c)[1]
+        elif coeff_src is not None:
+            raise ValueError('coeff_src needs FrameEngine(secc_renderer=...)')
+        elif cond_cano is None:
+            raise ValueError('begin_planes(cano_planes, cond_cano, cond_src)')
         from .secc2plane import canonical_planes_cl
         cl = canonical_planes_cl(cano_planes.to(self.device))
         if self._cano_cl is not None and self._cano_cl.data.shape == cl.data.shape:
@@ -229,11 +255,14 @@ class FrameEngine:
         self.secc.begin_clip(cond_cano.to(self.device), None if cond_src is None else cond_src.to(self.device))
 
     def _planes(self, planes):
-        """The render's plane sets: with secc2plane, `planes` is the driving SECC image and the backbone runs here (inside the capture)."""
+        """The render's plane sets: with secc2plane, `planes` is the driving SECC image (or, with a secc_renderer, the coefficients it is
+        rendered from) and the backbone runs here (inside the capture)."""
         if self.secc is None:
             return planes
         if self._cano_cl is None:
             raise RuntimeError('secc2plane: call begin_planes(cano_planes, cond_cano, cond_src) before the first step')
+        if self.secc_r is not None:
+            planes = self.secc_r.render(planes)[1]
         return (self._cano_cl, self.secc.planes_cl(planes))
 
     def end_clip(self) -> None:
@@ -271,7 +300,15 @@ class FrameEngine:
 
     def _capture_graph(self, planes, cameras, u_coarse, u_fine=None, kp_d=None):
         if self.torso and not self.warper_in_graph:
-            return self._capture_split(planes, cameras, u_coarse, u_fine, kp_d)
+            g, out = self._capture_split(planes, cameras, u_coarse, u_fine, kp_d)
+        else:
+            g, out = self._capture_whole(planes, cameras, u_coarse, u_fine, kp_d)
+        # the renderer's buffers the graph reads and writes (basis, faces, NCC code, key buffer) belong to the graph too: another engine built on
+        # the same renderer, or a .to() of it, then cannot free memory the graph keeps writing to
+        g.keep_alive = self.secc_r.graph_buffers(_frames_of(planes)) if self.secc_r is not None else ()
+        return g, out
+
+    def _capture_whole(self, planes, cameras, u_coarse, u_fine=None, kp_d=None):
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
@@ -355,14 +392,24 @@ class FrameEngine:
 
     @torch.no_grad()
     def step(self, planes, cameras: torch.Tensor, u_coarse: Optional[torch.Tensor] = None, u_fine: Optional[torch.Tensor] = None,
-             frame_index: Optional[int] = None, *, kp_d: Optional[torch.Tensor] = None, cond_tgt: Optional[torch.Tensor] = None) -> torch.Tensor:
+             frame_index: Optional[int] = None, *, kp_d: Optional[torch.Tensor] = None, cond_tgt: Optional[torch.Tensor] = None,
+             coeff: Optional[torch.Tensor] = None) -> torch.Tensor:
         """planes [B,3,32,256,256] | PlanesCL | (cano, secc); cameras [B,25]; u_coarse [B,4096,S,1], u_fine [B*4096,S_imp] (drawn here if None)
         -> this rank's frames: fp32 [B,3,512,512] in [-1,1] or uint8 [B,512,512,3]; with exchange='allgather' the gathered
         [world*B,...] (rank-major); with exchange='p2p' the frames are additionally pushed into the open clip at `frame_index`.
         kp_d [B,68,3]: the frames' driving key points, the torso head's only per-frame condition (torso engines only).
         cond_tgt [B,3,H,W]: the driving SECC image, in place of planes (pass None), for FrameEngine(secc2plane=...).
+        coeff [B,144]: the frames' [id | exp] coefficients, in place of cond_tgt, for FrameEngine(secc2plane=..., secc_renderer=...).
         The returned tensor is reused by the next step."""
-        if self.secc is not None:
+        if self.secc_r is not None:
+            if planes is not None or cond_tgt is not None or coeff is None:
+                raise ValueError('secc_renderer engine: step(None, cameras, ..., coeff=c [B,144])')
+            if coeff.ndim != 2 or coeff.shape[1] != self.secc_r.n_id + self.secc_r.n_exp:
+                raise ValueError(f'step: coeff must be [B,{self.secc_r.n_id + self.secc_r.n_exp}], got {tuple(coeff.shape)}')
+            planes = coeff
+        elif coeff is not None:
+            raise ValueError('coeff needs FrameEngine(secc2plane=..., secc_renderer=...)')
+        elif self.secc is not None:
             if planes is not None or cond_tgt is None:
                 raise ValueError('secc2plane engine: step(None, cameras, ..., cond_tgt=drv_secc)')
             planes = cond_tgt
@@ -551,7 +598,8 @@ class FrameEngine:
                     dst.copy_(src, non_blocking=True)
             hp['in_ready'][k].record(hp['copy_in'])
         cur.wait_event(hp['in_ready'][k])
-        p0, tgt = (None, {'cond_tgt': stage[0]}) if self.secc is not None else (stage[0], {})      # secc2plane: h_planes is the driving SECC image
+        # secc2plane: h_planes is the driving SECC image, or the coefficients it is rendered from with a secc_renderer
+        p0, tgt = (None, {'coeff' if self.secc_r is not None else 'cond_tgt': stage[0]}) if self.secc is not None else (stage[0], {})
         out = self.step(p0, *stage[1:4], kp_d=stage[4], **tgt) if self.torso else self.step(p0, *stage[1:], **tgt)
         self.wait_gather()
         hp['in_free'][k].record(cur)

@@ -8,7 +8,7 @@ row-major normalised intrinsics (9) with focal 4.2647 and principal point 0.5.""
 from __future__ import annotations
 
 import math
-from typing import Dict, Tuple
+from typing import Dict, Optional, Tuple
 
 import torch
 
@@ -210,3 +210,80 @@ def make_warp_inputs(n: int, seed: int = 7) -> Dict[str, torch.Tensor]:
 
 WARP_HPARAMS = {'torso_model_version': 'v2', 'htbsr_head_weight_fuse_mode': 'v2', 'htbsr_head_threshold': 0.9, 'torso_kp_num': 4,
                 'torso_inp_mode': 'rgb_alpha', 'weight_fuse': True}
+
+
+# ---- SECC renderer: a synthetic BFM (the real BFM_model_front.mat is licensed and not shipped) ----------------------------------
+BFM_ID, BFM_EXP = 80, 64
+
+
+def make_bfm(seed: int = 0, rows: int = 150, cols: int = 238) -> Dict[str, 'np.ndarray']:
+    """A head-like mesh at BFM scale with the BFM's file contents (float64 numpy; the loader casts like the reference):
+    meanshape [1, 3N] (xyz interleaved, not centred: the loader recentres it), idBase [3N, 80], exBase [3N, 64], tri [F, 3] 1-based,
+    ncc [3, N] in [0, 1], right_eye / left_eye: disjoint 1-based face lists.  Default size 150 x 238 = 35 700 vertices, 70 626 faces.
+
+    The surface is a grid on an ellipsoidal shell (semi-axes 0.75 / 0.9 / 0.7, facing +z, i.e. the camera after to_camera) over 0.15-0.85 pi
+    of polar angle and +-0.8 pi of azimuth, so part of the back is meshed too, with a nose bump that occludes the cheek under yaw.  The id and exp
+    bases are smooth low-frequency fields: N(0,1) coefficients move a vertex by a few hundredths.  Face 0 sits on the forehead, where every
+    image with |yaw| <= 0.6 sees it."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    th = np.linspace(0.15 * np.pi, 0.85 * np.pi, rows)[:, None]
+    ph = np.linspace(-0.8 * np.pi, 0.8 * np.pi, cols)[None, :]
+    nose = 0.22 * np.exp(-((th - 0.56 * np.pi) ** 2 / 0.02 + ph ** 2 / 0.012))
+    rad = 1.0 + nose
+    P = np.stack([0.75 * rad * np.sin(th) * np.sin(ph), 0.9 * np.cos(th) * np.ones_like(ph), 0.7 * rad * np.sin(th) * np.cos(ph)], -1)
+    P = P.reshape(-1, 3) + np.array([0.02, 0.05, -0.03])             # off-centre: recentring at load moves it back
+    n = P.shape[0]
+    u, w = (th[:, 0] - th.min()) / np.ptp(th), (ph[0] - ph.min()) / np.ptp(ph)
+
+    def basis(k, amp):                                                 # separable fields a cos(pi f u + p) cos(pi g w + q) per column and axis
+        f = rng.integers(1, 4, size=(k, 3, 2))
+        p = rng.uniform(0, 2 * np.pi, size=(k, 3, 2))
+        a = rng.normal(size=(k, 3, 1)) * amp
+        fu = a * np.cos(np.pi * f[..., :1] * u + p[..., :1])           # [k, 3, rows]
+        fw = np.cos(np.pi * f[..., 1:] * w + p[..., 1:])               # [k, 3, cols]
+        return np.einsum('kar,kac->rcak', fu, fw).reshape(3 * n, k)   # rows 3v + axis, v = row * cols + col
+    id_base, ex_base = basis(BFM_ID, 0.006), basis(BFM_EXP, 0.004)
+    idx = np.arange(n).reshape(rows, cols)
+    q0, q1, q2, q3 = idx[:-1, :-1].reshape(-1), idx[:-1, 1:].reshape(-1), idx[1:, :-1].reshape(-1), idx[1:, 1:].reshape(-1)
+    tri = np.concatenate([np.stack([q0, q2, q1], 1), np.stack([q1, q2, q3], 1)], 0)
+    cen = P[tri].mean(1)
+    front = np.argmin(np.abs(cen[:, 0]) + np.abs(cen[:, 1] - 0.45) + np.abs(cen[:, 2] - cen[:, 2].max()) * 0.1)
+    tri[[0, front]] = tri[[front, 0]]                                  # face 0: the forehead
+    cen = P[tri].mean(1)
+    eyes = []
+    for sx in (-1, 1):                                                 # right eye (image left), then left eye
+        d = (cen[:, 0] - sx * 0.28) ** 2 + (cen[:, 1] - 0.18) ** 2
+        sel = np.nonzero((d < 0.06 ** 2) & (cen[:, 2] > 0))[0]
+        eyes.append(sel[sel != 0] + 1)
+    ncc = ((P - P.min(0)) / np.ptp(P, 0)).T
+    return {'meanshape': P.reshape(1, -1), 'idBase': id_base, 'exBase': ex_base, 'tri': (tri + 1).astype(np.float64), 'ncc': ncc,
+            'right_eye': eyes[0].astype(np.int64), 'left_eye': eyes[1].astype(np.int64)}
+
+
+def write_bfm_folder(path: str, bfm: Optional[dict] = None, seed: int = 0) -> Dict[str, object]:
+    """Write a BFM in the reference's file layout under `path` (BFM/BFM_model_front.mat with 1-based tri, ncc_code.npy [3,N],
+    bfm_{right,left}_eye_faces.npy 1-based) and return the SECC_Renderer keyword arguments that read it."""
+    import numpy as np
+    import os
+    import scipy.io
+    bfm = make_bfm(seed) if bfm is None else bfm
+    os.makedirs(os.path.join(path, 'BFM'), exist_ok=True)
+    scipy.io.savemat(os.path.join(path, 'BFM', 'BFM_model_front.mat'),
+                     {k: bfm[k] for k in ('meanshape', 'idBase', 'exBase', 'tri')})
+    np.save(os.path.join(path, 'ncc_code.npy'), bfm['ncc'].astype(np.float32))
+    eyes = (os.path.join(path, 'bfm_right_eye_faces.npy'), os.path.join(path, 'bfm_left_eye_faces.npy'))
+    np.save(eyes[0], bfm['right_eye'])
+    np.save(eyes[1], bfm['left_eye'])
+    return {'bfm_folder': os.path.join(path, 'BFM'), 'ncc_path': os.path.join(path, 'ncc_code.npy'), 'eye_faces': eyes}
+
+
+def make_coeffs(n: int, seed: int = 0, yaw: float = 0.0) -> Dict[str, torch.Tensor]:
+    """id [n,80], exp [n,64] ~ N(0,1); euler [n,3] with yaw ~ U[-yaw, yaw] and pitch / roll a fifth of it; trans [n,3] ~ 0.02 N(0,1) when yaw > 0
+    (zero otherwise, as real3d_infer.py:392-393 drives the renderer)."""
+    g = torch.Generator().manual_seed(seed)
+    c = {'id': torch.randn(n, BFM_ID, generator=g), 'exp': torch.randn(n, BFM_EXP, generator=g)}
+    e = (torch.rand(n, 3, generator=g) * 2 - 1) * yaw * torch.tensor([0.2, 1.0, 0.2])
+    t = 0.02 * torch.randn(n, 3, generator=g) * (1.0 if yaw > 0 else 0.0)
+    c.update({'euler': e, 'trans': t})
+    return c

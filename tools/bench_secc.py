@@ -6,7 +6,11 @@ Also: per-launch times of the conv stack (a profiled pass of its own), and the c
   torch      the PyTorch backbone, then FrameEngine on the (canonical, secc) pair (what a user pays without this library's backbone)
   engine     FrameEngine(secc2plane=...): backbone and render in one CUDA graph
 
-    python tools/bench_secc.py [--batch 4] [--iters 20]"""
+The `render` section times SECC_Renderer (synthetic BFM at the real BFM's size, 512^2): per call at batch 4 and 50, per launch (with the vertex
+pass's GB/s on its algorithmic bytes: basis + mean + coefficients + vertices out), the clip step fed coefficients (secc_renderer engine) against
+the same engine fed resident SECC images, and the step_host loop with coefficients against SECC images.  There is no pytorch3d comparator.
+
+    python tools/bench_secc.py [--batch 4] [--iters 20] [--section all|backbone|render]"""
 import argparse
 import json
 import os
@@ -62,10 +66,116 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--batch', type=int, default=4)
     ap.add_argument('--iters', type=int, default=20)
+    ap.add_argument('--section', choices=('all', 'backbone', 'render'), default='all')
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit('bench_secc needs a CUDA device')
     q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.sm', '--format=csv,noheader'], capture_output=True, text=True).stdout.strip()
+    out = {'gpu': q}
+    if args.section in ('all', 'backbone'):
+        out.update(bench_backbone(args))
+    if args.section in ('all', 'render'):
+        out['render'] = bench_render(args)
+    print(json.dumps(out))
+
+
+def _clock():
+    return subprocess.run(['nvidia-smi', '--query-gpu=clocks.sm', '--format=csv,noheader'], capture_output=True, text=True).stdout.strip()
+
+
+def _alternate(arms, iters, clocks):
+    """Warm every arm, then 3 rounds of the arms in turn; -> {arm: {'ms': median, 'runs_ms': [...]}}."""
+    with torch.no_grad():
+        for fn in arms.values():
+            for _ in range(3):
+                fn()
+        torch.cuda.synchronize()
+        res = {k: [] for k in arms}
+        for _ in range(3):
+            for k, fn in arms.items():
+                res[k].append(timed(fn, iters))
+            clocks.append(_clock())
+    return {k: {'ms': round(statistics.median(v), 4), 'runs_ms': [round(t, 4) for t in v]} for k, v in res.items()}
+
+
+def bench_render(args):
+    import tempfile
+    dev, B, S = 'cuda:0', args.batch, 512
+    kw = syn.write_bfm_folder(tempfile.mkdtemp(prefix='r3dp_bfm_'), seed=0)
+    r = r3.SECC_Renderer(S, device=dev, **kw)
+    clocks = []
+    calls = {}
+    for n in (B, 50):
+        c = {k: v.to(dev) for k, v in syn.make_coeffs(n, seed=1).items()}
+        calls[n] = c
+    call = _alternate({f'call_b{n}': (lambda c=c: r(c['id'], c['exp'], c['euler'], c['trans'])) for n, c in calls.items()}, args.iters, clocks)
+    # per-launch times: a profiled pass of its own (CUDA events around each launch)
+    per_launch = {}
+    with torch.no_grad():
+        for n, c in calls.items():
+            capi.PROF = capi.Profiler()
+            try:
+                for _ in range(args.iters):
+                    r(c['id'], c['exp'], c['euler'], c['trans'])
+                t = {k.split('.', 1)[1]: v / args.iters for k, v in capi.PROF.totals().items() if k.startswith('secc_render.')}
+            finally:
+                capi.PROF = None
+            nbytes = r.basis.numel() * 4 + r.mean_shape.numel() * 4 + n * (r.n_id + r.n_exp) * 4 + n * r.n_verts * 16
+            per_launch[f'b{n}'] = {k: round(v * 1e3, 1) for k, v in t.items()}
+            per_launch[f'b{n}']['unit'] = 'us'
+            per_launch[f'b{n}']['vertices_GBps'] = round(nbytes / (t['vertices'] * 1e-3) / 1e9, 1)
+            per_launch[f'b{n}']['vertices_bytes'] = nbytes
+    # the clip step, batch B, uint8 frames, secc2plane engine: fed coefficients vs fed resident SECC images
+    m = r3.SegFormerSECC2PlaneBackbone()
+    m.load_state_dict(ref.make_params({k: v.shape for k, v in m.state_dict().items()}, 7), strict=True)
+    m = m.to(dev).eval()
+
+    def mk(**k):
+        e = engine.FrameEngine(batch=B, sr_mode='tc', hp={'num_samples_fine': 0}, out_uint8=True, secc2plane=m, **k)
+        e.load_params(syn.make_decoder_params(seed=4), syn.make_sr_params(seed=5))
+        return e
+    src = syn.make_coeffs(1, seed=2)
+    coeff_src = torch.cat([src['id'], src['exp']], 1).to(dev)
+    cano_c = coeff_src.clone()
+    cano_c[:, r.n_id:] = 0
+    cano_planes = syn.make_planes(1, seed=0).to(dev)
+    e_coef, e_img = mk(secc_renderer=r), mk()
+    with torch.no_grad():
+        e_coef.begin_planes(cano_planes, coeff_src=coeff_src)
+        e_img.begin_planes(cano_planes, r.render(cano_c)[1], r.render(coeff_src)[1])
+    drv = syn.make_coeffs(B, seed=3)
+    coeff = torch.cat([drv['id'], drv['exp']], 1).to(dev)
+    with torch.no_grad():
+        img = r.render(coeff)[1].clone()
+    cams = syn.make_cameras(B, seed=1).to(dev)
+    u_c = syn.make_jitter(B, 4096, 48, 0, seed=2)[0].to(dev)
+    with torch.no_grad():
+        e_coef.prepare([(coeff, cams, u_c)])
+        e_img.prepare([(img, cams, u_c)])
+    step = _alternate({'coeff': lambda: e_coef.step(None, cams, u_c, coeff=coeff),
+                       'resident_image': lambda: e_img.step(None, cams, u_c, cond_tgt=img)}, args.iters, clocks)
+    # the step_host loop: pinned host inputs -> pinned host frames, coefficients vs SECC images
+    h_cams, h_u = cams.cpu().pin_memory(), u_c.cpu().pin_memory()
+    h_coeff, h_img = coeff.cpu().pin_memory(), img.cpu().pin_memory()
+    h_out = torch.empty(B, 512, 512, 3, dtype=torch.uint8).pin_memory()
+    eh_coef, eh_img = mk(secc_renderer=r), mk()
+    with torch.no_grad():
+        eh_coef.begin_planes(cano_planes, coeff_src=coeff_src)
+        eh_img.begin_planes(cano_planes, r.render(cano_c)[1], r.render(coeff_src)[1])
+
+    def host_loop(e, h):
+        def run():
+            e.step_host(h, h_cams, h_u, h_out)
+        return run
+    host = _alternate({'coeff': host_loop(eh_coef, h_coeff), 'image': host_loop(eh_img, h_img)}, args.iters, clocks)
+    for k, h in (('coeff', h_coeff), ('image', h_img)):
+        host[k]['planes_slot_h2d_bytes_per_step'] = h.numel() * h.element_size()
+    return {'size': S, 'batch': B, 'faces': r.n_faces, 'vertices': r.n_verts, 'sm_clock_samples': clocks, 'per_call_ms': call,
+            'per_launch': per_launch, 'clip_step_uint8': step, 'step_host_loop': host,
+            'comparator': 'none: no pytorch3d arm (no speed-up over the reference renderer is claimed)'}
+
+
+def bench_backbone(args):
     dev = 'cuda:0'
     B, H = args.batch, 512
     m = r3.SegFormerSECC2PlaneBackbone()
@@ -140,7 +250,7 @@ def main():
                 step_res[k].append(timed(fn, args.iters))
             clocks.append(subprocess.run(['nvidia-smi', '--query-gpu=clocks.sm', '--format=csv,noheader'], capture_output=True, text=True).stdout.strip())
     gf = gflop(H) * B
-    out = {'gpu': q, 'sm_clock_samples': clocks, 'batch': B, 'size': H, 'gflop_per_call': round(gf, 2),
+    out = {'sm_clock_samples': clocks, 'batch': B, 'size': H, 'gflop_per_call': round(gf, 2),
            'torch_default_tf32_flags': list(default_tf32)}
     for k, v in res.items():
         ms = statistics.median(v)
@@ -148,7 +258,7 @@ def main():
     out['conv_stack_ms_per_launch'] = prof
     out['clip_step_uint8'] = {k: {'ms': round(statistics.median(v), 3), 'frames_per_s': round(B * 1e3 / statistics.median(v), 1),
                                   'runs_ms': [round(t, 3) for t in v]} for k, v in step_res.items()}
-    print(json.dumps(out))
+    return out
 
 
 if __name__ == '__main__':
