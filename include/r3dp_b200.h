@@ -451,6 +451,19 @@ int r3dp_secc_raster(const float* verts, int N, const int* faces, int F, int B, 
 int r3dp_secc_resolve(const float* verts, int N, const int* faces, const float* ncc, int B, int S, int drop_face0, void* keys, float* secc,
                       float* mask, r3dp_stream_t stream);
 
+/* ------------------------------------------------ SECC blink: blink_eye_for_secc (inference/edit_secc.py) ---
+ * r3dp_secc_blink     edits secc [B,3,S,S] fp32 (r3dp_secc_resolve's layout) in place, 64 <= S <= 1024: closes the eye holes of each image to
+ *                     the fraction p (DESIGN.md, "SECC blink") and quantises the image to the reference's 8-bit codes (q / 127.5 - 1).
+ *                     Control per image, exactly one of: p [B] double (outside [0, 1] or NaN = untouched), or rows (fp32, row stride
+ *                     row_stride) whose first two values are (t, T): p = -4/T^2 t^2 + 4/T t in double; T <= 0, t < 0 or t >= T = untouched.
+ *                     Untouched images are not written; p == 0 only quantises.  Images on which the reference raises (no non-face pixel
+ *                     in either prior eye region, or no face pixel left around the eyes after the erosion) are left as they are and
+ *                     add one to *faults (int32, device).  scratch: r3dp_secc_blink_scratch_bytes(B, S) bytes, 256-byte aligned, any
+ *                     content (each call initialises what it reads).  Four launches, no host synchronisation. */
+size_t r3dp_secc_blink_scratch_bytes(int B, int S);
+int r3dp_secc_blink(float* secc, int B, int S, const double* p, const float* rows, int row_stride, void* scratch, int* faults,
+                    r3dp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -135,6 +135,8 @@ _SIGNATURES = {
     'r3dp_secc_vertices': (_I, [_P, _P, _I, _I, _I, _P, _I, _P, _I, _P, _P, _I, _F, _F, _P, _P]),
     'r3dp_secc_raster': (_I, [_P, _I, _P, _I, _I, _I, _P, _P]),
     'r3dp_secc_resolve': (_I, [_P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P]),
+    'r3dp_secc_blink_scratch_bytes': (_Z, [_I, _I]),
+    'r3dp_secc_blink': (_I, [_P, _I, _I, _P, _P, _I, _P, _P, _P]),
 }
 
 

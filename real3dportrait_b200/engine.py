@@ -133,12 +133,17 @@ class FrameEngine:
     coeff=c [B,144]) renders the driving image inside the step (and its graph), in front of the backbone.  Each step is one renderer call, so
     face 0 is background in the first frame of every step, i.e. every `batch`-th frame of the clip.  The reference renders a clip in 50-frame
     calls and loses face 0 only in frames 0, 50, 100, ...: the engine's frames differ from it where face 0 wins in the other frames that start a
-    step (one triangle, a few pixels).  prepare() tuples and step_host() then carry the coefficients in the planes slot."""
+    step (one triangle, a few pixels).  prepare() tuples and step_host() then carry the coefficients in the planes slot.
+    blink (with secc_renderer): the engine also closes the eyes of each driving image as real3d_infer.py's default blink_mode='period' does
+    (blink_eye_for_secc): coefficient rows become [B, n_id + n_exp + 2] = [id | exp | t | T] (fp32; period_blink_schedule gives (t, T), T = 0
+    leaves a frame untouched) and the edit runs in place between the render and the backbone, inside the step's graph.  blink_faults() counts
+    the frames on which the reference would raise (left unedited).  begin_planes() is unchanged: the reference blinks only the driving images."""
 
     def __init__(self, batch: int = 4, sr_mode: str = 'fp32', device=None, world: int = 1, rank: int = 0, dist=None, hp: Optional[dict] = None,
                  static_styles: bool = True, use_graph: bool = True, out_uint8: bool = False, exchange: str = 'allgather',
                  torso_model: Optional[torch.nn.Module] = None, warper_in_graph: bool = False, torso_stage2: str = 'torch',
-                 torso_motion: str = 'torch', secc2plane: Optional[torch.nn.Module] = None, secc_renderer: Optional[torch.nn.Module] = None):
+                 torso_motion: str = 'torch', secc2plane: Optional[torch.nn.Module] = None, secc_renderer: Optional[torch.nn.Module] = None,
+                 blink: bool = False):
         assert exchange in ('allgather', 'p2p', 'none')
         if secc2plane is not None and (hp or {}).get('phase1_plane_fusion_mode', 'add') != 'add':
             raise NotImplementedError('secc2plane: only phase1_plane_fusion_mode="add" (cano + secc, secc_img2plane.py:76-77) is built')
@@ -160,6 +165,9 @@ class FrameEngine:
         if secc_renderer is not None and secc2plane is None:
             raise ValueError('secc_renderer renders the input of the SECC -> plane backbone: FrameEngine(secc2plane=..., secc_renderer=...)')
         self.secc_r = secc_renderer.to(self.device) if secc_renderer is not None else None
+        if blink and self.secc_r is None:
+            raise ValueError('blink edits the images the SECC renderer draws: FrameEngine(secc2plane=..., secc_renderer=..., blink=True)')
+        self.blink = bool(blink)
         self.out_uint8 = bool(out_uint8)
         if self.out_uint8 and self.head.superresolution.sr_mode not in ('tc', 'tc_exact'):     # the head's effective mode: a torso head maps 'fp32' to 'tc'
             raise NotImplementedError('uint8 frames are written by the tensor-core SR epilogue (sr_mode="tc")')
@@ -262,8 +270,17 @@ class FrameEngine:
         if self._cano_cl is None:
             raise RuntimeError('secc2plane: call begin_planes(cano_planes, cond_cano, cond_src) before the first step')
         if self.secc_r is not None:
-            planes = self.secc_r.render(planes)[1]
+            secc = self.secc_r.render(planes)[1]
+            if self.blink:
+                self.secc_r.blink(secc, rows=planes[:, self.secc_r.n_id + self.secc_r.n_exp:])
+            planes = secc
         return (self._cano_cl, self.secc.planes_cl(planes))
+
+    def blink_faults(self) -> int:
+        """blink=True engines: the frames left unedited since the last call because the reference raises on them (resets; one sync)."""
+        if not self.blink:
+            raise ValueError('blink_faults() is for FrameEngine(..., blink=True)')
+        return self.secc_r.blink_faults()
 
     def end_clip(self) -> None:
         """Release the clip's constants, and the graphs that read them."""
@@ -305,7 +322,7 @@ class FrameEngine:
             g, out = self._capture_whole(planes, cameras, u_coarse, u_fine, kp_d)
         # the renderer's buffers the graph reads and writes (basis, faces, NCC code, key buffer) belong to the graph too: another engine built on
         # the same renderer, or a .to() of it, then cannot free memory the graph keeps writing to
-        g.keep_alive = self.secc_r.graph_buffers(_frames_of(planes)) if self.secc_r is not None else ()
+        g.keep_alive = self.secc_r.graph_buffers(_frames_of(planes), blink=self.blink) if self.secc_r is not None else ()
         return g, out
 
     def _capture_whole(self, planes, cameras, u_coarse, u_fine=None, kp_d=None):
@@ -399,13 +416,15 @@ class FrameEngine:
         [world*B,...] (rank-major); with exchange='p2p' the frames are additionally pushed into the open clip at `frame_index`.
         kp_d [B,68,3]: the frames' driving key points, the torso head's only per-frame condition (torso engines only).
         cond_tgt [B,3,H,W]: the driving SECC image, in place of planes (pass None), for FrameEngine(secc2plane=...).
-        coeff [B,144]: the frames' [id | exp] coefficients, in place of cond_tgt, for FrameEngine(secc2plane=..., secc_renderer=...).
+        coeff [B,144]: the frames' [id | exp] coefficients, in place of cond_tgt, for FrameEngine(secc2plane=..., secc_renderer=...);
+        [B,146] = [id | exp | t | T] with blink=True.
         The returned tensor is reused by the next step."""
         if self.secc_r is not None:
             if planes is not None or cond_tgt is not None or coeff is None:
                 raise ValueError('secc_renderer engine: step(None, cameras, ..., coeff=c [B,144])')
-            if coeff.ndim != 2 or coeff.shape[1] != self.secc_r.n_id + self.secc_r.n_exp:
-                raise ValueError(f'step: coeff must be [B,{self.secc_r.n_id + self.secc_r.n_exp}], got {tuple(coeff.shape)}')
+            K = self.secc_r.n_id + self.secc_r.n_exp + (2 if self.blink else 0)
+            if coeff.ndim != 2 or coeff.shape[1] != K:
+                raise ValueError(f'step: coeff must be [B,{K}]{" (id | exp | t | T)" if self.blink else ""}, got {tuple(coeff.shape)}')
             planes = coeff
         elif coeff is not None:
             raise ValueError('coeff needs FrameEngine(secc2plane=..., secc_renderer=...)')

@@ -10,7 +10,12 @@ The `render` section times SECC_Renderer (synthetic BFM at the real BFM's size, 
 pass's GB/s on its algorithmic bytes: basis + mean + coefficients + vertices out), the clip step fed coefficients (secc_renderer engine) against
 the same engine fed resident SECC images, and the step_host loop with coefficients against SECC images.  There is no pytorch3d comparator.
 
-    python tools/bench_secc.py [--batch 4] [--iters 20] [--section all|backbone|render]"""
+The `blink` section times the SECC blink (SECC_Renderer.blink) at 512^2: one batch call with every frame blinking (p = 1 and p = 0.44) and with
+no frame blinking (each call re-copies the rendered batch first; the copy alone is timed too), the coefficient clip step with blink=True
+against blink=False (a step with no blinking frame, a step whose frames all blink, and 500 frames under a period_blink_schedule), and for
+context the reference-semantics CPU cost of one frame through the numpy restatement (tests/blink_reference.py).
+
+    python tools/bench_secc.py [--batch 4] [--iters 20] [--section all|backbone|render|blink]"""
 import argparse
 import json
 import os
@@ -66,7 +71,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--batch', type=int, default=4)
     ap.add_argument('--iters', type=int, default=20)
-    ap.add_argument('--section', choices=('all', 'backbone', 'render'), default='all')
+    ap.add_argument('--section', choices=('all', 'backbone', 'render', 'blink'), default='all')
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit('bench_secc needs a CUDA device')
@@ -76,6 +81,8 @@ def main():
         out.update(bench_backbone(args))
     if args.section in ('all', 'render'):
         out['render'] = bench_render(args)
+    if args.section in ('all', 'blink'):
+        out['blink'] = bench_blink(args)
     print(json.dumps(out))
 
 
@@ -173,6 +180,79 @@ def bench_render(args):
     return {'size': S, 'batch': B, 'faces': r.n_faces, 'vertices': r.n_verts, 'sm_clock_samples': clocks, 'per_call_ms': call,
             'per_launch': per_launch, 'clip_step_uint8': step, 'step_host_loop': host,
             'comparator': 'none: no pytorch3d arm (no speed-up over the reference renderer is claimed)'}
+
+
+def bench_blink(args):
+    import random
+    import tempfile
+    import time
+    import blink_reference as bref
+    dev, B, S = 'cuda:0', args.batch, 512
+    kw = syn.write_bfm_folder(tempfile.mkdtemp(prefix='r3dp_bfm_'), seed=0)
+    r = r3.SECC_Renderer(S, device=dev, **kw)
+    clocks = []
+    drv = syn.make_coeffs(B, seed=3)
+    coeff = torch.cat([drv['id'], drv['exp']], 1).to(dev)
+    with torch.no_grad():
+        src = r.render(coeff)[1].clone()
+    work = src.clone()
+
+    def call(p):
+        def run():
+            work.copy_(src)
+            r.blink(work, p=p)
+        return run
+    p1, p44, none = (torch.full((B,), v, dtype=torch.float64, device=dev) for v in (1.0, 0.44, -1.0))
+    calls = _alternate({'all_blink_p1': call(p1), 'all_blink_p044': call(p44), 'none_blink': call(none), 'copy_only': lambda: work.copy_(src)},
+                       args.iters, clocks)
+    assert r.blink_faults() == 0
+    m = r3.SegFormerSECC2PlaneBackbone()
+    m.load_state_dict(ref.make_params({k: v.shape for k, v in m.state_dict().items()}, 7), strict=True)
+    m = m.to(dev).eval()
+
+    def mk(**k):
+        e = engine.FrameEngine(batch=B, sr_mode='tc', hp={'num_samples_fine': 0}, out_uint8=True, secc2plane=m, secc_renderer=r, **k)
+        e.load_params(syn.make_decoder_params(seed=4), syn.make_sr_params(seed=5))
+        return e
+    s0 = syn.make_coeffs(1, seed=2)
+    coeff_src = torch.cat([s0['id'], s0['exp']], 1).to(dev)
+    cano_planes = syn.make_planes(1, seed=0).to(dev)
+    e_blink, e_plain = mk(blink=True), mk()
+    with torch.no_grad():
+        e_blink.begin_planes(cano_planes, coeff_src=coeff_src)
+        e_plain.begin_planes(cano_planes, coeff_src=coeff_src)
+    cams = syn.make_cameras(B, seed=1).to(dev)
+    u_c = syn.make_jitter(B, 4096, 48, 0, seed=2)[0].to(dev)
+
+    def rows_of(tT):
+        return torch.cat([coeff, torch.tensor(tT, dtype=torch.float32, device=dev)], 1).contiguous()
+    r_none, r_all = rows_of([[0, 0]] * B), rows_of([[t, 10] for t in range(1, B + 1)])
+    step = _alternate({'blink_none_blinking': lambda: e_blink.step(None, cams, u_c, coeff=r_none),
+                       'blink_all_blinking': lambda: e_blink.step(None, cams, u_c, coeff=r_all),
+                       'no_blink': lambda: e_plain.step(None, cams, u_c, coeff=coeff)}, args.iters, clocks)
+    # 500 frames: steps of B frames with a period_blink_schedule (random.Random(0)), every step's rows resident
+    N = 500
+    sched = r3.period_blink_schedule(N, rng=random.Random(0)).float().to(dev)
+    clip_rows = [torch.cat([coeff, sched[i:i + B]], 1).contiguous() for i in range(0, N - N % B, B)]
+
+    def clip(e, wide):
+        def run():
+            for rw in clip_rows:
+                e.step(None, cams, u_c, coeff=rw if wide else coeff)
+        return run
+    clip_ms = _alternate({'blink': clip(e_blink, True), 'no_blink': clip(e_plain, False)}, 1, clocks)
+    assert e_blink.blink_faults() == 0
+    # context: the reference semantics on the CPU, one frame (numpy restatement; the reference itself adds two k-d trees per frame)
+    x = src[0].cpu().numpy()
+    t0 = time.perf_counter()
+    for _ in range(3):
+        bref.blink(x, 0.44)
+    cpu_ms = (time.perf_counter() - t0) / 3 * 1e3
+    net = {k: round(calls[k]['ms'] - calls['copy_only']['ms'], 4) for k in ('all_blink_p1', 'all_blink_p044', 'none_blink')}
+    return {'size': S, 'batch': B, 'sm_clock_samples': clocks, 'call_ms': calls, 'call_net_of_copy_ms': net, 'clip_step_uint8': step,
+            'step_overhead_pct': {k: round(100 * (step[k]['ms'] / step['no_blink']['ms'] - 1), 2) for k in ('blink_none_blinking', 'blink_all_blinking')},
+            'clip_500_frames_ms': clip_ms, 'blinking_frames_in_500': int((sched[:, 1] > 0).sum()),
+            'cpu_restatement_ms_per_frame': round(cpu_ms, 1)}
 
 
 def bench_backbone(args):
