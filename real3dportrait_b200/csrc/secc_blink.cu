@@ -53,7 +53,8 @@ __device__ __forceinline__ bool control(const double* pv, const float* rows, int
     }
     const float ft = rows[(size_t)b * row_stride], fT = rows[(size_t)b * row_stride + 1];
     if (!(fT > 0.f) || !(ft >= 0.f) || !(ft < fT) || fT > 4096.f) return false;
-    const int t = (int)ft, T = (int)fT;
+    const int t = (int)ft, T = (int)fT;                             // truncated, as int() does
+    if (t >= T) return false;                                       // fractional rows: 0 < T < 1 (T = 0 after truncation), or int(t) = int(T)
     // real3d_infer.py's -4/T**2 * t**2 + 4/T * t: ((-4 / T^2) t^2) + ((4 / T) t), each step rounded once
     p = __dadd_rn(__dmul_rn(__ddiv_rn(-4.0, (double)(T * T)), (double)(t * t)), __dmul_rn(__ddiv_rn(4.0, (double)T), (double)t));
     return true;

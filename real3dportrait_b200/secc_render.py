@@ -125,7 +125,8 @@ class SECC_Renderer(nn.Module):
         return it.  Per image, exactly one of:
           p     a float per image (a sequence, or a float64 CUDA tensor [B]): the close-eye fraction; a negative value leaves the image untouched.
           rows  [B, >= 2] fp32 CUDA whose columns 0 and 1 hold (t, T) (a column slice such as coeff[:, 144:] is read in place): p is
-                -4/T**2 * t**2 + 4/T * t in double; T = 0 (or t >= T) leaves the image untouched.
+                -4/T**2 * t**2 + 4/T * t in double on int(t), int(T).  The image is untouched unless 0 <= t < T <= 4096 and
+                int(t) < int(T): T = 0, t >= T, negative, NaN and infinite entries and T > 4096 leave it untouched.
         Untouched images are not written; p = 0 only quantises.  An image on which the reference raises is left as it is and counted
         (blink_faults()).  No host synchronisation (capturable), except to copy a host sequence p."""
         return _blink(self._blink, secc, p, rows)

@@ -41,6 +41,22 @@ def schedule_p(t, T):
     return -4 / T ** 2 * t ** 2 + 4 / T * t
 
 
+def rows_control(t, T):
+    """The control of an image given by an fp32 row (t, T) (SECC_Renderer.blink's docstring, DESIGN.md "SECC blink"): None (untouched)
+    unless 0 <= t < T <= 4096 and int(t) < int(T); else p = schedule_p(int(t), int(T)) in double."""
+    t, T = float(np.float32(t)), float(np.float32(T))
+    if not (T > 0 and t >= 0 and t < T and T <= 4096):
+        return None
+    ti, Ti = int(t), int(T)
+    return None if ti >= Ti else schedule_p(ti, Ti)
+
+
+def p_control(p):
+    """The control of an image given by a double p: None (untouched) unless 0 <= p <= 1 (so NaN is untouched and -0.0 is p = 0)."""
+    p = float(p)
+    return p if 0.0 <= p <= 1.0 else None
+
+
 def _disk_dilate(m, radius=5):
     H, W = m.shape
     pad = np.zeros((H + 2 * radius, W + 2 * radius), dtype=bool)

@@ -15,18 +15,13 @@ import torch
 
 import secc2plane_reference as s2p_ref
 import secc_render_reference as ref
+import secc_launch_reference as lr
+from secc_launch_reference import U, value_bar, vertex_bar
 import real3dportrait_b200 as r3
 from real3dportrait_b200 import _capi as capi, engine, synthetic as syn
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
-U = 2.0 ** -24
-
-
-def gamma(n):
-    return n * U / (1 - n * U)
-
-
 @pytest.fixture(scope='module')
 def bfm(tmp_path_factory):
     kw = syn.write_bfm_folder(str(tmp_path_factory.mktemp('bfm')), seed=0)
@@ -50,28 +45,6 @@ def _vertices(r, c, B):
     assert torch.isnan(big[:G]).all() and torch.isnan(big[-G:]).all(), 'vertex guard overwritten'
     assert not torch.isnan(verts).any(), 'vertex element not written'
     return verts
-
-
-def vertex_bar(m, c):
-    """float64 reference vertices [B,N,3] and their fp32 error bound [B,N,3]."""
-    cpu = {k: v.cpu().double().numpy() for k, v in c.items()}
-    s, terms = ref.shape(m, cpu['id'], cpu['exp'])
-    K = cpu['id'].shape[1] + cpu['exp'].shape[1]
-    e_s = gamma(K + 1) * terms
-    R = ref.rotation(cpu['euler'])
-    e_r = 8 * U + 2 * U * np.abs(cpu['euler']).max()                 # sincospif of x / pi: argument and result rounding, 2-3 factor products
-    aR = np.abs(R)
-    t = cpu['trans']
-    e_v = np.einsum('bij,bnj->bni', aR, e_s) + e_r * np.abs(s).sum(-1, keepdims=True) \
-        + gamma(3) * (np.einsum('bij,bnj->bni', aR, np.abs(s)) + np.abs(t)[:, None])
-    v = ref.vertices(m, cpu['id'], cpu['exp'], cpu['euler'], t)
-    z = v[..., 2]
-    e_z = e_v[..., 2] + U * np.abs(z)
-    rel = e_z / z + 3 * U
-    tz = z * ref.TAN_HALF
-    e_x = e_v[..., 0] / tz + np.abs(v[..., 0]) * rel
-    e_y = e_v[..., 1] / tz + np.abs(v[..., 1]) * rel
-    return v, np.stack([e_x, e_y, e_z], -1)
 
 
 @pytest.fixture(scope='module')
@@ -118,69 +91,9 @@ def _raster_case(r, m, c, B, S, drop_face0=True):
     return verts, face, secc, mask
 
 
-def value_bar(m, vb, f, d_ndc):
-    """Per pixel and channel, the fp32 bar of secc for winning faces f [n] of one frame (vertices vb [N,3]) with vertex error d_ndc:
-    |dw_i| <= (d_ndc 2 perimeter / |A| + 4u) (zmax / zmin)^2 for each barycentric, times 2 spread(ncc) as sum_i dw_i ~ 0, + 12u of rounding.
-    -> (bar [n,3], the faces' NCC codes [n,3 verts,3 ch])."""
-    fv = m['faces'][f]
-    P = vb[fv]                                                          # [n,3 verts,3]
-    A = np.abs((P[:, 0, 0] - P[:, 1, 0]) * (P[:, 2, 1] - P[:, 1, 1]) - (P[:, 0, 1] - P[:, 1, 1]) * (P[:, 2, 0] - P[:, 1, 0]))
-    per = sum(np.hypot(*(P[:, i, :2] - P[:, (i + 1) % 3, :2]).T) for i in range(3))
-    zr = (P[:, :, 2].max(1) / P[:, :, 2].min(1)) ** 2
-    dw = 3 * (d_ndc * 2 * per / A + 4 * U) * zr
-    ncc = m['ncc'][fv]
-    return 2 * dw[:, None] * (ncc.max(1) - ncc.min(1)) + 12 * U, ncc
-
-
 def check_raster(m, c, B, S, face, secc, mask, label, drop_face0=True):
     v, bar = vertex_bar(m, c)
-    faces = m['faces']
-    stats = {'decisive': 0, 'ambiguous': 0, 'value_ratio': 0.0, 'value_err': 0.0}
-    for b in range(B):
-        e_xy = bar[b, :, :2].max()
-        d_ndc = 2 * e_xy + 4 * U                                       # vertex error + the pixel centre's rounding
-        d_px = d_ndc * S / 2 + 1e-6
-        d_z = (bar[b, :, 2] / v[b, :, 2]).max() + 16 * U
-        pairs = ref.raster_pairs(v[b], faces, S, slack_px=4 * d_px)
-        f_ref, w_ref = ref.resolve(pairs, S)
-        near = pairs['dist'] > -d_px
-        pix, pf, ppz, pd = pairs['pix'][near], pairs['face'][near], pairs['pz'][near], pairs['dist'][near]
-        # the winner's own pair
-        win = f_ref[pix] == pf
-        wpz = np.full(S * S, np.inf)
-        wd = np.full(S * S, -np.inf)
-        wpz[pix[win & pairs['covered'][near]]] = ppz[win & pairs['covered'][near]]
-        wd[pix[win & pairs['covered'][near]]] = pd[win & pairs['covered'][near]]
-        amb = np.zeros(S * S, bool)
-        amb[pix[~win & ~(ppz > wpz[pix] * (1 + d_z))]] = True           # another face within delta and not clearly farther
-        amb |= (f_ref >= 0) & (wd <= d_px)                              # the centre is within delta of the winner's boundary
-        amb |= (f_ref < 0) & np.isin(np.arange(S * S), pix)             # no winner, but a face comes within delta
-        got = face[b].reshape(-1)
-        dec = ~amb
-        bad = dec & (got != f_ref)
-        assert not bad.any(), f'{label} b={b}: {bad.sum()} decisive pixels differ, e.g. {np.nonzero(bad)[0][:5]}'
-        allowed = set((pix.astype(np.int64) * (faces.shape[0] + 1) + pf).tolist())
-        ai = np.nonzero(amb)[0]
-        for q in ai:
-            assert got[q] == -1 or int(q) * (faces.shape[0] + 1) + int(got[q]) in allowed, f'{label} b={b} pixel {q}: face {got[q]}'
-        stats['decisive'] += int(dec.sum())
-        stats['ambiguous'] += int(amb.sum())
-        # values where the faces agree
-        same = np.nonzero((got == f_ref) & (f_ref >= 0))[0]
-        vbar, ncc = value_bar(m, v[b], f_ref[same], d_ndc)
-        col = (w_ref[same][:, :, None] * ncc).sum(1)
-        drop = (b == 0) & (f_ref[same] == 0) & drop_face0               # the packed face 0: background
-        want = np.where(drop[:, None], -1.0, 2 * col - 1)
-        gotv = secc[b].reshape(3, -1)[:, same].T
-        err = np.abs(gotv - want)
-        stats['value_ratio'] = max(stats['value_ratio'], float((err / vbar).max(initial=0)))
-        stats['value_err'] = max(stats['value_err'], float(err.max(initial=0)))
-        assert (err <= vbar).all(), f'{label} b={b}: value error {err.max():.2e}'
-        bg = (got < 0) | ((b == 0) & (got == 0) & drop_face0)
-        assert (secc[b].reshape(3, -1)[:, bg] == -1).all() and (mask[b, 0].reshape(-1)[bg] == 0).all()
-    print(f'{label}: decisive {stats["decisive"]}, ambiguous {stats["ambiguous"]}, secc max |err| {stats["value_err"]:.2e}, '
-          f'worst err/bar {stats["value_ratio"]:.3f}')
-    return stats
+    return lr.check_raster(m, v, lr.raster_err(v, bar), S, face, secc, mask, label, drop_face0)
 
 
 @pytest.mark.parametrize('S,B,yaw', [(512, 1, 0.0), (512, 4, 0.6), (224, 4, 0.6), (97, 2, 0.6)])
