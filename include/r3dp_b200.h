@@ -405,9 +405,12 @@ int r3dp_mf_occlusion(const void* x_f16, int N, int D, int H, int W, int C, int 
  * r3dp_sp_embed           prenet + patch_embed1.proj (7x7 stride 4 pad 3, segformer.py:206-232) -> y fp32 [N, ceil(H/4)*ceil(W/4), 32], before its
  *                         LayerNorm.  Prenet output = (base ? base[1,3,H,W] : bpre[3]) + w [3,cin] . x[N,cin,H,W]; wpe [32,3,7,7], bpe [32]
  * r3dp_sp_layernorm       v = x + t (t may be NULL); xo = v if non-NULL (xo may be x: the in-place residual add of Block.forward, segformer.py:236-239);
- *                         u = LayerNorm(v)(g, b, eps) (segformer.py:118,216,411) -> yf fp32 [R,C] and/or yh fp16 with row stride yhs; C % 32 == 0, <= 256
+ *                         u = LayerNorm(v)(g, b, eps) (segformer.py:118,216,411) -> yf fp32 [R,C] and/or yh fp16 with row stride yhs; C % 32 == 0, <= 1024
  * r3dp_sp_patches         y fp16 [N*Ho*Wo, k*k*C], column (ky*k + kx)*C + c = x[n, oy*s - p + ky, ox*s - p + kx, c] (zero outside): GEMM rows of
  *                         the 3x3/2 patch embeds (segformer.py:286-291) and of Attention.sr (k = s = sr_ratio, segformer.py:126-128); C % 8 == 0
+ * r3dp_sp_patches_dil     the same rows for a conv of dilation d (x[n, oy*s - p + ky*d, ox*s - p + kx*d, c]), each row ldy halves long (ldy % 8 == 0,
+ *                         >= k*k*C) with columns from k*k*C on zero, so that the GEMM's K can be a multiple of 32; r3dp_sp_patches is d = 1,
+ *                         ldy = k*k*C
  * r3dp_sp_attention       Attention.forward's core (segformer.py:130-150) for head_dim 32: q fp16 [N,Tq, >= heads*32] (row stride qs), kv fp16
  *                         [N,Tk, >= 2*heads*32] (k in channels [0, 32 heads), v after it), Tk <= 256 -> o fp16 (row stride os), channel head*32 + d;
  *                         fp32 scores and an exact full-row softmax
@@ -424,6 +427,7 @@ int r3dp_sp_embed(const float* x, int N, int cin, int H, int W, const float* wpr
 int r3dp_sp_layernorm(const float* x, const float* t, int R, int C, const float* g, const float* b, float eps, float* xo, float* yf, void* yh_f16,
                       int yhs, r3dp_stream_t stream);
 int r3dp_sp_patches(const void* x_f16, int N, int H, int W, int C, int k, int s, int p, void* y_f16, r3dp_stream_t stream);
+int r3dp_sp_patches_dil(const void* x_f16, int N, int H, int W, int C, int k, int s, int p, int d, void* y_f16, int ldy, r3dp_stream_t stream);
 int r3dp_sp_attention(const void* q_f16, int qs, const void* kv_f16, int kvs, int N, int Tq, int Tk, int heads, float scale, void* o_f16, int os,
                       r3dp_stream_t stream);
 int r3dp_sp_dwconv_gelu(const void* x_f16, int N, int H, int W, int C, const float* w, const float* b, void* y_f16, r3dp_stream_t stream);
@@ -431,6 +435,33 @@ int r3dp_sp_head_fuse(const float* g1, int h1, const float* g2, int h2, const fl
                       void* y_f16, r3dp_stream_t stream);
 int r3dp_sp_leaky(void* x_f16, long long n, float slope, r3dp_stream_t stream);
 int r3dp_sp_upsample2_flip(const void* x_f16, int N, int h, int w, int C, void* yr_f16, void* yrc_f16, r3dp_stream_t stream);
+
+/* ------------------------------------------------ canonical plane backbone: Img2PlaneModel ---
+ * (modules/img2plane/img2plane_model.py:12-81; run once per clip on the source image by cal_cano_plane, modules/real3d/secc_img2plane.py:50-62).
+ * Activations NHWC fp16; token tensors row-major [N, h*w, C].  Convolutions and token GEMMs run on r3dp_mf_conv3d (strided and dilated convs on
+ * r3dp_sp_patches_dil rows), LayerNorm on r3dp_sp_layernorm, the Mlp's DWConv + GELU on r3dp_sp_dwconv_gelu.
+ * r3dp_ip_attention      Attention.forward's core (segformer/base.py:101-122) for head_dim 256 on wgmma: q fp16 [N,Tq, >= heads*256] (row stride
+ *                        qs), kv fp16 [N,Tk, >= 2*heads*256] (k in channels [0, 256 heads), v after it) -> o fp16 (row stride os), channel
+ *                        head*256 + d.  Any Tq, Tk >= 1; qs, kvs multiples of 8; q, kv 16-byte aligned.  Online softmax in fp32, P rounded to
+ *                        fp16 for P.V; no Tq x Tk buffer
+ * r3dp_ip_input          x fp32 [N,3,H,W] -> y fp16 [N,H,W,8] = (rgb, i/H, j/H, 0, 0, 0): the coordinate channels of img2plane_model.py:59-64
+ * r3dp_ip_maxpool        nn.MaxPool2d(3, 2, 1): x fp16 NHWC [N,H,W,C] -> y [N, (H-1)/2+1, (W-1)/2+1, C]; C % 8 == 0
+ * r3dp_ip_channel_mean   AdaptiveAvgPool2d(1): x fp16 [N,HW,C] -> y fp16 [N,C]; C % 32 == 0
+ * r3dp_ip_broadcast      y[n, p, yc0 + c] = v[n, c] for every pixel p < HW (pixel stride ys): ASPPPooling's upsampling of a 1x1 map
+ * r3dp_ip_pixel_shuffle  nn.PixelShuffle(2) of tokens x (+ t, may be NULL) fp32 [N, h*w, 4C] -> y fp16 [N,2h,2w] pixels of ys halves, channels
+ *                        [yc0, yc0 + C): y[n, 2a+i, 2b+j, c] = x[n, a*w + b, 4c + 2i + j]
+ * r3dp_ip_upsample2      nn.UpsamplingBilinear2d(x2) (align_corners=True): x fp16 NHWC [N,h,w,C] -> y [N,2h,2w,C]; C % 8 == 0
+ * r3dp_ip_flip_hwpc      the last conv's x fp32 [N,H,W,96] -> planes fp32 [N,H,W,3,32] (the render's hwpc layout) with the flips of
+ *                        img2plane_model.py:72-81: out[n,Y,X,p,c] = x[n, H-1-Y, p < 2 ? X : W-1-X, 32p + c] */
+int r3dp_ip_attention(const void* q_f16, int qs, const void* kv_f16, int kvs, int N, int Tq, int Tk, int heads, float scale, void* o_f16, int os,
+                      r3dp_stream_t stream);
+int r3dp_ip_input(const float* x, int N, int H, int W, void* y_f16, r3dp_stream_t stream);
+int r3dp_ip_maxpool(const void* x_f16, int N, int H, int W, int C, void* y_f16, r3dp_stream_t stream);
+int r3dp_ip_channel_mean(const void* x_f16, int N, int HW, int C, void* y_f16, r3dp_stream_t stream);
+int r3dp_ip_broadcast(const void* v_f16, int N, int HW, int C, void* y_f16, int ys, int yc0, r3dp_stream_t stream);
+int r3dp_ip_pixel_shuffle(const float* x, const float* t, int N, int h, int w, int C, void* y_f16, int ys, int yc0, r3dp_stream_t stream);
+int r3dp_ip_upsample2(const void* x_f16, int N, int h, int w, int C, void* y_f16, r3dp_stream_t stream);
+int r3dp_ip_flip_hwpc(const float* x, int N, int H, int W, float* out, r3dp_stream_t stream);
 
 /* ------------------------------------------------ SECC renderer: SECC_Renderer (deep_3drecon/secc_renderer.py) ---
  * The 3DMM face mesh rasterised at S x S with pytorch3d's rules (blur 0, one face per pixel, perspective-correct barycentrics, no culling

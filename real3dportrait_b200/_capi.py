@@ -127,11 +127,20 @@ _SIGNATURES = {
     'r3dp_sp_embed': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     'r3dp_sp_layernorm': (_I, [_P, _P, _I, _I, _P, _P, _F, _P, _P, _P, _I, _P]),
     'r3dp_sp_patches': (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
+    'r3dp_sp_patches_dil': (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P]),
     'r3dp_sp_attention': (_I, [_P, _I, _P, _I, _I, _I, _I, _I, _F, _P, _I, _P]),
     'r3dp_sp_dwconv_gelu': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P]),
     'r3dp_sp_head_fuse': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _I, _P, _P, _P]),
     'r3dp_sp_leaky': (_I, [_P, C.c_longlong, _F, _P]),
     'r3dp_sp_upsample2_flip': (_I, [_P, _I, _I, _I, _I, _P, _P, _P]),
+    'r3dp_ip_attention': (_I, [_P, _I, _P, _I, _I, _I, _I, _I, _F, _P, _I, _P]),
+    'r3dp_ip_input': (_I, [_P, _I, _I, _I, _P, _P]),
+    'r3dp_ip_maxpool': (_I, [_P, _I, _I, _I, _I, _P, _P]),
+    'r3dp_ip_channel_mean': (_I, [_P, _I, _I, _I, _P, _P]),
+    'r3dp_ip_broadcast': (_I, [_P, _I, _I, _I, _P, _I, _I, _P]),
+    'r3dp_ip_pixel_shuffle': (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _I, _P]),
+    'r3dp_ip_upsample2': (_I, [_P, _I, _I, _I, _I, _P, _P]),
+    'r3dp_ip_flip_hwpc': (_I, [_P, _I, _I, _I, _P, _P]),
     'r3dp_secc_vertices': (_I, [_P, _P, _I, _I, _I, _P, _I, _P, _I, _P, _P, _I, _F, _F, _P, _P]),
     'r3dp_secc_raster': (_I, [_P, _I, _P, _I, _I, _I, _P, _P]),
     'r3dp_secc_resolve': (_I, [_P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P]),

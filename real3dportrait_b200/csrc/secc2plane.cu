@@ -1,9 +1,9 @@
 // SegFormerSECC2PlaneBackbone (modules/real3d/segformer.py:673-733, MiT-b0) on sm_90a: the kernels around the token GEMMs.
 //   sp_prenet_kernel        the prenet's 1x1 conv (Conv2dLayer, networks_stylegan2.py:139-183) on the per-clip channels: the constant image
 //   sp_embed_kernel         prenet (constant image + tgt part, or the whole input) fused with patch_embed1's 7x7 stride-4 conv (segformer.py:206-232)
-//   sp_layernorm_kernel     optional residual add, then LayerNorm of each C <= 256 row in fp32 (one warp per row)
-//   sp_patches_kernel       k x k stride-s patches of an NHWC fp16 image as GEMM rows: the 3x3/2 patch embeds of stages 2-4 and the
-//                           spatial-reduction conv (k = stride = sr_ratio, segformer.py:126-128)
+//   sp_layernorm_kernel     optional residual add, then LayerNorm of each C <= 1024 row in fp32 (one warp per row)
+//   sp_patches_kernel       k x k stride-s dilation-d patches of an NHWC fp16 image as GEMM rows: the 3x3/2 patch embeds of stages 2-4 and
+//                           the spatial-reduction conv (k = stride = sr_ratio, segformer.py:126-128); Img2PlaneModel's strided and dilated convs
 //   sp_attention_kernel     softmax(q k^T * scale) v for head_dim 32 and <= 256 keys (segformer.py:130-150), exact fp32 softmax
 //   sp_dwconv_gelu_kernel   DWConv 3x3 + bias + exact GELU (segformer.py:82-84,459-468)
 //   sp_head_fuse_kernel     SegFormerHead with linear_c* and the BN'd linear_fuse folded into the per-level maps G_i (the caller's GEMMs):
@@ -82,17 +82,19 @@ __global__ void __launch_bounds__(128) sp_embed_kernel(const float* __restrict__
     for (int i = 0; i < kEmbedC / 4; ++i) out[i] = make_float4(acc[4 * i], acc[4 * i + 1], acc[4 * i + 2], acc[4 * i + 3]);
 }
 
-// One warp per row; lane holds channels lane + 32 i.  Two-pass statistics in fp32 (nn.LayerNorm: biased variance).
+// One warp per row; lane holds channels lane + 32 i, i < NV (8: C <= 256, 32: C <= 1024).  Two-pass statistics in fp32 (nn.LayerNorm:
+// biased variance).
+template <int NV>
 __global__ void __launch_bounds__(256) sp_layernorm_kernel(const float* x, const float* __restrict__ t, int R, int C, const float* __restrict__ g,
                                                            const float* __restrict__ b, float eps, float* xo, float* __restrict__ yf,
                                                            __half* __restrict__ yh, int yhs) {
     const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (row >= R) return;
     const int nv = C / 32;
-    float v[8];
+    float v[NV];
     float s = 0.f;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
+    for (int i = 0; i < NV; ++i) {
         if (i < nv) {
             const size_t o = (size_t)row * C + lane + 32 * i;
             v[i] = x[o] + (t ? t[o] : 0.f);
@@ -104,13 +106,13 @@ __global__ void __launch_bounds__(256) sp_layernorm_kernel(const float* x, const
     const float mean = s / C;
     float q = 0.f;
 #pragma unroll
-    for (int i = 0; i < 8; ++i)
+    for (int i = 0; i < NV; ++i)
         if (i < nv) { const float d = v[i] - mean; q = fmaf(d, d, q); }
 #pragma unroll
     for (int m = 16; m; m >>= 1) q += __shfl_xor_sync(0xffffffffu, q, m);
     const float rstd = rsqrtf(q / C + eps);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
+    for (int i = 0; i < NV; ++i) {
         if (i >= nv) break;
         const int c = lane + 32 * i;
         const size_t o = (size_t)row * C + c;
@@ -121,21 +123,22 @@ __global__ void __launch_bounds__(256) sp_layernorm_kernel(const float* x, const
     }
 }
 
-// y[(n, oy, ox)][(ky*k + kx)*C + c] = x[n, oy*s - p + ky, ox*s - p + kx, c] (0 outside); 8 channels per thread.
-__global__ void sp_patches_kernel(const __half* __restrict__ x, int N, int H, int W, int C, int k, int s, int p, int Ho, int Wo,
+// y[(n, oy, ox)][(ky*k + kx)*C + c] = x[n, oy*s - p + ky*d, ox*s - p + kx*d, c] (0 outside), rows of ldy halves with columns from k*k*C
+// on zero; 8 channels per thread.
+__global__ void sp_patches_kernel(const __half* __restrict__ x, int N, int H, int W, int C, int k, int s, int p, int d, int Ho, int Wo, int ldy,
                                   __half* __restrict__ y) {
-    const int c8 = C / 8;
-    const long long total = (long long)N * Ho * Wo * k * k * c8;
+    const int c8 = C / 8, l8 = ldy / 8;
+    const long long total = (long long)N * Ho * Wo * l8;
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= total) return;
     long long t = idx;
-    const int cc = (int)(t % c8); t /= c8;
-    const int tap = (int)(t % (k * k)); t /= (k * k);
+    const int j = (int)(t % l8); t /= l8;
     const int ox = (int)(t % Wo); t /= Wo;
     const int oy = (int)(t % Ho); const int n = (int)(t / Ho);
-    const int iy = oy * s - p + tap / k, ix = ox * s - p + tap % k;
+    const int tap = j / c8, cc = j - tap * c8;
+    const int iy = oy * s - p + (tap / k) * d, ix = ox * s - p + (tap % k) * d;
     uint4 v = make_uint4(0, 0, 0, 0);
-    if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = *reinterpret_cast<const uint4*>(x + (((size_t)n * H + iy) * W + ix) * C + cc * 8);
+    if (tap < k * k && iy >= 0 && iy < H && ix >= 0 && ix < W) v = *reinterpret_cast<const uint4*>(x + (((size_t)n * H + iy) * W + ix) * C + cc * 8);
     *reinterpret_cast<uint4*>(y + idx * 8) = v;
 }
 
@@ -338,23 +341,33 @@ extern "C" int r3dp_sp_embed(const float* x, int N, int cin, int H, int W, const
 extern "C" int r3dp_sp_layernorm(const float* x, const float* t, int R, int C, const float* g, const float* b, float eps, float* xo, float* yf,
                                  void* yh_f16, int yhs, r3dp_stream_t stream) {
     R3DP_REQUIRE(x && g && b && (xo || yf || yh_f16), "sp_layernorm: null pointer");
-    R3DP_REQUIRE(R > 0 && C % 32 == 0 && C >= 32 && C <= 256 && (!yh_f16 || yhs >= C), "sp_layernorm: C must be a multiple of 32, at most 256");
-    sp_layernorm_kernel<<<blocks(R, 8), 256, 0, as_stream(stream)>>>(x, t, R, C, g, b, eps, xo, yf, reinterpret_cast<__half*>(yh_f16), yhs);
+    R3DP_REQUIRE(R > 0 && C % 32 == 0 && C >= 32 && C <= 1024 && (!yh_f16 || yhs >= C), "sp_layernorm: C must be a multiple of 32, at most 1024");
+    if (C <= 256)
+        sp_layernorm_kernel<8><<<blocks(R, 8), 256, 0, as_stream(stream)>>>(x, t, R, C, g, b, eps, xo, yf, reinterpret_cast<__half*>(yh_f16), yhs);
+    else
+        sp_layernorm_kernel<32><<<blocks(R, 8), 256, 0, as_stream(stream)>>>(x, t, R, C, g, b, eps, xo, yf, reinterpret_cast<__half*>(yh_f16), yhs);
+    R3DP_LAUNCH_CHECK();
+    count_launches(1);
+    return 0;
+}
+
+extern "C" int r3dp_sp_patches_dil(const void* x_f16, int N, int H, int W, int C, int k, int s, int p, int d, void* y_f16, int ldy,
+                                   r3dp_stream_t stream) {
+    R3DP_REQUIRE(x_f16 && y_f16, "sp_patches: null pointer");
+    const int ke = d * (k - 1) + 1;                               // the dilated window's extent
+    R3DP_REQUIRE(N > 0 && H > 0 && W > 0 && C % 8 == 0 && C > 0 && k > 0 && s > 0 && p >= 0 && d > 0 && H + 2 * p >= ke && W + 2 * p >= ke &&
+                 ldy >= k * k * C && ldy % 8 == 0, "sp_patches: bad shape");
+    const int Ho = (H + 2 * p - ke) / s + 1, Wo = (W + 2 * p - ke) / s + 1;
+    const long long n = (long long)N * Ho * Wo * (ldy / 8);
+    sp_patches_kernel<<<blocks(n, 256), 256, 0, as_stream(stream)>>>(reinterpret_cast<const __half*>(x_f16), N, H, W, C, k, s, p, d, Ho, Wo, ldy,
+                                                                     reinterpret_cast<__half*>(y_f16));
     R3DP_LAUNCH_CHECK();
     count_launches(1);
     return 0;
 }
 
 extern "C" int r3dp_sp_patches(const void* x_f16, int N, int H, int W, int C, int k, int s, int p, void* y_f16, r3dp_stream_t stream) {
-    R3DP_REQUIRE(x_f16 && y_f16, "sp_patches: null pointer");
-    R3DP_REQUIRE(N > 0 && H > 0 && W > 0 && C % 8 == 0 && k > 0 && s > 0 && p >= 0 && H + 2 * p >= k && W + 2 * p >= k, "sp_patches: bad shape");
-    const int Ho = (H + 2 * p - k) / s + 1, Wo = (W + 2 * p - k) / s + 1;
-    const long long n = (long long)N * Ho * Wo * k * k * (C / 8);
-    sp_patches_kernel<<<blocks(n, 256), 256, 0, as_stream(stream)>>>(reinterpret_cast<const __half*>(x_f16), N, H, W, C, k, s, p, Ho, Wo,
-                                                                     reinterpret_cast<__half*>(y_f16));
-    R3DP_LAUNCH_CHECK();
-    count_launches(1);
-    return 0;
+    return r3dp_sp_patches_dil(x_f16, N, H, W, C, k, s, p, 1, y_f16, k * k * C, stream);
 }
 
 extern "C" int r3dp_sp_attention(const void* q_f16, int qs, const void* kv_f16, int kvs, int N, int Tq, int Tk, int heads, float scale, void* o_f16,

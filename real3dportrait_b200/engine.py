@@ -137,13 +137,16 @@ class FrameEngine:
     blink (with secc_renderer): the engine also closes the eyes of each driving image as real3d_infer.py's default blink_mode='period' does
     (blink_eye_for_secc): coefficient rows become [B, n_id + n_exp + 2] = [id | exp | t | T] (fp32; period_blink_schedule gives (t, T), T = 0
     leaves a frame untouched) and the edit runs in place between the render and the backbone, inside the step's graph.  blink_faults() counts
-    the frames on which the reference would raise (left unedited).  begin_planes() is unchanged: the reference blinks only the driving images."""
+    the frames on which the reference would raise (left unedited).  begin_planes() is unchanged: the reference blinks only the driving images.
+    img2plane (with secc2plane): an Img2PlaneModel; begin_planes(img=ref_head_img [1,3,512,512], ...) then makes the clip's canonical planes
+    from the source image (cal_cano_plane, secc_img2plane.py:50-62) straight into the engine's canonical buffer, once per clip and outside
+    the step's graph, in place of begin_planes(cano_planes, ...)."""
 
     def __init__(self, batch: int = 4, sr_mode: str = 'fp32', device=None, world: int = 1, rank: int = 0, dist=None, hp: Optional[dict] = None,
                  static_styles: bool = True, use_graph: bool = True, out_uint8: bool = False, exchange: str = 'allgather',
                  torso_model: Optional[torch.nn.Module] = None, warper_in_graph: bool = False, torso_stage2: str = 'torch',
                  torso_motion: str = 'torch', secc2plane: Optional[torch.nn.Module] = None, secc_renderer: Optional[torch.nn.Module] = None,
-                 blink: bool = False):
+                 blink: bool = False, img2plane: Optional[torch.nn.Module] = None):
         assert exchange in ('allgather', 'p2p', 'none')
         if secc2plane is not None and (hp or {}).get('phase1_plane_fusion_mode', 'add') != 'add':
             raise NotImplementedError('secc2plane: only phase1_plane_fusion_mode="add" (cano + secc, secc_img2plane.py:76-77) is built')
@@ -168,6 +171,9 @@ class FrameEngine:
         if blink and self.secc_r is None:
             raise ValueError('blink edits the images the SECC renderer draws: FrameEngine(secc2plane=..., secc_renderer=..., blink=True)')
         self.blink = bool(blink)
+        if img2plane is not None and secc2plane is None:
+            raise ValueError('img2plane makes the canonical planes of a secc2plane clip: FrameEngine(secc2plane=..., img2plane=...)')
+        self.img2p = img2plane.to(self.device).eval() if img2plane is not None else None
         self.out_uint8 = bool(out_uint8)
         if self.out_uint8 and self.head.superresolution.sr_mode not in ('tc', 'tc_exact'):     # the head's effective mode: a torso head maps 'fp32' to 'tc'
             raise NotImplementedError('uint8 frames are written by the tensor-core SR epilogue (sr_mode="tc")')
@@ -231,14 +237,22 @@ class FrameEngine:
         self._consts.update({'ref_torso_img': ref_torso_img, 'bg_img': bg_img})
 
     @torch.no_grad()
-    def begin_planes(self, cano_planes: torch.Tensor, cond_cano: Optional[torch.Tensor] = None, cond_src: Optional[torch.Tensor] = None, *,
-                     coeff_src: Optional[torch.Tensor] = None) -> None:
+    def begin_planes(self, cano_planes: Optional[torch.Tensor] = None, cond_cano: Optional[torch.Tensor] = None,
+                     cond_src: Optional[torch.Tensor] = None, *, coeff_src: Optional[torch.Tensor] = None,
+                     img: Optional[torch.Tensor] = None) -> None:
         """secc2plane engines: the clip's canonical planes [1,3,32,256,256] and the backbone's per-clip SECC images [1,3,H,W] (cond_src only in
         'cano_src_tgt').  With a secc_renderer the images come from the source frame's coefficients coeff_src [1,144] = [id | exp] instead:
-        cond_src = r(id, exp), cond_cano = r(id, 0 exp), zero pose (real3d_infer.py:404-405).  A later begin_planes() refills the same buffers in
-        place, so graphs captured for an earlier clip render the new one."""
+        cond_src = r(id, exp), cond_cano = r(id, 0 exp), zero pose (real3d_infer.py:404-405).  With FrameEngine(img2plane=...), img = the
+        source head image [1,3,512,512] in place of cano_planes: the backbone writes the canonical planes straight into the engine's buffer.
+        A later begin_planes() refills the same buffers in place, so graphs captured for an earlier clip render the new one."""
         if self.secc is None:
             raise ValueError('begin_planes() needs FrameEngine(secc2plane=...)')
+        if (cano_planes is None) == (img is None):
+            raise ValueError('begin_planes: pass exactly one of cano_planes and img (the source image, with FrameEngine(img2plane=...))')
+        if img is not None and self.img2p is None:
+            raise ValueError('begin_planes(img=...) needs FrameEngine(secc2plane=..., img2plane=Img2PlaneModel)')
+        if img is not None and (img.ndim != 4 or img.shape[0] != 1):
+            raise ValueError(f'begin_planes: img must be one source image [1,3,H,W], got {tuple(img.shape)}')
         if self.secc_r is not None:
             if coeff_src is None or cond_cano is not None or cond_src is not None:
                 raise ValueError('secc_renderer engine: begin_planes(cano_planes, coeff_src=c [1,144]) (the engine renders cond_cano / cond_src)')
@@ -253,13 +267,23 @@ class FrameEngine:
             raise ValueError('coeff_src needs FrameEngine(secc_renderer=...)')
         elif cond_cano is None:
             raise ValueError('begin_planes(cano_planes, cond_cano, cond_src)')
-        from .secc2plane import canonical_planes_cl
-        cl = canonical_planes_cl(cano_planes.to(self.device))
-        if self._cano_cl is not None and self._cano_cl.data.shape == cl.data.shape:
-            self._cano_cl.data.copy_(cl.data)
+        if img is not None:
+            img = img.to(self.device)
+            H2 = img.shape[-1] // 2
+            old = self._cano_cl
+            keep = old is not None and tuple(old.data.shape) == (1, H2, H2, 3, 32)
+            cl = self.img2p.planes_cl(img, out=old.data if keep else None)
+            if not keep:
+                self._cano_cl = cl
+                self.graph, self.inplace = None, {}
         else:
-            self._cano_cl = cl
-            self.graph, self.inplace = None, {}
+            from .secc2plane import canonical_planes_cl
+            cl = canonical_planes_cl(cano_planes.to(self.device))
+            if self._cano_cl is not None and self._cano_cl.data.shape == cl.data.shape:
+                self._cano_cl.data.copy_(cl.data)
+            else:
+                self._cano_cl = cl
+                self.graph, self.inplace = None, {}
         self.secc.begin_clip(cond_cano.to(self.device), None if cond_src is None else cond_src.to(self.device))
 
     def _planes(self, planes):
