@@ -373,8 +373,9 @@ int r3dp_tw_hid_to_nchw(const void* x_f16, int N, int C, int H, int W, int cs, i
  * r3dp_mf_conv3d       3-D conv on wgmma (stride 1, zero padding): box taps kd x kh x kw (odd) centred, or with up != 0 the 4 output-parity
  *                      phases of nn.Upsample((1,2,2), nearest) + 3x3x3 conv as kd x 2 x 2 taps on the low-resolution input (layers.py:77-93).
  *                      M space = the input grid N x D x H x W; x channels [0, cin) (cin % 32 == 0); wp [nph][taps][cop][cin (x2 split)] fp16,
- *                      bias [cop]; y = relu? (conv + bias) (+ res, same layout as y) stored at channels [yc0, yc0 + cout) of voxels of ys
- *                      halves (up: output grid D x 2H x 2W), fp16 or fp32 (out_f32, no residual)
+ *                      bias [cop]; y = act(conv + bias) (+ res, same layout as y) stored at channels [yc0, yc0 + cout) of voxels of ys
+ *                      halves (up: output grid D x 2H x 2W), fp16 or fp32 (out_f32, no residual); act (the `relu` argument): 0 none,
+ *                      1 ReLU, 2 exact GELU (nn.GELU(), erf form)
  * r3dp_mf_input        create_heatmap_representations + create_sparse_motions + create_deformed_source_image (func_utils.py:130-191, Rs = Rd = I):
  *                      fc [N or 1,D,H,W,4] fp32 (the compressed source), kp_s / kp_d [N,K,3] -> channel k*5 + j of y, zeros up to cpad
  * r3dp_mf_pool         AvgPool3d((1,2,2)) (layers.py:58-74); H, W: the pooled size
@@ -494,6 +495,32 @@ int r3dp_secc_resolve(const float* verts, int N, const int* faces, const float* 
 size_t r3dp_secc_blink_scratch_bytes(int B, int S);
 int r3dp_secc_blink(float* secc, int B, int S, const double* p, const float* rows, int row_stride, void* scratch, int* faults,
                     r3dp_stream_t stream);
+
+/* ------------------------------------------------ audio2motion: the audio2secc VAE (modules/audio2motion/vae.py, inference path) ---
+ * PitchContourVAEModel / VAEModel: audio features and f0 -> expression coefficients.  Activations are channels-last rows per frame; split fp16
+ * rows hold [hi | lo] of each value, weights [hi | lo] of w * 2^10 (as r3dp_mf_conv3d with split).  The convolutions and GEMMs around the
+ * WaveNets run on r3dp_mf_conv3d (1-D as D = H = 1, W = T).
+ * r3dp_a2m_wn_layer  one WaveNet layer (flow_base.py:70-96) fused, (hidden, k) = (64, 3) or (256, 5), dilation 1, x_mask = 1: x [B,T,hidden]
+ *                    fp32 -> x_out = x + res_skip[:hidden] (not last; a buffer other than x), skip [B,T,hidden] fp32 (+)= res_skip[hidden:]
+ *                    (first: =), last: out [B,T, hi hidden | lo hidden] split fp16 = skip + res_skip.  cond: per-frame rows of cs floats,
+ *                    this layer's cond_layer output with the in_layer bias added, rows interleaved (2c: tanh half, 2c + 1: sigmoid half of
+ *                    channel c).  w: the packed steps of the in_layer and res_skip weights (audio2motion.py, pack_wn_layer); bias: res_skip's.
+ * r3dp_a2m_input     audio [B,Tx,A] fp32 downsampled x0.5 (mean = 0: frame 2i, nearest; 1: the mean of frames 2i, 2i+1, linear) into split
+ *                    rows of y (ys halves, lo at ylo): channels [0, A) the features, [A, Ap) zero; with pitch_table [300,128] fp32 also
+ *                    [Ap, Ap+128) pitch_table[f0_to_coarse(f0[2i])] (mel_min, mel_span: pitch_utils' f0_mel_min, f0_mel_max - f0_mel_min)
+ *                    and the 32 split channels of yb (ybs halves, lo at yblo): blink[2i] == 0, blink[2i] == 1 (int64 [B,Tx], NULL = 0),
+ *                    mouth_amp[b], eye_amp[b] (NULL = 0), zeros
+ * r3dp_a2m_split     x [R,C] fp32 -> y1 split rows [R, hi C | lo C] and / or y4 split rows per group of four [R/4, hi 4C | lo 4C]
+ * r3dp_a2m_latent    z [B,16,T4] fp32 x temperature -> split rows [B*T4, hi 32 | lo 32] (channels 16..31 zero)
+ * r3dp_a2m_store     x [N,C] fp32 x mask[n] (NULL = 1) -> out[n * ld + c] */
+int r3dp_a2m_wn_layer(const float* x, float* x_out, const float* cond, int cs, const void* w_f16, const float* bias, float* skip, void* out_f16,
+                      int B, int T, int hidden, int k, int first, int last, r3dp_stream_t stream);
+int r3dp_a2m_input(const float* audio, int B, int Tx, int A, int Ap, int mean, const float* f0, const long long* blink, const float* mouth_amp,
+                   const float* eye_amp, const float* pitch_table, float mel_min, float mel_span, void* y_f16, int ys, int ylo, void* yb_f16, int ybs,
+                   int yblo, r3dp_stream_t stream);
+int r3dp_a2m_split(const float* x, long long R, int C, void* y1_f16, void* y4_f16, r3dp_stream_t stream);
+int r3dp_a2m_latent(const float* z, int B, int T4, float temperature, void* y_f16, r3dp_stream_t stream);
+int r3dp_a2m_store(const float* x, const float* mask, long long N, int C, float* out, long long ld, r3dp_stream_t stream);
 
 #ifdef __cplusplus
 }

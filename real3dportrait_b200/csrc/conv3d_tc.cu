@@ -36,7 +36,7 @@ struct Conv3dArgs {
     int kd, kh, kw, oz, oy, ox;          // taps dz in [-oz, kd - oz) etc.; phase (p, q) shifts the origin to oy - p, ox - q
     int sy, sx;                          // output voxel (d, h * sy + p, w * sx + q) of a grid D x H*sy x W*sx
     int ys, yc0, ylo, cout, cop;
-    int relu, out_f32;
+    int relu, out_f32;                   // relu: 0 none, 1 ReLU, 2 exact GELU
     float acc_scale;
 };
 
@@ -186,7 +186,8 @@ __global__ void __launch_bounds__(kThreads) conv3d_tc_kernel(const Conv3dArgs a)
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
             float u = SPLIT ? __fmaf_rn(acc[i + e], a.acc_scale, a.bias[col + (two ? e : 0)]) : __fadd_rn(acc[i + e], a.bias[col + (two ? e : 0)]);
-            if (a.relu) u = fmaxf(u, 0.f);
+            if (a.relu == 1) u = fmaxf(u, 0.f);
+            else if (a.relu == 2) u = 0.5f * u * (1.f + erff(u * 0.70710678118654752f));   // nn.GELU() (exact erf form)
             v[e] = u;
         }
         if (a.res) {
