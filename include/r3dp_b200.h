@@ -522,6 +522,36 @@ int r3dp_a2m_split(const float* x, long long R, int C, void* y1_f16, void* y4_f1
 int r3dp_a2m_latent(const float* z, int B, int T4, float temperature, void* y_f16, r3dp_stream_t stream);
 int r3dp_a2m_store(const float* x, const float* mask, long long N, int C, float* out, long long ld, r3dp_stream_t stream);
 
+/* ------------------------------------------------ audio features: HuBERT (transformers' HubertModel, hubert-large architecture) ---
+ * Split fp16 rows hold [hi | lo] of each value; weights are [N][hi Kp | lo Kp] of w * 2^10.  Every GEMM operand is split (three MMAs, fp32
+ * accumulation).
+ * r3dp_hb_gemm       y = A W^T + bias on wgmma (TMA producer warp, two consumer warpgroups, n128 tiles, 64-channel K steps).  A: M rows of
+ *                    a_width halves, a_stride halves apart (a_stride < a_width reads overlapping windows: a strided conv's A row t is the k
+ *                    frames from frame s t, a_stride = s * 2 seg); K channel kk sits at column (kk / seg) * 2 seg + kk % seg (hi), + seg (lo).
+ *                    w [N][hi Kp | lo Kp].  epi 0: split rows into y (fp16, ldy halves, lo at ylo); 1: GELU, then as 0; 2: y fp32 (ldy floats)
+ *                    += result; 3: y fp32 = result.  bias may be NULL.  Any M >= 1, N even; Kp and seg multiples of 64
+ * r3dp_hb_pos_conv   the positional conv (k128, pad 64, last frame dropped, groups of 64 channels) on each of nseg segments of Lseg frames
+ *                    with its own zero padding: y fp32 [M][H] += GELU(conv(x) + bias).  x: split rows [nseg * Lseg][hi H | lo H], rows >= M
+ *                    zero; w [H][hi 8192 | lo 8192], K channel 64 j + i = tap j, input channel i of the output's group
+ * r3dp_hb_attention  softmax(q k^T) v per head (head_dim 64; scale folded into q) within each of nseg consecutive segments of seg_len[i]
+ *                    rows (<= 64 segments, lengths >= 1): qkv split rows [rows][ld], q / k / v of head h at columns 64 h, H + 64 h,
+ *                    2H + 64 h (hi) and lo + those (lo), H = 64 heads.  o: split rows (os halves), hi at 64 h, lo at olo + 64 h
+ * r3dp_hb_stats      stats = (mean, 1 / sqrt(var + 1e-7)) of x[0, L) in fp64 (Wav2Vec2FeatureExtractor's normalisation), deterministic
+ * r3dp_hb_conv0      feature extractor layer 0 on F frames: ((x - mean) * rstd) conv w [C][10] (stride 5) + bias (may be NULL), LayerNorm
+ *                    (g, b, eps), GELU -> split rows y (ys halves, lo at ylo); C a multiple of 32, at most 512
+ * r3dp_hb_layernorm  LayerNorm of x [R][C] fp32 (C <= 1024), * g + b if given, GELU if gelu; yf fp32 rows (yfs floats) and / or split rows
+ *                    yh (yhs halves, lo at yhlo) */
+int r3dp_hb_gemm(const void* a_f16, int M, int a_width, int a_stride, int seg, const void* w_f16, int N, int Kp, const float* bias, int epi,
+                 void* y, int ldy, int ylo, r3dp_stream_t stream);
+int r3dp_hb_pos_conv(const void* x_f16, int nseg, int Lseg, int M, int H, const void* w_f16, const float* bias, float* y, r3dp_stream_t stream);
+int r3dp_hb_attention(const void* qkv_f16, int rows, int ld, int lo, int heads, const int* seg_len, int nseg, void* o_f16, int os, int olo,
+                      r3dp_stream_t stream);
+int r3dp_hb_stats(const float* x, long long L, double* stats, r3dp_stream_t stream);
+int r3dp_hb_conv0(const float* x, const double* stats, int F, int C, const float* w, const float* bias, const float* g, const float* b,
+                  float eps, void* y_f16, int ys, int ylo, r3dp_stream_t stream);
+int r3dp_hb_layernorm(const float* x, int R, int C, const float* g, const float* b, float eps, int gelu, float* yf, int yfs, void* yh_f16,
+                      int yhs, int yhlo, r3dp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -151,6 +151,12 @@ _SIGNATURES = {
     'r3dp_a2m_split': (_I, [_P, C.c_longlong, _I, _P, _P, _P]),
     'r3dp_a2m_latent': (_I, [_P, _I, _I, _F, _P, _P]),
     'r3dp_a2m_store': (_I, [_P, _P, C.c_longlong, _I, _P, C.c_longlong, _P]),
+    'r3dp_hb_gemm': (_I, [_P, _I, _I, _I, _I, _P, _I, _I, _P, _I, _P, _I, _I, _P]),
+    'r3dp_hb_pos_conv': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P]),
+    'r3dp_hb_attention': (_I, [_P, _I, _I, _I, _I, C.POINTER(_I), _I, _P, _I, _I, _P]),
+    'r3dp_hb_stats': (_I, [_P, C.c_longlong, _P, _P]),
+    'r3dp_hb_conv0': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _F, _P, _I, _I, _P]),
+    'r3dp_hb_layernorm': (_I, [_P, _I, _I, _P, _P, _F, _I, _P, _I, _P, _I, _I, _P]),
 }
 
 

@@ -16,7 +16,6 @@
 #include "tc_prims.cuh"
 #include <cuda_fp16.h>
 #include <math.h>
-#include <mutex>
 
 namespace r3dp {
 namespace ip {
@@ -32,32 +31,6 @@ constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 constexpr int kTile = kBKV * kHd * 2;      // one 64 x 256 fp16 tile: 4 column blocks of 64 rows x 128 B (SWIZZLE_128B atoms)
 constexpr int kBlk = 64 * 128;             // one column block
 constexpr int kFaSmem = 2 * kTile + 2 * kSlots * kTile + 1024 + 64;
-
-// D[64 x 64] += A[64 x 16] (registers, the accumulator layout of S rounded to fp16) * B, B from an MN-major (transposed) SWIZZLE_128B tile:
-// V rows (keys) of 128 B hold 64 head dims, 8-key groups 1024 B apart.
-__device__ __forceinline__ void wgmma_rs_m64n64k16_tb(float* d, const uint32_t* a, uint64_t desc_b) {
-    asm volatile(
-        "{\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
-        "{%32,%33,%34,%35}, %36, 1, 1, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b));
-}
-// SWIZZLE_128B descriptor with both byte offsets 1024: the 8-row group stride of a K-major tile, and of an MN-major tile one atom (64
-// elements) wide, whichever of the two fields the MN-major form reads it from.
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3ffff) >> 4);
-    d |= (uint64_t)(1024 >> 4) << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 62;
-    return d;
-}
-__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
 
 // grid (ceil(Tq / 128), heads, N).  Tensor maps: q [N][Tq][qs] and kv [N][Tk][kvs] fp16, boxes of 64 channels x 64 rows, zero fill past Tq / Tk.
 __global__ void __launch_bounds__(kFaThreads, 1) ip_flash_attention_kernel(const __grid_constant__ CUtensorMap tmQ,
@@ -327,21 +300,6 @@ __global__ void ip_flip_hwpc_kernel(const float* __restrict__ x, int N, int H, i
 inline unsigned blocks(long long n, int t) { return (unsigned)((n + t - 1) / t); }
 
 // ---- host side: tensor maps ----------------------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    });
-    return fn;
-}
-
 // fp16 rows [N][T][stride] read in 64-channel x 64-row boxes (128-byte swizzle), zero fill past T
 static int token_map(CUtensorMap* m, const void* ptr, int N, int T, int stride) {
     EncodeTiledFn fn = encode_fn();

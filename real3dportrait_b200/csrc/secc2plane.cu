@@ -1,7 +1,7 @@
 // SegFormerSECC2PlaneBackbone (modules/real3d/segformer.py:673-733, MiT-b0) on sm_90a: the kernels around the token GEMMs.
 //   sp_prenet_kernel        the prenet's 1x1 conv (Conv2dLayer, networks_stylegan2.py:139-183) on the per-clip channels: the constant image
 //   sp_embed_kernel         prenet (constant image + tgt part, or the whole input) fused with patch_embed1's 7x7 stride-4 conv (segformer.py:206-232)
-//   sp_layernorm_kernel     optional residual add, then LayerNorm of each C <= 1024 row in fp32 (one warp per row)
+//   layernorm_rows_kernel   (layernorm.cuh) optional residual add, then LayerNorm of each C <= 1024 row in fp32 (one warp per row)
 //   sp_patches_kernel       k x k stride-s dilation-d patches of an NHWC fp16 image as GEMM rows: the 3x3/2 patch embeds of stages 2-4 and
 //                           the spatial-reduction conv (k = stride = sr_ratio, segformer.py:126-128); Img2PlaneModel's strided and dilated convs
 //   sp_attention_kernel     softmax(q k^T * scale) v for head_dim 32 and <= 256 keys (segformer.py:130-150), exact fp32 softmax
@@ -13,6 +13,7 @@
 // The GEMMs themselves (q, kv, proj, fc1, fc2, patch embeds 2-4, sr, G_i, the last conv) run on r3dp_mf_conv3d; to_plane_cnn.0/2/4 on
 // r3dp_sr_tc_conv.  Activations fp16, residual stream / LayerNorm / softmax / GELU in fp32.
 #include "common.cuh"
+#include "layernorm.cuh"
 #include <cuda_fp16.h>
 #include <math.h>
 
@@ -80,47 +81,6 @@ __global__ void __launch_bounds__(128) sp_embed_kernel(const float* __restrict__
     float4* out = reinterpret_cast<float4*>(y + idx * kEmbedC);
 #pragma unroll
     for (int i = 0; i < kEmbedC / 4; ++i) out[i] = make_float4(acc[4 * i], acc[4 * i + 1], acc[4 * i + 2], acc[4 * i + 3]);
-}
-
-// One warp per row; lane holds channels lane + 32 i, i < NV (8: C <= 256, 32: C <= 1024).  Two-pass statistics in fp32 (nn.LayerNorm:
-// biased variance).
-template <int NV>
-__global__ void __launch_bounds__(256) sp_layernorm_kernel(const float* x, const float* __restrict__ t, int R, int C, const float* __restrict__ g,
-                                                           const float* __restrict__ b, float eps, float* xo, float* __restrict__ yf,
-                                                           __half* __restrict__ yh, int yhs) {
-    const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (row >= R) return;
-    const int nv = C / 32;
-    float v[NV];
-    float s = 0.f;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-        if (i < nv) {
-            const size_t o = (size_t)row * C + lane + 32 * i;
-            v[i] = x[o] + (t ? t[o] : 0.f);
-            s += v[i];
-        }
-    }
-#pragma unroll
-    for (int m = 16; m; m >>= 1) s += __shfl_xor_sync(0xffffffffu, s, m);
-    const float mean = s / C;
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < NV; ++i)
-        if (i < nv) { const float d = v[i] - mean; q = fmaf(d, d, q); }
-#pragma unroll
-    for (int m = 16; m; m >>= 1) q += __shfl_xor_sync(0xffffffffu, q, m);
-    const float rstd = rsqrtf(q / C + eps);
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-        if (i >= nv) break;
-        const int c = lane + 32 * i;
-        const size_t o = (size_t)row * C + c;
-        if (xo) xo[o] = v[i];
-        const float u = fmaf((v[i] - mean) * rstd, g[c], b[c]);
-        if (yf) yf[o] = u;
-        if (yh) yh[(size_t)row * yhs + c] = __float2half_rn(u);
-    }
 }
 
 // y[(n, oy, ox)][(ky*k + kx)*C + c] = x[n, oy*s - p + ky*d, ox*s - p + kx*d, c] (0 outside), rows of ldy halves with columns from k*k*C
@@ -343,9 +303,9 @@ extern "C" int r3dp_sp_layernorm(const float* x, const float* t, int R, int C, c
     R3DP_REQUIRE(x && g && b && (xo || yf || yh_f16), "sp_layernorm: null pointer");
     R3DP_REQUIRE(R > 0 && C % 32 == 0 && C >= 32 && C <= 1024 && (!yh_f16 || yhs >= C), "sp_layernorm: C must be a multiple of 32, at most 1024");
     if (C <= 256)
-        sp_layernorm_kernel<8><<<blocks(R, 8), 256, 0, as_stream(stream)>>>(x, t, R, C, g, b, eps, xo, yf, reinterpret_cast<__half*>(yh_f16), yhs);
+        layernorm_rows_kernel<8><<<blocks(R, 8), 256, 0, as_stream(stream)>>>(x, t, R, C, g, b, eps, xo, yf, C, reinterpret_cast<__half*>(yh_f16), yhs, 0, 0);
     else
-        sp_layernorm_kernel<32><<<blocks(R, 8), 256, 0, as_stream(stream)>>>(x, t, R, C, g, b, eps, xo, yf, reinterpret_cast<__half*>(yh_f16), yhs);
+        layernorm_rows_kernel<32><<<blocks(R, 8), 256, 0, as_stream(stream)>>>(x, t, R, C, g, b, eps, xo, yf, C, reinterpret_cast<__half*>(yh_f16), yhs, 0, 0);
     R3DP_LAUNCH_CHECK();
     count_launches(1);
     return 0;

@@ -814,21 +814,6 @@ __global__ void __launch_bounds__(256) torgb_f16_kernel(const __half* __restrict
 }
 
 // ---- host side: tensor maps -----------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    });
-    return fn;
-}
-
 // fp16 tensor [d3][d2][d1][d0] (d0 innermost, dense) read in boxes of box[0..3] elements, zero fill outside
 static int make_map(CUtensorMap* m, const void* ptr, const cuuint64_t (&dims)[4], const cuuint32_t (&box)[4], CUtensorMapSwizzle swizzle,
                     CUtensorMapL2promotion l2) {
