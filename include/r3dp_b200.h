@@ -468,10 +468,11 @@ int r3dp_ip_flip_hwpc(const float* x, int N, int H, int W, float* out, r3dp_stre
  * The 3DMM face mesh rasterised at S x S with pytorch3d's rules (blur 0, one face per pixel, perspective-correct barycentrics, no culling
  * or clipping; DESIGN.md) and shaded with the per-vertex NCC code.  All fp32.
  * r3dp_secc_vertices  basis [3N, n_id + n_exp] (row 3v + axis, id columns then exp columns, 16-byte aligned), mean [3N] (recentred),
- *                     id [B, >= n_id] (row stride ids), exp [B, >= n_exp] (row stride exps), euler, trans [B,3] (NULL = zero)
+ *                     id [B, >= n_id] (row stride ids), exp [B, >= n_exp] (row stride exps; a stride of 0 reads row 0 for every frame),
+ *                     euler, trans [B,3] (NULL = zero)
  *                     -> verts [B,N,4] = (x_ndc, y_ndc, z_view, 0): s = basis . [id|exp] + mean, v = Rz Ry Rx s + t (bfm.py:204-238,260-270),
  *                     z = cam_dist - v_z, x_ndc = -v_x / (z tan_half), y_ndc = v_y / (z tan_half).  n_id + n_exp <= 256, a multiple of 4.
- *                     Each basis row is read once per call for all B frames.
+ *                     Each basis row is read once per chunk of frames: one chunk when N fills the GPU, more for small N.
  * r3dp_secc_raster    verts [B,N,4], faces int32 [F,3] (0-based) -> keys [B,S,S] uint64: atomicMin of (bits of pz) << 32 | face over every
  *                     covered pixel centre (nearest pz, ties to the lower face).  keys must hold ~0 (empty) on entry.
  * r3dp_secc_resolve   keys -> secc [B,3,S,S] = 2 mask sum_i w_i ncc[v_i] - 1 (-1 where empty) and mask [B,1,S,S] (may be NULL); ncc [N,4]
@@ -495,6 +496,22 @@ int r3dp_secc_resolve(const float* verts, int N, const int* faces, const float* 
 size_t r3dp_secc_blink_scratch_bytes(int B, int S);
 int r3dp_secc_blink(float* secc, int B, int S, const double* p, const float* rows, int row_stride, void* scratch, int* faults,
                     r3dp_stream_t stream);
+
+/* ------------------------------------------------ clip motion: cameras and torso key points (real3d_infer.py:271-321, 428-452) ---
+ * r3dp_motion_camera     per frame i < T: the pose (fp32, as the reference): driving row mirror_index(i, P) of drv_euler / drv_trans [P,3]
+ *                        (pass the source pose with P = 1 for the 'static' pose), z translation of frame 0, + (src - pose[0]) when
+ *                        map_to_init_pose -> euler, trans [T,3]; and cameras [T,25] = row-major c2w (16) and intrinsics (9) of
+ *                        get_eg3d_convention_camera_pose_intrinsic, smoothed by smooth_camera_sequence over the truncated 7-frame window
+ *                        (translation mean; rotation mean = top eigenvector of sum q q^T, in double).
+ * r3dp_motion_keypoints  verts_s [K,4] / verts_d [T,K,4] (r3dp_secc_vertices at the key points, 16-byte aligned) -> kp_s [K,3] =
+ *                        (clamp(-x_ndc), clamp(-y_ndc), 0) (clamp to [-1, 1]), kp_d [T,K,3] = the same smoothed by smooth_features_xd
+ *                        (7-tap box filter over frames, the first and last three mirrored); T >= 3.
+ * r3dp_motion_lm2d       verts [n,4] -> lm2d [n,2] = (1 - x_ndc, 1 - y_ndc) / 2 (Face3DHelper.reconstruct_lm2d's coordinates).
+ * No host synchronisation and no allocation: capturable in a CUDA graph. */
+int r3dp_motion_camera(const float* src_euler, const float* src_trans, const float* drv_euler, const float* drv_trans, int P, int T,
+                       int map_to_init_pose, float* euler, float* trans, float* cameras, r3dp_stream_t stream);
+int r3dp_motion_keypoints(const float* verts_s, const float* verts_d, int T, int K, float* kp_s, float* kp_d, r3dp_stream_t stream);
+int r3dp_motion_lm2d(const float* verts, long long n, float* lm2d, r3dp_stream_t stream);
 
 /* ------------------------------------------------ audio2motion: the audio2secc VAE (modules/audio2motion/vae.py, inference path) ---
  * PitchContourVAEModel / VAEModel: audio features and f0 -> expression coefficients.  Activations are channels-last rows per frame; split fp16

@@ -1,8 +1,10 @@
 // SECC_Renderer (deep_3drecon/secc_renderer.py) on sm_90a: the BFM face mesh from 3DMM coefficients, rasterised and shaded with the NCC code.
 //   secc_vertices_kernel   shape = basis . [id | exp] + mean (bfm.py:102-115), pose v = R s + t (bfm.py:204-238, 260-270), to_camera z = 10 - z,
 //                          the renderer's x negation (mesh_renderer.py:69-71), FoV projection -> (x_ndc, y_ndc, z_view, 0) per vertex.
-//                          One warp per vertex holds its three basis rows in registers and loops over every frame of the call: the basis
-//                          (61.7 MB for the BFM) is read from memory once per call whatever the batch.
+//                          One warp per vertex holds its three basis rows in registers and loops over the frames of its block's frame
+//                          chunk (blockIdx.y): the basis (61.7 MB for the BFM) is read from memory once per chunk.  A mesh with enough vertices
+//                          to fill the GPU runs one chunk of every frame; a small one (the 68 key points of motion.py) splits the frames into
+//                          chunks of whole 32-frame tiles, which computes every frame exactly as one chunk does.
 //   secc_raster_kernel     one thread per (frame, face): pytorch3d's per-face culls, then every pixel centre of the face's bounding box; a covered
 //                          centre does a 64-bit atomicMin of (bits of pz) << 32 | face into the frame's key buffer: nearest pz, ties to the lower face.
 //   secc_resolve_kernel    one thread per pixel: decodes the key, recomputes the winner's corrected barycentrics, interpolates the NCC code
@@ -27,8 +29,8 @@ inline unsigned blocks(long long n, int t) { return (unsigned)((n + t - 1) / t);
 __global__ void __launch_bounds__(kVertWarps * 32) secc_vertices_kernel(const float* __restrict__ basis, const float* __restrict__ mean, int N,
                                                                         int n_id, int n_exp, const float* __restrict__ id, int ids,
                                                                         const float* __restrict__ exp, int exps, const float* __restrict__ euler,
-                                                                        const float* __restrict__ trans, int B, float cam_dist, float tan_half,
-                                                                        float4* __restrict__ verts) {
+                                                                        const float* __restrict__ trans, int B, int chunk, float cam_dist,
+                                                                        float tan_half, float4* __restrict__ verts) {
     __shared__ __align__(16) float s_coef[kFrameTile * kMaxK];
     __shared__ float s_pose[kFrameTile * 12];                      // R row-major (9), t (3)
     const int K = n_id + n_exp, K4 = K / 4;
@@ -45,6 +47,15 @@ __global__ void __launch_bounds__(kVertWarps * 32) secc_vertices_kernel(const fl
     float m0 = 0.f, m1 = 0.f, m2 = 0.f;
     if (live) {
         m0 = mean[3 * v]; m1 = mean[3 * v + 1]; m2 = mean[3 * v + 2];
+    }
+    {                                                              // this block's chunk of frames (chunk: a multiple of kFrameTile)
+        const int f0 = blockIdx.y * chunk;
+        B = min(chunk, B - f0);
+        id += (size_t)f0 * ids;
+        exp += (size_t)f0 * exps;
+        if (euler) euler += 3 * f0;
+        if (trans) trans += 3 * f0;
+        verts += (size_t)f0 * N;
     }
     for (int b0 = 0; b0 < B; b0 += kFrameTile) {
         const int nb = min(kFrameTile, B - b0);
@@ -216,11 +227,16 @@ extern "C" int r3dp_secc_vertices(const float* basis, const float* mean, int N, 
     R3DP_REQUIRE(basis && mean && id && exp && verts, "secc_vertices: null pointer");
     const int K = n_id + n_exp;
     R3DP_REQUIRE(N > 0 && B > 0 && n_id >= 0 && n_exp >= 0 && K > 0 && K % 4 == 0 && K <= kMaxK, "secc_vertices: bad shape (0 < id+exp <= %d, a multiple of 4)", kMaxK);
-    R3DP_REQUIRE(ids >= n_id && exps >= n_exp, "secc_vertices: bad row strides");
+    R3DP_REQUIRE((ids >= n_id || ids == 0) && (exps >= n_exp || exps == 0), "secc_vertices: bad row strides");
     R3DP_REQUIRE(((uintptr_t)basis & 15) == 0 && ((uintptr_t)verts & 15) == 0, "secc_vertices: basis and verts must be 16-byte aligned");
-    secc_vertices_kernel<<<blocks(N, kVertWarps), kVertWarps * 32, 0, as_stream(stream)>>>(basis, mean, N, n_id, n_exp, id, ids, exp, exps, euler,
-                                                                                           trans, B, cam_dist, tan_half,
-                                                                                           reinterpret_cast<float4*>(verts));
+    // fewer vertex blocks than two waves of the GPU: split the frames into chunks of whole tiles so the grid fills it
+    const unsigned vb = blocks(N, kVertWarps);
+    const int tiles = (B + kFrameTile - 1) / kFrameTile, want = 2 * sm_count();
+    const int split = (int)vb >= want ? 1 : min(tiles, (want + (int)vb - 1) / (int)vb);
+    const int chunk = (tiles + split - 1) / split * kFrameTile;
+    const dim3 grid(vb, (unsigned)((B + chunk - 1) / chunk));
+    secc_vertices_kernel<<<grid, kVertWarps * 32, 0, as_stream(stream)>>>(basis, mean, N, n_id, n_exp, id, ids, exp, exps, euler, trans, B, chunk,
+                                                                         cam_dist, tan_half, reinterpret_cast<float4*>(verts));
     R3DP_LAUNCH_CHECK();
     count_launches(1);
     return 0;

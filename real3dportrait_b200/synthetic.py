@@ -261,16 +261,43 @@ def make_bfm(seed: int = 0, rows: int = 150, cols: int = 238) -> Dict[str, 'np.n
             'right_eye': eyes[0].astype(np.int64), 'left_eye': eyes[1].astype(np.int64)}
 
 
-def write_bfm_folder(path: str, bfm: Optional[dict] = None, seed: int = 0) -> Dict[str, object]:
+def make_keypoints(bfm: dict, seed: int = 0, rows: int = 150, cols: int = 238) -> 'np.ndarray':
+    """68 landmark vertices of make_bfm's head as BFM_model_front.mat stores them: [68, 1] float64, 1-based.  The layout follows the 68-point
+    scheme (jaw 17, brows 10, nose 9, eyes 12, mouth 20) on the front of the head; the jaw reaches x = +-0.7 and the chin y = -0.75, so
+    translations of a few tenths push key points past +-1 in NDC.  Each target is jittered by a generator of its own (seed + 1000), not
+    make_bfm's: the bases and every output drawn from them stay as they are."""
+    import numpy as np
+    rng = np.random.default_rng(seed + 1000)
+    P = np.asarray(bfm['meanshape'], np.float64).reshape(-1, 3)
+    jaw = [(0.7 * np.sin(a), 0.15 - 0.9 * np.cos(a)) for a in np.linspace(-1.45, 1.45, 17)]
+    brows = [(sx * x, 0.3 + 0.04 * np.sin(np.pi * (x - 0.12) / 0.3)) for sx in (-1, 1) for x in np.linspace(0.12, 0.42, 5)]
+    nose = [(0.0, y) for y in np.linspace(0.12, -0.12, 4)] + [(x, -0.2) for x in np.linspace(-0.1, 0.1, 5)]
+    eyes = [(sx * (0.28 + 0.08 * np.cos(a)), 0.18 + 0.035 * np.sin(a)) for sx in (-1, 1) for a in np.linspace(0, 2 * np.pi, 7)[:-1]]
+    outer = [(0.2 * np.cos(a), -0.42 + 0.09 * np.sin(a)) for a in np.linspace(0, 2 * np.pi, 13)[:-1]]
+    inner = [(0.12 * np.cos(a), -0.42 + 0.04 * np.sin(a)) for a in np.linspace(0, 2 * np.pi, 9)[:-1]]
+    tgt = np.array(jaw + brows + nose + eyes + outer + inner) + rng.normal(scale=0.01, size=(68, 2))
+    front = np.nonzero(P[:, 2] > P[:, 2].mean())[0]
+    d = ((P[front, None, :2] - tgt[None]) ** 2).sum(-1)
+    v = front[np.argmin(d, 0)]
+    assert v.max() + 1 < P.shape[0]                                   # the reference reads vertex v + 1 (no - 1): it must exist
+    return (v + 1).astype(np.float64).reshape(68, 1)
+
+
+def write_bfm_folder(path: str, bfm: Optional[dict] = None, seed: int = 0, keypoints: bool = False) -> Dict[str, object]:
     """Write a BFM in the reference's file layout under `path` (BFM/BFM_model_front.mat with 1-based tri, ncc_code.npy [3,N],
-    bfm_{right,left}_eye_faces.npy 1-based) and return the SECC_Renderer keyword arguments that read it."""
+    bfm_{right,left}_eye_faces.npy 1-based) and return the SECC_Renderer keyword arguments that read it.  keypoints=True also writes the
+    68 key points (make_keypoints) and zero placeholders for the other keys Face3DHelper loads (meantex, texBase, point_buf)."""
     import numpy as np
     import os
     import scipy.io
     bfm = make_bfm(seed) if bfm is None else bfm
     os.makedirs(os.path.join(path, 'BFM'), exist_ok=True)
-    scipy.io.savemat(os.path.join(path, 'BFM', 'BFM_model_front.mat'),
-                     {k: bfm[k] for k in ('meanshape', 'idBase', 'exBase', 'tri')})
+    mat = {k: bfm[k] for k in ('meanshape', 'idBase', 'exBase', 'tri')}
+    if keypoints:
+        n = bfm['meanshape'].size // 3
+        mat.update({'keypoints': make_keypoints(bfm, seed), 'meantex': np.zeros((1, 3 * n)), 'texBase': np.zeros((3 * n, 1)),
+                    'point_buf': np.zeros((n, 8))})
+    scipy.io.savemat(os.path.join(path, 'BFM', 'BFM_model_front.mat'), mat)
     np.save(os.path.join(path, 'ncc_code.npy'), bfm['ncc'].astype(np.float32))
     eyes = (os.path.join(path, 'bfm_right_eye_faces.npy'), os.path.join(path, 'bfm_left_eye_faces.npy'))
     np.save(eyes[0], bfm['right_eye'])
