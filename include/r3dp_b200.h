@@ -569,6 +569,33 @@ int r3dp_hb_conv0(const float* x, const double* stats, int F, int C, const float
 int r3dp_hb_layernorm(const float* x, int R, int C, const float* g, const float* b, float eps, int gelu, float* yf, int yfs, void* yh_f16,
                       int yhs, int yhlo, r3dp_stream_t stream);
 
+/* ------------------------------------------------ source images: ref_head_img, ref_torso_img and bg_img (real3d_infer.py:243-260) ---
+ * img uint8 [H,W,3] RGB; seg [6,H,W] float32 (seg_u8 = 0) or uint8 (seg_u8 = 1) in _cal_seg_map's channel order (0 bg, 1 hair, 2 body skin,
+ * 3 face skin, 4 clothes, 5 others).  64 <= H, W <= 1024.  Float outputs are [3,H,W] planes of (u - 127.5) / 127.5 in float32.
+ * r3dp_src_inpaint      inpaint_torso_job up to the blur: img2 uint8 [H,W,3] = img with head pixels ((s1 + s3 + s5) != 0) zeroed, the torso
+ *                       (9 rows) and neck (53 rows, after the torso) darkened copies written, numpy's negative-row wrap; flags uint8 [H,W]:
+ *                       bit 0 kept in torso_img, bit 1 neck-inpainted.  tab_torso [9] / tab_neck [53]: numpy's 0.98 ** np.arange(L), float64
+ * r3dp_src_compose      cv2.GaussianBlur(img2, (5,5), 4) at the neck-inpainted pixels, zero outside the torso mask -> torso_f32 and / or
+ *                       torso_u8 [H,W,3]; head_f32 = img where s1 + s3 + s5 > 0.5, else 0 (each output may be NULL, not all)
+ * r3dp_src_bg_distance  extract_background's first pass over F selected frames (segs + f seg_stride elements): each pixel's max over frames of
+ *                       the squared distance to the frame's nearest non-bg (s0 == 0) pixel, maxd2 int32 [H,W], and the first frame
+ *                       attaining it, argmax int32 [H,W]; has_fg int32 [F] = 1 where the frame has a non-bg pixel.  g: int16 scratch
+ *                       [chunk,H,W] (frames are processed chunk at a time)
+ * r3dp_src_bg_fill      the second pass: every pixel takes the colour of frame argmax[q] at q = its nearest pixel with maxd2 > 100 (itself
+ *                       when maxd2 > 100; ties: smallest column, then smallest row) -> bg_u8 [H,W,3] and / or bg_f32.  frames: the selected
+ *                       frames, uint8 [H,W,3] each, frame_stride bytes apart; g: int16 scratch [H,W]; has_bc int32 = 1 + the raster index of
+ *                       the last pixel with maxd2 > 100 (0: none).  Pixel 0, when maxd2 > 100 there, takes the frame argmax has of that last
+ *                       pixel, as the reference's fancy-index assignment leaves it
+ * No host synchronisation and no allocation: capturable in a CUDA graph. */
+int r3dp_src_inpaint(const unsigned char* img, const void* seg, int seg_u8, int H, int W, const double* tab_torso, const double* tab_neck,
+                     unsigned char* img2, unsigned char* flags, r3dp_stream_t stream);
+int r3dp_src_compose(const unsigned char* img, const void* seg, int seg_u8, const unsigned char* img2, const unsigned char* flags, int H, int W,
+                     float* head_f32, float* torso_f32, unsigned char* torso_u8, r3dp_stream_t stream);
+int r3dp_src_bg_distance(const void* segs, int seg_u8, long long seg_stride, int F, int H, int W, short* g, int chunk, int* maxd2, int* argmax,
+                         int* has_fg, r3dp_stream_t stream);
+int r3dp_src_bg_fill(const unsigned char* frames, long long frame_stride, const int* maxd2, const int* argmax, int H, int W, short* g,
+                     int* has_bc, unsigned char* bg_u8, float* bg_f32, r3dp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

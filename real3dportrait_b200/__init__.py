@@ -17,10 +17,12 @@ from .secc_render import SECC_Renderer, blink_eye_for_secc, period_blink_schedul
 from .audio2motion import PitchContourVAEModel, VAEModel
 from .hubert import HubertModel, get_hubert_from_16k_speech, hubert_frames
 from .motion import ClipMotion
+from .source import extract_background, inpaint_torso, prepare_source
 
 __all__ = ['RaySampler', 'ImportanceRenderer', 'PlanesCL', 'generate_planes', 'planes_to_channels_last',
            'sample_from_planes', 'sample_from_trigrids', 'grids_to_channels_last', 'producer_view', 'MipRayMarcher2', 'FullyConnectedLayer', 'OSGDecoder', 'SuperresolutionHybrid8XDC',
            'SynthesisBlock', 'SynthesisLayer', 'ToRGBLayer', 'SuperresolutionHybrid8XDC_Warp', 'SynthesisBlockNoUp', 'RenderHead',
            'SegFormerSECC2PlaneBackbone', 'canonical_planes_cl', 'Img2PlaneModel', 'SECC_Renderer',
            'blink_eye_for_secc', 'period_blink_schedule', 'PitchContourVAEModel', 'VAEModel',
-           'HubertModel', 'get_hubert_from_16k_speech', 'hubert_frames', 'ClipMotion']
+           'HubertModel', 'get_hubert_from_16k_speech', 'hubert_frames', 'ClipMotion',
+           'prepare_source', 'inpaint_torso', 'extract_background']

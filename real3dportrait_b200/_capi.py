@@ -160,6 +160,10 @@ _SIGNATURES = {
     'r3dp_hb_stats': (_I, [_P, C.c_longlong, _P, _P]),
     'r3dp_hb_conv0': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _F, _P, _I, _I, _P]),
     'r3dp_hb_layernorm': (_I, [_P, _I, _I, _P, _P, _F, _I, _P, _I, _P, _I, _I, _P]),
+    'r3dp_src_inpaint': (_I, [_P, _P, _I, _I, _I, _P, _P, _P, _P, _P]),
+    'r3dp_src_compose': (_I, [_P, _P, _I, _P, _P, _I, _I, _P, _P, _P, _P]),
+    'r3dp_src_bg_distance': (_I, [_P, _I, C.c_longlong, _I, _I, _I, _P, _I, _P, _P, _P, _P]),
+    'r3dp_src_bg_fill': (_I, [_P, C.c_longlong, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
 }
 
 

@@ -314,3 +314,66 @@ def make_coeffs(n: int, seed: int = 0, yaw: float = 0.0) -> Dict[str, torch.Tens
     t = 0.02 * torch.randn(n, 3, generator=g) * (1.0 if yaw > 0 else 0.0)
     c.update({'euler': e, 'trans': t})
     return c
+
+
+# ---- source images: a portrait-like segmap and a smooth image (the segmap itself comes from mediapipe and is not shipped) ---------------
+SEG_BG, SEG_HAIR, SEG_BODY, SEG_FACE, SEG_CLOTHES, SEG_OTHERS = range(6)
+
+
+def make_segmap(H: int = 512, W: int = 512, seed: int = 0, *, center: float = 0.5, torso_top: float = 0.72, torso: bool = True,
+                neck_width: float = 0.09, neck_gaps: int = 0, roll: int = 0, fractional: bool = False) -> 'np.ndarray':
+    """A [6,H,W] float32 one-hot map in _cal_seg_map's channel order: a head ellipse (face skin, hair on top, an 'others' band for glasses)
+    centred on column center * W, a neck (body skin) from inside the head down to the torso, clothes from row torso_top * H to the bottom
+    (torso=False: none) widening downward, background elsewhere; every boundary wobbles per column with the seed.  neck_width: the neck's
+    half width / W (wider than the head's bottom gives neck columns without head above them).  neck_gaps: that many 10-row background gaps
+    cut into random neck columns (a neck that is not contiguous within a column).  roll: np.roll of the rows (a negative roll of the torso's
+    top puts the torso on row 0 and the head on the last rows).  fractional: soft values, so that (s1 + s3 + s5) != 0 and > 0.5 disagree on
+    part of the image and s0 is fractional but nonzero on the background."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    y, x = np.mgrid[0:H, 0:W].astype(np.float64)
+    wob = lambda amp: amp * np.sin(x[0] / W * rng.uniform(4, 12) + rng.uniform(0, 6.3))[None, :]   # noqa: E731  per-column wobble
+    cy, cx, ry, rx = 0.36 * H, center * W, 0.2 * H, 0.16 * W
+    cls = np.full((H, W), SEG_BG, np.int64)
+    t0 = torso_top * H + wob(0.02 * H)
+    if torso:
+        cls[(y >= t0) & (np.abs(x - cx) <= 0.22 * W + 0.5 * (y - t0) + wob(0.01 * W))] = SEG_CLOTHES
+    neck = (y >= cy) & (y < t0) & (np.abs(x - cx) <= neck_width * W + wob(0.01 * W))
+    cls[neck] = SEG_BODY
+    head = ((y - cy) / ry) ** 2 + ((x - cx) / rx) ** 2 <= 1 + wob(0.05)
+    cls[head] = SEG_FACE
+    cls[head & (y < cy - 0.45 * ry + wob(0.04 * H))] = SEG_HAIR
+    cls[head & (np.abs(y - (cy - 0.1 * ry)) < 0.04 * H) & (np.abs(x - cx) < 0.7 * rx)] = SEG_OTHERS
+    cols = np.nonzero(neck.any(0))[0]
+    for _ in range(neck_gaps):
+        if cols.size:
+            c = rng.choice(cols)
+            r = np.nonzero(cls[:, c] == SEG_BODY)[0]
+            if r.size > 16:
+                r0 = rng.integers(r[0] + 2, r[-1] - 12)
+                cls[r0:r0 + 10, c] = SEG_BG
+    seg = (np.arange(6)[:, None, None] == cls[None]).astype(np.float32)
+    if fractional:
+        u = rng.uniform(0.0, 1.0, (H, W)).astype(np.float32)
+        soft = rng.uniform(0.0, 1.0, (H, W)) < 0.3
+        seg[SEG_HAIR][soft & (cls != SEG_HAIR)] = 0.4 * u[soft & (cls != SEG_HAIR)]       # head sum in (0, 0.4]: != 0 yet not > 0.5
+        seg[SEG_FACE][soft & (cls == SEG_FACE)] = 0.2 + 0.6 * u[soft & (cls == SEG_FACE)]
+        seg[SEG_BG][soft & (cls == SEG_BG)] = 0.25 + 0.5 * u[soft & (cls == SEG_BG)]
+    if roll:
+        seg = np.roll(seg, roll, axis=1)
+    return np.ascontiguousarray(seg)
+
+
+def make_source_image(H: int = 512, W: int = 512, seed: int = 0) -> 'np.ndarray':
+    """A smooth uint8 [H,W,3] RGB image: a few seeded low-frequency waves per channel."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    y, x = np.mgrid[0:H, 0:W].astype(np.float64)
+    img = np.empty((H, W, 3))
+    for ch in range(3):
+        v = rng.uniform(60, 190) + np.zeros((H, W))
+        for _ in range(3):
+            fy, fx, ph = rng.uniform(0.5, 4, 2).tolist() + [rng.uniform(0, 6.3)]
+            v += rng.uniform(20, 40) * np.sin(2 * np.pi * (fy * y / H + fx * x / W) + ph)
+        img[..., ch] = v
+    return np.clip(np.rint(img), 0, 255).astype(np.uint8)
