@@ -513,6 +513,27 @@ int r3dp_motion_camera(const float* src_euler, const float* src_trans, const flo
 int r3dp_motion_keypoints(const float* verts_s, const float* verts_d, int T, int K, float* kp_s, float* kp_d, r3dp_stream_t stream);
 int r3dp_motion_lm2d(const float* verts, long long n, float* lm2d, r3dp_stream_t stream);
 
+/* ------------------------------------------------ 3DMM fit: coefficients from mediapipe landmarks (data_gen/utils/process_{image,video}/fit_3dmm_landmark.py) ---
+ * The parameters x [80 + 70 T] fp64: id [80], then per frame exp [64], euler [3], trans [3]; Adam's m and v share that layout.  The 468 key
+ * points are 8 chunks of 64 (the last 44 padded): basis [8][192][144] fp32 (chunk rows x | y | z blocks of 64 points, columns id | exp),
+ * mean [8][192], weight [512] (the landmark loss's per-point weights, 0 on the padding).
+ * r3dp_fit_grad  one iteration's landmark-loss gradient (mean over T 468 2 of w (proj - lms)^2) at x; lms [T, L, 2] mediapipe pixels (y down,
+ *                L >= 468 points per frame, 8-byte aligned), img_size the image side.  stage 1: the mean shape (id and exp unused, basis may be
+ *                NULL), writes part_frame only.  stage 2: the shape mean + [id | exp] basis^T.  Writes (never accumulates):
+ *                  part_frame [8][T][12]  fp64, per chunk and frame dL/dR (R = Rz Ry Rx, row-major) and dL/dtrans
+ *                  part_exp   [8][T][64]  per chunk and frame dL/dexp
+ *                  part_id    [8][16][80] fp64, per chunk and frame-tile CTA dL/did (min(ceil(T / 64), 16) CTAs per chunk)
+ * r3dp_fit_adam  sums the partials in a fixed order, adds lam_id mean(id^2) + lam_exp mean(exp^2) + lam_lap (lap(exp) + 0.3 lap(euler) +
+ *                0.3 lap(trans)) (cal_lap_loss over frames) when step_idexp > 0, and takes torch's Adam step (lr, betas 0.9 / 0.999, eps
+ *                1e-8) from x into x_next (not x): euler / trans at step step_frame, id / exp at step_idexp (0: copied unchanged, no
+ *                regulariser).  grad (NULL or [80 + 70 T]) receives the gradient.
+ * No host synchronisation and no allocation: a whole fit is capturable in a CUDA graph. */
+int r3dp_fit_grad(const float* basis, const float* mean, const float* weight, const float* lms, int T, int L, int img_size, const double* x,
+                  int stage, double* part_frame, float* part_exp, double* part_id, r3dp_stream_t stream);
+int r3dp_fit_adam(const double* part_frame, const float* part_exp, const double* part_id, int T, int step_frame, int step_idexp, double lr,
+                  double lam_id, double lam_exp, double lam_lap, const double* x, double* x_next, double* m, double* v, double* grad,
+                  r3dp_stream_t stream);
+
 /* ------------------------------------------------ audio2motion: the audio2secc VAE (modules/audio2motion/vae.py, inference path) ---
  * PitchContourVAEModel / VAEModel: audio features and f0 -> expression coefficients.  Activations are channels-last rows per frame; split fp16
  * rows hold [hi | lo] of each value, weights [hi | lo] of w * 2^10 (as r3dp_mf_conv3d with split).  The convolutions and GEMMs around the

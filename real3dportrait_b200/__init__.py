@@ -17,6 +17,7 @@ from .secc_render import SECC_Renderer, blink_eye_for_secc, period_blink_schedul
 from .audio2motion import PitchContourVAEModel, VAEModel
 from .hubert import HubertModel, get_hubert_from_16k_speech, hubert_frames
 from .motion import ClipMotion
+from .fit3dmm import Fit3DMM
 from .source import extract_background, inpaint_torso, prepare_source
 
 __all__ = ['RaySampler', 'ImportanceRenderer', 'PlanesCL', 'generate_planes', 'planes_to_channels_last',
@@ -24,5 +25,5 @@ __all__ = ['RaySampler', 'ImportanceRenderer', 'PlanesCL', 'generate_planes', 'p
            'SynthesisBlock', 'SynthesisLayer', 'ToRGBLayer', 'SuperresolutionHybrid8XDC_Warp', 'SynthesisBlockNoUp', 'RenderHead',
            'SegFormerSECC2PlaneBackbone', 'canonical_planes_cl', 'Img2PlaneModel', 'SECC_Renderer',
            'blink_eye_for_secc', 'period_blink_schedule', 'PitchContourVAEModel', 'VAEModel',
-           'HubertModel', 'get_hubert_from_16k_speech', 'hubert_frames', 'ClipMotion',
+           'HubertModel', 'get_hubert_from_16k_speech', 'hubert_frames', 'ClipMotion', 'Fit3DMM',
            'prepare_source', 'inpaint_torso', 'extract_background']

@@ -149,6 +149,8 @@ _SIGNATURES = {
     'r3dp_motion_camera': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P]),
     'r3dp_motion_keypoints': (_I, [_P, _P, _I, _I, _P, _P, _P]),
     'r3dp_motion_lm2d': (_I, [_P, C.c_longlong, _P, _P]),
+    'r3dp_fit_grad': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _I, _P, _P, _P, _P]),
+    'r3dp_fit_adam': (_I, [_P, _P, _P, _I, _I, _I, C.c_double, C.c_double, C.c_double, C.c_double, _P, _P, _P, _P, _P, _P]),
     'r3dp_a2m_wn_layer': (_I, [_P, _P, _P, _I, _P, _P, _P, _P] + [_I] * 6 + [_P]),
     'r3dp_a2m_input': (_I, [_P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _F, _F, _P, _I, _I, _P, _I, _I, _P]),
     'r3dp_a2m_split': (_I, [_P, C.c_longlong, _I, _P, _P, _P]),

@@ -21,27 +21,38 @@ import torch.nn as nn
 from . import _capi as capi
 from .secc_render import CAMERA_DISTANCE, CENTER, FOCAL
 
-def load_keypoint_bfm(bfm_folder: str):
-    """BFM_model_front.mat -> float32 numpy: mean [N,3] recentred (bfm.py:78-81), id_base [3N,n_id], exp_base [3N,n_exp], keypoints int64 [68]
-    as stored (1-based in the file; read without the - 1, see ClipMotion)."""
+def load_bfm(bfm_folder: str, who: str, keys=()):
+    """BFM_model_front.mat -> float32 numpy: mean [N,3] recentred (bfm.py:78-81), id_base [3N,n_id], exp_base [3N,n_exp], and the raw
+    entries `keys` (which must be present too).  who names the caller in error messages."""
     from scipy.io import loadmat
     path = os.path.join(bfm_folder, 'BFM_model_front.mat')
     if not os.path.isfile(path):
-        raise FileNotFoundError(f'ClipMotion: BFM_model_front.mat not found at {path!r}')
+        raise FileNotFoundError(f'{who}: BFM_model_front.mat not found at {path!r}')
     mat = loadmat(path)
-    missing = [k for k in ('meanshape', 'idBase', 'exBase', 'keypoints') if k not in mat]
+    missing = [k for k in ('meanshape', 'idBase', 'exBase') + tuple(keys) if k not in mat]
     if missing:
-        raise KeyError(f'ClipMotion: BFM_model_front.mat lacks {missing}')
+        raise KeyError(f'{who}: BFM_model_front.mat lacks {missing}')
     mean = mat['meanshape'].astype(np.float32).reshape(-1, 3)
     mean = mean - np.mean(mean, axis=0, keepdims=True)
     id_base, exp_base = mat['idBase'].astype(np.float32), mat['exBase'].astype(np.float32)
     n = mean.shape[0]
     if id_base.shape[0] != 3 * n or exp_base.shape[0] != 3 * n:
-        raise ValueError(f'ClipMotion: idBase {id_base.shape} / exBase {exp_base.shape} do not match {n} vertices')
-    kp = np.squeeze(mat['keypoints']).astype(np.int64).reshape(-1)
+        raise ValueError(f'{who}: idBase {id_base.shape} / exBase {exp_base.shape} do not match {n} vertices')
+    out = {'mean': mean, 'id_base': id_base, 'exp_base': exp_base}
+    out.update({k: mat[k] for k in keys})
+    return out
+
+
+def load_keypoint_bfm(bfm_folder: str):
+    """BFM_model_front.mat -> load_bfm's arrays and keypoints int64 [68] as stored (1-based in the file; read without the - 1, see
+    ClipMotion)."""
+    m = load_bfm(bfm_folder, 'ClipMotion', ('keypoints',))
+    n = m['mean'].shape[0]
+    kp = np.squeeze(m['keypoints']).astype(np.int64).reshape(-1)
     if kp.size == 0 or kp.min() < 0 or kp.max() >= n:
         raise ValueError(f'ClipMotion: keypoints must index the {n} vertices as stored (the reference gathers them without - 1)')
-    return {'mean': mean, 'id_base': id_base, 'exp_base': exp_base, 'keypoints': kp}
+    m['keypoints'] = kp
+    return m
 
 
 class ClipMotion(nn.Module):

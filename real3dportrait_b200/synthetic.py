@@ -283,10 +283,27 @@ def make_keypoints(bfm: dict, seed: int = 0, rows: int = 150, cols: int = 238) -
     return (v + 1).astype(np.float64).reshape(68, 1)
 
 
-def write_bfm_folder(path: str, bfm: Optional[dict] = None, seed: int = 0, keypoints: bool = False) -> Dict[str, object]:
+#: the 8 mediapipe points without a BFM vertex (index -1 in index_mp468_from_mesh35709.npy; weight 0 in the fit's landmark loss)
+MP_UNMATCHED = (93, 127, 132, 234, 323, 356, 361, 454)
+
+
+def make_mp468_index(bfm: dict, seed: int = 0) -> 'np.ndarray':
+    """index_mp468_from_mesh35709.npy for make_bfm's head: int64 [468], 0-based vertex indices of 468 distinct vertices spread over the front
+    of the face (|x| < 0.6, -0.8 < y < 0.55), -1 at MP_UNMATCHED.  A generator of its own (seed + 2000), so make_bfm's outputs stay as they are."""
+    import numpy as np
+    rng = np.random.default_rng(seed + 2000)
+    P = np.asarray(bfm['meanshape'], np.float64).reshape(-1, 3)
+    front = np.nonzero((P[:, 2] > P[:, 2].mean()) & (np.abs(P[:, 0]) < 0.6) & (P[:, 1] > -0.8) & (P[:, 1] < 0.55))[0]
+    idx = rng.choice(front, size=468, replace=False).astype(np.int64)
+    idx[list(MP_UNMATCHED)] = -1
+    return idx
+
+
+def write_bfm_folder(path: str, bfm: Optional[dict] = None, seed: int = 0, keypoints: bool = False, mp468: bool = False) -> Dict[str, object]:
     """Write a BFM in the reference's file layout under `path` (BFM/BFM_model_front.mat with 1-based tri, ncc_code.npy [3,N],
     bfm_{right,left}_eye_faces.npy 1-based) and return the SECC_Renderer keyword arguments that read it.  keypoints=True also writes the
-    68 key points (make_keypoints) and zero placeholders for the other keys Face3DHelper loads (meantex, texBase, point_buf)."""
+    68 key points (make_keypoints) and zero placeholders for the other keys Face3DHelper loads (meantex, texBase, point_buf).  mp468=True
+    writes BFM/index_mp468_from_mesh35709.npy (make_mp468_index) and placeholders for every key ParametricFaceModel(is_train=True) loads."""
     import numpy as np
     import os
     import scipy.io
@@ -297,6 +314,13 @@ def write_bfm_folder(path: str, bfm: Optional[dict] = None, seed: int = 0, keypo
         n = bfm['meanshape'].size // 3
         mat.update({'keypoints': make_keypoints(bfm, seed), 'meantex': np.zeros((1, 3 * n)), 'texBase': np.zeros((3 * n, 1)),
                     'point_buf': np.zeros((n, 8))})
+    if mp468:
+        n = bfm['meanshape'].size // 3
+        mat.setdefault('keypoints', make_keypoints(bfm, seed))
+        for k, v in (('meantex', np.zeros((1, 3 * n))), ('texBase', np.zeros((3 * n, 1))), ('point_buf', np.ones((n, 8))),
+                     ('frontmask2_idx', np.ones((n, 1))), ('tri_mask2', bfm['tri'][:16]), ('skinmask', np.ones((1, n)))):
+            mat.setdefault(k, v)
+        np.save(os.path.join(path, 'BFM', 'index_mp468_from_mesh35709.npy'), make_mp468_index(bfm, seed))
     scipy.io.savemat(os.path.join(path, 'BFM', 'BFM_model_front.mat'), mat)
     np.save(os.path.join(path, 'ncc_code.npy'), bfm['ncc'].astype(np.float32))
     eyes = (os.path.join(path, 'bfm_right_eye_faces.npy'), os.path.join(path, 'bfm_left_eye_faces.npy'))
