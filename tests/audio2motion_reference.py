@@ -5,8 +5,11 @@ train=False; flow_base.py WN / ResidualCouplingBlock), seeded parameters and inp
                                                   Flips, the cond_proj concatenation), float64
   forward_folded(P, batch, z, temperature, pitch) the same network on fold_weights(model): the layouts the kernels run (paired gate rows,
                                                   absorbed Flips, the one-hot blink / amplitude block, g_pre_net over groups of four
-                                                  frames, the transposed conv as a GEMM), float64
+                                                  frames, the transposed conv as a GEMM), float64; with `operands`, every GEMM and conv
+                                                  operand rounded as the kernels read it (split fp16, or fp16 alone at one launch)
+  launch_plan(kind, A, B, Tx, hp)                 every kernel launch of the module's forward, restated from the architecture
 The pitch bins are computed by f0_to_coarse_ref (the reference's float32 formula) in both."""
+import ctypes
 import math
 import os
 import socket
@@ -22,6 +25,14 @@ F0_BIN, F0_MIN, F0_MAX = 256, 50.0, 1100.0
 F0_MEL_MIN = 1127 * np.log(1 + F0_MIN / 700)
 F0_MEL_MAX = 1127 * np.log(1 + F0_MAX / 700)
 HP_PITCH = {'use_mouth_amp_embed': True, 'use_eye_amp_embed': False}
+#: the end-to-end bar of the CUDA forward: max |got - exp64| <= E2E_BAR max |exp64|.  Measured on an H100 80GB HBM3 (700 W power limit):
+#: worst 1.43e-5 (VAEModel, A = 1024), 1.30e-5 for the released pitch config, 5.1e-6 at A = 13.  The fp32 accumulation of enc1's K = 3072
+#: products dominates it (that launch alone is 1.1e-5 of its max |ref|); the float64 emulation of split operands sits near 2e-7 and
+#: float32 eager near 7e-7.  One launch reading fp16 operands alone moves the emulation by 2.9e-5 or more
+#: (tests/test_cpu_audio2motion_launches.py); the per-launch rows of tests/test_gpu_audio2motion_launches.py tell those apart with 4x
+#: margin or more
+E2E_BAR = 2e-5
+SPLIT_WEIGHT_SCALE = 1024.0                 # split weights are stored as [hi | lo] of w * 2^10
 
 
 def reference_checkout():
@@ -189,19 +200,62 @@ def forward(sd, batch, z, temperature, pitch=True, hp=HP_PITCH, dt=torch.float64
 
 
 # ---- the folded network (the kernels' layouts), float64 ---------------------------------------------------------------------------------
-def _conv_cl(x, w, b, k):
+def _hi(v):
+    return v.to(torch.float16).double()
+
+
+class _Operands:
+    """How forward_folded reads the operands of each GEMM / conv launch (tag as in launch_plan):
+      'exact'  float64 as given;
+      'split'  every operand as the kernels read it: activations hi + lo of their fp16 split, weights (hi + lo) / 2^10 of the split of w * 2^10;
+      'hi'     fp16 hi halves alone (activations fp16(x), weights fp16(w * 2^10) / 2^10) at launch `site`, split everywhere else (site None:
+               every launch hi-only)."""
+
+    def __init__(self, mode='exact', site=None):
+        assert mode in ('exact', 'split', 'hi'), mode
+        self.mode, self.site, self.seen = mode, site, set()
+
+    def _hi_only(self, tag):
+        self.seen.add(tag)
+        return self.mode == 'hi' and (self.site is None or self.site == tag)
+
+    def x(self, tag, v):
+        if self.mode == 'exact':
+            return v
+        h = _hi(v)
+        return h if self._hi_only(tag) else h + _hi(v - h)
+
+    def w(self, tag, v):
+        if self.mode == 'exact':
+            return v
+        s = v * SPLIT_WEIGHT_SCALE
+        h = _hi(s)
+        return (h if self._hi_only(tag) else h + _hi(s - h)) / SPLIT_WEIGHT_SCALE
+
+
+def _conv_cl(x, w, b, k, ops=None, tag=None):
     """channels-last [B, T, I] conv with w [O, I, k] (same padding) -> [B, T, O]"""
+    if ops is not None:
+        x, w = ops.x(tag, x), ops.w(tag, w)
     return F.conv1d(x.transpose(1, 2), w, b, padding=k // 2).transpose(1, 2)
 
 
-def _wavenet_folded(x, layers, cond, H):
-    """x [B, T, H]; layers [(w_in [2H, H, k], w_rs [NO, H], b_rs)]; cond [B, T, L*2H] paired rows with the in_layer bias added."""
+def _gemm(x, w, b, ops, tag):
+    """rows x [..., I] @ w [O, I]^T + b"""
+    return ops.x(tag, x) @ ops.w(tag, w).t() + b
+
+
+def _wavenet_folded(x, layers, cond, H, ops=None, prefix='wn'):
+    """x [B, T, H]; layers [(w_in [2H, H, k], w_rs [NO, H], b_rs)]; cond [B, T, L*2H] paired rows with the in_layer bias added.
+    Layer i is launch `{prefix}{i}`: its in_layer conv and res_skip GEMM read their operands through `ops`."""
+    ops = ops or _Operands()
     skip = None
     for i, (wi, wr, br) in enumerate(layers):
+        tag = f'{prefix}{i}'
         wi = wi[torch.stack([torch.arange(H), torch.arange(H) + H], 1).reshape(-1)]
-        a = _conv_cl(x, wi, None, wi.shape[2]) + cond[:, :, 2 * H * i:2 * H * (i + 1)]
+        a = _conv_cl(x, wi, None, wi.shape[2], ops, tag) + cond[:, :, 2 * H * i:2 * H * (i + 1)]
         gated = torch.tanh(a[:, :, 0::2]) * torch.sigmoid(a[:, :, 1::2])
-        rs = gated @ wr.t() + br
+        rs = _gemm(gated, wr, br, ops, tag)
         if i < len(layers) - 1:
             x = x + rs[:, :, :H]
             skip = rs[:, :, H:] if skip is None else skip + rs[:, :, H:]
@@ -210,7 +264,9 @@ def _wavenet_folded(x, layers, cond, H):
     return skip
 
 
-def forward_folded(P, batch, z, temperature, pitch=True, hp=HP_PITCH):
+def forward_folded(P, batch, z, temperature, pitch=True, hp=HP_PITCH, operands='exact', site=None):
+    """The forward on fold_weights(model) in float64.  operands / site: how each launch reads its GEMM / conv operands (_Operands)."""
+    ops = _Operands(operands, site)
     audio = batch['audio'].double()
     B, Tx, A = audio.shape
     T, T4 = Tx // 2, Tx // 8
@@ -221,13 +277,13 @@ def forward_folded(P, batch, z, temperature, pitch=True, hp=HP_PITCH):
     (w1, b1), w2 = P['enc1'], P['enc2']
     w1p = torch.zeros(w1.shape[0], Ap, 3, dtype=torch.float64)
     w1p[:, :A] = w1
-    h = F.gelu(_conv_cl(xin, w1p, b1, 3))
+    h = F.gelu(_conv_cl(xin, w1p, b1, 3, ops, 'enc1'))
     if pitch:
         gcat = torch.zeros(B, T, 288, dtype=torch.float64)
-        gcat[:, :, :128] = _conv_cl(h, w2, None, 3)
+        gcat[:, :, :128] = _conv_cl(h, w2, None, 3, ops, 'enc2')
         emb = P['pitch_table'][f0_to_coarse_ref(batch['f0'].float()[:, ::2])]
         (p1, pb1), p2 = P['penc1'], P['penc2']
-        gcat[:, :, 128:256] = _conv_cl(F.gelu(_conv_cl(emb, p1, pb1, 3)), p2, None, 3)
+        gcat[:, :, 128:256] = _conv_cl(F.gelu(_conv_cl(emb, p1, pb1, 3, ops, 'penc1')), p2, None, 3, ops, 'penc2')
         blink = batch.get('blink', torch.zeros(B, Tx, 1, dtype=torch.long))[:, ::2, 0]
         gcat[:, :, 256] = (blink == 0).double()
         gcat[:, :, 257] = (blink == 1).double()
@@ -236,26 +292,109 @@ def forward_folded(P, batch, z, temperature, pitch=True, hp=HP_PITCH):
         if hp.get('use_eye_amp_embed', False):
             gcat[:, :, 259] = batch.get('eye_amp', torch.full((B, 1), 0.4)).double()
         wc, bc = P['cond_proj']
-        g = gcat @ wc.t() + bc
+        g = _gemm(gcat, wc, bc, ops, 'cond_proj')
     else:
-        g = _conv_cl(h, w2, None, 3)
+        g = _conv_cl(h, w2, None, 3, ops, 'enc2')
     gin = g.shape[2]
     wq, bq = P['g_pre']
-    gs = _conv_cl(g.reshape(B, T4, 4 * gin), wq, bq, 3)
+    gs = _conv_cl(g.reshape(B, T4, 4 * gin), wq, bq, 3, ops, 'g_pre')
     zs = torch.zeros(B, T4, 32, dtype=torch.float64)
     zs[:, :, :16] = z.double().transpose(1, 2) * temperature
     if 'flows' in P:
         wcf, bcf = P['flow_cond']
-        cf = gs @ wcf.t() + bcf
+        cf = _gemm(gs, wcf, bcf, ops, 'flow_cond')
         for n, f in enumerate(P['flows']):
             wp, bp = f['pre']
-            hh = zs @ wp.t() + bp
-            out = _wavenet_folded(hh, f['wn'], cf[:, :, 512 * n:512 * (n + 1)], 64)
+            hh = _gemm(zs, wp, bp, ops, f'flow{n}.pre')
+            out = _wavenet_folded(hh, f['wn'], cf[:, :, 512 * n:512 * (n + 1)], 64, ops, f'flow{n}.wn')
             wpo, bpo = f['post']
-            zs[:, :, f['yc0']:f['yc0'] + 8] += out @ wpo.t() + bpo
+            zs[:, :, f['yc0']:f['yc0'] + 8] += _gemm(out, wpo, bpo, ops, f'flow{n}.post')
     wd, bd = P['dec_pre']
-    x = (zs @ wd.t() + bd).reshape(B, T, 256)
+    x = _gemm(zs, wd, bd, ops, 'dec_pre').reshape(B, T, 256)
     wcd, bcd = P['dec_cond']
-    y = _wavenet_folded(x, P['dec_wn'], g @ wcd.t() + bcd, 256)
+    y = _wavenet_folded(x, P['dec_wn'], _gemm(g, wcd, bcd, ops, 'dec_cond'), 256, ops, 'dec.wn')
     wo, bo = P['out_proj']
-    return (y @ wo.t() + bo) * batch['y_mask'].double()[:, :, None]
+    out = _gemm(y, wo, bo, ops, 'out_proj') * batch['y_mask'].double()[:, :, None]
+    assert site is None or site in ops.seen, f'no launch {site!r} reads GEMM operands'
+    return out
+
+
+# ---- the library's launch sequence, restated from the architecture ----------------------------------------------------------------------
+def launch_signature(fn, args):
+    """(entry point, non-pointer arguments) with every float argument rounded to fp32, as the C side receives it."""
+    return fn, tuple(ctypes.c_float(a).value if isinstance(a, float) else a for a in args)
+
+
+def cop_of(cout):
+    """Packed couts of an r3dp_mf_conv3d launch: cout rounded up to its cout tile (16, 32, 64 or 128)."""
+    bn = 16 if cout <= 16 else 32 if cout <= 32 else 64 if cout <= 64 else 128
+    return -(-cout // bn) * bn
+
+
+#: launches that are not GEMMs or convolutions: no operand rounding to emulate
+PACK_LAUNCHES = ('r3dp_a2m_input', 'r3dp_a2m_split', 'r3dp_a2m_latent', 'r3dp_a2m_store')
+
+
+def launch_plan(kind, A, B, Tx, hp=HP_PITCH, temperature=1.0, ld=64):
+    """Every kernel launch of PitchContourVAEModel (kind 'pitch') / VAEModel ('vae') forward on [B, T_x, A] features, as (tag, C entry
+    point, the non-pointer arguments in C order), written from the architecture (vae.py, flow_base.py) and DESIGN.md's layouts rather than
+    from the module's code.  T = T_x / 2 frames, T4 = T / 4 latent frames; every operand split fp16 ([hi | lo], lo at half the row).
+    The blink / amplitude inputs (hp, batch['blink']) change pointers only, not a launch; temperature and the destination's row stride `ld`
+    are arguments of r3dp_a2m_latent and r3dp_a2m_store.
+      input                          audio (+ pitch row) -> xin [B*T, hi C | lo C], C = Ap (+ 128); the blink / amplitude block into gcat
+      enc1, enc2 / penc1, penc2      k3 convs over B sequences of T frames (enc1 / penc1 with the GELU epilogue); the pitch model's second
+                                     convs write column slices [0, 128) / [128, 256) of gcat [B*T, hi 288 | lo 288]
+      cond_proj                      GEMM over gcat (K = 288) -> fp32 g [B*T, 128]   (VAEModel: enc2 writes g directly)
+      split                          g -> split rows per frame and per group of four frames
+      g_pre                          k3 conv over B sequences of T4 groups of four frames (K = 3 * 4 C_g)
+      latent                         the draw x temperature -> zb [B*T4, hi 32 | lo 32]
+      flow_cond                      the four coupling layers' cond_layers as one GEMM -> fp32 [B*T4, 2048]
+      flow{n}.pre / .wn{i} / .post   per coupling layer (reversed order): pre GEMM (32 -> 64, fp32), four WaveNet layers (hidden 64, k 3), post
+                                     GEMM (64 -> 8, cop 16) added in place into zb's channels [yc0, yc0 + 8), yc0 = 0 for flows 0, 2 (flipped)
+      dec_cond, dec_pre              the decoder's cond GEMM -> fp32 [B*T, 2048]; the transposed conv as a GEMM 32 -> 1024 = 4 frames x 256
+      dec.wn{i}, out_proj, store     four WaveNet layers (hidden 256, k 5), out_proj 256 -> 64 fp32, x y_mask into the destination"""
+    assert kind in ('pitch', 'vae') and A in (1024, 13) and Tx % 8 == 0 and Tx > 0 and B > 0
+    pitch = kind == 'pitch'
+    T, T4 = Tx // 2, Tx // 8
+    Ap = (A + 31) // 32 * 32
+    C = Ap + (128 if pitch else 0)
+    gin = 128 if pitch else 64
+    c1 = gin
+    plan = []
+
+    def add(tag, fn, *args):
+        plan.append((tag, fn, tuple(args)))
+
+    def conv(tag, xs, xlo, cin, N, W, k, O, relu, ys, yc0, ylo, f32):
+        add(tag, 'r3dp_mf_conv3d', xs, xlo, cin, N, 1, 1, W, 1, 1, k, 0, O, cop_of(O), relu, ys, yc0, ylo, int(f32), 1)
+
+    def gemm(tag, K, R, O, ys, yc0=0, ylo=0, f32=True):
+        conv(tag, 2 * K, K, K, 1, R, 1, O, 0, ys, yc0, ylo, f32)
+
+    def wavenet(prefix, T_, hidden, k):
+        for i in range(4):
+            add(f'{prefix}{i}', 'r3dp_a2m_wn_layer', 2048, B, T_, hidden, k, int(i == 0), int(i == 3))
+
+    add('input', 'r3dp_a2m_input', B, Tx, A, Ap, int(not pitch), float(F0_MEL_MIN), float(F0_MEL_MAX - F0_MEL_MIN), 2 * C, C, 576, 288)
+    conv('enc1', 2 * C, C, Ap, B, T, 3, c1, 2, 2 * c1, 0, c1, False)
+    if pitch:
+        conv('enc2', 256, 128, 128, B, T, 3, 128, 0, 576, 0, 288, False)
+        conv('penc1', 2 * C, C, 128, B, T, 3, 128, 2, 256, 0, 128, False)
+        conv('penc2', 256, 128, 128, B, T, 3, 128, 0, 576, 128, 288, False)
+        gemm('cond_proj', 288, B * T, gin, gin)
+    else:
+        conv('enc2', 2 * c1, c1, c1, B, T, 3, gin, 0, gin, 0, 0, True)
+    add('split', 'r3dp_a2m_split', B * T, gin)
+    conv('g_pre', 8 * gin, 4 * gin, 4 * gin, B, T4, 3, gin, 0, 2 * gin, 0, gin, False)
+    add('latent', 'r3dp_a2m_latent', B, T4, float(temperature))
+    gemm('flow_cond', gin, B * T4, 2048, 2048)
+    for n in range(4):
+        gemm(f'flow{n}.pre', 32, B * T4, 64, 64)
+        wavenet(f'flow{n}.wn', T4, 64, 3)
+        gemm(f'flow{n}.post', 64, B * T4, 8, 64, yc0=0 if n % 2 == 0 else 8, ylo=32, f32=False)
+    gemm('dec_cond', gin, B * T, 2048, 2048)
+    gemm('dec_pre', 32, B * T4, 1024, 1024)
+    wavenet('dec.wn', T, 256, 5)
+    gemm('out_proj', 256, B * T, 64, 64)
+    add('store', 'r3dp_a2m_store', B * T, 64, ld)
+    return plan

@@ -1,8 +1,10 @@
 """PitchContourVAEModel / VAEModel forward on the GPU against the float64 restatement (tests/audio2motion_reference.py, itself pinned to the
 reference's own outputs): T_x from 8 to 30000 (ten minutes of audio at 50 Hz features), temperatures 0 and 0.2, mouth_amp 0.45, blink
 ids on, a masked tail, and `out=` into a strided slice of [id | exp | t | T] rows with the other columns untouched.  End-to-end bar:
-max |err| <= 1e-4 max |exp| (DESIGN.md, "Audio-to-motion").  Also: the seeded draw, the rejected inputs that need the device, and the
-peak memory of a 30000-frame forward."""
+max |err| <= E2E_BAR max |exp| = 2e-5 max |exp| (audio2motion_reference.E2E_BAR; DESIGN.md, "Audio-to-motion"): the float64 emulation of
+split operands sits more than 10x below it, with any one launch reading its fp16 hi halves alone above it (tests/
+test_cpu_audio2motion_launches.py).  Also: the seeded draw, the rejected inputs that need the device, and the peak memory of a
+30000-frame forward."""
 import pytest
 import torch
 
@@ -11,7 +13,7 @@ from real3dportrait_b200 import PitchContourVAEModel, VAEModel
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
-TOL = 1e-4
+TOL = ref.E2E_BAR
 
 
 def _model(kind, A, seed=11):
@@ -59,6 +61,7 @@ def test_forward_matches_float64(models, case, temperature, Tx):
     assert ret['pred'] is got and ret['mask'] is not None
     scale = float(want.abs().max())
     err = float((got.double() - want).abs().max())
+    print(f'{kind}{A} T_x={Tx} temperature={temperature}: max |err| / max |exp| = {err / scale:.3e} (bar {TOL:.0e})')
     assert err <= TOL * scale, (err / scale)
     # z= replaces the draw
     got_z = m(_to(batch, DEV), {}, temperature=temperature, z=z_ref.to(DEV))
