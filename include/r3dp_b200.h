@@ -617,6 +617,22 @@ int r3dp_src_bg_distance(const void* segs, int seg_u8, long long seg_stride, int
 int r3dp_src_bg_fill(const unsigned char* frames, long long frame_stride, const int* maxd2, const int* argmax, int H, int W, short* g,
                      int* has_bc, unsigned char* bg_u8, float* bg_f32, r3dp_stream_t stream);
 
+/* ------------------------------------------------ the 'concat_debug' video frames (real3d_infer.py:494-521) --------------------------------
+ * A frame is a uint8 RGB strip [512][2560][3]: panels source | driving SECC | image_raw | depth | image, 512 x 512 each.  dst is byte 0 of
+ * frame 0's strip; frames are frame_stride bytes apart, rows row_pitch (>= 7680) bytes apart, so a strip may be a slice of a wider buffer.
+ * Every panel is converted as the reference's float64 torch.cat makes it: clamp(-1, 1), then ((x + 1) / 2 * 255).int() in float64.
+ * r3dp_debug_panels       panels 0, 1, 2 and 4 of B frames.  ref_gt [3,512,512] fp32 (the source image, every frame); secc [B,3,512,512]
+ *                         fp32 (as ((secc + 1) * 127.5).int() / 127.5 - 1); feat [B,4096,feat_c] fp32, the render's channels-last features
+ *                         with rgb in channels 0-2 (x8 nearest); image [B,3,512,512] fp32, the final frame.  Writes nothing else
+ * r3dp_debug_depth_panel  panel 3 of F frames: depth [F,64,64] fp32, normalised by its min and max over all F frames in float32, x8
+ *                         nearest, the one channel three times (a constant clip gives 0 / 0 = NaN, i.e. byte 0).  minmax: 2 unsigned of
+ *                         device scratch.  Two launches; the min and max never leave the device
+ * No host synchronisation and no allocation: capturable in a CUDA graph. */
+int r3dp_debug_panels(const float* ref_gt, const float* secc, const float* feat, int feat_c, const float* image, int B, unsigned char* dst,
+                      long long frame_stride, long long row_pitch, r3dp_stream_t stream);
+int r3dp_debug_depth_panel(const float* depth, int F, unsigned* minmax, unsigned char* dst, long long frame_stride, long long row_pitch,
+                           r3dp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,6 +19,7 @@ from .hubert import HubertModel, get_hubert_from_16k_speech, hubert_frames
 from .motion import ClipMotion
 from .fit3dmm import Fit3DMM
 from .source import extract_background, inpaint_torso, prepare_source
+from .debug_frames import concat_debug_frames
 
 __all__ = ['RaySampler', 'ImportanceRenderer', 'PlanesCL', 'generate_planes', 'planes_to_channels_last',
            'sample_from_planes', 'sample_from_trigrids', 'grids_to_channels_last', 'producer_view', 'MipRayMarcher2', 'FullyConnectedLayer', 'OSGDecoder', 'SuperresolutionHybrid8XDC',
@@ -26,4 +27,4 @@ __all__ = ['RaySampler', 'ImportanceRenderer', 'PlanesCL', 'generate_planes', 'p
            'SegFormerSECC2PlaneBackbone', 'canonical_planes_cl', 'Img2PlaneModel', 'SECC_Renderer',
            'blink_eye_for_secc', 'period_blink_schedule', 'PitchContourVAEModel', 'VAEModel',
            'HubertModel', 'get_hubert_from_16k_speech', 'hubert_frames', 'ClipMotion', 'Fit3DMM',
-           'prepare_source', 'inpaint_torso', 'extract_background']
+           'prepare_source', 'inpaint_torso', 'extract_background', 'concat_debug_frames']

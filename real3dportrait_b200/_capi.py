@@ -166,6 +166,8 @@ _SIGNATURES = {
     'r3dp_src_compose': (_I, [_P, _P, _I, _P, _P, _I, _I, _P, _P, _P, _P]),
     'r3dp_src_bg_distance': (_I, [_P, _I, C.c_longlong, _I, _I, _I, _P, _I, _P, _P, _P, _P]),
     'r3dp_src_bg_fill': (_I, [_P, C.c_longlong, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
+    'r3dp_debug_panels': (_I, [_P, _P, _P, _I, _P, _I, _P, C.c_longlong, C.c_longlong, _P]),
+    'r3dp_debug_depth_panel': (_I, [_P, _I, _P, _P, C.c_longlong, C.c_longlong, _P]),
 }
 
 

@@ -13,7 +13,10 @@ With out_uint8 the last SR epilogue writes uint8 HWC video frames (the reference
 
 With torso_model=... the engine runs the torso head (OSAvatarSECC_Img2plane_Torso, SuperresolutionHybrid8XDC_Warp): begin_clip() takes the
 constants of a clip (ref_torso_img, bg_img, segmap, kp_s; real3d_infer.py:463-467) and every step takes the frames' kp_d.  The torso warper is
-the caller's PyTorch module; it need not be capturable: by default a step replays two graphs around an eager warper call."""
+the caller's PyTorch module; it need not be capturable: by default a step replays two graphs around an eager warper call.
+
+With out_mode='concat_debug' every frame is the reference's default debug strip [512,2560,3] (real3d_infer.py:494-521): source | driving
+SECC | raw render | depth | final, see debug_frames.py.  The depth panel is normalised over the whole clip, so close_clip() writes it."""
 from __future__ import annotations
 
 import contextlib
@@ -23,6 +26,7 @@ from typing import Callable, Dict, Optional
 import torch
 
 from . import _capi as capi
+from .debug_frames import FRAME_SHAPE as DEBUG_FRAME_SHAPE, RES as DEBUG_RES, debug_panels, depth_panel
 from .renderer import PlanesCL
 from .synthesis import RenderHead
 
@@ -140,14 +144,31 @@ class FrameEngine:
     the frames on which the reference would raise (left unedited).  begin_planes() is unchanged: the reference blinks only the driving images.
     img2plane (with secc2plane): an Img2PlaneModel; begin_planes(img=ref_head_img [1,3,512,512], ...) then makes the clip's canonical planes
     from the source image (cal_cano_plane, secc_img2plane.py:50-62) straight into the engine's canonical buffer, once per clip and outside
-    the step's graph, in place of begin_planes(cano_planes, ...)."""
+    the step's graph, in place of begin_planes(cano_planes, ...).
+    out_mode='concat_debug' (with secc2plane and out_uint8=True): frames are the reference's default debug strips uint8 [512,2560,3]
+    (real3d_infer.py:494-521).  open_clip(frames_per_rank, ref_gt_img=...) takes the source image of panel 0, every step needs the open clip
+    and its frame_index, and close_clip() writes the depth panel, normalised over the whole clip.  Panel 1 is the SECC image the step used
+    (cond_tgt, or the rendered and blinked image).  Needs exchange='p2p' at world > 1; step_host() is not built for it."""
 
     def __init__(self, batch: int = 4, sr_mode: str = 'fp32', device=None, world: int = 1, rank: int = 0, dist=None, hp: Optional[dict] = None,
                  static_styles: bool = True, use_graph: bool = True, out_uint8: bool = False, exchange: str = 'allgather',
                  torso_model: Optional[torch.nn.Module] = None, warper_in_graph: bool = False, torso_stage2: str = 'torch',
                  torso_motion: str = 'torch', secc2plane: Optional[torch.nn.Module] = None, secc_renderer: Optional[torch.nn.Module] = None,
-                 blink: bool = False, img2plane: Optional[torch.nn.Module] = None):
+                 blink: bool = False, img2plane: Optional[torch.nn.Module] = None, out_mode: str = 'final'):
         assert exchange in ('allgather', 'p2p', 'none')
+        if out_mode not in ('final', 'concat_debug'):
+            raise ValueError(f"out_mode must be 'final' or 'concat_debug', got {out_mode!r}")
+        if out_mode == 'concat_debug':
+            if secc2plane is None:
+                raise ValueError("out_mode='concat_debug' shows the driving SECC image: FrameEngine(secc2plane=..., out_mode='concat_debug')")
+            if not out_uint8:
+                raise ValueError("out_mode='concat_debug' writes uint8 video frames: FrameEngine(out_uint8=True, out_mode='concat_debug')")
+            if world > 1 and exchange != 'p2p':
+                raise NotImplementedError("out_mode='concat_debug' at world > 1 collects the clip on rank 0 with exchange='p2p' only")
+            if (hp or {}).get('mask_invalid_rays', False):
+                raise NotImplementedError("out_mode='concat_debug' reads the lean render path, which mask_invalid_rays does not take")
+        self.debug = out_mode == 'concat_debug'
+        self.out_mode = out_mode
         if secc2plane is not None and (hp or {}).get('phase1_plane_fusion_mode', 'add') != 'add':
             raise NotImplementedError('secc2plane: only phase1_plane_fusion_mode="add" (cano + secc, secc_img2plane.py:76-77) is built')
         self.batch, self.world, self.rank, self.dist = batch, world, rank, dist
@@ -189,9 +210,13 @@ class FrameEngine:
         self.inplace = {}                 # input pointers -> (graph, output, the inputs kept alive): see prepare()
         self._pool = None
         self._clip = None
+        self._ref_gt = None               # concat_debug: panel 0's source image [1,3,512,512] (open_clip)
+        self._clip_depth = None           # concat_debug: the clip's depths [world*frames_per_rank,64,64] on rank 0
 
     # ---- output geometry -------------------------------------------------------------------------------------------------------------
     def frame_shape(self):
+        if self.debug:
+            return DEBUG_FRAME_SHAPE
         return (512, 512, 3) if self.out_uint8 else (3, 512, 512)
 
     def frame_dtype(self):
@@ -298,6 +323,8 @@ class FrameEngine:
             if self.blink:
                 self.secc_r.blink(secc, rows=planes[:, self.secc_r.n_id + self.secc_r.n_exp:])
             planes = secc
+        if self.debug:
+            self._secc_used = planes                                   # the step's driving SECC image: panel 1 of its debug frames
         return (self._cano_cl, self.secc.planes_cl(planes))
 
     def blink_faults(self) -> int:
@@ -337,7 +364,18 @@ class FrameEngine:
     @torch.no_grad()
     def _body(self, planes, cameras, u_coarse, u_fine=None, kp_d=None) -> torch.Tensor:
         cond = self._cond(kp_d) if self.torso else None
+        if self.debug:
+            ret = self.head.synthesis(self._planes(planes), cameras, cond=cond, lean=True, keep_render=True, **self._over(u_coarse, u_fine))
+            return self._debug_frames(ret['image'], ret['render_feat'], ret['render_depth'], self._secc_used)
         return self.head.synthesis(self._planes(planes), cameras, cond=cond, lean=True, out_uint8=self.out_uint8, **self._over(u_coarse, u_fine))['image']
+
+    def _debug_frames(self, image, feat, depth, secc):
+        """concat_debug: the step's strips with panels 0, 1, 2 and 4 (panel 3 is written into the clip by close_clip), and its depths
+        [B,64,64] for the clip.  image: the SR's clamped fp32 frames; the panel kernel converts them as the reference's float64 cat does."""
+        B = image.shape[0]
+        frames = torch.empty((B,) + DEBUG_FRAME_SHAPE, dtype=torch.uint8, device=self.device)
+        debug_panels(self._ref_gt, capi.f32(secc), feat, capi.f32(image), frames)
+        return frames, depth.view(B, DEBUG_RES, DEBUG_RES)
 
     def _capture_graph(self, planes, cameras, u_coarse, u_fine=None, kp_d=None):
         if self.torso and not self.warper_in_graph:
@@ -369,14 +407,25 @@ class FrameEngine:
     def _capture_split(self, planes, cameras, u_coarse, u_fine, kp_d):
         """Torso step as graph A -> eager warper -> graph B (see _TorsoGraphs); returns (graphs, output buffer)."""
         sr, over = self.head.superresolution, self._over(u_coarse, u_fine)
-        pre = lambda: self.head.torso_pre(self._planes(planes), cameras, self._cond(kp_d), self.out_uint8, **over)   # noqa: E731
+        if self.debug:                                               # graph B writes the debug frames: graph A's render and SECC image stay alive in st
+            over['keep_render'] = True
+
+        def pre():
+            st = self.head.torso_pre(self._planes(planes), cameras, self._cond(kp_d), self.out_uint8 and not self.debug, **over)
+            if self.debug:
+                st['debug_secc'] = self._secc_used
+            return st
+
+        def post(st, rgb_torso, ret):
+            out = sr.forward_post(st, rgb_torso, ret)
+            return self._debug_frames(out, st['render_feat'], st['render_depth'], st['debug_secc']) if self.debug else out
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side), torch.no_grad():
             for _ in range(2):                                       # warm-up outside capture, as in _capture_graph
                 st = pre()
                 rgb_torso, ret = sr.run_torso(st)
-                sr.forward_post(st, rgb_torso, ret)
+                post(st, rgb_torso, ret)
             b_in = tuple(capi.f32(t).clone() for t in (rgb_torso, ret['deformed_torso_hid'], ret['occlusion_2']))
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
@@ -388,7 +437,7 @@ class FrameEngine:
             with torch.cuda.graph(a, pool=self._pool):
                 st = pre()
             with torch.cuda.graph(b, pool=self._pool):
-                out = sr.forward_post(st, b_in[0], {'deformed_torso_hid': b_in[1], 'occlusion_2': b_in[2]})
+                out = post(st, b_in[0], {'deformed_torso_hid': b_in[1], 'occlusion_2': b_in[2]})
         self.launches_per_step = int(capi.lib().r3dp_launch_count() - c0)
         return _TorsoGraphs(sr, a, st, b_in, b), out
 
@@ -415,6 +464,8 @@ class FrameEngine:
         the steps run eagerly (see `eager_reason`) and nothing is captured."""
         if not self.use_graph or self.eager_reason is not None:
             return 0
+        if self.debug and self._ref_gt is None:
+            raise RuntimeError("out_mode='concat_debug': open_clip(frames_per_rank, ref_gt_img=...) before prepare()")
         for item in inputs:
             planes, cameras, u_coarse = item[:3]
             u_fine = item[3] if len(item) > 3 else None
@@ -438,6 +489,8 @@ class FrameEngine:
         """planes [B,3,32,256,256] | PlanesCL | (cano, secc); cameras [B,25]; u_coarse [B,4096,S,1], u_fine [B*4096,S_imp] (drawn here if None)
         -> this rank's frames: fp32 [B,3,512,512] in [-1,1] or uint8 [B,512,512,3]; with exchange='allgather' the gathered
         [world*B,...] (rank-major); with exchange='p2p' the frames are additionally pushed into the open clip at `frame_index`.
+        out_mode='concat_debug': this rank's debug strips uint8 [B,512,2560,3], pushed with their depths into the open clip at `frame_index`
+        (both required).  Their panel 3 is NOT written: it is normalised over the whole clip, and close_clip() writes it into the clip.
         kp_d [B,68,3]: the frames' driving key points, the torso head's only per-frame condition (torso engines only).
         cond_tgt [B,3,H,W]: the driving SECC image, in place of planes (pass None), for FrameEngine(secc2plane=...).
         coeff [B,144]: the frames' [id | exp] coefficients, in place of cond_tgt, for FrameEngine(secc2plane=..., secc_renderer=...);
@@ -459,6 +512,9 @@ class FrameEngine:
         elif cond_tgt is not None:
             raise ValueError('cond_tgt needs FrameEngine(secc2plane=...)')
         self._check_kp_d(kp_d)
+        if self.debug and (self._clip is None or frame_index is None or not 0 <= frame_index < self._fpr):
+            raise RuntimeError("out_mode='concat_debug': every step needs an open clip (open_clip(frames_per_rank, ref_gt_img=...)) and its "
+                               f"frame_index in [0, frames_per_rank), got frame_index={frame_index}")
         drawn = u_coarse is None or (u_fine is None and self._needs_fine())
         u_coarse, u_fine = self._draw(cameras.shape[0], cameras.device, u_coarse, u_fine)
         graphable = self.use_graph and capi.PROF is None and cameras.shape[0] == self.batch and self.eager_reason is None
@@ -482,6 +538,11 @@ class FrameEngine:
             out = self.s_out
         else:
             out = self._body(planes, cameras, u_coarse, u_fine, kp_d)
+        if self.debug:
+            frames, depth = out
+            with capi.region('exchange'):
+                self._push(frames, frame_index, depth)
+            return frames
         if self.exchange == 'allgather':
             if capi.PROF is not None:                                   # profiling pass: serial, so the region time is the collective's own
                 gathered = torch.empty((self.world * self.batch,) + tuple(out.shape[1:]), dtype=out.dtype, device=self.device)
@@ -529,69 +590,92 @@ class FrameEngine:
             torch.cuda.current_stream().wait_stream(self._p2p['stream'])
 
     # ---- exchange: peer pushes into the clip on rank 0 -----------------------------------------------------------------------------------
-    def open_clip(self, frames_per_rank: int) -> Optional[torch.Tensor]:
+    def open_clip(self, frames_per_rank: int, ref_gt_img: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
         """Allocate the output clip [world*frames_per_rank, ...] on rank 0 and map it into every other rank (CUDA IPC); returns the clip on
-        rank 0, None elsewhere.  Frame f of rank r lands at clip[r*frames_per_rank + f].  With world == 1 the clip is a local buffer."""
+        rank 0, None elsewhere.  Frame f of rank r lands at clip[r*frames_per_rank + f].  With world == 1 the clip is a local buffer.
+        out_mode='concat_debug': ref_gt_img [1,3,512,512] is the source image of panel 0 (real3d_infer.py's ref_gt_img), and rank 0 also
+        holds the clip's depths [world*frames_per_rank,64,64] for close_clip()."""
+        if self.debug:
+            if ref_gt_img is None or tuple(ref_gt_img.shape) != (1, 3, 512, 512):
+                raise ValueError("out_mode='concat_debug': open_clip(frames_per_rank, ref_gt_img=[1,3,512,512]), got "
+                                 f"{None if ref_gt_img is None else tuple(ref_gt_img.shape)}")
+            if self._ref_gt is None:
+                self._ref_gt = torch.empty(1, 3, 512, 512, device=self.device)
+            self._ref_gt.copy_(ref_gt_img)                             # in place: graphs captured for an earlier clip read the new image
+        elif ref_gt_img is not None:
+            raise ValueError("ref_gt_img is panel 0 of the debug frames: FrameEngine(out_mode='concat_debug')")
         shape = (self.world * frames_per_rank,) + self.frame_shape()
+        dshape = (self.world * frames_per_rank, DEBUG_RES, DEBUG_RES)
         self._fpr = frames_per_rank
         if self.world == 1 or self.exchange != 'p2p':
             self._clip = torch.empty(shape, dtype=self.frame_dtype(), device=self.device) if self.rank == 0 else None
             self._clip_view = self._clip
+            self._clip_depth = torch.empty(dshape, device=self.device) if self.debug and self.rank == 0 else None
             self._p2p = None
             return self._clip
         from torch.multiprocessing.reductions import reduce_tensor
         payload = [None]
         if self.rank == 0:
             self._clip = torch.empty(shape, dtype=self.frame_dtype(), device=self.device)
-            payload = [reduce_tensor(self._clip)]
+            self._clip_depth = torch.empty(dshape, device=self.device) if self.debug else None
+            payload = [(reduce_tensor(self._clip), None if self._clip_depth is None else reduce_tensor(self._clip_depth))]
         self.dist.broadcast_object_list(payload, src=0)
         if self.rank == 0:
             self._clip_view = self._clip
         else:
-            fn, args = payload[0]
+            (fn, args), dep = payload[0]
             self._clip_view = fn(*args)                                # rank 0's buffer, mapped into this process (lives on rank 0's device)
             self._clip = self._clip_view                               # pushes only; never read here
+            self._clip_depth = dep[0](*dep[1]) if dep is not None else None
         self._p2p = {'stream': torch.cuda.Stream(device=self.device), 'k': 0, 'stage': None,
                      'done': [torch.cuda.Event() for _ in range(2)], 'ready': [torch.cuda.Event() for _ in range(2)]}
         for e in self._p2p['done']:
             e.record(torch.cuda.current_stream())
         return self._clip if self.rank == 0 else None
 
-    def _push(self, out: torch.Tensor, frame_index: int) -> None:
+    def _push(self, out: torch.Tensor, frame_index: int, depth: Optional[torch.Tensor] = None) -> None:
+        """Frames (and, for concat_debug, their depths [B,64,64]) into the clip at this rank's frame_index."""
         n = min(out.shape[0], self._fpr - frame_index)
         if n <= 0:
             return
-        dst = self._clip_view[self.rank * self._fpr + frame_index: self.rank * self._fpr + frame_index + n]
+        g0 = self.rank * self._fpr + frame_index
+        pairs = [(out, self._clip_view)] + ([(depth, self._clip_depth)] if depth is not None else [])
         if self._p2p is None:                                          # single rank / local clip: plain device copy on the compute stream
-            dst.copy_(out[:n], non_blocking=True)
+            for src, clip in pairs:
+                clip[g0:g0 + n].copy_(src[:n], non_blocking=True)
             return
         p = self._p2p
         k = p['k'] & 1
         p['k'] += 1
         cur = torch.cuda.current_stream()
         if p['stage'] is None:
-            p['stage'] = [torch.empty_like(out) for _ in range(2)]
+            p['stage'] = [[torch.empty_like(src) for src, _ in pairs] for _ in range(2)]
         cur.wait_event(p['done'][k])
-        p['stage'][k].copy_(out, non_blocking=True)                     # the graph's output buffer is rewritten by the next replay
+        for stage, (src, _) in zip(p['stage'][k], pairs):
+            stage[:src.shape[0]].copy_(src, non_blocking=True)         # the graph's output buffer is rewritten by the next replay
         p['ready'][k].record(cur)
         with torch.cuda.stream(p['stream']):
             p['stream'].wait_event(p['ready'][k])
-            src = p['stage'][k][:n]
-            # peer copy over NVLink by the copy engine (no SMs), enqueued directly: torch's cross-device copy_ brackets every copy with
-            # event record/wait pairs on BOTH devices' current streams (measured: 1.3 ms/step of host-side stalls at 2 GPUs)
-            capi.check(capi.lib().r3dp_peer_copy(dst.data_ptr(), dst.device.index, src.data_ptr(), src.device.index,
-                                                 src.numel() * src.element_size(), capi.stream()))
+            for stage, (_, clip) in zip(p['stage'][k], pairs):
+                dst, src = clip[g0:g0 + n], stage[:n]
+                # peer copy over NVLink by the copy engine (no SMs), enqueued directly: torch's cross-device copy_ brackets every copy with
+                # event record/wait pairs on BOTH devices' current streams (measured: 1.3 ms/step of host-side stalls at 2 GPUs)
+                capi.check(capi.lib().r3dp_peer_copy(dst.data_ptr(), dst.device.index, src.data_ptr(), src.device.index,
+                                                     src.numel() * src.element_size(), capi.stream()))
             p['done'][k].record(p['stream'])
 
     def close_clip(self) -> Optional[torch.Tensor]:
-        """Wait until every rank's pushes have landed; returns the finished clip on rank 0."""
+        """Wait until every rank's pushes have landed; returns the finished clip on rank 0.  concat_debug: rank 0 then writes every frame's
+        depth panel, normalised by the min and max over the whole clip (two launches on the current stream)."""
         self.wait_gather()
         torch.cuda.synchronize(self.device)
         if self.world > 1 and self.dist is not None:
             self.dist.barrier()
         clip = self._clip if self.rank == 0 else None
+        if self.debug and self.rank == 0 and clip is not None:
+            depth_panel(self._clip_depth, clip)
         if self.rank != 0 and getattr(self, '_p2p', None) is not None:      # drop this process's mapping of rank 0's buffer before rank 0 may free it
-            self._clip_view = self._clip = None
+            self._clip_view = self._clip = self._clip_depth = None
             torch.cuda.ipc_collect()
         if self.world > 1 and self.dist is not None and getattr(self, '_p2p', None) is not None:
             self.dist.barrier()
@@ -617,6 +701,8 @@ class FrameEngine:
         """Same step, from PINNED HOST tensors to a pinned host output (frames of THIS rank), fully asynchronous: the call
         enqueues H2D (copy-in stream) -> step (current stream) -> D2H (copy-out stream) and returns; with two staging slots the
         copy of step i+1 runs under the compute of step i.  Call `sync_host()` before reading `h_out`.  h_kp_d: the torso head's kp_d."""
+        if self.debug:
+            raise NotImplementedError("out_mode='concat_debug' collects a device-resident clip; step_host() has no clip design for it")
         self._check_kp_d(h_kp_d)
         hp = self._host_pipeline()
         k = hp['k'] & 1

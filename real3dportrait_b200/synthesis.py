@@ -80,26 +80,34 @@ class RenderHead(torch.nn.Module):
                                                 rgb_from_x=True, out_clamp=True, out_uint8=out_uint8)
 
     @torch.no_grad()
-    def torso_pre(self, planes, camera: torch.Tensor, cond: Dict, out_uint8: bool = False, **render_overrides) -> Dict:
+    def torso_pre(self, planes, camera: torch.Tensor, cond: Dict, out_uint8: bool = False, keep_render: bool = False, **render_overrides) -> Dict:
         """Lean torso step up to the torso_model call: render, then the first half of the torso SR head (forward_pre) on the renderer's
         channels-last output.  Continue with superresolution.run_torso(state) and superresolution.forward_post(state, ...) -> the image,
-        clamped to [-1,1] (uint8 HWC frames with out_uint8)."""
-        feat, _, wsum, _ = self._render(planes, camera, render_overrides)
-        return self._torso_pre_from(feat, wsum, cond, out_uint8)
+        clamped to [-1,1] (uint8 HWC frames with out_uint8).  keep_render: the state also holds the render's channels-last features
+        'render_feat' [N,4096,C] and depths 'render_depth' [N,4096,1]."""
+        feat, depth, wsum, _ = self._render(planes, camera, render_overrides)
+        st = self._torso_pre_from(feat, wsum, cond, out_uint8)
+        if keep_render:
+            st['render_feat'], st['render_depth'] = feat, depth
+        return st
 
     @torch.no_grad()
     def synthesis(self, planes, camera: torch.Tensor, ret: Optional[Dict] = None, cond: Optional[Dict] = None, **render_overrides) -> Dict[str, torch.Tensor]:
         """planes [N,3,C,H,W], camera [N,25] -> ret dict with the reference's keys (secc_img2plane.py:134-136).
         lean=True (tensor-core SR, no mask_invalid_rays): the frame-loop fast path of FrameEngine; only ret['image'] (plus ret['is_ray_valid']
-        for the plain head) is filled, clamped to [-1,1], or as uint8 HWC frames [N,512,512,3] with out_uint8=True."""
+        for the plain head) is filled, clamped to [-1,1], or as uint8 HWC frames [N,512,512,3] with out_uint8=True; keep_render=True adds the
+        render's channels-last features ret['render_feat'] [N,4096,C] and depths ret['render_depth'] [N,4096,1] (no copies)."""
         if ret is None:
             ret = {}
         res = self.neural_rendering_resolution
         lean = bool(render_overrides.pop('lean', False))
         out_uint8 = bool(render_overrides.pop('out_uint8', False))
+        keep_render = bool(render_overrides.pop('keep_render', False))
         feat, depth, wsum, valid = self._render(planes, camera, render_overrides)
         N = feat.shape[0]
         if lean and self._lean():
+            if keep_render:
+                ret['render_feat'], ret['render_depth'] = feat, depth
             # frame-loop fast path (FrameEngine): only ret['image'] is wanted, so the NCHW copies of the feature / weight images, the
             # clamped raw image and the per-call ones_ws are not materialised; the SR reads the renderer's channels-last output directly.
             # The clamp (and, if asked, the uint8 HWC conversion of real3d_infer.py:519) happen in the last SR epilogue

@@ -7,7 +7,9 @@ Every rank renders `steps` batches of its own frames; with exchange='p2p' the fr
 locally (sent through an independent NCCL gather at the end) - bit for bit - and prints the per-step cost of both exchanges.
 With --torso the engines run the torso head (synthetic.StubTorsoModel as the warper, the clip constants of begin_clip(), kp_d per frame);
 --no-weight-fuse runs its weight_fuse=False configuration and --torso-v1 its torso_model_version 'v1' (synthetic.StubTorsoModelV1); either implies
---torso."""
+--torso.
+With --concat-debug the engines run the secc2plane head with out_mode='concat_debug' (exchange='p2p'): rank 0's clip of debug strips, whose
+depth panel is normalised over every rank's frames, must equal the clip one GPU renders from the same frames alone."""
 import os
 import sys
 
@@ -18,11 +20,58 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from real3dportrait_b200 import engine, renderer as ren, synthetic as syn   # noqa: E402
 
 
+def concat_debug(rank, world, dev):
+    """Rank 0's concat_debug clip at `world` GPUs == the clip of a single-GPU engine over every rank's frames, bit for bit."""
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests'))
+    import real3dportrait_b200 as r3
+    import secc2plane_reference as s2p_ref
+    B, steps = 4, 3
+
+    def make(**kw):
+        bb = r3.SegFormerSECC2PlaneBackbone()
+        bb.load_state_dict(s2p_ref.make_params({k: v.shape for k, v in bb.state_dict().items()}, 7), strict=True)
+        eng = engine.FrameEngine(batch=B, sr_mode='tc', device=dev, hp={'num_samples_fine': 0}, secc2plane=bb, out_uint8=True,
+                                 out_mode='concat_debug', **kw)
+        eng.load_params(syn.make_decoder_params(seed=4), syn.make_sr_params(seed=5))
+        c = s2p_ref.make_inputs(1, 512, 1)
+        eng.begin_planes(syn.make_planes(1, seed=1).to(dev), c[0].to(dev), c[1].to(dev))
+        return eng
+
+    def frames_of(r, s):
+        tgt = s2p_ref.make_inputs(B, 512, 100 * r + s)[2].to(dev)
+        return tgt, syn.make_cameras(B, seed=100 * r + s + 50).to(dev), syn.make_jitter(B, 4096, 48, 0, seed=100 * r + s + 70)[0].to(dev)
+    ref_gt = ((torch.randint(0, 256, (1, 3, 512, 512), generator=torch.Generator().manual_seed(5)).float() - 127.5) / 127.5).to(dev)
+    eng = make(world=world, rank=rank, dist=dist, exchange='p2p')
+    eng.open_clip(steps * B, ref_gt_img=ref_gt)
+    for s in range(steps):
+        tgt, cams, u = frames_of(rank, s)
+        eng.step(None, cams, u, cond_tgt=tgt, frame_index=s * B)
+    clip = eng.close_clip()
+    ok = True
+    if rank == 0:
+        one = make()
+        one.open_clip(world * steps * B, ref_gt_img=ref_gt)
+        for r in range(world):
+            for s in range(steps):
+                tgt, cams, u = frames_of(r, s)
+                one.step(None, cams, u, cond_tgt=tgt, frame_index=(r * steps + s) * B)
+        ok = torch.equal(clip, one.close_clip())
+        print(f'concat_debug world={world}: rank 0 clip == single-GPU clip: {ok}')
+    dist.barrier()
+    return ok
+
+
 def main():
     rank, world, local = int(os.environ['RANK']), int(os.environ['WORLD_SIZE']), int(os.environ['LOCAL_RANK'])
     torch.cuda.set_device(local)
     dev = torch.device('cuda', local)
     dist.init_process_group('nccl', device_id=dev)
+    if '--concat-debug' in sys.argv[1:]:
+        ok = concat_debug(rank, world, dev)
+        if rank == 0:
+            print('EXCHANGE_OK' if ok else 'EXCHANGE_MISMATCH')
+        dist.destroy_process_group()
+        return
     cfg = {}
     if '--no-weight-fuse' in sys.argv[1:]:
         cfg['weight_fuse'] = False
