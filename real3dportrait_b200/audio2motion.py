@@ -29,8 +29,8 @@ import torch
 import torch.distributions as dist
 import torch.nn as nn
 
-from . import _capi as capi
-from .torso_warp import pack_conv3d
+from . import _capi as capi, conv3d
+from .conv3d import pack_conv3d
 
 F16 = torch.float16
 LATENT = 16
@@ -242,10 +242,6 @@ def fold_weights(model: nn.Module) -> dict:
     return P
 
 
-def _ceil32(n: int) -> int:
-    return (n + 31) // 32 * 32
-
-
 def f0_to_coarse(f0: torch.Tensor) -> torch.Tensor:
     """utils/commons/pitch_utils.py:17-26 on a float32 tensor (the reference's formula and evaluation order, without its assert)."""
     f0_mel = 1127 * (1 + f0 / 700).log()
@@ -291,22 +287,22 @@ class _Audio2Motion(nn.Module):
         with torch.no_grad():
             P = fold_weights(self)
 
-            def conv(wb, cin, split=True):                                  # [O, I, k] or [O, I] -> r3dp_mf_conv3d taps along W
+            def conv(wb, cin):                                              # [O, I, k] or [O, I] -> r3dp_mf_conv3d taps along W
                 w, b = wb
                 if w.dim() == 2:
                     w = w[:, :, None]
-                return pack_conv3d(w[None, :, :, None, None, :], b, cin, split)
+                return pack_conv3d(w[None, :, :, None, None, :], b, cin, True)
 
             def wn(layers):
                 return [(pack_wn_layer(wi, wr).to(dev), br.to(dev, torch.float32).contiguous()) for wi, wr, br in layers]
 
-            A, Ap = self.audio_in_dim, _ceil32(self.audio_in_dim)
+            A, Ap = self.audio_in_dim, conv3d.ceil32(self.audio_in_dim)
             Q = {'A': A, 'Ap': Ap, 'gin': P['enc2'].shape[0]}
             Q['enc1'] = conv(P['enc1'], Ap)
-            Q['enc2'] = conv((P['enc2'], torch.zeros(P['enc2'].shape[0], dtype=torch.float64, device=dev)), P['enc2'].shape[1])
+            Q['enc2'] = conv((P['enc2'], None), P['enc2'].shape[1])
             if self.pitch:
                 Q['penc1'] = conv(P['penc1'], 128)
-                Q['penc2'] = conv((P['penc2'], torch.zeros(128, dtype=torch.float64, device=dev)), 128)
+                Q['penc2'] = conv((P['penc2'], None), 128)
                 Q['pitch_table'] = P['pitch_table'].to(torch.float32).contiguous()
                 Q['cond_proj'] = conv(P['cond_proj'], 288)
             Q['g_pre'] = conv(P['g_pre'], 4 * Q['gin'])
@@ -407,12 +403,6 @@ class _Audio2Motion(nn.Module):
         def at(t, halves=0):
             return ctypes.c_void_p(t.data_ptr() + 2 * halves)
 
-        def conv(xp, xs, xlo, cin, pk, rows, k=1, batch=1, relu=0, res=None, y=None, ys=0, yc0=0, ylo=0, out_f32=False):
-            """r3dp_mf_conv3d on `batch` sequences of `rows` frames (k taps, zero padded per sequence); split operands."""
-            wp, bias, O, cop = pk
-            capi.check(L.r3dp_mf_conv3d(xp, xs, xlo, cin, ptr(wp, F16), ptr(bias), res, batch, 1, 1, rows, 1, 1, k, 0, O, cop, relu,
-                                        ctypes.c_void_p(y.data_ptr()), ys, yc0, ylo, int(out_f32), 1, st))
-
         def wavenet(x, layers, cond, cs, hidden, k, rows, wn_out):
             """x fp32 [B*rows, hidden] (clobbered) -> wn_out split [B*rows, hi | lo]; cond fp32 rows (cs floats), layer i at 2 * hidden * i."""
             xb = torch.empty_like(x)
@@ -439,16 +429,16 @@ class _Audio2Motion(nn.Module):
             c1 = Q['enc1'][2]
             h1 = torch.empty(B * T, 2 * c1, device=dev, dtype=F16)
             gf = torch.empty(B * T, gin, device=dev)
-            conv(at(xin), 2 * C, C, Ap, Q['enc1'], T, k=3, batch=B, relu=2, y=h1, ys=2 * c1, ylo=c1)
+            conv3d.launch(Q['enc1'], xin, 2 * C, C, Ap, (B, 1, 1, T), (1, 1, 3), h1, 2 * c1, ylo=c1, relu=2, stream=st)
             if self.pitch:
-                conv(at(h1), 256, 128, 128, Q['enc2'], T, k=3, batch=B, y=gcat, ys=576, yc0=0, ylo=288)
-                conv(at(xin, Ap), 2 * C, C, 128, Q['penc1'], T, k=3, batch=B, relu=2, y=h1, ys=256, ylo=128)
-                conv(at(h1), 256, 128, 128, Q['penc2'], T, k=3, batch=B, y=gcat, ys=576, yc0=128, ylo=288)
+                conv3d.launch(Q['enc2'], h1, 256, 128, 128, (B, 1, 1, T), (1, 1, 3), gcat, 576, 0, 288, stream=st)
+                conv3d.launch(Q['penc1'], at(xin, Ap), 2 * C, C, 128, (B, 1, 1, T), (1, 1, 3), h1, 256, 0, 128, relu=2, stream=st)
+                conv3d.launch(Q['penc2'], h1, 256, 128, 128, (B, 1, 1, T), (1, 1, 3), gcat, 576, 128, 288, stream=st)
                 del h1
-                conv(at(gcat), 576, 288, 288, Q['cond_proj'], B * T, y=gf, ys=gin, out_f32=True)
+                conv3d.launch(Q['cond_proj'], gcat, 576, 288, 288, (1, 1, 1, B * T), (1, 1, 1), gf, gin, stream=st)
                 del gcat
             else:
-                conv(at(h1), 2 * c1, c1, c1, Q['enc2'], T, k=3, batch=B, y=gf, ys=gin, out_f32=True)
+                conv3d.launch(Q['enc2'], h1, 2 * c1, c1, c1, (B, 1, 1, T), (1, 1, 3), gf, gin, stream=st)
                 del h1
             del xin
             g = torch.empty(B * T, 2 * gin, device=dev, dtype=F16)
@@ -456,34 +446,34 @@ class _Audio2Motion(nn.Module):
             capi.check(L.r3dp_a2m_split(ptr(gf), B * T, gin, ptr(g, F16), ptr(g4, F16), st))
             del gf
             gs = torch.empty(B * T4, 2 * gin, device=dev, dtype=F16)
-            conv(at(g4), 8 * gin, 4 * gin, 4 * gin, Q['g_pre'], T4, k=3, batch=B, y=gs, ys=2 * gin, ylo=gin)
+            conv3d.launch(Q['g_pre'], g4, 8 * gin, 4 * gin, 4 * gin, (B, 1, 1, T4), (1, 1, 3), gs, 2 * gin, 0, gin, stream=st)
             del g4
             # prior flow, reversed
             zb = torch.empty(B * T4, 64, device=dev, dtype=F16)
             capi.check(L.r3dp_a2m_latent(ptr(z), B, T4, temperature, ptr(zb, F16), st))
             if 'flows' in Q:
                 cf = torch.empty(B * T4, 2048, device=dev)
-                conv(at(gs), 2 * gin, gin, gin, Q['flow_cond'], B * T4, y=cf, ys=2048, out_f32=True)
+                conv3d.launch(Q['flow_cond'], gs, 2 * gin, gin, gin, (1, 1, 1, B * T4), (1, 1, 1), cf, 2048, stream=st)
                 h = torch.empty(B * T4, 64, device=dev)
                 ho = torch.empty(B * T4, 128, device=dev, dtype=F16)
                 for n, f in enumerate(Q['flows']):
-                    conv(at(zb), 64, 32, 32, f['pre'], B * T4, y=h, ys=64, out_f32=True)
+                    conv3d.launch(f['pre'], zb, 64, 32, 32, (1, 1, 1, B * T4), (1, 1, 1), h, 64, stream=st)
                     wavenet(h, f['wn'], cf[:, 512 * n:], 2048, 64, 3, T4, ho)
-                    conv(at(ho), 128, 64, 64, f['post'], B * T4, res=at(zb), y=zb, ys=64, yc0=f['yc0'], ylo=32)
+                    conv3d.launch(f['post'], ho, 128, 64, 64, (1, 1, 1, B * T4), (1, 1, 1), zb, 64, f['yc0'], 32, res=zb, stream=st)
                 del cf, h, ho
             del gs
             # decoder
             cd = torch.empty(B * T, 2048, device=dev)
-            conv(at(g), 2 * gin, gin, gin, Q['dec_cond'], B * T, y=cd, ys=2048, out_f32=True)
+            conv3d.launch(Q['dec_cond'], g, 2 * gin, gin, gin, (1, 1, 1, B * T), (1, 1, 1), cd, 2048, stream=st)
             del g
             x = torch.empty(B * T, 256, device=dev)
-            conv(at(zb), 64, 32, 32, Q['dec_pre'], B * T4, y=x, ys=1024, out_f32=True)
+            conv3d.launch(Q['dec_pre'], zb, 64, 32, 32, (1, 1, 1, B * T4), (1, 1, 1), x, 1024, stream=st)
             del zb
             ho = torch.empty(B * T, 512, device=dev, dtype=F16)
             wavenet(x, Q['dec_wn'], cd, 2048, 256, 5, T, ho)
             del x, cd
             y = torch.empty(B * T, 64, device=dev)
-            conv(at(ho), 512, 256, 256, Q['out_proj'], B * T, y=y, ys=64, out_f32=True)
+            conv3d.launch(Q['out_proj'], ho, 512, 256, 256, (1, 1, 1, B * T), (1, 1, 1), y, 64, stream=st)
             del ho
             capi.check(L.r3dp_a2m_store(ptr(y), ptr(mask), B * T, 64, ctypes.c_void_p(out.data_ptr()), out.stride(0), st))
         return out

@@ -24,9 +24,10 @@ from typing import Optional
 import torch
 import torch.nn as nn
 
-from . import _capi as capi
+from . import _capi as capi, conv3d, sr_tc
+from .conv3d import pack_gemm, pack_taps
 from .renderer import PlanesCL
-from .secc2plane import _conv_rows, _pack_gemm, _pack_taps
+from .secc2plane import _conv_rows
 
 F16 = torch.float16
 DIM = 1024                          # both ViTs' embed dim (segformer/models.py:19,103)
@@ -165,10 +166,6 @@ def fold_conv_bn(conv_w: torch.Tensor, bn: nn.BatchNorm2d):
     return conv_w.detach().double() * s[:, None, None, None], bias
 
 
-def _ceil32(n: int) -> int:
-    return (n + 31) // 32 * 32
-
-
 class _Conv:
     """One convolution's packed weights.  Stride-1 undilated 3x3 convs run as r3dp_mf_conv3d (1,3,3) taps, or on r3dp_sr_tc_conv where it
     applies (128 or 256 outputs, a dense input of a multiple of 64 channels, W % 128 == 0: packed for both, chosen per launch); 1x1 stride-1
@@ -185,19 +182,17 @@ class _Conv:
         self.gemm = k == 1 and s == 1
         self.tc = None
         if self.box:
-            self.pk = _pack_taps(w, b, dev)
+            self.pk = pack_taps(w, b, dev)
             if O in (128, 256) and I % 64 == 0:
-                wf = w.to(dev, torch.float32).contiguous()
-                self.tc = torch.empty(9 * O * I, device=dev, dtype=F16)
-                capi.check(capi.lib().r3dp_sr_tc_pack_weights(capi.ptr(wf), 1, O, I, capi.ptr(self.tc, F16), capi.stream()))
+                self.tc = sr_tc.pack_plain_weights(w.to(dev)[None], b.to(dev), I)[0]
         elif self.gemm:
-            self.pk = _pack_gemm(w[:, :, 0, 0], b, dev)
+            self.pk = pack_gemm(w[:, :, 0, 0], b, dev)
         else:
             rows = _conv_rows(w)
-            self.ldy = _ceil32(rows.shape[1])
+            self.ldy = conv3d.ceil32(rows.shape[1])
             wp = torch.zeros(O, self.ldy, dtype=torch.float64, device=w.device)
             wp[:, :rows.shape[1]] = rows
-            self.pk = _pack_gemm(wp, b, dev)
+            self.pk = pack_gemm(wp, b, dev)
 
     def out_size(self, h: int) -> int:
         return (h + 2 * self.p - self.d * (self.k - 1) - 1) // self.s + 1
@@ -289,17 +284,15 @@ class Img2PlaneModel(nn.Module):
         P['aspp_proj'] = conv(aspp.project[0], 1, 1, 0)
         P['dec'] = conv(dec_conv)
         ln = lambda m: (f32(m.weight), f32(m.bias), float(m.eps))           # noqa: E731
+        lin = lambda m: pack_gemm(d(m.weight), d(m.bias), dev)             # noqa: E731
 
         def vit(v, sr):
             blocks = []
             for i in range(1, v.num_blocks + 1):
                 blk = getattr(v, f'block{i}')
                 at = blk.attn
-                e = {'norm1': ln(blk.norm1), 'norm2': ln(blk.norm2),
-                     'q': _pack_gemm(d(at.q.weight), d(at.q.bias), dev), 'kv': _pack_gemm(d(at.kv.weight), d(at.kv.bias), dev),
-                     'proj': _pack_gemm(d(at.proj.weight), d(at.proj.bias), dev),
-                     'fc1': _pack_gemm(d(blk.mlp.fc1.weight), d(blk.mlp.fc1.bias), dev),
-                     'fc2': _pack_gemm(d(blk.mlp.fc2.weight), d(blk.mlp.fc2.bias), dev),
+                e = {'norm1': ln(blk.norm1), 'norm2': ln(blk.norm2), 'q': lin(at.q), 'kv': lin(at.kv), 'proj': lin(at.proj),
+                     'fc1': lin(blk.mlp.fc1), 'fc2': lin(blk.mlp.fc2),
                      'dw': (f32(blk.mlp.dwconv.dwconv.weight.reshape(-1, 9)), f32(blk.mlp.dwconv.dwconv.bias))}
                 if sr > 1:
                     e['sr'] = conv(at.sr, sr, sr, 0)
@@ -363,13 +356,10 @@ class Img2PlaneModel(nn.Module):
         def at(t, halves=0):                                        # a device pointer into an fp16 buffer, `halves` elements in
             return ctypes.c_void_p(t.data_ptr() + 2 * halves)
 
-        def gemm_raw(a, xs, cin, rows, pk, relu=False, res=None, y=None, ys=None, yc0=0, out_f32=False):
-            wp, bias, O, cop = pk
-            if y is None:
-                y = torch.empty(rows, O, device=dev, dtype=torch.float32 if out_f32 else F16)
-                ys = O
-            capi.check(L.r3dp_mf_conv3d(a, xs, 0, cin, ptr(wp, F16), ptr(bias), None if res is None else ptr(res, F16), 1, 1, rows, 1, 1, 1, 1, 0,
-                                        O, cop, int(relu), ctypes.c_void_p(y.data_ptr()), ys, yc0, 0, int(out_f32), 0, st))
+        def gemm(a, pk, relu=False, out_f32=False):                 # a [rows, K] fp16 -> [rows, cout]
+            rows, K = a.shape
+            y = torch.empty(rows, pk.cout, device=dev, dtype=torch.float32 if out_f32 else F16)
+            conv3d.launch(pk, a, K, 0, K, (1, 1, rows, 1), (1, 1, 1), y, pk.cout, relu=int(relu), stream=st)
             return y
 
         def conv(xp, xs, h, cv, act=None, res=None, y=None, ys=None, yc0=0, out_f32=False, src=None):
@@ -381,26 +371,21 @@ class Img2PlaneModel(nn.Module):
                 y = torch.empty(B, ho, ho, cv.cout, device=dev, dtype=torch.float32 if out_f32 else F16)
                 ys = cv.cout
             assert act != 'leaky' or (own and not out_f32)
-            wp, bias, O, cop = cv.pk
-            rp = None if res is None else ptr(res, F16)
-            yp = ctypes.c_void_p(y.data_ptr())
-            relu = act == 'relu'
+            relu = int(act == 'relu')
             if cv.tc is not None and xs == cv.cin and h % 128 == 0 and own and res is None and not out_f32:
                 # r3dp_sr_tc_conv (tiles of 128-pixel rows); epilogue act 3 = ReLU, 2 = LeakyReLU(0.01)
-                capi.check(L.r3dp_sr_tc_conv(xp, ptr(cv.tc, F16), ptr(bias), B, 1, cv.cin, O, h, h, 3, {None: 0, 'leaky': 2, 'relu': 3}[act], yp, st))
+                capi.check(L.r3dp_sr_tc_conv(xp, ptr(cv.tc, F16), ptr(cv.pk.bias), B, 1, cv.cin, cv.cout, h, h, 3, {None: 0, 'leaky': 2, 'relu': 3}[act],
+                                             ptr(y, F16), st))
                 return y, ho
             if cv.box:
-                capi.check(L.r3dp_mf_conv3d(xp, xs, 0, cv.cin, ptr(wp, F16), ptr(bias), rp, B, 1, h, h, 1, 3, 3, 0, O, cop, int(relu), yp, ys, yc0,
-                                            0, int(out_f32), 0, st))
+                conv3d.launch(cv.pk, xp, xs, 0, cv.cin, (B, 1, h, h), (1, 3, 3), y, ys, yc0, relu=relu, res=res, stream=st)
             elif cv.gemm:
-                capi.check(L.r3dp_mf_conv3d(xp, xs, 0, cv.cin, ptr(wp, F16), ptr(bias), rp, 1, 1, B * h * h, 1, 1, 1, 1, 0, O, cop, int(relu), yp, ys,
-                                            yc0, 0, int(out_f32), 0, st))
+                conv3d.launch(cv.pk, xp, xs, 0, cv.cin, (1, 1, B * h * h, 1), (1, 1, 1), y, ys, yc0, relu=relu, res=res, stream=st)
             else:
                 assert src is not None and xs == src.shape[-1] == cv.cin
                 pt = torch.empty(B * ho * ho, cv.ldy, device=dev, dtype=F16)
                 capi.check(L.r3dp_sp_patches_dil(ptr(src, F16), B, h, h, cv.cin, cv.k, cv.s, cv.p, cv.d, ptr(pt, F16), cv.ldy, st))
-                capi.check(L.r3dp_mf_conv3d(ptr(pt, F16), cv.ldy, 0, cv.ldy, ptr(wp, F16), ptr(bias), rp, 1, 1, B * ho * ho, 1, 1, 1, 1, 0, O, cop,
-                                            int(relu), yp, ys, yc0, 0, int(out_f32), 0, st))
+                conv3d.launch(cv.pk, pt, cv.ldy, 0, cv.ldy, (1, 1, B * ho * ho, 1), (1, 1, 1), y, ys, yc0, relu=relu, res=res, stream=st)
             if act == 'leaky':
                 capi.check(L.r3dp_sp_leaky(ptr(y, F16), y.numel(), 0.01, st))
             return y, ho
@@ -425,28 +410,28 @@ class Img2PlaneModel(nn.Module):
             a = torch.empty(R, DIM, device=dev, dtype=F16)
             layernorm(xres, None, R, V['blocks'][0]['norm1'], yh=a)
             for bi, bw in enumerate(V['blocks']):
-                q = gemm_raw(ptr(a, F16), DIM, DIM, R, bw['q'])
+                q = gemm(a, bw['q'])
                 if sr > 1:
                     r, hk = dense(a.view(B, hv, hv, DIM), bw['sr'], hv, out_f32=True)
                     a2 = torch.empty(B * hk * hk, DIM, device=dev, dtype=F16)
                     layernorm(r, None, B * hk * hk, bw['sr_norm'], yh=a2)
                     del r
-                    kv, tk = gemm_raw(ptr(a2, F16), DIM, DIM, B * hk * hk, bw['kv']), hk * hk
+                    kv, tk = gemm(a2, bw['kv']), hk * hk
                     del a2
                 else:
-                    kv, tk = gemm_raw(ptr(a, F16), DIM, DIM, R, bw['kv']), hv * hv
+                    kv, tk = gemm(a, bw['kv']), hv * hv
                 o = torch.empty(R, DIM, device=dev, dtype=F16)
                 with capi.region('img2plane.attention'):
                     capi.check(L.r3dp_ip_attention(ptr(q, F16), DIM, ptr(kv, F16), 2 * DIM, B, hv * hv, tk, HEADS, 1.0 / 16.0, ptr(o, F16), DIM, st))
                 del q, kv
-                t = gemm_raw(ptr(o, F16), DIM, DIM, R, bw['proj'], out_f32=True)
+                t = gemm(o, bw['proj'], out_f32=True)
                 del o
                 layernorm(xres, t, R, bw['norm2'], xo=xres, yh=a)
-                f1 = gemm_raw(ptr(a, F16), DIM, DIM, R, bw['fc1'])
+                f1 = gemm(a, bw['fc1'])
                 f2 = torch.empty_like(f1)
                 capi.check(L.r3dp_sp_dwconv_gelu(ptr(f1, F16), B, hv, hv, MLP, ptr(bw['dw'][0]), ptr(bw['dw'][1]), ptr(f2, F16), st))
                 del f1
-                t = gemm_raw(ptr(f2, F16), MLP, MLP, R, bw['fc2'], out_f32=True)
+                t = gemm(f2, bw['fc2'], out_f32=True)
                 del f2
                 if bi + 1 < len(V['blocks']):
                     layernorm(xres, t, R, V['blocks'][bi + 1]['norm1'], xo=xres, yh=a)
@@ -462,8 +447,8 @@ class Img2PlaneModel(nn.Module):
                 pt = torch.empty(B * h1 * h1, cs.ldy, device=dev, dtype=F16)
                 capi.check(L.r3dp_sp_patches_dil(ptr(xin, F16), B, H, H, 8, 7, 2, 3, 1, ptr(pt, F16), cs.ldy, st))
                 del xin
-                e = gemm_raw(ptr(pt, F16), cs.ldy, cs.ldy, B * h1 * h1, cs.pk, relu=True).view(B, h1, h1, 64)
-                hi = gemm_raw(ptr(pt, F16), cs.ldy, cs.ldy, B * h1 * h1, P['high_first'].pk).view(B, h1, h1, 64)
+                e = gemm(pt, cs.pk, relu=True).view(B, h1, h1, 64)
+                hi = gemm(pt, P['high_first'].pk).view(B, h1, h1, 64)
                 del pt
                 h = (h1 - 1) // 2 + 1
                 y = torch.empty(B, h, h, 64, device=dev, dtype=F16)
@@ -485,7 +470,7 @@ class Img2PlaneModel(nn.Module):
                     dense(y, cv, h8, act='relu', y=cat, ys=1280, yc0=256 * (i + 1))
                 mean = torch.empty(B, 512, device=dev, dtype=F16)
                 capi.check(L.r3dp_ip_channel_mean(ptr(y, F16), B, h8 * h8, 512, ptr(mean, F16), st))
-                pooled = gemm_raw(ptr(mean, F16), 512, 512, B, P['aspp_pool'].pk, relu=True)
+                pooled = gemm(mean, P['aspp_pool'].pk, relu=True)
                 capi.check(L.r3dp_ip_broadcast(ptr(pooled, F16), B, h8 * h8, 256, ptr(cat, F16), 1280, 1024, st))
                 del y, mean, pooled
                 proj, _ = dense(cat, P['aspp_proj'], h8, act='relu')

@@ -18,7 +18,8 @@ from typing import Optional
 import torch
 import torch.nn as nn
 
-from . import _capi as capi
+from . import _capi as capi, conv3d, sr_tc
+from .conv3d import pack_gemm as _pack_gemm, pack_taps as _pack_taps
 from .renderer import PlanesCL, producer_view
 
 F16 = torch.float16
@@ -140,34 +141,6 @@ def fold_head(head: _SegFormerHead):
     return G, bias
 
 
-def _cop(cout: int) -> int:
-    bn = 16 if cout <= 16 else 32 if cout <= 32 else 64 if cout <= 64 else 128      # r3dp_mf_conv3d's cout tile
-    return (cout + bn - 1) // bn * bn
-
-
-def _pack_gemm(w: torch.Tensor, b: Optional[torch.Tensor], dev):
-    """GEMM weights [O, K] -> (fp16 [cop, K], fp32 bias [cop], O, cop) for r3dp_mf_conv3d with 1x1x1 taps."""
-    O, K = w.shape
-    cop = _cop(O)
-    wp = torch.zeros(cop, K, dtype=torch.float64, device=w.device)
-    wp[:O] = w
-    bp = torch.zeros(cop, dtype=torch.float64, device=w.device)
-    if b is not None:
-        bp[:O] = b
-    return wp.to(dev, F16).contiguous(), bp.to(dev, torch.float32).contiguous(), O, cop
-
-
-def _pack_taps(w: torch.Tensor, b: torch.Tensor, dev):
-    """3x3 conv weights [O, I, 3, 3] (float64) -> r3dp_mf_conv3d (1, 3, 3) taps: fp16 [9, cop, I], tap ky*3 + kx."""
-    O, I = w.shape[:2]
-    cop = _cop(O)
-    wp = torch.zeros(9, cop, I, dtype=torch.float64, device=w.device)
-    wp[:, :O] = w.permute(2, 3, 0, 1).reshape(9, O, I)
-    bp = torch.zeros(cop, dtype=torch.float64, device=w.device)
-    bp[:O] = b
-    return wp.to(dev, F16).contiguous(), bp.to(dev, torch.float32).contiguous(), O, cop
-
-
 def _conv_rows(w: torch.Tensor) -> torch.Tensor:
     """Conv weights [O, I, k, k] -> GEMM [O, k*k*I], column (ky*k + kx)*I + c (the r3dp_sp_patches order)."""
     return w.permute(0, 2, 3, 1).reshape(w.shape[0], -1)
@@ -261,14 +234,8 @@ class SegFormerSECC2PlaneBackbone(nn.Module):
         G, hb = fold_head(self.fuse_head)
         P['G'] = [_pack_gemm(g, None, dev) for g in G]
         P['head_bias'] = f32(hb)
-        convs = []
-        for i in (0, 2, 4):
-            c = self.to_plane_cnn[i]
-            w = f32(c.weight)
-            wtc = torch.empty(9 * 256 * 256, device=dev, dtype=F16)
-            capi.check(capi.lib().r3dp_sr_tc_pack_weights(capi.ptr(w), 1, 256, 256, capi.ptr(wtc, F16), capi.stream()))
-            convs.append({'tc': wtc, 'mf': _pack_taps(d(c.weight), d(c.bias), dev), 'bias': f32(c.bias)})
-        P['convs'] = convs
+        P['convs'] = [{'tc': sr_tc.pack_plain(c, EMB), 'mf': _pack_taps(d(c.weight), d(c.bias), dev)}
+                      for c in (self.to_plane_cnn[i] for i in (0, 2, 4))]
         last = self.to_plane_cnn[7]
         w7, b7 = d(last.weight), d(last.bias)
         P['last_r'] = _pack_taps(w7[:64].flip(2), b7[:64], dev)          # planes 0, 1: rows mirrored
@@ -332,11 +299,9 @@ class SegFormerSECC2PlaneBackbone(nn.Module):
         ptr = capi.ptr
 
         def gemm(a, R, pk, out_f32):
-            wp, bias, O, cop = pk
-            K = wp.shape[1]
-            y = torch.empty(R, O, device=dev, dtype=torch.float32 if out_f32 else F16)
-            capi.check(L.r3dp_mf_conv3d(ptr(a, F16), K, 0, K, ptr(wp, F16), ptr(bias), None, 1, 1, 1, R, 1, 1, 1, 0, O, cop, 0,
-                                        ptr(y, torch.float32 if out_f32 else F16), O, 0, 0, int(out_f32), 0, st))
+            K = pk.w.shape[1]
+            y = torch.empty(R, pk.cout, device=dev, dtype=torch.float32 if out_f32 else F16)
+            conv3d.launch(pk, a, K, 0, K, (1, 1, 1, R), (1, 1, 1), y, pk.cout, stream=st)
             return y
 
         def layernorm(xv, t, R, C, p, xo=None, yf=None, yh=None):
@@ -397,11 +362,10 @@ class SegFormerSECC2PlaneBackbone(nn.Module):
                 z = torch.empty_like(y)
                 with capi.region(f'secc2plane.conv{2 * ci}'):         # per-launch times of the conv stack (tools/bench_secc.py)
                     if h1 % 128 == 0:          # r3dp_sr_tc_conv tiles 128-pixel rows
-                        capi.check(L.r3dp_sr_tc_conv(ptr(y, F16), ptr(cv['tc'], F16), ptr(cv['bias']), B, 1, EMB, EMB, h1, h1, 3, 2, ptr(z, F16), st))
+                        wp, bias, _ = cv['tc']
+                        capi.check(L.r3dp_sr_tc_conv(ptr(y, F16), ptr(wp, F16), ptr(bias), B, 1, EMB, EMB, h1, h1, 3, 2, ptr(z, F16), st))
                     else:
-                        wp, bias, O, cop = cv['mf']
-                        capi.check(L.r3dp_mf_conv3d(ptr(y, F16), EMB, 0, EMB, ptr(wp, F16), ptr(bias), None, B, 1, h1, h1, 1, 3, 3, 0, O, cop, 0,
-                                                    ptr(z, F16), EMB, 0, 0, 0, 0, st))
+                        conv3d.launch(cv['mf'], y, EMB, 0, EMB, (B, 1, h1, h1), (1, 3, 3), z, EMB, stream=st)
                         capi.check(L.r3dp_sp_leaky(ptr(z, F16), z.numel(), 0.01, st))
                 y = z
             H2 = 2 * h1
@@ -414,9 +378,8 @@ class SegFormerSECC2PlaneBackbone(nn.Module):
             elif tuple(out.shape) != (B, H2, H2, 3, 32) or out.dtype != torch.float32 or not out.is_contiguous():
                 raise ValueError(f'planes_cl: out must be a contiguous fp32 [{B},{H2},{H2},3,32] tensor')
             with capi.region('secc2plane.conv7'):
-                for src, (wp, bias, O, cop), c0 in ((ur, P['last_r'], 0), (urc, P['last_rc'], 64)):
-                    capi.check(L.r3dp_mf_conv3d(ptr(src, F16), EMB, 0, EMB, ptr(wp, F16), ptr(bias), None, B, 1, H2, H2, 1, 3, 3, 0, O, cop, 0,
-                                                ptr(out), 96, c0, 0, 1, 0, st))
+                for src, pk, c0 in ((ur, P['last_r'], 0), (urc, P['last_rc'], 64)):
+                    conv3d.launch(pk, src, EMB, 0, EMB, (B, 1, H2, H2), (1, 3, 3), out, 96, c0, stream=st)
         return out
 
 

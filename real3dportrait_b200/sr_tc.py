@@ -78,23 +78,29 @@ def to_nhwc_f16(x: torch.Tensor, size: int, split: bool = False) -> torch.Tensor
     return y
 
 
-def pack_plain(conv: torch.nn.Conv2d, in_tensor_channels: int, out_pad: int = 128, split: bool = False):
-    """nn.Conv2d (k = 1|3) -> packed fp16 weights [1,9,Opad,Ipad] + fp32 bias [Opad]; output channels padded to a multiple of
-    `out_pad` with zero filters, input channels padded (zero weights) to the channel count of the activation tensor it reads."""
-    w = conv.weight.detach().float()
-    O, I, k, _ = w.shape
-    Op = (O + out_pad - 1) // out_pad * out_pad
-    w9 = torch.zeros(1, Op, in_tensor_channels, 3, 3, device=w.device)
+def pack_plain_weights(w: torch.Tensor, b: torch.Tensor, in_tensor_channels: int, split: bool = False):
+    """Conv weights [nw,O,I,k,k] (k = 1|3, float32 or float64, rounded to fp32 first) and bias [O] -> packed fp16 weights [nw,9,Opad,Ipad]
+    (a 1x1 in tap 4) + fp32 bias [Opad] + k; output channels padded to a multiple of 128 with zero filters, input channels padded (zero
+    weights) to the channel count of the activation tensor it reads."""
+    w = w.detach()
+    nw, O, I, k = w.shape[:4]
+    Op = (O + 127) // 128 * 128
+    w9 = torch.zeros(nw, Op, in_tensor_channels, 3, 3, device=w.device)
     if k == 3:
-        w9[0, :O, :I] = w
+        w9[:, :O, :I] = w
     else:
-        w9[0, :O, :I, 1, 1] = w[:, :, 0, 0]
+        w9[:, :O, :I, 1, 1] = w[..., 0, 0]
     Ip = (in_tensor_channels + 63) // 64 * 64
-    packed = torch.empty(1, 9, Op, Ip * (2 if split else 1), device=w.device, dtype=torch.float16)
-    capi.check(_fn('pack_weights', split)(capi.ptr(w9), 1, Op, in_tensor_channels, capi.ptr(packed, torch.float16), capi.stream()))
+    packed = torch.empty(nw, 9, Op, Ip * (2 if split else 1), device=w.device, dtype=torch.float16)
+    capi.check(_fn('pack_weights', split)(capi.ptr(w9), nw, Op, in_tensor_channels, capi.ptr(packed, torch.float16), capi.stream()))
     bias = torch.zeros(Op, device=w.device)
-    bias[:O] = conv.bias.detach().float()
+    bias[:O] = b.detach()
     return packed, bias, k
+
+
+def pack_plain(conv: torch.nn.Conv2d, in_tensor_channels: int, split: bool = False):
+    """nn.Conv2d (k = 1|3) -> pack_plain_weights of its weight and bias."""
+    return pack_plain_weights(conv.weight[None], conv.bias, in_tensor_channels, split)
 
 
 def conv_plain(x16: torch.Tensor, packed, act: int, residual: Optional[torch.Tensor] = None, split: bool = False) -> torch.Tensor:

@@ -23,7 +23,8 @@ import torch
 import torch.nn.functional as F
 
 from . import _capi as capi
-from . import sr_tc
+from . import conv3d, sr_tc
+from .conv3d import pack_conv3d
 
 KP_IDX = {4: [0, 8, 16, 27], 9: [0, 3, 6, 8, 10, 13, 16, 27, 33]}     # model2.py:238-243
 
@@ -72,28 +73,10 @@ class Stage2Weights:
         dev = next(gen.parameters()).device
         f32 = lambda t: t.float().contiguous().to(dev)                                    # noqa: E731
 
-        def pack(w, b, in_ch, nw=1):
-            # w [nw,O,I,3,3] float64 -> packed fp16 [nw,9,Opad,Ipad] (Opad = 128 | 256), bias [Opad] fp32
-            O, I = w.shape[1:3]
-            Op = max(128, (O + 127) // 128 * 128)
-            w9 = torch.zeros(nw, Op, in_ch, 3, 3, dtype=torch.float64, device=w.device)
-            w9[:, :O, :I] = w
-            Ip = (in_ch + 63) // 64 * 64
-            out = torch.empty(nw, 9, Op, Ip * (2 if split else 1), device=dev, dtype=torch.float16)
-            capi.check(sr_tc._fn('pack_weights', split)(capi.ptr(f32(w9)), nw, Op, in_ch, capi.ptr(out, torch.float16), capi.stream()))
-            bias = torch.zeros(Op, device=dev)
-            bias[:O] = f32(b)
-            return out, bias
-
-        def k1_as_3x3(w):
-            w3 = w.new_zeros(w.shape[0], w.shape[1], 3, 3)
-            w3[:, :, 1, 1] = w[:, :, 0, 0]
-            return w3
-
         w, b = fold_cna(gen.in_conv)
-        self.in_conv = pack(w[None], b, w.shape[1])
+        self.in_conv = sr_tc.pack_plain_weights(w[None], b, w.shape[1], split)
         mc = gen.mid_conv
-        self.mid_conv = pack(k1_as_3x3(mc.weight.detach().double())[None], mc.bias.detach().double(), mc.in_channels)
+        self.mid_conv = sr_tc.pack_plain(mc, mc.in_channels, split)
         self.res = []
         for rb in gen.res:
             nac1, nac2 = rb.layers[0].layers, rb.layers[1].layers                       # NAC: BN, ReLU, conv
@@ -101,11 +84,12 @@ class Stage2Weights:
             s2, t2 = bn_affine(nac2[0])
             w1, b1 = sn_weight(nac1[2]), nac1[2].bias.detach().double()
             w2, b2 = sn_weight(nac2[2]), nac2[2].bias.detach().double()
-            self.res.append((f32(s1), f32(t1), pack((w1 * s2[:, None, None, None])[None], b1 * s2 + t2, w1.shape[1]), pack(w2[None], b2, w2.shape[1])))
+            self.res.append((f32(s1), f32(t1), sr_tc.pack_plain_weights((w1 * s2[:, None, None, None])[None], b1 * s2 + t2, w1.shape[1], split),
+                             sr_tc.pack_plain_weights(w2[None], b2, w2.shape[1], split)))
         self.up = []
         for ub in gen.up:
             w, b = fold_cna(ub.layers[1])
-            self.up.append((pack(compose_nearest_up(w), b, w.shape[1], nw=4), w.shape[0]))
+            self.up.append((sr_tc.pack_plain_weights(compose_nearest_up(w), b, w.shape[1], split), w.shape[0]))
         oc = gen.out_conv
         self.out_conv = (f32(oc.weight.detach().double().permute(2, 3, 1, 0)), f32(oc.bias.detach().double()), oc.kernel_size[0])
         self.occ = [(f32(c.weight.detach().double().permute(2, 3, 1, 0)), f32(c.bias.detach().double())) for c in (occ[0], occ[2], occ[4])]
@@ -125,21 +109,21 @@ def stage2(wts: Stage2Weights, fs_ndhwc: torch.Tensor, deformation: torch.Tensor
     with capi.region('torso_stage2'):
         capi.check(L.r3dp_tw_gather3d(capi.ptr(fs_ndhwc), int(shared), capi.ptr(deformation), N, C, D, h, w, capi.ptr(g, torch.float16), int(sp), st))
 
-        def conv(x, packed, H, W, slope, residual=None, k=3):
-            wp, bias = packed
+        def conv(x, packed, H, W, slope, residual=None):
+            wp, bias, k = packed
             y = torch.empty(N, H, W, wp.shape[2] * wide, device=dev, dtype=torch.float16)
             capi.check(L.r3dp_tw_conv(capi.ptr(x, torch.float16), capi.ptr(wp, torch.float16), capi.ptr(bias), N, x.shape[-1] // wide, wp.shape[2], H, W,
                                       k, slope, capi.ptr(residual, torch.float16), capi.ptr(y, torch.float16), int(sp), st))
             return y
 
-        x = conv(conv(g, wts.in_conv, h, w, 0.2), wts.mid_conv, h, w, 1.0, k=1)
+        x = conv(conv(g, wts.in_conv, h, w, 0.2), wts.mid_conv, h, w, 1.0)
         C0 = x.shape[-1] // wide
         for s1, t1, c1, c2 in wts.res:
             a = torch.empty_like(x)
             capi.check(L.r3dp_tw_affine_relu(capi.ptr(x, torch.float16), capi.ptr(s1), capi.ptr(t1), N, h, w, C0, int(sp), capi.ptr(a, torch.float16), st))
             x = conv(conv(a, c1, h, w, 0.0), c2, h, w, 1.0, residual=x)
         H, W = h, w
-        for (wp, bias), O in wts.up:
+        for (wp, bias, _), O in wts.up:
             y = torch.empty(N, 2 * H, 2 * W, wp.shape[2] * wide, device=dev, dtype=torch.float16)
             capi.check(L.r3dp_tw_conv_up_nearest(capi.ptr(x, torch.float16), capi.ptr(wp, torch.float16), capi.ptr(bias), N, x.shape[-1] // wide,
                                                  wp.shape[2], H, W, 0.0, capi.ptr(y, torch.float16), int(sp), st))
@@ -179,27 +163,6 @@ def compose_nearest_up3d(w: torch.Tensor) -> torch.Tensor:
 MOTION_D, MOTION_HW = 16, 64
 
 
-def pack_conv3d(w: torch.Tensor, b: torch.Tensor, cin: int, split: bool, cin_map=None, cout_tile: Optional[int] = None):
-    """Folded float64 weights [nph,O,I,kd,kh,kw] -> (packed fp16 [nph, taps, cop, cin (x2 split: [hi | lo] of w * 2^10)], bias [cop] fp32,
-    O, cop).  cin: the channels the conv reads (a multiple of 32); cin_map: the physical input channel of each of the I logical channels."""
-    nph, O, I = w.shape[:3]
-    taps = w.shape[3] * w.shape[4] * w.shape[5]
-    tile = cout_tile or (16 if O <= 16 else 32 if O <= 32 else 64 if O <= 64 else 128)
-    cop = (O + tile - 1) // tile * tile
-    idx = torch.as_tensor(list(range(I)) if cin_map is None else cin_map, dtype=torch.long, device=w.device)
-    wt = torch.zeros(nph, taps, cop, cin, dtype=torch.float64, device=w.device)
-    wt[:, :, :O].index_copy_(3, idx, w.permute(0, 3, 4, 5, 1, 2).reshape(nph, taps, O, I))
-    if split:
-        s = wt * 1024.0
-        hi = s.half()
-        packed = torch.cat([hi, (s - hi.double()).half()], dim=-1)
-    else:
-        packed = wt.half()
-    bias = torch.zeros(cop, dtype=torch.float32, device=w.device)
-    bias[:O] = b.float()
-    return packed.contiguous(), bias, O, cop
-
-
 def estimator_shape_error(mfe: torch.nn.Module) -> Optional[str]:
     """Why `mfe` is not the estimator the kernels restate (MotionFieldEstimator('standard', 34, K in {4, 9}), predict_multiref_occ), or None."""
     try:
@@ -232,7 +195,7 @@ class MotionWeights:
         d = lambda t: t.detach().double()                                               # noqa: E731
         c0 = mfe.down[0].layers[0].layers[0].in_channels
         self.K = c0 // 5 - 1
-        self.c0, self.P0 = c0, (c0 + 31) // 32 * 32                        # input channels, padded to the 32-channel K step
+        self.c0, self.P0 = c0, conv3d.ceil32(c0)                           # input channels, padded to the 32-channel K step
         self.CF = self.P0 + 64                                             # fuser input: [input c0 | pad | up output 32 | head features 32]
         self.compress = (d(mfe.compress.weight)[:, :, 0, 0, 0], d(mfe.compress.bias))
         self.down = []
@@ -292,32 +255,26 @@ def motion(wts: MotionWeights, fc: torch.Tensor, kp_s: torch.Tensor, kp_d: torch
     f16 = torch.float16
     P0, CF = wts.P0, wts.CF
 
-    def conv(x, xs, xlo, cin, packed, dims, taps, relu, y, ys, yc0, ylo, up=0, res=None, out_f32=0):
-        wp, bias, O, cop = packed
-        n, dd, h, w = dims
-        capi.check(L.r3dp_mf_conv3d(capi.ptr(x, f16), xs, xlo, cin, capi.ptr(wp, f16), capi.ptr(bias), capi.ptr(res, f16), n, dd, h, w, *taps, up, O, cop,
-                                    relu, capi.ptr(y, torch.float32 if out_f32 else f16), ys, yc0, ylo, out_f32, int(sp), st))
-
     with capi.region('torso_motion'):
         xf = torch.empty(N, D, S, S, CF * wide, device=dev, dtype=f16)                 # the fuser input; its first P0 channels feed the down path
         capi.check(L.r3dp_mf_input(capi.ptr(fc), int(fc.shape[0] == 1 and N > 1), capi.ptr(kp_s), capi.ptr(kp_d), N, K, D, S, S, P0,
                                    capi.ptr(xf, f16), CF * wide, CF, int(sp), st))
         x, xs, xlo, cin, hw = xf, CF * wide, CF, P0, S
         for packed in wts.down:
-            O = packed[2]
+            O = packed.cout
             y = torch.empty(N, D, hw, hw, O * wide, device=dev, dtype=f16)
-            conv(x, xs, xlo, cin, packed, (N, D, hw, hw), (3, 3, 3), 1, y, O * wide, 0, O)
+            conv3d.launch(packed, x, xs, xlo, cin, (N, D, hw, hw), (3, 3, 3), y, O * wide, 0, O, relu=1, stream=st)
             hw //= 2
             x = torch.empty(N, D, hw, hw, O * wide, device=dev, dtype=f16)
             capi.check(L.r3dp_mf_pool(capi.ptr(y, f16), N, D, hw, hw, O, O * wide, O, capi.ptr(x, f16), O * wide, O, int(sp), st))
             xs, xlo, cin = O * wide, O, O
         for i, packed in enumerate(wts.up):
-            O = packed[2]
+            O = packed.cout
             if i + 1 < len(wts.up):
                 y, ys, yc0, ylo = torch.empty(N, D, 2 * hw, 2 * hw, O * wide, device=dev, dtype=f16), O * wide, 0, O
             else:                                                                          # the last up block writes its slice of the fuser input
                 y, ys, yc0, ylo = xf, CF * wide, P0, CF
-            conv(x, xs, xlo, cin, packed, (N, D, hw, hw), (3, 2, 2), 1, y, ys, yc0, ylo, up=1)
+            conv3d.launch(packed, x, xs, xlo, cin, (N, D, hw, hw), (3, 2, 2), y, ys, yc0, ylo, relu=1, up=1, stream=st)
             x, xs, xlo, cin, hw = y, O * wide, O, O, 2 * hw
         # tgt-head encoder at 128^2 (D = 1), then its 2x2 mean broadcast over depth into the fuser input
         if tuple(rgb_256.shape) != (N, 3, 4 * S, 4 * S) or tuple(weights_256.shape) != (N, 1, 4 * S, 4 * S):
@@ -328,22 +285,22 @@ def motion(wts: MotionWeights, fc: torch.Tensor, kp_s: torch.Tensor, kp_d: torch
                                         int(sp), st))
         dims2 = (N, 1, H2, H2)
         x = torch.empty_like(e)
-        conv(e, 32 * wide, 32, 32, wts.enc0, dims2, (1, 7, 7), 1, x, 32 * wide, 0, 32)
+        conv3d.launch(wts.enc0, e, 32 * wide, 32, 32, dims2, (1, 7, 7), x, 32 * wide, 0, 32, relu=1, stream=st)
         for s1, t1, c1, c2 in wts.res:
             a = torch.empty_like(x)
             capi.check(L.r3dp_tw_affine_relu(capi.ptr(x, f16), capi.ptr(s1), capi.ptr(t1), N, H2, H2, 32, int(sp), capi.ptr(a, f16), st))
             t = torch.empty_like(x)
-            conv(a, 32 * wide, 32, 32, c1, dims2, (1, 3, 3), 1, t, 32 * wide, 0, 32)
+            conv3d.launch(c1, a, 32 * wide, 32, 32, dims2, (1, 3, 3), t, 32 * wide, 0, 32, relu=1, stream=st)
             xn = torch.empty_like(x)
-            conv(t, 32 * wide, 32, 32, c2, dims2, (1, 3, 3), 0, xn, 32 * wide, 0, 32, res=x)
+            conv3d.launch(c2, t, 32 * wide, 32, 32, dims2, (1, 3, 3), xn, 32 * wide, 0, 32, res=x, stream=st)
             x = xn
         capi.check(L.r3dp_mf_head_bcast(capi.ptr(x, f16), N, D, S, S, 32, 32 * wide, 32, capi.ptr(xf, f16), CF * wide, P0 + 32, CF, int(sp), st))
         # fuser (7^3, no activation), mask logits (fp32), softmax + deformation, the occlusion pair
         fx = torch.empty(N, D, S, S, 32 * wide, device=dev, dtype=f16)
-        conv(xf, CF * wide, CF, CF, wts.fuser, (N, D, S, S), (7, 7, 7), 0, fx, 32 * wide, 0, 32)
+        conv3d.launch(wts.fuser, xf, CF * wide, CF, CF, (N, D, S, S), (7, 7, 7), fx, 32 * wide, 0, 32, stream=st)
         ls = (K + 2) // 2 * 2                                                           # K+1 logits per voxel, an even stride
         logits = torch.empty(N, D, S, S, ls, device=dev)
-        conv(fx, 32 * wide, 32, 32, wts.mask, (N, D, S, S), (7, 7, 7), 0, logits, ls, 0, 0, out_f32=1)
+        conv3d.launch(wts.mask, fx, 32 * wide, 32, 32, (N, D, S, S), (7, 7, 7), logits, ls, stream=st)
         deformation = torch.empty(N, D, S, S, 3, device=dev)
         capi.check(L.r3dp_mf_deform(capi.ptr(logits), ls, capi.ptr(kp_s), capi.ptr(kp_d), N, K, D, S, S, capi.ptr(deformation), st))
         occ = torch.empty(N, 1, S, S, device=dev)
