@@ -1,6 +1,7 @@
 """HuBERT on the GPU: r3dp_hb_gemm at every (N, K, epilogue) of the hubert-large forward and r3dp_hb_attention on mixed segment batches,
 each against float64 of the split operands they read, with sentinel guards; the small config against the reference's extract_hubert
-(fixture); hubert-large with formula weights against the float64 restatement; out=, determinism and CUDA-graph capture."""
+(fixture) and the float64 chunk loop at its edges up to T = 30 001; hubert-large with formula weights against the float64 restatement,
+up to three launch groups; all within hubert_reference.E2E_BAR; out=, determinism and CUDA-graph capture, one group and three."""
 import ctypes
 import os
 import sys
@@ -185,8 +186,28 @@ def test_small_against_fixture(L):
     got = get_hubert_from_16k_speech(hr.wave(L), m).double().cpu()
     assert got.shape == ref.shape
     err = float((got - ref).abs().max()) / float(ref.abs().max())
-    print(f'small L={L}: max|err| / max|ref| = {err:.2e}')
-    assert err <= 1e-4
+    print(f'small L={L}: max|err| / max|ref| = {err:.2e} (bar {hr.E2E_BAR:.0e})')
+    assert err <= hr.E2E_BAR
+
+
+@pytest.mark.parametrize('k', [1, 4, 30])
+@pytest.mark.parametrize('r', [79, 80, 399, 400])
+def test_small_chunk_edges(k, r):
+    """L = 320 000 k + r: the reference's chunk loop drops a last chunk of fewer than 400 samples (r < 400) and cuts its last full chunk
+    short when r < 80, so T = 1000 k - 1, 1000 k, 1000 k, 1000 k + 1; k = 4 ends a launch group, k = 30 runs eight groups."""
+    m, _ = small_model()
+    cfg = hr.small_config()
+    sd = {key: v.to(DEV) for key, v in hr.formula_params({key: tuple(v.shape) for key, v in m.state_dict().items()}).items()}
+    L = 320_000 * k + r
+    T = hubert_frames(L)
+    assert T == 1000 * k + (r - 80) // 320
+    speech = torch.from_numpy(hr.wave(L))
+    got = get_hubert_from_16k_speech(speech, m).double()
+    ref = hr.get_hubert(sd, cfg, speech.to(DEV))
+    assert got.shape == ref.shape == (T, 128)
+    err = float((got - ref).abs().max()) / float(ref.abs().max())
+    print(f'small L={L} (T={T}): max|err| / max|ref| = {err:.2e} (bar {hr.E2E_BAR:.0e})')
+    assert err <= hr.E2E_BAR
 
 
 @pytest.fixture(scope='module')
@@ -197,8 +218,10 @@ def large():
     return m.to(DEV), {k: v.to(DEV) for k, v in sd.items()}
 
 
-@pytest.mark.parametrize('T', [1, 49, 999, 1000, 1031, 2500])
+@pytest.mark.parametrize('T', [1, 49, 999, 1000, 1031, 2500, 4000, 4001, 9000])
 def test_large_against_restatement(large, T):
+    """T = 4000 fills one launch group of four segments; 4001 adds a second group of one 1-frame segment; 9000 runs three groups, the last
+    with one segment."""
     m, sd = large
     L = 320 * T + 80 + (T % 7) * 37
     assert hubert_frames(L) == T
@@ -206,8 +229,8 @@ def test_large_against_restatement(large, T):
     got = get_hubert_from_16k_speech(speech, m).double()
     ref = hr.get_hubert(sd, LARGE, speech.to(DEV))
     err = float((got - ref).abs().max()) / float(ref.abs().max())
-    print(f'large T={T}: max|err| / max|ref| = {err:.2e} (bar 1e-4)')
-    assert err <= 1e-4
+    print(f'large T={T}: max|err| / max|ref| = {err:.2e} (bar {hr.E2E_BAR:.0e})')
+    assert err <= hr.E2E_BAR
 
 
 def test_out_padding_determinism_and_graph(large):
@@ -224,6 +247,32 @@ def test_out_padding_determinism_and_graph(large):
     assert r.data_ptr() == audio[0].data_ptr() and torch.equal(audio[0, :T], a)
     assert bool((audio[0, T:] == 0).all()) and bool(audio[1].isnan().all())
     # CUDA graph at fixed L: replay is bit-identical to eager
+    out = torch.empty(T, 1024, device=DEV)
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        get_hubert_from_16k_speech(x, m, out=out)
+    torch.cuda.current_stream().wait_stream(s)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        get_hubert_from_16k_speech(x, m, out=out)
+    out.zero_()
+    g.replay()
+    torch.cuda.synchronize()
+    assert torch.equal(out, a)
+
+
+@torch.no_grad()
+def test_multi_group_out_and_graph(large):
+    """A clip of three launch groups (T = 9000): out= into a wider row-strided buffer and a CUDA-graph replay, both bit-identical to eager."""
+    m, _ = large
+    T = 9000
+    x = torch.from_numpy(hr.wave(320 * T + 80 + 211)).to(DEV)
+    a = get_hubert_from_16k_speech(x, m)
+    buf = torch.full((T + 13, 1024 + 64), float('nan'), device=DEV)
+    r = get_hubert_from_16k_speech(x, m, out=buf[:, :1024])
+    assert r.data_ptr() == buf.data_ptr() and torch.equal(buf[:T, :1024], a)
+    assert bool((buf[T:, :1024] == 0).all()) and bool(buf[:, 1024:].isnan().all())
     out = torch.empty(T, 1024, device=DEV)
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())

@@ -1,7 +1,7 @@
 """HuBERT's front-end and positional-conv entry points on the GPU, each against float64 of the operands it reads, with sentinel guards around
 every output: r3dp_hb_stats and r3dp_hb_conv0 (normalisation, k10 s5 conv, LayerNorm, GELU, split rows), r3dp_hb_layernorm in every output
 form, r3dp_hb_pos_conv at segment edges; and the chain waveform -> HubertModel (out=batch['audio'][0]) -> PitchContourVAEModel (z= given)
-against float64 HuBERT -> the VAE's float64 restatement (tests/audio2motion_reference.py), within the VAE's bar.
+against float64 HuBERT -> the VAE's float64 restatement (tests/audio2motion_reference.py), within the VAE's end-to-end bar E2E_BAR.
 
 The LayerNorm inputs have a small variance (std ~0.05 around an offset), so an eps slip or an unbiased variance moves the output by
 1e-3 or more of its scale, far above the bars (3e-5 of |gamma| (|z| + 1) + |beta|, times GELU's slope bound 1.13, plus 2^-21 of the output
@@ -223,5 +223,5 @@ def test_hubert_into_vae():
     ref_batch['audio'] = feats
     want = a2m.forward({k: val.to(DEV) for k, val in vsd.items()}, ref_batch, z.to(DEV), 0.2, pitch=True)
     err = float((got.double() - want).abs().max()) / float(want.abs().max())
-    print(f'waveform -> HuBERT -> VAE: max|err| / max|ref| = {err:.2e} (bar 1e-4)')
-    assert err <= 1e-4
+    print(f'waveform -> HuBERT -> VAE: max|err| / max|ref| = {err:.2e} (bar {a2m.E2E_BAR:.0e})')
+    assert err <= a2m.E2E_BAR
