@@ -10,6 +10,9 @@ from real3dportrait_b200.img2plane import Img2PlaneModel
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
+#: stays at 3e-3: fp16 operand rounding alone moves the planes by ~1.25e-3 max|ref|, and accumulating the same rounded operands in fp32
+#: instead of float64 moves them ~1e-3 again (tests/test_cpu_img2plane_launches.py), so no emulation tightens it; faults below it are
+#: the per-launch tests' (tests/test_gpu_img2plane_launches.py)
 BAR = 3e-3
 
 

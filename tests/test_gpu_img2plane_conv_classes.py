@@ -48,6 +48,8 @@ ROWS = [
     ('layer4 conv2 dilated patch rows + identity', 'gemm', 4608, 512, False, True, False, 4608, 0, 512, 0, True),
     # ASPP and the decoder conv (bias-free convs)
     ('aspp 1x1 into slice 0 of 1280', 'gemm', 512, 256, True, False, False, 512, 0, 1280, 0, False),
+    ('aspp rate-12 patch rows into slice 256 of 1280', 'gemm', 4608, 256, True, False, False, 4608, 0, 1280, 256, False),
+    ('aspp rate-24 patch rows into slice 512 of 1280', 'gemm', 4608, 256, True, False, False, 4608, 0, 1280, 512, False),
     ('aspp rate-36 patch rows into slice 768 of 1280', 'gemm', 4608, 256, True, False, False, 4608, 0, 1280, 768, False),
     ('aspp pooled rows', 'gemm', 512, 256, True, False, False, 512, 0, 256, 0, False),
     ('aspp project', 'gemm', 1280, 256, True, False, False, 1280, 0, 256, 0, False),

@@ -276,6 +276,13 @@ SECC_PRODUCTION = [
     ('conv_res', 1, 1, 256, 256, 128, 128, {'act': 2}),
 ]
 PRODUCTION += SECC_PRODUCTION
+#: Img2PlaneModel's r3dp_sr_tc_conv launches at 512^2, forward at B = 4 and 1: LowResolutionViT's conv_after_upsample1 / 2 (ReLU, act 3)
+#: and TriplanePredictorViT's second_conv, second_conv_after_cat and third_conv_after_cat (LeakyReLU(0.01), act 2); not in the benchmarked
+#: step, so test_launches_have_rows (tests/test_gpu_img2plane_launches.py) keeps these launched
+IMG2PLANE_PRODUCTION = [(fam, B, 1, I, O, h, h, opt) for B in (4, 1) for fam, I, O, h, opt in (
+    ('conv_res', 256, 128, 128, {'act': 3}), ('conv_res', 128, 128, 256, {'act': 3}), ('conv_res', 256, 128, 256, {'act': 2}),
+    ('conv_res', 128, 128, 256, {'act': 2}))]
+PRODUCTION += IMG2PLANE_PRODUCTION
 #: block1's two layers with per-sample weights: weight-tap addressing per image at tiles_x = 4 and in the 2048-item FIR pass
 PER_SAMPLE = [
     ('layer2', 4, 4, 256, 128, 256, 256, {}),
@@ -496,7 +503,8 @@ def test_benchmarked_launches_have_rows(monkeypatch):
     assert {row[0] for _, t, row in launches.values()} >= {'composed', 'layer_torgb', 'layer2', 'last', 'conv_res', 'layer1', 'noup'}
     missing = [f'{name}: {row} (in {t})' for key, (name, t, row) in launches.items() if key not in have]
     assert not missing, 'launches of the benchmarked step without a float64 row:\n' + '\n'.join(missing)
-    stale = [row for row in PRODUCTION if row not in SECC_PRODUCTION and ('CASES', _signature('CASES', row)) not in launches]
+    stale = [row for row in PRODUCTION if row not in SECC_PRODUCTION and row not in IMG2PLANE_PRODUCTION
+             and ('CASES', _signature('CASES', row)) not in launches]
     assert not stale, f'PRODUCTION rows the benchmarked step no longer launches: {stale}'
 
 
