@@ -9,7 +9,6 @@ train=False; flow_base.py WN / ResidualCouplingBlock), seeded parameters and inp
                                                   operand rounded as the kernels read it (split fp16, or fp16 alone at one launch)
   launch_plan(kind, A, B, Tx, hp)                 every kernel launch of the module's forward, restated from the architecture
 The pitch bins are computed by f0_to_coarse_ref (the reference's float32 formula) in both."""
-import ctypes
 import math
 import os
 import socket
@@ -20,6 +19,8 @@ import zlib
 import numpy as np
 import torch
 import torch.nn.functional as F
+
+from launch_harness import launch_signature  # noqa: F401  (the launch tests call it through this module)
 
 F0_BIN, F0_MIN, F0_MAX = 256, 50.0, 1100.0
 F0_MEL_MIN = 1127 * np.log(1 + F0_MIN / 700)
@@ -320,11 +321,6 @@ def forward_folded(P, batch, z, temperature, pitch=True, hp=HP_PITCH, operands='
 
 
 # ---- the library's launch sequence, restated from the architecture ----------------------------------------------------------------------
-def launch_signature(fn, args):
-    """(entry point, non-pointer arguments) with every float argument rounded to fp32, as the C side receives it."""
-    return fn, tuple(ctypes.c_float(a).value if isinstance(a, float) else a for a in args)
-
-
 def cop_of(cout):
     """Packed couts of an r3dp_mf_conv3d launch: cout rounded up to its cout tile (16, 32, 64 or 128)."""
     bn = 16 if cout <= 16 else 32 if cout <= 32 else 64 if cout <= 64 else 128

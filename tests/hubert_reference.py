@@ -3,11 +3,12 @@ the architecture: `forward_unfolded` as transformers writes it (from a state_dic
 weights in the kernels' layouts (GEMM rows, the conv windows' K order, the pos conv's tap-major K order), exact or with every GEMM,
 attention and positional-conv operand rounded as the kernels read it (split fp16, or fp16 hi halves alone at one launch), and
 `launch_plan`, every kernel launch of the module restated from the architecture."""
-import ctypes
 import math
 
 import torch
 import torch.nn.functional as Fn
+
+from launch_harness import launch_signature  # noqa: F401  (the launch tests call it through this module)
 
 KERNELS, STRIDES = (10, 3, 3, 3, 3, 2, 2), (5, 2, 2, 2, 2, 2, 2)
 #: the end-to-end bar of get_hubert_from_16k_speech: max |got - exp64| <= E2E_BAR max |exp64|.  Measured on an H100 80GB HBM3 (700 W power
@@ -259,11 +260,6 @@ def wave(L):
 
 # ---- the library's launch sequence, restated from the architecture ----------------------------------------------------------------------
 SEG, GROUP = 1000, 4                        # frames per encoder segment; segments per launch group (DESIGN.md "Audio features")
-
-
-def launch_signature(fn, args):
-    """(entry point, non-pointer arguments) with every float argument rounded to fp32, as the C side receives it."""
-    return fn, tuple(ctypes.c_float(a).value if isinstance(a, float) else a for a in args)
 
 
 def groups(T):

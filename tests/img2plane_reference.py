@@ -4,7 +4,6 @@ the tests compare the library against it, and it against the fixture the referen
 
 Also here: the seeded synthetic parameters and inputs the fixture and the tests share, and the shims that let the reference's class be
 built without timm, pretrainedmodels, the global hparams or a network connection (tests/golden/make_golden_img2plane.py)."""
-import ctypes
 import math
 import os
 import socket
@@ -15,6 +14,8 @@ from typing import NamedTuple, Optional
 
 import torch
 import torch.nn.functional as F
+
+from launch_harness import launch_signature
 
 LAYERS = [3, 4, 6, 3]
 DILATION = [1, 1, 2, 4]
@@ -212,11 +213,6 @@ def cop_of(cout):
     """Packed couts of an r3dp_mf_conv3d launch: cout rounded up to its cout tile (16, 32, 64 or 128)."""
     bn = 16 if cout <= 16 else 32 if cout <= 32 else 64 if cout <= 64 else 128
     return -(-cout // bn) * bn
-
-
-def launch_signature(fn, args):
-    """(entry point, non-pointer arguments) with every float argument rounded to fp32, as the C side receives it."""
-    return fn, tuple(ctypes.c_float(a).value if isinstance(a, float) else a for a in args)
 
 
 def row_key(fn, args, reads, writes):

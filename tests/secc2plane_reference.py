@@ -4,7 +4,6 @@ fixture the reference's own class wrote (tests/golden/secc2plane_small.npz).
 
 Also here: the seeded synthetic parameters and inputs the fixture and the tests share, and the shims that let the reference's segformer.py
 import without timm / mmcv (tests/golden/make_golden_secc2plane.py)."""
-import ctypes
 import math
 import sys
 import types
@@ -13,6 +12,8 @@ import zlib
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+
+from launch_harness import launch_signature  # noqa: F401  (the launch tests call it through this module)
 
 EMBED = [32, 64, 160, 256]
 HEADS = [1, 2, 5, 8]
@@ -147,11 +148,6 @@ def to64(sd, device='cpu'):
 
 # ---- the library's launch sequence, restated from the architecture ----------------------------------------------------------------------
 EMB = 256
-
-
-def launch_signature(fn, args):
-    """(entry point, non-pointer arguments) with every float argument rounded to fp32, as the C side receives it."""
-    return fn, tuple(ctypes.c_float(a).value if isinstance(a, float) else a for a in args)
 
 
 def cop_of(cout):

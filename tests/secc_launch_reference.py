@@ -16,6 +16,7 @@ import ctypes
 import numpy as np
 
 import secc_render_reference as ref
+from launch_harness import given
 
 U = 2.0 ** -24
 CAMERA_DISTANCE = 10.0
@@ -143,14 +144,8 @@ def signature(fn, args, types):
     """A call of one of LAUNCHES -> (entry point, its non-pointer arguments with floats rounded to fp32 as the C side receives them, the
     non-NULL flags of its optional pointers).  types: the entry point's ctypes argument types (capi._SIGNATURES[fn][1])."""
     vals = tuple(ctypes.c_float(a).value if t is ctypes.c_float else a for a, t in zip(args, types) if t is not ctypes.c_void_p)
-    nonnull = tuple(_nonnull(args[i]) for i in OPTIONAL[fn])
+    nonnull = tuple(given(args[i]) for i in OPTIONAL[fn])
     return fn, vals, nonnull
-
-
-def _nonnull(p):
-    if isinstance(p, ctypes.c_void_p):
-        return p.value is not None and p.value != 0
-    return p is not None and p != 0
 
 
 def render_rows(N, F, n_id, n_exp, ids, exps, B, S, pose, drop_face0, with_mask, tan_half):

@@ -12,22 +12,13 @@ import torch
 import torch.nn.functional as F
 
 import audio2motion_reference as ref
+from launch_harness import guarded, guards_intact
 from real3dportrait_b200 import _capi as capi
 from real3dportrait_b200.audio2motion import F0_MEL_MAX, F0_MEL_MIN, gate_order, pack_wn_layer
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
-GUARD = 4096
 SENT = -12345.0
-
-
-def _guarded(n, dtype=torch.float32, fill=SENT):
-    buf = torch.full((n + 2 * GUARD,), fill, device=DEV, dtype=dtype)
-    return buf, buf[GUARD:GUARD + n]
-
-
-def _guards_intact(buf, n, fill=SENT):
-    return bool((buf[:GUARD] == fill).all()) and bool((buf[GUARD + n:] == fill).all())
 
 
 def _layer64(H, k, NO, B, T, seed, first, last):
@@ -69,13 +60,13 @@ def test_wn_layer_matches_float64(H, k, T, B, pos):
     x, w_in, w_rs, b_rs, cond, skip = (None if t is None else t.to(DEV) for t in _layer64(H, k, NO, B, T, seed=H + 7 * T + B, first=first, last=last))
     rs, ers = _reference(x, w_in, w_rs, b_rs, cond, skip, H)
     n = B * T * H
-    xb, xd = _guarded(n)
+    xb, xd = guarded(n, torch.float32, fill=SENT, device=DEV)
     xd.copy_(x.flatten().float())
-    ob, od = _guarded(n)
-    sb, sd = _guarded(n)
+    ob, od = guarded(n, torch.float32, fill=SENT, device=DEV)
+    sb, sd = guarded(n, torch.float32, fill=SENT, device=DEV)
     if skip is not None:
         sd.copy_(skip.flatten().float())
-    hb, hd = _guarded(2 * n, torch.float16, fill=-3.0)
+    hb, hd = guarded(2 * n, torch.float16, fill=-3.0, device=DEV)
     cond_buf = torch.full((B * T, 2 * H + 6), SENT, device=DEV)                   # a row stride beyond the slice
     cond_buf[:, :2 * H] = cond.reshape(B * T, 2 * H).float()
     w = pack_wn_layer(w_in, w_rs)
@@ -85,24 +76,24 @@ def test_wn_layer_matches_float64(H, k, T, B, pos):
                                    capi.ptr(bias), capi.ptr(sd), ctypes.c_void_p(hd.data_ptr()) if last else None, B, T, H, k,
                                    int(first), int(last), capi.stream()))
     torch.cuda.synchronize()
-    assert _guards_intact(xb, n) and torch.equal(xd, x.flatten().float())          # the input is never written
+    assert guards_intact(xb, n, fill=SENT) and torch.equal(xd, x.flatten().float())          # the input is never written
     if last:
         want = skip + rs
         bar = ers + 2.0 ** -22 * want.abs()
         h = hd.view(B, T, 2 * H).double()
         got = h[..., :H] + h[..., H:]
-        assert _guards_intact(hb, 2 * n, fill=-3.0) and _guards_intact(ob, n) and bool((od == SENT).all())
+        assert guards_intact(hb, 2 * n, fill=-3.0) and guards_intact(ob, n, fill=SENT) and bool((od == SENT).all())
     else:
         got_x = od.view(B, T, H).double()
         err_x = (got_x - (x + rs[..., :H])).abs()
         bar_x = ers[..., :H] + 2.0 ** -23 * (x + rs[..., :H]).abs()
-        assert _guards_intact(ob, n)
+        assert guards_intact(ob, n, fill=SENT)
         assert bool((err_x <= bar_x).all()), float((err_x / bar_x).max())
         want = rs[..., H:] if first else skip + rs[..., H:]
         bar = ers[..., H:] + 2.0 ** -23 * want.abs()
         got = sd.view(B, T, H).double()
         assert bool((hd == -3.0).all())
-    assert _guards_intact(sb, n)
+    assert guards_intact(sb, n, fill=SENT)
     err = (got - want).abs()
     # the ends of each sequence and the tile boundaries are where the halo and the zero padding act: report them on their own
     for t in sorted({0, T - 1} | {t for t in (63, 64, 127, 128) if t < T}):

@@ -19,14 +19,14 @@ check that keeps these tables equal to what the module launches.
   r3dp_a2m_split, r3dp_a2m_latent and r3dp_a2m_store: exact against torch between guards, at B*T up to 15000.
 * test_forward_launches_have_rows records both classes' forward at several sizes: the calls equal launch_plan (42 for the released
   config), every launch has a row here or in test_gpu_audio2motion_kernels.py, and every conv row of the largest size is still launched."""
-import ctypes
-
 import pytest
 import torch
 import torch.nn.functional as F
 
 import audio2motion_reference as ref
 import sr_conv_reference as scr
+from launch_harness import (Recorder, assert_plan, assert_rows, at, bits, call_signature, conv3d, guarded, guards_intact, hi_w, inside, join, split,
+                            untouched)
 from real3dportrait_b200 import PitchContourVAEModel, VAEModel, _capi as capi
 from real3dportrait_b200.audio2motion import F0_MEL_MAX, F0_MEL_MIN, fold_weights
 
@@ -37,20 +37,12 @@ F16, F32 = torch.float16, torch.float32
 PLANS = [('pitch', 1024, 1, 8), ('pitch', 1024, 2, 400), ('pitch', 1024, 3, 1032), ('pitch', 1024, 1, 30000), ('vae', 13, 2, 400),
          ('vae', 1024, 2, 400)]
 LARGEST = PLANS[3]
-SENTINEL = {F16: (torch.int16, 0x7E55), F32: (torch.int32, 0x7FC01234)}
-GUARD = 4096
 GELU_LIP = 1.13                               # max |GELU'(x)| = 1.1289
 #: beta per K = taps x cin (the products of one output; split runs three MMAs per product).  Worst excess / S over the rows on an H100
 #: 80GB HBM3 (700 W power limit): 1.59e-6 at K = 3072 (enc1), 1.00e-6 at K = 1536 (g_pre), 6.6e-7 at K <= 384; every row's hi-only
 #: weights break its beta by 4x or more (enc1: 1.58e-5 against 2^-19)
 def beta_of(K):
     return 2.0 ** -19 if K > 384 else 2.0 ** -20
-
-
-def signature(fn, args):
-    """A recorded call -> (entry point, its non-pointer arguments), as launch_plan lists it."""
-    types = capi._SIGNATURES[fn][1]
-    return ref.launch_signature(fn, [a for a, t in zip(args, types) if t is not capi._P])
 
 
 def _label(kind, A, B, Tx):
@@ -75,30 +67,6 @@ def _id(key):
     kind, A, tag, label = CONV3D[key]
     a = key[1]
     return f'{label}-{tag}-K{a[9] * a[2]}-N{a[3]}xW{a[6]}-O{a[11]}'
-
-
-# ---- guarded buffers -----------------------------------------------------------------------------------------------------------------------
-def _guarded(n, dt):
-    buf = torch.empty(n + 2 * GUARD, device=DEV, dtype=dt)
-    buf.view(SENTINEL[dt][0]).fill_(SENTINEL[dt][1])
-    return buf, buf[GUARD:GUARD + n]
-
-
-def _untouched(t):
-    return t.view(SENTINEL[t.dtype][0]) == SENTINEL[t.dtype][1]
-
-
-def _guards_intact(buf):
-    return bool(_untouched(buf[:GUARD]).all()) and bool(_untouched(buf[-GUARD:]).all())
-
-
-def _split(v):
-    hi = v.half()
-    return hi, (v - hi.float()).half()
-
-
-def _join(y, c0, n, lo):
-    return y[:, c0:c0 + n].double() + y[:, lo + c0:lo + c0 + n].double()
 
 
 # ---- the models' packed and float64 weights ------------------------------------------------------------------------------------------------
@@ -127,25 +95,10 @@ def _weights(Q, P, tag):
     return q, (w if w.dim() == 3 else w[:, :, None], b)
 
 
-def _hi_w(w):
-    return (w * 1024.0).half().double() / 1024.0
-
-
 def _conv64(x, w, b, k):
     """x [N, W, I] float64, w [O, I, k] -> [N, W, O] (zero padding per sequence)."""
     y = F.conv1d(x.transpose(1, 2), w, None, padding=k // 2).transpose(1, 2)
     return y if b is None else y + b
-
-
-def _launch(a, x, wp, bias, res, y, N, W):
-    """r3dp_mf_conv3d with the row's arguments a (launch_plan order), N / W replaced; x, res, y: pointers."""
-    xs, xlo, cin, _, D, H, _, kd, kh, kw, up, O, cop, relu, ys, yc0, ylo, out_f32, split = a
-    capi.check(capi.lib().r3dp_mf_conv3d(x, xs, xlo, cin, capi.ptr(wp, F16), capi.ptr(bias), res, N, D, H, W, kd, kh, kw, up, O, cop, relu,
-                                         y, ys, yc0, ylo, out_f32, split, capi.stream()))
-
-
-def _at(t, elems=0):
-    return ctypes.c_void_p(t.data_ptr() + t.element_size() * elems)
 
 
 @torch.no_grad()
@@ -165,39 +118,36 @@ def test_conv3d_launch_vs_float64(models, key):
     # input rows: split random fp32 in [0, cin) and [xlo, xlo + cin), NaN in every other half of the row
     xv = torch.randn(M, cin, generator=g, device=DEV)
     xb = torch.full((M, xs), float('nan'), device=DEV, dtype=F16)
-    xb[:, :cin], xb[:, xlo:xlo + cin] = _split(xv)
+    xb[:, :cin], xb[:, xlo:xlo + cin] = split(xv)
     dt = F32 if out_f32 else F16
-    buf, y = _guarded(M * ys, dt)
+    buf, y = guarded(M * ys, dt, device=DEV)
     yv = y.view(M, ys)
-    inside = torch.zeros(ys, dtype=torch.bool, device=DEV)
-    inside[yc0:yc0 + O] = True
-    if not out_f32:
-        inside[ylo + yc0:ylo + yc0 + O] = True
+    mask = inside(ys, yc0, O, ylo, not out_f32, device=DEV)
     if post:                                  # zb as the module holds it: split state in every channel, post adds into its slice
         rv = torch.randn(M, 32, generator=g, device=DEV)
-        yv[:, :32], yv[:, 32:] = _split(rv)
+        yv[:, :32], yv[:, 32:] = split(rv)
         before = yv.clone()
-    _launch(a, _at(xb), wp, bias, _at(y) if post else None, _at(y), N, W)
+    conv3d(a, at(xb), wp, bias, at(y) if post else None, at(y))
     torch.cuda.synchronize()
-    assert _guards_intact(buf), f'{name}: written outside the output'
+    assert guards_intact(buf, y.numel()), f'{name}: written outside the output'
     if post:
-        assert torch.equal(yv[:, ~inside].view(torch.int16), before[:, ~inside].view(torch.int16)), f'{name}: other channels of zb changed'
+        assert torch.equal(yv[:, ~mask].view(torch.int16), before[:, ~mask].view(torch.int16)), f'{name}: other channels of zb changed'
     else:
-        assert not bool(_untouched(yv[:, inside]).any()), f'{name}: an output element was not written'
-        assert bool(_untouched(yv[:, ~inside]).all()), f'{name}: written outside the channel slice'
-    got = (yv[:, yc0:yc0 + O].double() if out_f32 else _join(yv, yc0, O, ylo)).view(N, W, O)
+        assert not bool(untouched(yv[:, mask]).any()), f'{name}: an output element was not written'
+        assert bool(untouched(yv[:, ~mask]).all()), f'{name}: written outside the channel slice'
+    got = (yv[:, yc0:yc0 + O].double() if out_f32 else join(yv, yc0, O, ylo)).view(N, W, O)
 
     x64 = xv.double().view(N, W, cin)[..., :I]
     pre = _conv64(x64, w64, b64, k)
     S = _conv64(x64.abs(), w64.abs(), b64.abs(), k)
-    pre_hi = _conv64(x64.half().double(), _hi_w(w64), b64, k)             # every operand its hi half alone
-    pre_hw = _conv64(x64, _hi_w(w64), b64, k)                             # the weights' hi halves alone
+    pre_hi = _conv64(x64.half().double(), hi_w(w64), b64, k)             # every operand its hi half alone
+    pre_hw = _conv64(x64, hi_w(w64), b64, k)                             # the weights' hi halves alone
     if relu == 2:
         want, want_hi, want_hw, S = F.gelu(pre), F.gelu(pre_hi), F.gelu(pre_hw), GELU_LIP * S
     else:
         want, want_hi, want_hw = pre, pre_hi, pre_hw
     if post:
-        r64 = _join(before, yc0, O, ylo).view(N, W, O)
+        r64 = join(before, yc0, O, ylo).view(N, W, O)
         want, want_hi, want_hw, S = want + r64, want_hi + r64, want_hw + r64, S + r64.abs()
     alpha = scr.ALPHA_F32 if out_f32 else scr.ALPHA_SPLIT
     extra = None if out_f32 else scr.FLOOR_F16                            # the lo half's fp16 subnormal floor
@@ -221,14 +171,14 @@ def test_conv3d_launch_vs_float64(models, key):
     r = W if k == 3 else min(W, 300)
     if k == 3 and N == 1:
         return
-    one_buf, one = _guarded(r * ys, dt)
+    one_buf, one = guarded(r * ys, dt, device=DEV)
     ov = one.view(r, ys)
     if post:
         ov.copy_(before[M - r:])
-    _launch(a, _at(xb, (M - r) * xs), wp, bias, _at(one) if post else None, _at(one), 1, r)
+    conv3d(a, at(xb, (M - r) * xs), wp, bias, at(one) if post else None, at(one), N=1, W=r)
     torch.cuda.synchronize()
-    assert _guards_intact(one_buf)
-    assert torch.equal(ov.view(SENTINEL[dt][0]), yv[M - r:].view(SENTINEL[dt][0])), f'{name}: last {r} rows vs a launch on them alone'
+    assert guards_intact(one_buf, one.numel())
+    assert torch.equal(bits(ov), bits(yv[M - r:])), f'{name}: last {r} rows vs a launch on them alone'
 
 
 # ---- r3dp_a2m_input ------------------------------------------------------------------------------------------------------------------------
@@ -250,14 +200,14 @@ def test_input_frame_mean(A, B, Tx):
     C = Ap
     ys = 2 * C + 8                                                        # a frame stride beyond ylo + C
     audio = torch.randn(B, Tx, A, generator=torch.Generator().manual_seed(Tx + A), device='cpu').to(DEV)
-    buf, y = _guarded(B * T * ys, F16)
+    buf, y = guarded(B * T * ys, F16, device=DEV)
     capi.check(capi.lib().r3dp_a2m_input(capi.ptr(audio), B, Tx, A, Ap, 1, None, None, None, None, None, float(F0_MEL_MIN),
-                                         float(F0_MEL_MAX - F0_MEL_MIN), _at(y), ys, C, None, 576, 288, capi.stream()))
+                                         float(F0_MEL_MAX - F0_MEL_MIN), at(y), ys, C, None, 576, 288, capi.stream()))
     torch.cuda.synchronize()
     yv = y.view(B * T, ys)
-    assert _guards_intact(buf) and bool(_untouched(yv[:, 2 * C:]).all()), 'written beyond ylo + C'
+    assert guards_intact(buf, y.numel()) and bool(untouched(yv[:, 2 * C:]).all()), 'written beyond ylo + C'
     want = 0.5 * (audio[:, 0::2].double() + audio[:, 1::2].double())
-    got = _join(yv, 0, C, C).view(B, T, C)
+    got = join(yv, 0, C, C).view(B, T, C)
     assert _close(got[..., :A], want)
     assert bool((yv[:, A:C] == 0).all()) and bool((yv[:, C + A:2 * C] == 0).all()), 'pad columns not zero'
 
@@ -277,25 +227,25 @@ def test_input_blink_and_amplitudes(mouth, eye, blink):
     eye_d = torch.tensor([0.2, 0.7, 3.1], device=DEV) if eye else None
     audio, f0 = batch['audio'].to(DEV), batch['f0'].to(DEV)
     table = torch.randn(300, 128, generator=torch.Generator().manual_seed(2)).to(DEV)
-    xbuf, xin = _guarded(B * T * 2 * C, F16)
-    gbuf, gcat = _guarded(B * T * 576, F16)
+    xbuf, xin = guarded(B * T * 2 * C, F16, device=DEV)
+    gbuf, gcat = guarded(B * T * 576, F16, device=DEV)
     capi.check(capi.lib().r3dp_a2m_input(capi.ptr(audio), B, Tx, A, Ap, 0, capi.ptr(f0), capi.ptr(bl_d, torch.int64), capi.ptr(mouth_d),
-                                         capi.ptr(eye_d), capi.ptr(table), float(F0_MEL_MIN), float(F0_MEL_MAX - F0_MEL_MIN), _at(xin), 2 * C, C,
-                                         _at(gcat, 256), 576, 288, capi.stream()))
+                                         capi.ptr(eye_d), capi.ptr(table), float(F0_MEL_MIN), float(F0_MEL_MAX - F0_MEL_MIN), at(xin), 2 * C, C,
+                                         at(gcat, 256), 576, 288, capi.stream()))
     torch.cuda.synchronize()
-    assert _guards_intact(xbuf) and _guards_intact(gbuf)
+    assert guards_intact(xbuf, xin.numel()) and guards_intact(gbuf, gcat.numel())
     gv = gcat.view(B * T, 576)
     block = torch.zeros(576, dtype=torch.bool, device=DEV)
     block[256:288] = block[544:576] = True
-    assert bool(_untouched(gv[:, ~block]).all()), 'the block written outside gcat columns 256..287 / 544..575'
-    got = _join(gv, 256, 32, 288).view(B, T, 32)
+    assert bool(untouched(gv[:, ~block]).all()), 'the block written outside gcat columns 256..287 / 544..575'
+    got = join(gv, 256, 32, 288).view(B, T, 32)
     b0 = bl[:, ::2].to(DEV) if blink == 'runs' else torch.zeros(B, T, dtype=torch.long, device=DEV)
     assert torch.equal(got[..., 0], (b0 == 0).double()) and torch.equal(got[..., 1], (b0 == 1).double())
     for col, amp in ((2, mouth_d), (3, eye_d)):
         want = torch.zeros(B, T, dtype=torch.float64, device=DEV) if amp is None else amp.double()[:, None].expand(B, T)
         assert _close(got[..., col], want), col
     assert bool((gv[:, 260:288] == 0).all()) and bool((gv[:, 544:546] == 0).all()) and bool((gv[:, 548:576] == 0).all())
-    assert _close(_join(xin.view(B * T, 2 * C), 0, A, C).view(B, T, A), audio[:, ::2].double())
+    assert _close(join(xin.view(B * T, 2 * C), 0, A, C).view(B, T, A), audio[:, ::2].double())
 
 
 # ---- r3dp_a2m_split / _latent / _store -------------------------------------------------------------------------------------------------------
@@ -305,21 +255,21 @@ def test_input_blink_and_amplitudes(mouth, eye, blink):
 def test_split_exact(which, R, C):
     x = torch.randn(R, C, generator=torch.Generator().manual_seed(R + C), device='cpu').to(DEV) * 3.0
     x[0, :4] = torch.tensor([0.0, 1e-6, -7e-8, 65000.0])                  # zero, subnormal remainders, a large value
-    b1, y1 = _guarded(R * 2 * C, F16)
-    b4, y4 = _guarded(R * 2 * C, F16)
-    capi.check(capi.lib().r3dp_a2m_split(capi.ptr(x), R, C, _at(y1) if which != 'y4' else None, _at(y4) if which != 'y1' else None,
+    b1, y1 = guarded(R * 2 * C, F16, device=DEV)
+    b4, y4 = guarded(R * 2 * C, F16, device=DEV)
+    capi.check(capi.lib().r3dp_a2m_split(capi.ptr(x), R, C, at(y1) if which != 'y4' else None, at(y4) if which != 'y1' else None,
                                          capi.stream()))
     torch.cuda.synchronize()
-    hi, lo = _split(x)
-    assert _guards_intact(b1) and _guards_intact(b4)
+    hi, lo = split(x)
+    assert guards_intact(b1, y1.numel()) and guards_intact(b4, y4.numel())
     if which != 'y4':
         assert torch.equal(y1.view(R, 2 * C), torch.cat([hi, lo], 1))
     else:
-        assert bool(_untouched(y1).all())
+        assert bool(untouched(y1).all())
     if which != 'y1':
         assert torch.equal(y4.view(R // 4, 8 * C), torch.cat([hi.reshape(R // 4, 4 * C), lo.reshape(R // 4, 4 * C)], 1))
     else:
-        assert bool(_untouched(y4).all())
+        assert bool(untouched(y4).all())
 
 
 @torch.no_grad()
@@ -327,13 +277,13 @@ def test_split_exact(which, R, C):
 @pytest.mark.parametrize('B,T4', [(1, 1), (3, 129), (4, 3750)])
 def test_latent_exact(temperature, B, T4):
     z = torch.randn(B, 16, T4, generator=torch.Generator().manual_seed(B * T4), device='cpu').to(DEV)
-    buf, y = _guarded(B * T4 * 64, F16)
-    capi.check(capi.lib().r3dp_a2m_latent(capi.ptr(z), B, T4, temperature, _at(y), capi.stream()))
+    buf, y = guarded(B * T4 * 64, F16, device=DEV)
+    capi.check(capi.lib().r3dp_a2m_latent(capi.ptr(z), B, T4, temperature, at(y), capi.stream()))
     torch.cuda.synchronize()
     v = torch.zeros(B * T4, 32, device=DEV)
     v[:, :16] = (z * torch.tensor(temperature, dtype=F32, device=DEV)).transpose(1, 2).reshape(B * T4, 16)
-    hi, lo = _split(v)
-    assert _guards_intact(buf)
+    hi, lo = split(v)
+    assert guards_intact(buf, y.numel())
     yv = y.view(B * T4, 64)
     assert torch.equal(yv, torch.cat([hi, lo], 1)) and bool((yv[:, 16:32] == 0).all()) and bool((yv[:, 48:] == 0).all())
 
@@ -346,32 +296,15 @@ def test_store_exact(masked, ld, N):
     g = torch.Generator().manual_seed(N + ld)
     x = torch.randn(N, 64, generator=g).to(DEV)
     mask = (torch.rand(N, generator=g) < 0.8).float().to(DEV) if masked else None
-    buf, out = _guarded(N * ld, F32)
-    capi.check(capi.lib().r3dp_a2m_store(capi.ptr(x), capi.ptr(mask), N, 64, _at(out), ld, capi.stream()))
+    buf, out = guarded(N * ld, F32, device=DEV)
+    capi.check(capi.lib().r3dp_a2m_store(capi.ptr(x), capi.ptr(mask), N, 64, at(out), ld, capi.stream()))
     torch.cuda.synchronize()
     ov = out.view(N, ld)
-    assert _guards_intact(buf) and bool(_untouched(ov[:, 64:]).all())
+    assert guards_intact(buf, out.numel()) and bool(untouched(ov[:, 64:]).all())
     assert torch.equal(ov[:, :64], x * mask[:, None] if masked else x)
 
 
 # ---- the recorded launches -----------------------------------------------------------------------------------------------------------------
-class _Recorder:
-    """Stands in for the library object: records the arguments of every entry point the forward calls and passes each call on unchanged."""
-
-    def __init__(self, lib):
-        self.lib, self.calls = lib, []
-
-    def __getattr__(self, name):
-        fn = getattr(self.lib, name)
-        if not (name.startswith('r3dp_a2m_') or name == 'r3dp_mf_conv3d'):
-            return fn
-
-        def call(*args):
-            self.calls.append((name, args))
-            return fn(*args)
-        return call
-
-
 def _has_row(fn, a):
     """Whether a launch (entry point, non-pointer arguments) has a float64 row here or in test_gpu_audio2motion_kernels.py."""
     import test_gpu_audio2motion_kernels as kern
@@ -392,29 +325,25 @@ def _has_row(fn, a):
 
 
 @torch.no_grad()
-def test_forward_launches_have_rows(models, monkeypatch):
-    rec = _Recorder(capi.lib())
-    monkeypatch.setattr(capi, '_lib', rec)
+def test_forward_launches_have_rows(models):
     launched, missing = {}, []
-    for kind, A, B, Tx in PLANS:
-        m = models[(kind, A)][0]
-        batch = {k: v.to(DEV) for k, v in ref.make_batch(B, Tx, A, seed=Tx, pitch=kind == 'pitch').items()}
-        rec.calls.clear()
-        m(batch, {}, temperature=0.2)
-        got = [signature(n, a) for n, a in rec.calls]
-        want = [ref.launch_signature(f, a) for _, f, a in ref.launch_plan(kind, A, B, Tx, temperature=0.2)]
-        label = _label(kind, A, B, Tx)
-        assert got == want, f'{label}: the module launches ' + '; '.join(f'{x}' for x in got if x not in want) + \
-            ' not in launch_plan, which has ' + '; '.join(f'{x}' for x in want if x not in got)
-        if kind == 'pitch':
-            assert len(got) == 42
-        for fn, a in got:
-            launched.setdefault((fn, a), label)
-            if not _has_row(fn, a):
-                missing.append(f'{label}: {fn}{a}')
-    torch.cuda.synchronize()
-    assert not missing, 'launches without a float64 row:\n' + '\n'.join(missing)
+    with Recorder(capi.lib(), lambda n: n.startswith('r3dp_a2m_') or n == 'r3dp_mf_conv3d') as rec:
+        for kind, A, B, Tx in PLANS:
+            m = models[(kind, A)][0]
+            batch = {k: v.to(DEV) for k, v in ref.make_batch(B, Tx, A, seed=Tx, pitch=kind == 'pitch').items()}
+            rec.calls.clear()
+            m(batch, {}, temperature=0.2)
+            got = [call_signature(n, a) for n, a in rec.calls]
+            label = _label(kind, A, B, Tx)
+            assert_plan(got, [ref.launch_signature(f, a) for _, f, a in ref.launch_plan(kind, A, B, Tx, temperature=0.2)], label)
+            if kind == 'pitch':
+                assert len(got) == 42
+            for fn, a in got:
+                launched.setdefault((fn, a), label)
+                if not _has_row(fn, a):
+                    missing.append(f'{label}: {fn}{a}')
+        torch.cuda.synchronize()
     largest = _label(*LARGEST)
     rows = {ref.launch_signature(f, a) for _, f, a in ref.launch_plan(*LARGEST[:2], *LARGEST[2:]) if f == 'r3dp_mf_conv3d'}
     stale = [f'{CONV3D[k][2]}: {k}' for k in CONV3D if (k in rows or CONV3D[k][3] == largest) and k not in launched]
-    assert not stale, f'rows the {largest} forward no longer launches:\n' + '\n'.join(stale)
+    assert_rows(missing, stale, f'the {largest} forward')

@@ -13,26 +13,16 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
 import hubert_reference as hr  # noqa: E402
+from launch_harness import guarded, guards_intact  # noqa: E402
 from real3dportrait_b200 import _capi as capi  # noqa: E402
 from real3dportrait_b200 import hubert as hb  # noqa: E402
 from real3dportrait_b200 import HubertModel, get_hubert_from_16k_speech, hubert_frames  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-GUARD = 4096
 LARGE = dict(conv_dim=(512,) * 7, hidden_size=1024, num_attention_heads=16, intermediate_size=4096, num_hidden_layers=24,
              num_conv_pos_embeddings=128, num_conv_pos_embedding_groups=16, feat_extract_norm='layer', do_stable_layer_norm=True,
              conv_bias=True)
-
-
-def guarded(n, dtype, fill):
-    buf = torch.full((n + 2 * GUARD,), fill, dtype=dtype, device=DEV)
-    return buf, buf[GUARD:GUARD + n]
-
-
-def check_guards(buf, fill):
-    g = torch.cat([buf[:GUARD], buf[-GUARD:]])
-    assert bool((g == fill).all()) if not np.isnan(fill) else bool(g.isnan().all())
 
 
 def split_rows(x):
@@ -89,22 +79,22 @@ def test_gemm(case, M):
     if epi in (0, 1):
         if epi == 1:
             ref = hr.gelu(ref)
-        buf, y = guarded(M * 2 * N, torch.float16, -7.0)
+        buf, y = guarded(M * 2 * N, torch.float16, fill=-7.0, device=DEV)
         run_gemm(Arows, M, width, stride, seg, wp, N, K, bias, epi, y, 2 * N, N)
         torch.cuda.synchronize()
         y = y.view(M, 2 * N)
         got = y[:, :N].double() + y[:, N:].double()
-        check_guards(buf, -7.0)
+        assert guards_intact(buf, y.numel(), fill=-7.0)
     else:
         init = torch.randn(M, N, device=DEV) if epi == 2 else None
-        buf, y = guarded(M * N, torch.float32, float('nan') if epi == 3 else 0.0)
+        buf, y = guarded(M * N, torch.float32, fill=float('nan') if epi == 3 else 0.0, device=DEV)
         if epi == 2:
             y.copy_(init.view(-1))
             ref = ref + init.double()
         run_gemm(Arows, M, width, stride, seg, wp, N, K, bias, epi, y, N, 0)
         torch.cuda.synchronize()
         got = y.view(M, N).double()
-        check_guards(buf, float('nan') if epi == 3 else 0.0)
+        assert guards_intact(buf, y.numel(), fill=float('nan') if epi == 3 else 0.0)
     bar = 2.0 ** -17 * mag * (1.8 if epi == 1 else 1.0) + 2.0 ** -20 * ref.abs() + 1e-30
     ratio = float(((got - ref).abs() / bar).max())
     print(f'gemm {case} M={M}: worst err/bar {ratio:.3f}')
@@ -149,12 +139,12 @@ def test_attention(segs):
     torch.manual_seed(len(segs))
     x = torch.randn(R, 3 * H, device=DEV) * 2.0
     qkv, _ = split_rows(x)
-    buf, o = guarded(R * 2 * H, torch.float16, -7.0)
+    buf, o = guarded(R * 2 * H, torch.float16, fill=-7.0, device=DEV)
     lens = (ctypes.c_int * len(segs))(*segs)
     capi.check(capi.lib().r3dp_hb_attention(capi.ptr(qkv, torch.float16), R, 6 * H, 3 * H, 16, lens, len(segs), ctypes.c_void_p(o.data_ptr()),
                                             2 * H, H, capi.stream()))
     torch.cuda.synchronize()
-    check_guards(buf, -7.0)
+    assert guards_intact(buf, o.numel(), fill=-7.0)
     o = o.view(R, 2 * H)
     got = o[:, :H].double() + o[:, H:].double()
     ref, mag = attention_ref(qkv, segs, H)

@@ -19,24 +19,14 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
 import audio2motion_reference as a2m  # noqa: E402
 import hubert_reference as hr  # noqa: E402
+from launch_harness import guarded, guards_intact  # noqa: E402
 from real3dportrait_b200 import _capi as capi  # noqa: E402
 from real3dportrait_b200 import hubert as hb  # noqa: E402
 from real3dportrait_b200 import HubertModel, PitchContourVAEModel, get_hubert_from_16k_speech, hubert_frames  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-GUARD = 4096
 LN_REL = 3e-5
-
-
-def guarded(n, dtype, fill):
-    buf = torch.full((n + 2 * GUARD,), fill, dtype=dtype, device=DEV)
-    return buf, buf[GUARD:GUARD + n]
-
-
-def guards_ok(buf, fill):
-    g = torch.cat([buf[:GUARD], buf[-GUARD:]])
-    return bool(g.isnan().all()) if np.isnan(fill) else bool((g == fill).all())
 
 
 def split_value(y, C, lo):
@@ -59,10 +49,10 @@ def ln_bar(z, g, b, u, gelu):
 @pytest.mark.parametrize('L', [400, 100003, 3000001])
 def test_stats(L):
     x = (torch.from_numpy(hr.wave(L)) * 0.8 + 0.05).to(DEV)
-    buf, st = guarded(2, torch.float64, float('nan'))
+    buf, st = guarded(2, torch.float64, fill=float('nan'), device=DEV)
     capi.check(capi.lib().r3dp_hb_stats(capi.ptr(x), L, ctypes.c_void_p(st.data_ptr()), capi.stream()))
     torch.cuda.synchronize()
-    assert guards_ok(buf, float('nan'))
+    assert guards_intact(buf, st.numel(), fill=float('nan'))
     xd = x.double()
     mean, var = xd.mean(), xd.var(unbiased=False)
     assert abs(float(st[0] - mean)) <= 1e-13 * float(xd.abs().max())
@@ -81,11 +71,11 @@ def test_conv0(C, F):
     gam = (1 + 0.3 * torch.randn(C, generator=g)).to(DEV)
     bet = (0.2 * torch.randn(C, generator=g)).to(DEV)
     lo = C + 64
-    buf, y = guarded(F * (2 * C + 128), torch.float16, -7.0)
+    buf, y = guarded(F * (2 * C + 128), torch.float16, fill=-7.0, device=DEV)
     capi.check(capi.lib().r3dp_hb_conv0(capi.ptr(x), capi.ptr(stats, torch.float64), F, C, capi.ptr(w), capi.ptr(bias), capi.ptr(gam),
                                         capi.ptr(bet), 1e-5, ctypes.c_void_p(y.data_ptr()), 2 * C + 128, lo, capi.stream()))
     torch.cuda.synchronize()
-    assert guards_ok(buf, -7.0)
+    assert guards_intact(buf, y.numel(), fill=-7.0)
     y = y.view(F, 2 * C + 128)
     assert bool((y[:, C:lo] == -7.0).all()) and bool((y[:, lo + C:] == -7.0).all())      # the columns between the halves are not written
     xd = x.double()
@@ -115,31 +105,31 @@ def test_layernorm(mode, C, R):
     L = capi.lib()
     if mode.endswith('split'):
         ys, lo = 2 * C + 64, C + 32
-        buf, y = guarded(R * ys, torch.float16, -7.0)
+        buf, y = guarded(R * ys, torch.float16, fill=-7.0, device=DEV)
         capi.check(L.r3dp_hb_layernorm(capi.ptr(x), R, C, capi.ptr(gam), capi.ptr(bet), 1e-5, int(gelu), None, 0, ctypes.c_void_p(y.data_ptr()),
                                        ys, lo, capi.stream()))
         torch.cuda.synchronize()
-        assert guards_ok(buf, -7.0)
+        assert guards_intact(buf, y.numel(), fill=-7.0)
         y = y.view(R, ys)
         assert bool((y[:, C:lo] == -7.0).all()) and bool((y[:, lo + C:] == -7.0).all())
         got = split_value(y, C, lo)
     elif mode.endswith('strided'):
         ys = C + 40
-        buf, y = guarded(R * ys, torch.float32, float('nan'))
+        buf, y = guarded(R * ys, torch.float32, fill=float('nan'), device=DEV)
         capi.check(L.r3dp_hb_layernorm(capi.ptr(x), R, C, capi.ptr(gam), capi.ptr(bet), 1e-5, int(gelu), ctypes.c_void_p(y.data_ptr()), ys, None,
                                        0, 0, capi.stream()))
         torch.cuda.synchronize()
-        assert guards_ok(buf, float('nan'))
+        assert guards_intact(buf, y.numel(), fill=float('nan'))
         y = y.view(R, ys)
         assert bool(y[:, C:].isnan().all())
         got = y[:, :C].double()
     else:                                                                              # in place, as the feature projection's input runs
-        buf, y = guarded(R * C, torch.float32, float('nan'))
+        buf, y = guarded(R * C, torch.float32, fill=float('nan'), device=DEV)
         y.copy_(x.view(-1))
         capi.check(L.r3dp_hb_layernorm(ctypes.c_void_p(y.data_ptr()), R, C, capi.ptr(gam), capi.ptr(bet), 1e-5, int(gelu),
                                        ctypes.c_void_p(y.data_ptr()), C, None, 0, 0, capi.stream()))
         torch.cuda.synchronize()
-        assert guards_ok(buf, float('nan'))
+        assert guards_intact(buf, y.numel(), fill=float('nan'))
         got = y.view(R, C).double()
     bar = ln_bar(z, None if gam is None else gam.double(), None if bet is None else bet.double(), u, gelu)
     ratio = float(((got - ref).abs() / bar).max())
@@ -162,14 +152,14 @@ def test_pos_conv(H, nseg, Lseg, M):
     W = (wp[:, :8192].double() + wp[:, 8192:].double()) / 1024.0                      # [H, 128 * 64], K = tap-major
     W3 = W.view(H, 128, 64).permute(0, 2, 1).contiguous()                              # back to [H, 64, 128]
     bias = (0.1 * torch.randn(H, generator=g)).to(DEV)
-    buf, y = guarded(M * H + 3 * H, torch.float32, 0.0)
+    buf, y = guarded(M * H + 3 * H, torch.float32, fill=0.0, device=DEV)
     init = torch.randn(M, H, generator=g).to(DEV)
     y[:M * H].copy_(init.view(-1))
     y[M * H:].fill_(-3.0)                                                              # rows past M: not written
     capi.check(capi.lib().r3dp_hb_pos_conv(capi.ptr(xs, torch.float16), nseg, Lseg, M, H, capi.ptr(wp, torch.float16), capi.ptr(bias),
                                            ctypes.c_void_p(y.data_ptr()), capi.stream()))
     torch.cuda.synchronize()
-    assert guards_ok(buf, 0.0) and bool((y[M * H:] == -3.0).all())
+    assert guards_intact(buf, y.numel(), fill=0.0) and bool((y[M * H:] == -3.0).all())
     pre, mag = [], []
     for s in range(nseg):
         seg = X[s * Lseg:min((s + 1) * Lseg, M)]

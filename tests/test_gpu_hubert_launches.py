@@ -27,6 +27,8 @@ import torch.nn.functional as Fn
 import hubert_reference as hr
 import test_gpu_hubert as tgh
 import test_gpu_hubert_kernels as kern
+from launch_harness import (Recorder, assert_plan, assert_rows, assert_written, at, call_signature, guarded, guards_intact, hi_w, inside, split,
+                            untouched)
 from real3dportrait_b200 import _capi as capi
 from real3dportrait_b200 import hubert as hb
 from real3dportrait_b200 import get_hubert_from_16k_speech
@@ -37,8 +39,6 @@ F16, F32, F64 = torch.float16, torch.float32, torch.float64
 CFG = {'large': hr.LARGE, 'small': hr.small_config()}
 PLANS = [('large', T) for T in (1, 49, 1031, 4000, 4001)] + [('small', T) for T in (1, 49, 1031, 4001)]
 FORWARD_LX = 320 * 48 + 400 + 11                        # HubertModel.forward input length: T = 49, the rows of the T = 49 plans
-GUARD = 4096
-SENT16, SENT32 = 0x7E55, 0x7FC01234                      # NaN payloads no kernel writes
 GELU_LIP = 1.13
 ONE_ROW_DRAWS = 32
 
@@ -65,34 +65,6 @@ TABLES = {'r3dp_hb_gemm': GEMM, 'r3dp_hb_attention': ATTN, 'r3dp_hb_layernorm': 
 
 def _ids(table):
     return [f'{v[2]}-{v[1].split(".", 1)[1]}-' + 'x'.join(str(a) for a in k[1] if not isinstance(a, (tuple, float))) for k, v in table.items()]
-
-
-# ---- guarded buffers ---------------------------------------------------------------------------------------------------------------------
-def guarded(n, dt):
-    buf = torch.empty(n + 2 * GUARD, device=DEV, dtype=dt)
-    buf.view(torch.int16 if dt == F16 else torch.int32).fill_(SENT16 if dt == F16 else SENT32)
-    return buf, buf[GUARD:GUARD + n]
-
-
-def untouched(t):
-    return t.view(torch.int16) == SENT16 if t.dtype == F16 else t.view(torch.int32) == SENT32
-
-
-def guards_intact(buf):
-    return bool(untouched(buf[:GUARD]).all()) and bool(untouched(buf[-GUARD:]).all())
-
-
-def at(t, elems=0):
-    return ctypes.c_void_p(t.data_ptr() + t.element_size() * elems)
-
-
-def split(v):
-    hi = v.half()
-    return hi, (v - hi.float()).half()
-
-
-def hi_w(w):
-    return (w * 1024.0).half().double() / 1024.0
 
 
 def randn(shape, seed, scale=1.0):
@@ -179,9 +151,9 @@ def _gemm_draw(models, key, site, seed):
     mag = X.abs() @ W64.abs().t()
     pre_hx, pre_hw = Xh @ W64.t() + b64, X @ hi_w(W64).t() + b64
     if epi in (0, 1):
-        buf, y = guarded(M * ldy, F16)
+        buf, y = guarded(M * ldy, F16, device=DEV)
     else:
-        buf, y = guarded(M * ldy + 64 * ldy, F32)                             # + 64 rows past M
+        buf, y = guarded(M * ldy + 64 * ldy, F32, device=DEV)                 # + 64 rows past M
     yv = y[:M * ldy].view(M, ldy)
     init = None
     if epi == 2:
@@ -190,18 +162,16 @@ def _gemm_draw(models, key, site, seed):
     capi.check(capi.lib().r3dp_hb_gemm(at(A), M, width, stride, seg, capi.ptr(wp, F16), N, Kp, capi.ptr(bias), epi, at(y), ldy, ylo,
                                        capi.stream()))
     torch.cuda.synchronize()
-    assert guards_intact(buf), f'{what}: written outside the output'
-    inside = torch.zeros(ldy, dtype=torch.bool, device=DEV)
-    inside[:N] = True
+    assert guards_intact(buf, y.numel()), f'{what}: written outside the output'
+    mask = inside(ldy, 0, N, ylo, epi in (0, 1), device=DEV)
     if epi in (0, 1):
-        inside[ylo:ylo + N] = True
         got = yv[:, :N].double() + yv[:, ylo:ylo + N].double()
     else:
         got = yv[:, :N].double()
         assert bool(untouched(y[M * ldy:]).all()), f'{what}: rows past M written'
     if epi != 2:
-        assert not bool(untouched(yv[:, inside]).any()), f'{what}: an output element was not written'
-        assert bool(untouched(yv[:, ~inside]).all()), f'{what}: written outside the output halves'
+        assert not bool(untouched(yv[:, mask]).any()), f'{what}: an output element was not written'
+        assert bool(untouched(yv[:, ~mask]).all()), f'{what}: written outside the output halves'
     else:
         assert torch.equal(yv[:, N:], init[:, N:]), f'{what}: residual columns past N changed'
     if epi == 1:
@@ -242,14 +212,10 @@ def test_attention_launch(key):
     what = f'{label} {tag} lens {lens[:4]}'
     x = randn((rows, 3 * H), list(ATTN).index(key) + 50, 2.0)
     qkv = torch.cat(split(x), 1).contiguous()
-    buf, o = guarded(rows * os_, F16)
+    buf, o = guarded(rows * os_, F16, device=DEV)
     attention(at(qkv), rows, H, heads, lens, at(o), os_, olo)
-    torch.cuda.synchronize()
-    assert guards_intact(buf)
+    assert_written(buf, o, os_, inside(os_, 0, H, olo, True, device=DEV), what)
     ov = o.view(rows, os_)
-    inside = torch.zeros(os_, dtype=torch.bool, device=DEV)
-    inside[:H] = inside[olo:olo + H] = True
-    assert bool(untouched(ov[:, ~inside]).all()) and not bool(untouched(ov[:, inside]).any()), f'{what}: output columns'
     got = ov[:, :H].double() + ov[:, olo:olo + H].double()
     want, mag = attention64(qkv, lens, H)
     bar = 2.0 ** -17 * mag + 2.0 ** -20 * want.abs()
@@ -268,10 +234,10 @@ def test_attention_launch(key):
     assert ratio <= 1.0, f'{what}: err/bar {ratio:.3f}'
     assert mh > 1.0, f'{what}: the bar does not see hi-only q, k, v'
     last = lens[-1]
-    obuf, one = guarded(last * os_, F16)
+    obuf, one = guarded(last * os_, F16, device=DEV)
     attention(at(qkv, (rows - last) * 6 * H), last, H, heads, (last,), at(one), os_, olo)
     torch.cuda.synchronize()
-    assert guards_intact(obuf)
+    assert guards_intact(obuf, one.numel())
     assert torch.equal(one.view(torch.int16), o[(rows - last) * os_:].view(torch.int16)), f'{what}: the last segment vs a launch on it alone'
 
 
@@ -296,23 +262,21 @@ def test_layernorm_launch(models, key):
     want = hr.gelu(u) if gelu else u
     inplace = yfs and site.startswith('conv')
     if yhs:
-        buf, y = guarded(R * yhs, F16)
+        buf, y = guarded(R * yhs, F16, device=DEV)
         capi.check(capi.lib().r3dp_hb_layernorm(capi.ptr(x), R, C, capi.ptr(g), capi.ptr(b), eps, gelu, None, 0, at(y), yhs, yhlo,
                                                 capi.stream()))
-        inside = torch.zeros(yhs, dtype=torch.bool, device=DEV)
-        inside[:C] = inside[yhlo:yhlo + C] = True
+        mask = inside(yhs, 0, C, yhlo, True, device=DEV)
     else:
-        buf, y = guarded(R * yfs, F32)
+        buf, y = guarded(R * yfs, F32, device=DEV)
         if inplace:
             y.view(R, yfs)[:, :C].copy_(x)
         src = at(y) if inplace else capi.ptr(x)
         capi.check(capi.lib().r3dp_hb_layernorm(src, R, C, capi.ptr(g), capi.ptr(b), eps, gelu, at(y), yfs, None, 0, 0, capi.stream()))
-        inside = torch.zeros(yfs, dtype=torch.bool, device=DEV)
-        inside[:C] = True
+        mask = inside(yfs, 0, C, device=DEV)
     torch.cuda.synchronize()
-    assert guards_intact(buf), f'{what}: written outside the output'
+    assert guards_intact(buf, y.numel()), f'{what}: written outside the output'
     yv = y.view(R, -1)
-    assert bool(untouched(yv[:, ~inside]).all()), f'{what}: written between or past the output halves'
+    assert bool(untouched(yv[:, ~mask]).all()), f'{what}: written between or past the output halves'
     got = yv[:, :C].double() + (yv[:, yhlo:yhlo + C].double() if yhs else 0.0)
     ratio = float(((got - want).abs() / kern.ln_bar(z, None if g is None else g.double(), None if b is None else b.double(), u, gelu)).max())
     print(f'layernorm {what} R={R} C={C}: worst err/bar {ratio:.3f}')
@@ -331,15 +295,13 @@ def test_conv0_launch(models, key):
     x = (torch.from_numpy(hr.wave(n + 7)) * 1.3 - 0.2).to(DEV)[:n]
     xd = x.double()
     stats = torch.stack([xd.mean(), 1.0 / torch.sqrt(xd.var(unbiased=False) + 1e-7)])
-    buf, y = guarded(F * ys, F16)
+    buf, y = guarded(F * ys, F16, device=DEV)
     capi.check(capi.lib().r3dp_hb_conv0(capi.ptr(x), capi.ptr(stats, F64), F, C, capi.ptr(w0), capi.ptr(b0), capi.ptr(g0), capi.ptr(be0), eps,
                                         at(y), ys, ylo, capi.stream()))
     torch.cuda.synchronize()
-    assert guards_intact(buf)
+    assert guards_intact(buf, y.numel())
     yv = y.view(F, ys)
-    inside = torch.zeros(ys, dtype=torch.bool, device=DEV)
-    inside[:C] = inside[ylo:ylo + C] = True
-    assert bool(untouched(yv[:, ~inside]).all()), f'{label}: written between or past the halves'
+    assert bool(untouched(yv[:, ~inside(ys, 0, C, ylo, True, device=DEV)]).all()), f'{label}: written between or past the halves'
     win = ((xd - stats[0]) * stats[1]).unfold(0, 10, 5)
     pre = win @ w0.double().t() + b0.double()
     z, u = kern.ln64(pre, g0.double(), be0.double(), eps)
@@ -370,12 +332,12 @@ def test_pos_conv_launch(models, key):
     xs = torch.zeros(nseg * Ls, 2 * H, device=DEV, dtype=F16)              # rows past M: zero, as the module allocates them
     xs[:M, :H], xs[:M, H:] = split(xv)
     X = xs[:M, :H].double() + xs[:M, H:].double()
-    buf, y = guarded(M * H + 64 * H, F32)
+    buf, y = guarded(M * H + 64 * H, F32, device=DEV)
     init = randn((M, H), seed + 1)
     y[:M * H].copy_(init.view(-1))
     capi.check(capi.lib().r3dp_hb_pos_conv(capi.ptr(xs, F16), nseg, Ls, M, H, capi.ptr(wp, F16), capi.ptr(bias), at(y), capi.stream()))
     torch.cuda.synchronize()
-    assert guards_intact(buf) and bool(untouched(y[M * H:]).all()), f'{label}: written past row M'
+    assert guards_intact(buf, y.numel()) and bool(untouched(y[M * H:]).all()), f'{label}: written past row M'
     pre = _pos64(X, W3, H, nseg, Ls, M) + b64
     mag = _pos64(X.abs(), W3.abs(), H, nseg, Ls, M)
     want = init.double() + hr.gelu(pre)
@@ -396,11 +358,11 @@ def test_split_launch(key):
     R, H = key[1]
     x = randn((R, H), R + H, 3.0)
     rows = (R + 999) // 1000 * 1000
-    buf, y = guarded(rows * 2 * H, F16)
+    buf, y = guarded(rows * 2 * H, F16, device=DEV)
     y.zero_()
     capi.check(capi.lib().r3dp_a2m_split(capi.ptr(x), R, H, at(y), None, capi.stream()))
     torch.cuda.synchronize()
-    assert guards_intact(buf)
+    assert guards_intact(buf, y.numel())
     yv = y.view(rows, 2 * H)
     assert torch.equal(yv[:R], torch.cat(split(x), 1)) and bool((yv[R:] == 0).all())
 
@@ -414,34 +376,22 @@ def _has_row(fn, a):
     return (fn, a) in TABLES.get(fn, {})
 
 
-PTR = capi.ptr
-
-
-class _Recorder:
-    """Stands in for the library object: records every r3dp_hb_* and r3dp_a2m_split call as its signature (attention's segment lengths
-    copied out of their ctypes array) and passes each call on unchanged."""
+class _HubertCalls(Recorder):
+    """Records every r3dp_hb_* and r3dp_a2m_split call as its signature (attention's segment lengths copied out of their ctypes array), with
+    capi.ptr wrapped so that the split operands they read can be looked at."""
 
     def __init__(self, lib):
-        self.lib, self.calls, self.tensors, self.dead = lib, [], {}, []
-
-    def ptr(self, t, *a, **k):
-        """capi.ptr, remembering which tensor each pointer the module passes belongs to."""
-        if t is not None:
-            self.tensors[t.data_ptr()] = t
-        return PTR(t, *a, **k)
+        super().__init__(lib, lambda n: n.startswith('r3dp_hb_') or n == 'r3dp_a2m_split', ptrs=True)
+        self.dead = []
 
     def check_lo(self, name, args):
         """A split operand [rows, hi | lo] that a GEMM, attention or positional-conv launch reads: where |hi| >= 1/4 the lo half is a normal
         fp16 and zero only when the fp32 value is fp16-exact (about 2^-13 of values), so an operand written without its lo halves shows as
         zeros.  (Smaller values, e.g. GELU's tails, have lo halves that underflow to zero.)"""
-        if name == 'r3dp_hb_gemm':
-            t, half = self.tensors[args[0].value], args[4]
-        elif name == 'r3dp_hb_attention':
-            t, half = self.tensors[args[0].value], args[3]
-        elif name == 'r3dp_hb_pos_conv':
-            t, half = self.tensors[args[0].value], args[4]
-        else:
+        half = {'r3dp_hb_gemm': 4, 'r3dp_hb_attention': 3, 'r3dp_hb_pos_conv': 4}.get(name)
+        if half is None:
             return
+        t, half = self.tensor(args[0].value), args[half]
         torch.cuda.synchronize()
         t = t.view(t.shape[0], -1)
         hi, lo = t[:, :half], t[:, half:2 * half]
@@ -450,53 +400,40 @@ class _Recorder:
         if frac > 0.01:
             self.dead.append(f'{name}: {frac:.1%} of the operand\'s lo halves are zero')
 
-    def __getattr__(self, name):
-        fn = getattr(self.lib, name)
-        if not (name.startswith('r3dp_hb_') or name == 'r3dp_a2m_split'):
-            return fn
-        types = capi._SIGNATURES[name][1]
-
-        def call(*args):
-            self.check_lo(name, args)
-            a = [x for x, t in zip(args, types) if t is not capi._P]
-            if name == 'r3dp_hb_attention':
-                a[4] = tuple(a[4][i] for i in range(a[5]))
-            self.calls.append(hr.launch_signature(name, a))
-            return fn(*args)
-        return call
+    def record(self, name, args):
+        self.check_lo(name, args)
+        fn, a = call_signature(name, args)
+        if name == 'r3dp_hb_attention':
+            a = a[:4] + (tuple(a[4][i] for i in range(a[5])),) + a[5:]
+        return fn, a
 
 
 @torch.no_grad()
-def test_launches_have_rows(models, monkeypatch):
-    rec = _Recorder(capi.lib())
-    monkeypatch.setattr(capi, '_lib', rec)
-    monkeypatch.setattr(capi, 'ptr', rec.ptr)
+def test_launches_have_rows(models):
     launched, missing = set(), []
     runs = [(name, T, None) for name, T in PLANS] + [(name, None, 2) for name in CFG]
-    for name, T, B in runs:
-        m = models[name][0]
-        rec.calls.clear()
-        if B is None:
-            get_hubert_from_16k_speech(hr.wave(clip(T)), m)
-            want = hr.launch_plan(CFG[name], clip(T))
-            label = f'{name}-T{T}'
-        else:
-            m(randn((B, FORWARD_LX), 5))
-            want = hr.launch_plan(CFG[name], FORWARD_LX, B=B)
-            label = f'{name}-forward-B{B}'
-        want = [hr.launch_signature(f, a) for _, f, a in want]
-        got = rec.calls[:]
-        assert got == want, f'{label}: the module launches ' + '; '.join(f'{x}' for x in got if x not in want) + \
-            ' not in launch_plan, which has ' + '; '.join(f'{x}' for x in want if x not in got)
-        if name == 'large' and B is None:
-            print(f'{label}: {len(got)} launches = 1 + 186 x {(len(got) - 1) // 186} groups')
-            assert (len(got) - 1) % 186 == 0
-        for fn, a in got:
-            launched.add((fn, a))
-            if not _has_row(fn, a):
-                missing.append(f'{label}: {fn}{a}')
-    torch.cuda.synchronize()
+    with _HubertCalls(capi.lib()) as rec:
+        for name, T, B in runs:
+            m = models[name][0]
+            rec.clear()
+            if B is None:
+                get_hubert_from_16k_speech(hr.wave(clip(T)), m)
+                want = hr.launch_plan(CFG[name], clip(T))
+                label = f'{name}-T{T}'
+            else:
+                m(randn((B, FORWARD_LX), 5))
+                want = hr.launch_plan(CFG[name], FORWARD_LX, B=B)
+                label = f'{name}-forward-B{B}'
+            got = rec.calls[:]
+            assert_plan(got, [hr.launch_signature(f, a) for _, f, a in want], label)
+            if name == 'large' and B is None:
+                print(f'{label}: {len(got)} launches = 1 + 186 x {(len(got) - 1) // 186} groups')
+                assert (len(got) - 1) % 186 == 0
+            for fn, a in got:
+                launched.add((fn, a))
+                if not _has_row(fn, a):
+                    missing.append(f'{label}: {fn}{a}')
+        torch.cuda.synchronize()
     assert not rec.dead, 'split operands without their lo halves:\n' + '\n'.join(rec.dead[:20])
-    assert not missing, 'launches without a float64 row:\n' + '\n'.join(missing)
     stale = [f'{fn}: {v[1]} {k}' for fn, table in TABLES.items() for k, v in table.items() if k not in launched]
-    assert not stale, 'rows no forward launches:\n' + '\n'.join(stale)
+    assert_rows(missing, stale, 'the forwards')

@@ -41,7 +41,7 @@ def _rand(shape, seed, dtype=F32, scale=1.0):
     return (torch.randn(shape, generator=_g(seed), device=DEV) * scale).to(dtype).contiguous()
 
 
-def _check(name, got, ref, S=None):
+def check_bar(name, got, ref, S=None):
     ref = ref.to(F64)
     S = float(ref.abs().max()) if S is None else S
     excess = (got.to(F64) - ref).abs() - ALPHA[got.dtype] * ref.abs()
@@ -88,7 +88,7 @@ def test_attention(B, Tq, Tk):
             kh = kv[b, :, h * 256:(h + 1) * 256].to(F64)
             vh = kv[b, :, C + h * 256:C + (h + 1) * 256].to(F64)
             ref = ((qh @ kh.T) / 16.0).softmax(-1) @ vh
-            _check(f'attention B{B} Tq{Tq} Tk{Tk} b{b} h{h}', got[b, :, h * 256:(h + 1) * 256], ref, S)
+            check_bar(f'attention B{B} Tq{Tq} Tk{Tk} b{b} h{h}', got[b, :, h * 256:(h + 1) * 256], ref, S)
 
 
 # R of every C = 1024 LayerNorm launch: LowResolutionViT (H/16)^2 B, TriplanePredictorViT queries (H/4)^2 B and sr keys (H/8)^2 B, at
@@ -106,8 +106,8 @@ def test_layernorm_1024(R):
     v = x.to(F64) + t.to(F64)
     ref = F.layer_norm(v, (C,), g.to(F64), b.to(F64), 1e-5)
     assert torch.equal(xo, x + t)
-    _check(f'layernorm R{R} yf', yf, ref)
-    _check(f'layernorm R{R} yh', yh[:, :C], ref)
+    check_bar(f'layernorm R{R} yf', yf, ref)
+    check_bar(f'layernorm R{R} yh', yh[:, :C], ref)
     assert torch.isnan(yh[:, C:]).all()
 
 
@@ -166,7 +166,7 @@ def test_channel_mean_and_broadcast(B, HW, C):
     v = _rand((B, Cb), 11, F16)
     capi.check(lib().r3dp_ip_broadcast(P(v, F16), B, HW, Cb, P(y, F16), ys, yc0, capi.stream()))
     torch.cuda.synchronize()
-    _check(f'mean B{B} HW{HW}', m[:B], x.to(F64).mean(1))
+    check_bar(f'mean B{B} HW{HW}', m[:B], x.to(F64).mean(1))
     assert torch.isnan(m[B]).all()
     assert torch.equal(y[..., yc0:], v[:, None, :].expand(B, HW, Cb))
     assert torch.isnan(y[..., :yc0]).all()
@@ -193,7 +193,7 @@ def test_upsample2(B, h, C):
     capi.check(lib().r3dp_ip_upsample2(P(x, F16), B, h, h, C, P(y, F16), capi.stream()))
     torch.cuda.synchronize()
     ref = F.interpolate(x.permute(0, 3, 1, 2).to(F64), scale_factor=2.0, mode='bilinear', align_corners=True).permute(0, 2, 3, 1).reshape(-1, C)
-    _check(f'upsample2 B{B} h{h}', y[:-1], ref)
+    check_bar(f'upsample2 B{B} h{h}', y[:-1], ref)
     assert torch.isnan(y[-1]).all()
 
 

@@ -31,6 +31,9 @@ import img2plane_reference as ref
 import sr_conv_reference as scr
 import test_gpu_img2plane_kernels as ikern
 import test_gpu_secc2plane_kernels as skern
+import test_gpu_sr_conv_conformance as srcc
+from launch_harness import (GUARD, Recorder, assert_plan, assert_rows, at, bits, call_signature, conv3d, given, guarded, guards_intact, inside,
+                            untouched)
 from real3dportrait_b200 import _capi as capi
 from real3dportrait_b200 import img2plane as ip
 from real3dportrait_b200.img2plane import Img2PlaneModel
@@ -41,8 +44,6 @@ F16, F32, F64 = torch.float16, torch.float32, torch.float64
 #: (H, B) of the standard-scale forwards the rows come from; RECORDED adds 64^2 at the other two scales
 PLAN_SIZES = [(512, 4), (512, 1), (144, 3), (32, 3), (16, 1)]
 RECORDED = [(H, B, 'standard') for H, B in PLAN_SIZES] + [(64, 1, 'small'), (64, 1, 'large')]
-SENTINEL = {F16: (torch.int16, 0x7E55), F32: (torch.int32, 0x7FC01234)}
-GUARD = 4096
 #: r3dp_mf_conv3d's beta per tap count (1: GEMMs on token / patch rows, 9: the (1,3,3) convs), about 2x the worst ratio over the rows on
 #: an H100 80GB HBM3 (700 W power limit, max SM clock 1980 MHz): GEMMs 8.44e-7 (144^2 tri.block1.sr, K = 4096, fp32 out; fp16 out
 #: 4.52e-7, layer4.0.conv2 at K = 4608), convs 5.23e-7 (512^2 B = 4 tri.final_conv, fp32 out; fp16 out 2.49e-7)
@@ -70,35 +71,11 @@ def _id(key):
     return label + '-' + 'x'.join(f'{v:g}' if isinstance(v, float) else str(v) for v in launch.args)
 
 
-def at(t, elems=0):
-    return ctypes.c_void_p(t.data_ptr() + t.element_size() * elems)
-
-
 def _gen(key):
     return torch.Generator(device=DEV).manual_seed(list(ROWS).index(key) + 900)
 
 
-def _guarded(n, dt, tail=GUARD):
-    buf = torch.empty(GUARD + n + tail, device=DEV, dtype=dt)
-    buf.view(SENTINEL[dt][0]).fill_(SENTINEL[dt][1])
-    return buf, buf[GUARD:GUARD + n]
-
-
-def _untouched(t):
-    return t.view(SENTINEL[t.dtype][0]) == SENTINEL[t.dtype][1]
-
-
-def _guards_intact(buf, n):
-    return bool(_untouched(buf[:GUARD]).all()) and bool(_untouched(buf[GUARD + n:]).all())
-
-
 # ---- r3dp_mf_conv3d ------------------------------------------------------------------------------------------------------------------------
-def _launch_conv3d(x, xc0, wp, bias, res, a, N, H, y):
-    xs, _, cin, _, D, _, W, kd, kh, kw, up, O, cop, relu, ys, yc0, ylo, f32, split = a
-    capi.check(capi.lib().r3dp_mf_conv3d(at(x, xc0), xs, 0, cin, P(wp, F16), P(bias), None if res is None else P(res, F16), N, D, H, W, kd, kh, kw,
-                                         up, O, cop, relu, at(y), ys, yc0, ylo, f32, split, capi.stream()))
-
-
 @torch.no_grad()
 @pytest.mark.parametrize('key', _keys('r3dp_mf_conv3d'), ids=_id)
 def test_conv3d_launch(key):
@@ -122,15 +99,14 @@ def test_conv3d_launch(key):
     r = torch.randn(M, O, generator=g, device=DEV).half() if has_res else None
     assert not has_res or ys == O
     dt = F32 if f32 else F16
-    buf, y = _guarded(M * ys, dt, max(GUARD, (cop - O) * ys))
-    _launch_conv3d(x, xc0, wp, bias, r, a, N, H, y)
+    buf, y = guarded(M * ys, dt, tail=max(GUARD, (cop - O) * ys), device=DEV)
+    conv3d(a, at(x, xc0), wp, bias, r, at(y))
     torch.cuda.synchronize()
-    assert _guards_intact(buf, M * ys), f'{label}: written past the output'
+    assert guards_intact(buf, M * ys), f'{label}: written past the output'
     yv = y.view(M, ys)
-    inside = torch.zeros(ys, dtype=torch.bool, device=DEV)
-    inside[yc0:yc0 + O] = True
-    assert not bool(_untouched(yv[:, inside]).any()), f'{label}: an output element was not written'
-    assert bool(_untouched(yv[:, ~inside]).all()), f'{label}: written outside the channel slice'
+    mask = inside(ys, yc0, O, device=DEV)
+    assert not bool(untouched(yv[:, mask]).any()), f'{label}: an output element was not written'
+    assert bool(untouched(yv[:, ~mask]).all()), f'{label}: written outside the channel slice'
     alpha = scr.ALPHA_F32 if f32 else scr.ALPHA_F16
     extra = None if f32 else 2 * scr.FLOOR_F16
     bv = bias[:O].double()
@@ -164,17 +140,17 @@ def test_conv3d_launch(key):
     print(f'conv3d {_id(key)}: worst excess / S = {worst:.3e} (beta {BETA[9 if box else 1]:.2e})')
     # bit-exact: the last image of a box conv equals its N = 1 launch, the last rows of a GEMM a launch on those rows alone
     if box and N > 1:
-        ob, one = _guarded(H * W * ys, dt)
-        _launch_conv3d(x[(N - 1) * H * W:].contiguous(), xc0, wp, bias, None if r is None else r[(N - 1) * H * W:].contiguous(), a, 1, H, one)
+        ob, one = guarded(H * W * ys, dt, device=DEV)
+        conv3d(a, at(x[(N - 1) * H * W:].contiguous(), xc0), wp, bias, None if r is None else r[(N - 1) * H * W:].contiguous(), at(one), N=1)
         torch.cuda.synchronize()
-        assert torch.equal(one.view(H * W, ys)[:, inside].view(SENTINEL[dt][0]), yv[-H * W:, inside].view(SENTINEL[dt][0])), \
+        assert torch.equal(bits(one.view(H * W, ys)[:, mask]), bits(yv[-H * W:, mask])), \
             f'{label}: the last image vs its N = 1 launch'
     elif not box:
         t = min(M, 300)
-        ob, tail = _guarded(t * ys, dt)
-        _launch_conv3d(x[M - t:].contiguous(), xc0, wp, bias, None if r is None else r[M - t:].contiguous(), a, 1, t, tail)
+        ob, tail = guarded(t * ys, dt, device=DEV)
+        conv3d(a, at(x[M - t:].contiguous(), xc0), wp, bias, None if r is None else r[M - t:].contiguous(), at(tail), N=1, H=t)
         torch.cuda.synchronize()
-        assert torch.equal(tail.view(t, ys)[:, inside].view(SENTINEL[dt][0]), yv[-t:, inside].view(SENTINEL[dt][0])), \
+        assert torch.equal(bits(tail.view(t, ys)[:, mask]), bits(yv[-t:, mask])), \
             f'{label}: the last {t} rows vs a launch on them alone'
 
 
@@ -190,17 +166,17 @@ def test_layernorm_launch(key):
     t = torch.randn(R, C, generator=g, device=DEV) * 0.5 if 't' in roles else None
     gam = 1 + 0.1 * torch.randn(C, generator=g, device=DEV)
     bet = 0.1 * torch.randn(C, generator=g, device=DEV)
-    xbuf, x = _guarded(R * C, F32)
+    xbuf, x = guarded(R * C, F32, device=DEV)
     x.copy_(x0.view(-1))
     outs = {}
     for role, dt in (('xo', F32), ('yf', F32), ('yh', F16)):
         if role in roles and not (role == 'xo' and inplace):
-            outs[role] = _guarded(R * C, dt)
+            outs[role] = guarded(R * C, dt, device=DEV)
     xo = x if inplace else outs.get('xo', (None, None))[1]
     capi.check(capi.lib().r3dp_sp_layernorm(P(x), P(t), R, C, P(gam), P(bet), eps, P(xo), P(outs.get('yf', (None, None))[1]),
                                             P(outs.get('yh', (None, None))[1], F16), ldyh, capi.stream()))
     torch.cuda.synchronize()
-    assert _guards_intact(xbuf, R * C), f'{label}: written around x'
+    assert guards_intact(xbuf, R * C), f'{label}: written around x'
     v = x0.double() + (0.0 if t is None else t.double())
     want = F.layer_norm(v, (C,), gam.double(), bet.double(), eps)
     if 'xo' in roles:
@@ -208,9 +184,9 @@ def test_layernorm_launch(key):
     else:
         assert torch.equal(x.view(R, C), x0), f'{label}: x changed without an xo'
     for role, (buf, y) in outs.items():
-        assert _guards_intact(buf, R * C) and not bool(_untouched(y).any()), f'{label} {role}: output not written exactly'
+        assert guards_intact(buf, R * C) and not bool(untouched(y).any()), f'{label} {role}: output not written exactly'
         if role != 'xo':
-            skern._check(f'sp_layernorm {label} {role}', y.view(R, C), want)
+            skern.check_bar(f'sp_layernorm {label} {role}', y.view(R, C), want)
 
 
 @torch.no_grad()
@@ -221,14 +197,14 @@ def test_dwconv_gelu_launch(key):
     g = _gen(key)
     x = torch.randn(B, h, w, C, generator=g, device=DEV).half()
     wt, b = 0.3 * torch.randn(C, 9, generator=g, device=DEV), 0.1 * torch.randn(C, generator=g, device=DEV)
-    buf, y = _guarded(B * h * w * C, F16)
+    buf, y = guarded(B * h * w * C, F16, device=DEV)
     capi.check(capi.lib().r3dp_sp_dwconv_gelu(P(x, F16), B, h, w, C, P(wt), P(b), P(y, F16), capi.stream()))
     torch.cuda.synchronize()
-    assert _guards_intact(buf, y.numel()) and not bool(_untouched(y).any()), f'{label}: output not written exactly'
+    assert guards_intact(buf, y.numel()) and not bool(untouched(y).any()), f'{label}: output not written exactly'
     y = y.view(B, h, w, C)
     for n in range(B):
         want = F.gelu(F.conv2d(x[n:n + 1].double().permute(0, 3, 1, 2), wt.double().view(C, 1, 3, 3), b.double(), 1, 1, groups=C))
-        skern._check(f'sp_dwconv_gelu {label} image {n}', y[n], want[0].permute(1, 2, 0))
+        skern.check_bar(f'sp_dwconv_gelu {label} image {n}', y[n], want[0].permute(1, 2, 0))
 
 
 @torch.no_grad()
@@ -236,15 +212,15 @@ def test_dwconv_gelu_launch(key):
 def test_leaky_launch(key):
     label, launch = ROWS[key]
     n, slope = launch.args
-    buf, y = _guarded(n, F16)
+    buf, y = guarded(n, F16, device=DEV)
     y.copy_(torch.randn(n, generator=_gen(key), device=DEV).half())
     want = F.leaky_relu(y.double(), slope)
     capi.check(capi.lib().r3dp_sp_leaky(P(y, F16), n, slope, capi.stream()))
     torch.cuda.synchronize()
-    assert _guards_intact(buf, n)
+    assert guards_intact(buf, n)
     if slope == 0.0:
         assert torch.equal(y.double(), want), f'{label}: ReLU is exact'
-    skern._check(f'sp_leaky {label}', y, want)
+    skern.check_bar(f'sp_leaky {label}', y, want)
 
 
 # ---- r3dp_ip_* -------------------------------------------------------------------------------------------------------------------------------
@@ -258,10 +234,10 @@ def test_attention_launch(key):
     g = _gen(key)
     q = torch.randn(B * Tq, qs, generator=g, device=DEV).half()
     kv = torch.randn(B * Tk, kvs, generator=g, device=DEV).half()
-    buf, o = _guarded(B * Tq * os_, F16)
+    buf, o = guarded(B * Tq * os_, F16, device=DEV)
     capi.check(capi.lib().r3dp_ip_attention(P(q, F16), qs, P(kv, F16), kvs, B, Tq, Tk, heads, scale, P(o, F16), os_, capi.stream()))
     torch.cuda.synchronize()
-    assert _guards_intact(buf, o.numel()) and not bool(_untouched(o).any()), f'{label}: output not written exactly'
+    assert guards_intact(buf, o.numel()) and not bool(untouched(o).any()), f'{label}: output not written exactly'
     o, q, kv = o.view(B, Tq, os_), q.view(B, Tq, qs), kv.view(B, Tk, kvs)
     S = float(kv[..., C:].abs().max())
     for b in range(B):
@@ -270,7 +246,7 @@ def test_attention_launch(key):
             qh, kh = q[b, :, cs].double(), kv[b, :, cs].double()
             vh = kv[b, :, C + hh * hd:C + (hh + 1) * hd].double()
             want = ((qh @ kh.T) * scale).softmax(-1) @ vh
-            ikern._check(f'attention {label} b{b} h{hh}', o[b, :, cs], want, S)
+            ikern.check_bar(f'attention {label} b{b} h{hh}', o[b, :, cs], want, S)
 
 
 @torch.no_grad()
@@ -279,11 +255,11 @@ def test_channel_mean_launch(key):
     label, launch = ROWS[key]
     B, HW, C = launch.args
     x = torch.randn(B, HW, C, generator=_gen(key), device=DEV).half()
-    buf, m = _guarded(B * C, F16)
+    buf, m = guarded(B * C, F16, device=DEV)
     capi.check(capi.lib().r3dp_ip_channel_mean(P(x, F16), B, HW, C, P(m, F16), capi.stream()))
     torch.cuda.synchronize()
-    assert _guards_intact(buf, m.numel())
-    ikern._check(f'mean {label}', m.view(B, C), x.double().mean(1))
+    assert guards_intact(buf, m.numel())
+    ikern.check_bar(f'mean {label}', m.view(B, C), x.double().mean(1))
 
 
 @torch.no_grad()
@@ -292,12 +268,12 @@ def test_broadcast_launch(key):
     label, launch = ROWS[key]
     B, HW, Cb, ys, yc0 = launch.args
     v = torch.randn(B, Cb, generator=_gen(key), device=DEV).half()
-    buf, y = _guarded(B * HW * ys, F16)
+    buf, y = guarded(B * HW * ys, F16, device=DEV)
     capi.check(capi.lib().r3dp_ip_broadcast(P(v, F16), B, HW, Cb, P(y, F16), ys, yc0, capi.stream()))
     torch.cuda.synchronize()
-    assert _guards_intact(buf, y.numel())
+    assert guards_intact(buf, y.numel())
     y = y.view(B, HW, ys)
-    assert torch.equal(y[..., yc0:yc0 + Cb], v[:, None].expand(B, HW, Cb)) and bool(_untouched(y[..., :yc0]).all())
+    assert torch.equal(y[..., yc0:yc0 + Cb], v[:, None].expand(B, HW, Cb)) and bool(untouched(y[..., :yc0]).all())
 
 
 @torch.no_grad()
@@ -307,14 +283,14 @@ def test_pixel_shuffle_launch(key):
     B, h, w, C, ys, yc0 = launch.args
     g = _gen(key)
     x, t = torch.randn(B * h * w, 4 * C, generator=g, device=DEV), torch.randn(B * h * w, 4 * C, generator=g, device=DEV)
-    buf, y = _guarded(B * 4 * h * w * ys, F16)
+    buf, y = guarded(B * 4 * h * w * ys, F16, device=DEV)
     capi.check(capi.lib().r3dp_ip_pixel_shuffle(P(x), P(t), B, h, w, C, P(y, F16), ys, yc0, capi.stream()))
     torch.cuda.synchronize()
-    assert _guards_intact(buf, y.numel())
+    assert guards_intact(buf, y.numel())
     y = y.view(B, 2 * h, 2 * w, ys)
     want = F.pixel_shuffle((x + t).view(B, h, w, 4 * C).permute(0, 3, 1, 2), 2).permute(0, 2, 3, 1).half()
     assert torch.equal(y[..., yc0:yc0 + C], want), f'{label}: fp16(x + t), shuffled'
-    assert bool(_untouched(y[..., :yc0]).all()) and bool(_untouched(y[..., yc0 + C:]).all()), f'{label}: written outside its slice'
+    assert bool(untouched(y[..., :yc0]).all()) and bool(untouched(y[..., yc0 + C:]).all()), f'{label}: written outside its slice'
 
 
 @torch.no_grad()
@@ -323,14 +299,14 @@ def test_upsample2_launch(key):
     label, launch = ROWS[key]
     B, h, w, C = launch.args
     x = torch.randn(B, h, w, C, generator=_gen(key), device=DEV).half()
-    buf, y = _guarded(B * 4 * h * w * C, F16)
+    buf, y = guarded(B * 4 * h * w * C, F16, device=DEV)
     capi.check(capi.lib().r3dp_ip_upsample2(P(x, F16), B, h, w, C, P(y, F16), capi.stream()))
     torch.cuda.synchronize()
-    assert _guards_intact(buf, y.numel()) and not bool(_untouched(y).any())
+    assert guards_intact(buf, y.numel()) and not bool(untouched(y).any())
     y = y.view(B, 2 * h, 2 * w, C)
     for n in range(B):
         want = F.interpolate(x[n:n + 1].permute(0, 3, 1, 2).double(), scale_factor=2.0, mode='bilinear', align_corners=True)
-        ikern._check(f'upsample2 {label} image {n}', y[n], want[0].permute(1, 2, 0))
+        ikern.check_bar(f'upsample2 {label} image {n}', y[n], want[0].permute(1, 2, 0))
 
 
 @torch.no_grad()
@@ -342,7 +318,7 @@ def test_copy_launch(key):
     if fn == 'r3dp_ip_input':
         B, H, W = launch.args
         x = torch.rand(B, 3, H, W, generator=g, device=DEV) * 2 - 1
-        buf, y = _guarded(B * H * W * 8, F16)
+        buf, y = guarded(B * H * W * 8, F16, device=DEV)
         capi.check(capi.lib().r3dp_ip_input(P(x), B, H, W, P(y, F16), capi.stream()))
         want = ref.with_coords(x.double()).permute(0, 2, 3, 1)
         want = torch.cat([want, torch.zeros(B, H, W, 3, device=DEV, dtype=F64)], -1).half().reshape(-1)
@@ -350,107 +326,78 @@ def test_copy_launch(key):
         B, H, W, C = launch.args
         x = torch.randn(B, H, W, C, generator=g, device=DEV).half()
         ho, wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
-        buf, y = _guarded(B * ho * wo * C, F16)
+        buf, y = guarded(B * ho * wo * C, F16, device=DEV)
         capi.check(capi.lib().r3dp_ip_maxpool(P(x, F16), B, H, W, C, P(y, F16), capi.stream()))
         want = F.max_pool2d(x.permute(0, 3, 1, 2).float(), 3, 2, 1).permute(0, 2, 3, 1).half().reshape(-1)
     else:
         B, H, W = launch.args
         x = torch.randn(B, H, W, 96, generator=g, device=DEV)
-        buf, y = _guarded(B * H * W * 96, F32)
+        buf, y = guarded(B * H * W * 96, F32, device=DEV)
         capi.check(capi.lib().r3dp_ip_flip_hwpc(P(x), B, H, W, P(y), capi.stream()))
         want = ref.flip_planes(x.permute(0, 3, 1, 2)).permute(0, 3, 4, 1, 2).reshape(-1)
     torch.cuda.synchronize()
-    assert _guards_intact(buf, y.numel())
+    assert guards_intact(buf, y.numel())
     assert torch.equal(y, want), f'{label}: not an exact copy'
 
 
 # ---- the recorded launches -------------------------------------------------------------------------------------------------------------------
-_ENTRY = ('r3dp_ip_', 'r3dp_sp_')
+def _recorded(name):
+    return name.startswith(('r3dp_ip_', 'r3dp_sp_')) or name in ('r3dp_mf_conv3d', 'r3dp_sr_tc_conv')
 
 
-class _Recorder:
-    """Stands in for the library object: records every r3dp_ip_*, r3dp_sp_*, r3dp_mf_conv3d and r3dp_sr_tc_conv call as its row key and
-    passes it on unchanged.  capi.ptr is wrapped too, so an offset pointer (a channel slice of cat448) resolves to its tensor."""
+class _RowKeys(Recorder):
+    """Records every r3dp_ip_*, r3dp_sp_*, r3dp_mf_conv3d and r3dp_sr_tc_conv call as its row key; capi.ptr is wrapped too, so an offset
+    pointer (a channel slice of cat448) resolves to its tensor."""
 
     def __init__(self, lib):
-        self.lib, self.calls, self.tensors = lib, [], []
+        super().__init__(lib, _recorded, ptrs=True)
 
-    def ptr(self, t, *a, **k):
-        if t is not None:
-            self.tensors.append((t.data_ptr(), t.data_ptr() + t.numel() * t.element_size()))
-        return P(t, *a, **k)
-
-    def offset(self, p):
-        """Elements (fp16) from the start of the latest tensor holding address p."""
-        for lo, hi in reversed(self.tensors):
-            if lo <= p < hi:
-                return (p - lo) // 2
-        raise AssertionError(f'pointer {p:#x} into no tensor the module passed')
-
-    def key(self, name, args):
-        types = capi._SIGNATURES[name][1]
-        sig = ref.launch_signature(name, [a for a, t in zip(args, types) if t is not capi._P])
-        given = lambda v: (v.value if isinstance(v, ctypes.c_void_p) else v) is not None          # noqa: E731
+    def record(self, name, args):
+        sig = call_signature(name, args)
         if name == 'r3dp_mf_conv3d':
-            xs = args[1]
-            return sig + (given(args[6]), self.offset(args[0].value) % xs)
+            x = args[0].value                                   # its channel offset in the tensor it points into (fp16 elements)
+            return sig + (given(args[6]), (x - self.tensor(x).data_ptr()) // 2 % args[1])
         if name == 'r3dp_sp_layernorm':
             roles = tuple(r for r, v in zip(('t', 'xo', 'yf', 'yh'), (args[1], args[7], args[8], args[9])) if given(v))
             return sig + (roles, given(args[7]) and args[7].value == args[0].value)
         return sig
 
-    def __getattr__(self, name):
-        fn = getattr(self.lib, name)
-        if not (name.startswith(_ENTRY) or name in ('r3dp_mf_conv3d', 'r3dp_sr_tc_conv')):
-            return fn
-
-        def call(*args):
-            self.calls.append(self.key(name, args))
-            return fn(*args)
-        return call
-
 
 @torch.no_grad()
-def test_launches_have_rows(monkeypatch):
-    import test_gpu_sr_conv_conformance as srcc
+def test_launches_have_rows():
     models = {}
     for scale in ('small', 'standard', 'large'):
         m = Img2PlaneModel(hp={'img2plane_backbone_scale': scale})
         m.load_state_dict(ref.make_params({k: v.shape for k, v in m.state_dict().items()}, 5), strict=True)
         models[scale] = m.to(DEV).eval()
         models[scale]._prepared()                                # the weight packing, not recorded
-    rec = _Recorder(capi.lib())
-    monkeypatch.setattr(capi, '_lib', rec)
-    monkeypatch.setattr(capi, 'ptr', rec.ptr)
     launched, missing = set(), []
-    sr_rows = {srcc._signature('CASES', row) for row in srcc.CASES}
+    sr_rows = {srcc.row_signature(row) for row in srcc.CASES}
     patch_rows = {(B, H, H, C, k, s, p, d, (k * k * C + 31) // 32 * 32) for B, H, C, k, s, p, d in ikern.PATCH_ROWS}
-    for H, B, scale in RECORDED:
-        rec.calls.clear()
-        rec.tensors.clear()
-        models[scale](ref.make_inputs(B, H, 11).to(DEV))
-        want = [ref.row_key(launch.fn, launch.args, launch.reads, launch.writes) for launch in ref.launch_plan(H, B, scale)]
-        got = rec.calls[:]
-        assert got == want, f'{H}^2 B={B} {scale}: the module launches ' + '; '.join(f'{x}' for x in got if x not in want) + \
-            ' not in launch_plan, which has ' + '; '.join(f'{x}' for x in want if x not in got)
-        for k in got:
-            launched.add(k)
-            if k[0] == 'r3dp_sr_tc_conv':
-                N, Nw, I, O, h, w, ksize, act = k[1]
-                ok = srcc._signature('CASES', ('conv_res', N, Nw, I, O, h, w, {'ksize': ksize, 'act': act})) in sr_rows
-            elif k[0] == 'r3dp_sp_patches_dil':
-                ok = k[1] in patch_rows
-            else:
-                ok = k in ROWS
-            if not ok:
-                missing.append(f'{H}^2 B={B} {scale}: {k}')
-    torch.cuda.synchronize()
+    with _RowKeys(capi.lib()) as rec:
+        for H, B, scale in RECORDED:
+            rec.clear()
+            models[scale](ref.make_inputs(B, H, 11).to(DEV))
+            got = rec.calls[:]
+            assert_plan(got, [ref.row_key(launch.fn, launch.args, launch.reads, launch.writes) for launch in ref.launch_plan(H, B, scale)],
+                        f'{H}^2 B={B} {scale}')
+            for k in got:
+                launched.add(k)
+                if k[0] == 'r3dp_sr_tc_conv':
+                    N, Nw, I, O, h, w, ksize, act = k[1]
+                    ok = srcc.row_signature(('conv_res', N, Nw, I, O, h, w, {'ksize': ksize, 'act': act})) in sr_rows
+                elif k[0] == 'r3dp_sp_patches_dil':
+                    ok = k[1] in patch_rows
+                else:
+                    ok = k in ROWS
+                if not ok:
+                    missing.append(f'{H}^2 B={B} {scale}: {k}')
+        torch.cuda.synchronize()
     print(f'{len(launched)} distinct launches over {len(RECORDED)} forwards')
-    assert not missing, 'launches without a float64 row:\n' + '\n'.join(missing)
     stale = [ROWS[k][0] for k in ROWS if k not in launched]
     stale += [f'IMG2PLANE_PRODUCTION {row}' for row in srcc.IMG2PLANE_PRODUCTION
               if ('r3dp_sr_tc_conv', (*row[1:7], row[7].get('ksize', 3), row[7]['act'])) not in launched]
-    assert not stale, 'rows no forward launches:\n' + '\n'.join(stale)
+    assert_rows(missing, stale, 'the forwards')
 
 
 # ---- the teacher-forced forward ------------------------------------------------------------------------------------------------------------
@@ -545,7 +492,7 @@ def _same_bits(what, got, want, stats):
     assert int(d.max()) <= 1 and n <= max(2, d.numel() // 10000), f'{what}: {n} of {d.numel()} values differ from the fold (max {int(d.max())} ulp)'
 
 
-class _TeacherForcer(_Recorder):
+class _TeacherForcer(_RowKeys):
     """Runs forward launch by launch against launch_plan: after each launch, the float64 reference of what it wrote is computed from the
     snapshots of the buffers the plan says it reads (earlier launches' outputs), not from the pointers it was given, and its weights are
     checked against the state_dict's fold."""
@@ -559,18 +506,6 @@ class _TeacherForcer(_Recorder):
                 self.width[b] = max(self.width.get(b, 0), c1)
         self.store = {'img': x}
         self.stats = {'ties': 0, 'values': 0, 'launches': 0}
-        self.objs = []
-
-    def ptr(self, t, *a, **k):
-        if t is not None:
-            self.objs.append((t.data_ptr(), t.data_ptr() + t.numel() * t.element_size(), t))
-        return super().ptr(t, *a, **k)
-
-    def tensor(self, p):
-        for lo, hi, t in reversed(self.objs):
-            if lo <= p < hi:
-                return t
-        raise AssertionError(f'pointer {p:#x} into no tensor the module passed')
 
     def rd(self, launch, role):
         b, c0, c1 = launch.reads[role]
@@ -578,13 +513,13 @@ class _TeacherForcer(_Recorder):
 
     def __getattr__(self, name):
         fn = getattr(self.lib, name)
-        if not (name.startswith(_ENTRY) or name in ('r3dp_mf_conv3d', 'r3dp_sr_tc_conv')):
+        if not _recorded(name):
             return fn
 
         def call(*args):
             assert self.i < len(self.plan), f'{name}: a launch past the plan'
             launch = self.plan[self.i]
-            assert self.key(name, args) == ref.row_key(launch.fn, launch.args, launch.reads, launch.writes), f'launch {self.i}: {launch.tag}'
+            assert self.record(name, args) == ref.row_key(launch.fn, launch.args, launch.reads, launch.writes), f'launch {self.i}: {launch.tag}'
             rc = fn(*args)
             torch.cuda.synchronize()
             outs = {}
@@ -624,7 +559,7 @@ class _TeacherForcer(_Recorder):
             assert torch.equal(outs['y'], F.max_pool2d(x, 3, 2, 1).permute(0, 2, 3, 1).reshape(-1, C).half()), what
         elif fn == 'r3dp_ip_channel_mean':
             B, HW, C = a
-            ikern._check(f'mean {what}', outs['y'].reshape(B, C), self.rd(L, 'x').reshape(B, HW, C).double().mean(1))
+            ikern.check_bar(f'mean {what}', outs['y'].reshape(B, C), self.rd(L, 'x').reshape(B, HW, C).double().mean(1))
         elif fn == 'r3dp_ip_broadcast':
             B, HW, C, ys, yc0 = a
             got = outs['y'].reshape(B, HW, ys)[..., yc0:yc0 + C]
@@ -645,7 +580,7 @@ class _TeacherForcer(_Recorder):
             want = F.layer_norm(v, (C,), g.double(), b.double(), eps)
             for role in ('yf', 'yh'):
                 if role in outs:
-                    skern._check(f'sp_layernorm {what} {role}', outs[role], want)
+                    skern.check_bar(f'sp_layernorm {what} {role}', outs[role], want)
         elif fn == 'r3dp_ip_attention':
             qs, kvs, B, Tq, Tk, heads, scale, _ = a
             q, kv, o = self.rd(L, 'q').reshape(B, Tq, qs), self.rd(L, 'kv').reshape(B, Tk, kvs), outs['o'].reshape(B, Tq, -1)
@@ -655,7 +590,7 @@ class _TeacherForcer(_Recorder):
                 for h in range(heads):
                     cs = slice(h * hd, (h + 1) * hd)
                     want = ((q[bb, :, cs].double() @ kv[bb, :, cs].double().T) * scale).softmax(-1) @ kv[bb, :, qs + h * hd:qs + (h + 1) * hd].double()
-                    ikern._check(f'attention {what} b{bb} h{h}', o[bb, :, cs], want, S)
+                    ikern.check_bar(f'attention {what} b{bb} h{h}', o[bb, :, cs], want, S)
         elif fn == 'r3dp_sp_dwconv_gelu':
             B, h, w, C = a
             p, _ = _sd_keys(tag)
@@ -666,10 +601,10 @@ class _TeacherForcer(_Recorder):
             y = outs['y'].reshape(B, h, w, C)
             for n in range(B):
                 want = F.gelu(F.conv2d(x[n:n + 1].double().permute(0, 3, 1, 2), wt.double().view(C, 1, 3, 3), bt.double(), 1, 1, groups=C))
-                skern._check(f'sp_dwconv_gelu {what} image {n}', y[n], want[0].permute(1, 2, 0))
+                skern.check_bar(f'sp_dwconv_gelu {what} image {n}', y[n], want[0].permute(1, 2, 0))
         elif fn == 'r3dp_sp_leaky':
             n, slope = a
-            skern._check(f'sp_leaky {what}', outs['x'], F.leaky_relu(self.rd(L, 'x').double(), slope))
+            skern.check_bar(f'sp_leaky {what}', outs['x'], F.leaky_relu(self.rd(L, 'x').double(), slope))
         elif fn == 'r3dp_ip_pixel_shuffle':
             B, h, w, C, ys, yc0 = a
             v = (self.rd(L, 'x') + self.rd(L, 't')).reshape(B, h, w, 4 * C).permute(0, 3, 1, 2)
@@ -679,7 +614,7 @@ class _TeacherForcer(_Recorder):
             B, h, w, C = a
             x = self.rd(L, 'x').reshape(B, h, w, C).permute(0, 3, 1, 2).double()
             want = F.interpolate(x, scale_factor=2.0, mode='bilinear', align_corners=True).permute(0, 2, 3, 1)
-            ikern._check(f'upsample2 {what}', outs['y'].reshape(B, 2 * h, 2 * w, C), want)
+            ikern.check_bar(f'upsample2 {what}', outs['y'].reshape(B, 2 * h, 2 * w, C), want)
         elif fn == 'r3dp_ip_flip_hwpc':
             B, H, W = a
             x = self.rd(L, 'x').reshape(B, H, W, 96).permute(0, 3, 1, 2)
@@ -737,7 +672,7 @@ class _TeacherForcer(_Recorder):
 
 @torch.no_grad()
 @pytest.mark.parametrize('H,B', TEACHER, ids=lambda v: str(v))
-def test_teacher_forced_forward(H, B, monkeypatch):
+def test_teacher_forced_forward(H, B):
     """forward with make_params weights, each launch checked against float64 of the buffers launch_plan says it reads, as the earlier
     launches wrote them: a launch that reads the wrong buffer or slice, or races with its own in-place write, fails, as does a weight
     that is not the state_dict's (the wrong block's LayerNorm, a fold with another BatchNorm eps)."""
@@ -748,11 +683,9 @@ def test_teacher_forced_forward(H, B, monkeypatch):
     m._prepared()
     sd = {k: (v.to(DEV, F64) if v.is_floating_point() else v.to(DEV)) for k, v in sd.items()}
     x = ref.make_inputs(B, H, 11).to(DEV)
-    tf = _TeacherForcer(capi.lib(), ref.launch_plan(H, B), m, sd, x)
-    monkeypatch.setattr(capi, '_lib', tf)
-    monkeypatch.setattr(capi, 'ptr', tf.ptr)
-    out = m(x)
-    torch.cuda.synchronize()
+    with _TeacherForcer(capi.lib(), ref.launch_plan(H, B), m, sd, x) as tf:
+        out = m(x)
+        torch.cuda.synchronize()
     assert tf.i == len(tf.plan), f'{tf.i} of {len(tf.plan)} launches'
     assert torch.equal(out.permute(0, 3, 4, 1, 2).reshape(-1), tf.store['planes'].reshape(-1))
     print(f'teacher-forced {H}^2 B={B}: {tf.stats["launches"]} launches; weights: {tf.stats["ties"]} of {tf.stats["values"]} values 1 ulp '

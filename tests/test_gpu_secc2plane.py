@@ -18,24 +18,24 @@ DEV = 'cuda:0'
 BAR = 3e-3          # |got - ref| <= BAR * max|ref|; measured <= 9.0e-4 on an H100 (DESIGN.md)
 
 
-def _module(mode='cano_src_tgt', seed=7):
+def module(mode='cano_src_tgt', seed=7):
     m = r3.SegFormerSECC2PlaneBackbone(pncc_cond_mode=mode)
     m.load_state_dict(ref.make_params({k: v.shape for k, v in m.state_dict().items()}, seed), strict=True)
     return m.to(DEV).eval()
 
 
-def _rel(got, want):
+def rel(got, want):
     return float((got.double() - want.double()).abs().max()) / float(want.double().abs().max())
 
 
 @torch.no_grad()
 def test_backbone_matches_reference_fixture():
     g = load_golden('secc2plane_small')
-    m = _module(seed=int(g['param_seed']))
+    m = module(seed=int(g['param_seed']))
     cano, src, tgt = ref.make_inputs(1, int(g['size']), int(g['input_seed']))
     out = m(torch.cat([cano, src, tgt], 1).to(DEV))
     assert out.shape == (1, 3, 32, 64, 64)
-    r = _rel(out[..., ::2, ::2].cpu(), g['planes_s2'])
+    r = rel(out[..., ::2, ::2].cpu(), g['planes_s2'])
     print(f'secc2plane 128^2 vs reference fixture: max err / range = {r:.2e}')
     assert r < BAR, r
 
@@ -43,14 +43,14 @@ def test_backbone_matches_reference_fixture():
 @torch.no_grad()
 @pytest.mark.parametrize('mode', ['cano_src_tgt', 'cano_tgt'])
 def test_backbone_matches_float64_at_512(mode):
-    m = _module(mode)
+    m = module(mode)
     sd = ref.to64(m.state_dict(), DEV)
     cano, src, tgt = ref.make_inputs(4, 512, 3)
     parts = [cano, src] if mode == 'cano_src_tgt' else [cano]
     x = torch.cat([p.expand(4, -1, -1, -1) for p in parts] + [tgt], 1).to(DEV)
     out = m(x)
     want = ref.forward(sd, x.double())
-    r = _rel(out, want)
+    r = rel(out, want)
     print(f'secc2plane 512^2 B=4 ({mode}) vs float64: max err / range = {r:.2e}')
     assert r < BAR, r
     # image k of the batch is bit-identical to that frame alone
@@ -60,7 +60,7 @@ def test_backbone_matches_float64_at_512(mode):
 
 @torch.no_grad()
 def test_planes_cl_equals_forward():
-    m = _module()
+    m = module()
     cano, src, tgt = (t.to(DEV) for t in ref.make_inputs(2, 512, 5))
     full = m(torch.cat([cano.expand(2, -1, -1, -1), src.expand(2, -1, -1, -1), tgt], 1))
     m.begin_clip(cano, src)
@@ -76,7 +76,7 @@ def test_planes_cl_equals_forward():
 
 @torch.no_grad()
 def test_render_of_pair_equals_render_of_sum():
-    m = _module()
+    m = module()
     cano_in, src, tgt = (t.to(DEV) for t in ref.make_inputs(2, 512, 9))
     m.begin_clip(cano_in, src)
     secc_cl = m.planes_cl(tgt)

@@ -16,6 +16,7 @@ import torch.nn.functional as F
 
 from real3dportrait_b200 import _capi as capi
 import secc2plane_reference as sref
+from launch_harness import GUARD, guarded, guards_intact, untouched
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
@@ -42,7 +43,7 @@ def _beta(got, ref):
     return max(float(excess.max()), 0.0) / S
 
 
-def _check(name, got, ref):
+def check_bar(name, got, ref):
     b = _beta(got, ref)
     bar = BETA[name.split()[0]]
     print(f'{name}: beta = {b:.2e} (bar {bar:.1e})')
@@ -72,18 +73,18 @@ def test_prenet_and_embed(B):
     base = torch.empty(1, 3, H, H, device=DEV)
     capi.check(lib().r3dp_sp_prenet(P(cano_src), 1, 6, H, H, P(w[:, :6].contiguous()), P(b), P(base), st))
     ref_base = torch.einsum('cj,njhw->nchw', w[:, :6].double(), cano_src.double()) + b.double()[None, :, None, None]
-    _check('sp_prenet', base, ref_base)
+    check_bar('sp_prenet', base, ref_base)
     # per-frame embed on the cached image (the operands it reads: base, tgt, w[:, 6:])
     y = torch.empty(B, (H // 4) ** 2, 32, device=DEV)
     capi.check(lib().r3dp_sp_embed(P(tgt), B, 3, H, H, P(w[:, 6:].contiguous()), P(base), None, P(wpe), P(bpe), P(y), st))
     pre = base.double() + torch.einsum('cj,njhw->nchw', w[:, 6:].double(), tgt.double())
     ref = F.conv2d(pre, wpe.double(), bpe.double(), 4, 3).flatten(2).transpose(1, 2)
-    _check('sp_embed (cached image)', y, ref)
+    check_bar('sp_embed (cached image)', y, ref)
     # the whole 9-channel input, no cached image
     x = torch.cat([cano_src.expand(B, -1, -1, -1), tgt], 1).contiguous()
     capi.check(lib().r3dp_sp_embed(P(x), B, 9, H, H, P(w), None, P(b), P(wpe), P(bpe), P(y), st))
     pre = torch.einsum('cj,njhw->nchw', w.double(), x.double()) + b.double()[None, :, None, None]
-    _check('sp_embed (full input)', y, F.conv2d(pre, wpe.double(), bpe.double(), 4, 3).flatten(2).transpose(1, 2))
+    check_bar('sp_embed (full input)', y, F.conv2d(pre, wpe.double(), bpe.double(), 4, 3).flatten(2).transpose(1, 2))
 
 
 @pytest.mark.parametrize('B', [1, 4])
@@ -96,9 +97,9 @@ def test_layernorm(B, C, hw):
     capi.check(lib().r3dp_sp_layernorm(P(x), P(t), R, C, P(g), P(b), 1e-6, P(xo), P(yf), P(yh, F16), C, capi.stream()))
     v = x.double() + t.double()
     ref = F.layer_norm(v, (C,), g.double(), b.double(), 1e-6)
-    _check(f'sp_layernorm residual C={C}', xo, v)
-    _check(f'sp_layernorm fp32 C={C}', yf, ref)
-    _check(f'sp_layernorm fp16 C={C}', yh, ref)
+    check_bar(f'sp_layernorm residual C={C}', xo, v)
+    check_bar(f'sp_layernorm fp32 C={C}', yf, ref)
+    check_bar(f'sp_layernorm fp16 C={C}', yh, ref)
 
 
 @pytest.mark.parametrize('B', [1, 4])
@@ -126,7 +127,7 @@ def test_attention(B, hw, heads, tk):
     kh = kv.double()[..., :C].view(B, tk, heads, 32).transpose(1, 2)
     vh = kv.double()[..., C:].view(B, tk, heads, 32).transpose(1, 2)
     ref = ((qh @ kh.transpose(-2, -1)) * 32 ** -0.5).softmax(-1) @ vh
-    _check(f'sp_attention heads={heads}', o, ref.transpose(1, 2).reshape(B, T, C))
+    check_bar(f'sp_attention heads={heads}', o, ref.transpose(1, 2).reshape(B, T, C))
 
 
 @pytest.mark.parametrize('B', [1, 4])
@@ -137,7 +138,7 @@ def test_dwconv_gelu(B, hw, C):
     y = torch.empty_like(x)
     capi.check(lib().r3dp_sp_dwconv_gelu(P(x, F16), B, hw, hw, C, P(w), P(b), P(y, F16), capi.stream()))
     ref = F.gelu(F.conv2d(x.double().permute(0, 3, 1, 2), w.double().view(C, 1, 3, 3), b.double(), 1, 1, groups=C)).permute(0, 2, 3, 1)
-    _check(f'sp_dwconv_gelu C={C}', y, ref)
+    check_bar(f'sp_dwconv_gelu C={C}', y, ref)
 
 
 @pytest.mark.parametrize('B', [1, 4])
@@ -150,7 +151,7 @@ def test_head_fuse(B):
     acc = bias.double()[None, :, None, None] + g[0].double().permute(0, 3, 1, 2)
     for t in g[1:]:
         acc = acc + F.interpolate(t.double().permute(0, 3, 1, 2), size=(128, 128), mode='bilinear', align_corners=False)
-    _check('sp_head_fuse', y, torch.relu(acc).permute(0, 2, 3, 1))
+    check_bar('sp_head_fuse', y, torch.relu(acc).permute(0, 2, 3, 1))
 
 
 @pytest.mark.parametrize('B', [1, 4])
@@ -158,7 +159,7 @@ def test_leaky(B):
     x = _rand((B, 128, 128, 256), 60, F16)
     ref = F.leaky_relu(x.double(), 0.01)
     capi.check(lib().r3dp_sp_leaky(P(x, F16), x.numel(), 0.01, capi.stream()))
-    _check('sp_leaky', x, ref)
+    check_bar('sp_leaky', x, ref)
 
 
 @pytest.mark.parametrize('B', [1, 4])
@@ -167,8 +168,8 @@ def test_upsample2_flip(B):
     yr, yrc = torch.empty(B, 256, 256, 256, device=DEV, dtype=F16), torch.empty(B, 256, 256, 256, device=DEV, dtype=F16)
     capi.check(lib().r3dp_sp_upsample2_flip(P(x, F16), B, 128, 128, 256, P(yr, F16), P(yrc, F16), capi.stream()))
     up = F.interpolate(x.double().permute(0, 3, 1, 2), scale_factor=2.0, mode='bilinear', align_corners=True).permute(0, 2, 3, 1)
-    _check('sp_upsample2_flip rows', yr, up.flip(1))
-    _check('sp_upsample2_flip rows+cols', yrc, up.flip(1, 2))
+    check_bar('sp_upsample2_flip rows', yr, up.flip(1))
+    check_bar('sp_upsample2_flip rows+cols', yrc, up.flip(1, 2))
 
 
 # ---- every size class the module accepts ---------------------------------------------------------------------------------------------------
@@ -210,22 +211,15 @@ def _kid(k):
 
 
 def _guarded(shape, dtype):
-    """(output view, whole buffer): the output between two GUARD-element runs, all of it filled with a NaN pattern no kernel writes."""
-    n = math.prod(shape)
-    buf = torch.empty(n + 2 * GUARD, device=DEV, dtype=dtype)
-    buf.view(SENTINEL[dtype][0]).fill_(SENTINEL[dtype][1])
-    return buf[GUARD:GUARD + n].view(shape), buf
+    """(output view of `shape`, whole guarded buffer)."""
+    buf, y = guarded(math.prod(shape), dtype, device=DEV)
+    return y.view(shape), buf
 
 
 def _written(name, buf):
-    it, s = SENTINEL[buf.dtype]
-    b = buf.view(it)
-    assert bool((b[:GUARD] == s).all()) and bool((b[-GUARD:] == s).all()), f'{name}: written outside the output'
-    assert not bool((b[GUARD:-GUARD] == s).any()), f'{name}: output elements left unwritten'
-
-
-GUARD = 4096
-SENTINEL = {F16: (torch.int16, 0x7E55), F32: (torch.int32, 0x7FC01234)}
+    y = buf[GUARD:-GUARD]
+    assert guards_intact(buf, y.numel()), f'{name}: written outside the output'
+    assert not bool(untouched(y).any()), f'{name}: output elements left unwritten'
 
 
 @pytest.mark.parametrize('key', _keys('r3dp_sp_attention'), ids=_kid)
@@ -241,7 +235,7 @@ def test_attention_sizes(key):
     kh = kv.double()[..., :C].view(B, tk, heads, 32).transpose(1, 2)
     vh = kv.double()[..., C:].view(B, tk, heads, 32).transpose(1, 2)
     ref = ((qh @ kh.transpose(-2, -1)) * 32 ** -0.5).softmax(-1) @ vh
-    _check(f'sp_attention {_kid(key)}', o, ref.transpose(1, 2).reshape(B, T, C))
+    check_bar(f'sp_attention {_kid(key)}', o, ref.transpose(1, 2).reshape(B, T, C))
 
 
 @pytest.mark.parametrize('key', _keys('r3dp_sp_layernorm'), ids=_kid)
@@ -256,9 +250,9 @@ def test_layernorm_sizes(key):
         _written(f'{_kid(key)} {name}', buf)
     v = x.double() + t.double()
     ref = F.layer_norm(v, (C,), g.double(), b.double(), eps)
-    _check(f'sp_layernorm residual {_kid(key)}', xo, v)
-    _check(f'sp_layernorm fp32 {_kid(key)}', yf, ref)
-    _check(f'sp_layernorm fp16 {_kid(key)}', yh, ref)
+    check_bar(f'sp_layernorm residual {_kid(key)}', xo, v)
+    check_bar(f'sp_layernorm fp32 {_kid(key)}', yf, ref)
+    check_bar(f'sp_layernorm fp16 {_kid(key)}', yh, ref)
 
 
 @pytest.mark.parametrize('key', _keys('r3dp_sp_dwconv_gelu'), ids=_kid)
@@ -271,7 +265,7 @@ def test_dwconv_gelu_sizes(key):
     torch.cuda.synchronize()
     _written(_kid(key), buf)
     ref = F.gelu(F.conv2d(x.double().permute(0, 3, 1, 2), w.double().view(C, 1, 3, 3), b.double(), 1, 1, groups=C)).permute(0, 2, 3, 1)
-    _check(f'sp_dwconv_gelu {_kid(key)}', y, ref)
+    check_bar(f'sp_dwconv_gelu {_kid(key)}', y, ref)
 
 
 @pytest.mark.parametrize('key', _keys('r3dp_sp_head_fuse'), ids=_kid)
@@ -288,7 +282,7 @@ def test_head_fuse_sizes(key):
     acc = bias.double()[None, :, None, None] + g[0].double().permute(0, 3, 1, 2)
     for t in g[1:]:
         acc = acc + F.interpolate(t.double().permute(0, 3, 1, 2), size=(h1, h1), mode='bilinear', align_corners=False)
-    _check(f'sp_head_fuse {_kid(key)}', y, torch.relu(acc).permute(0, 2, 3, 1))
+    check_bar(f'sp_head_fuse {_kid(key)}', y, torch.relu(acc).permute(0, 2, 3, 1))
 
 
 @pytest.mark.parametrize('key', _keys('r3dp_sp_upsample2_flip'), ids=_kid)
@@ -301,8 +295,8 @@ def test_upsample2_flip_sizes(key):
     _written(f'{_kid(key)} rows', br)
     _written(f'{_kid(key)} rows+cols', brc)
     up = F.interpolate(x.double().permute(0, 3, 1, 2), scale_factor=2.0, mode='bilinear', align_corners=True).permute(0, 2, 3, 1)
-    _check(f'sp_upsample2_flip rows {_kid(key)}', yr, up.flip(1))
-    _check(f'sp_upsample2_flip rows+cols {_kid(key)}', yrc, up.flip(1, 2))
+    check_bar(f'sp_upsample2_flip rows {_kid(key)}', yr, up.flip(1))
+    check_bar(f'sp_upsample2_flip rows+cols {_kid(key)}', yrc, up.flip(1, 2))
 
 
 @pytest.mark.parametrize('key', _keys('r3dp_sp_leaky'), ids=_kid)
@@ -314,7 +308,7 @@ def test_leaky_sizes(key):
     capi.check(lib().r3dp_sp_leaky(P(y, F16), n, slope, capi.stream()))
     torch.cuda.synchronize()
     _written(_kid(key), buf)
-    _check(f'sp_leaky {_kid(key)}', y, ref)
+    check_bar(f'sp_leaky {_kid(key)}', y, ref)
 
 
 @pytest.mark.parametrize('key', _keys('r3dp_sp_embed'), ids=_kid)
@@ -331,7 +325,7 @@ def test_embed_sizes(key):
     torch.cuda.synchronize()
     _written(f'{_kid(key)} full input', buf)
     pre = torch.einsum('cj,njhw->nchw', w.double(), x.double()) + b.double()[None, :, None, None]
-    _check(f'sp_embed (full input) {_kid(key)}', y, F.conv2d(pre, wpe.double(), bpe.double(), 4, 3).flatten(2).transpose(1, 2))
+    check_bar(f'sp_embed (full input) {_kid(key)}', y, F.conv2d(pre, wpe.double(), bpe.double(), 4, 3).flatten(2).transpose(1, 2))
     y, buf = _guarded((B, ho * ho, 32), F32)
     tgt = x[:, -3:].contiguous()
     wt = w[:, -3:].contiguous()
@@ -339,7 +333,7 @@ def test_embed_sizes(key):
     torch.cuda.synchronize()
     _written(f'{_kid(key)} cached image', buf)
     pre = base.double() + torch.einsum('cj,njhw->nchw', wt.double(), tgt.double())
-    _check(f'sp_embed (cached image) {_kid(key)}', y, F.conv2d(pre, wpe.double(), bpe.double(), 4, 3).flatten(2).transpose(1, 2))
+    check_bar(f'sp_embed (cached image) {_kid(key)}', y, F.conv2d(pre, wpe.double(), bpe.double(), 4, 3).flatten(2).transpose(1, 2))
 
 
 @pytest.mark.parametrize('key', _keys('r3dp_sp_patches'), ids=_kid)
@@ -374,6 +368,6 @@ def test_attention_on_second_device():
             torch.cuda.synchronize()
             qh, kh, vh = q.double(), kv.double()[..., :C], kv.double()[..., C:]
             ref = ((qh @ kh.transpose(-2, -1)) * 32 ** -0.5).softmax(-1) @ vh
-            _check(f'sp_attention on {dev}', o, ref)
+            check_bar(f'sp_attention on {dev}', o, ref)
             outs.append(o.cpu())
     assert torch.equal(outs[0], outs[1])

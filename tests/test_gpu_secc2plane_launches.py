@@ -20,7 +20,10 @@ import real3dportrait_b200 as r3
 from real3dportrait_b200 import _capi as capi, secc2plane as sp
 import secc2plane_reference as ref
 import sr_conv_reference as scr
-from test_gpu_torso_motion import _ref_conv
+import test_gpu_secc2plane_kernels as kern
+import test_gpu_sr_conv_conformance as srcc
+from launch_harness import GUARD, Recorder, assert_plan, assert_rows, assert_written, call_signature, conv3d, guarded, inside
+from torso_motion_reference import ref_conv
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
@@ -28,20 +31,11 @@ F16, F32 = torch.float16, torch.float32
 #: (H, B) of the forward calls the table covers; the first three are the ones the recorded-launch test runs
 PLAN_SIZES = [(512, 4), (512, 1), (480, 3), (96, 3), (32, 3)]
 RECORDED = PLAN_SIZES[:3]
-#: fp16 and fp32 NaN bit patterns no kernel writes
-SENTINEL = {F16: (torch.int16, 0x7E55), F32: (torch.int32, 0x7FC01234)}
-GUARD = 4096
 #: beta per taps (1: the token GEMMs, 9: the 1x3x3 convs).  Worst ratio over the rows on an H100 80GB HBM3 (700 W power limit): GEMMs
 #: 4.4e-7 (s4.pe, K = 1440, fp32 out), convs 6.7e-7 (the 480^2 last conv, K = 2304, fp32 out); the fp16-output rows measure lower (GEMMs
 #: 4.8e-8, convs 1.7e-7) because the store's 2^-11 rounding absorbs most of the accumulation error.  A skipped K chunk or cout tile costs
 #: O(S), far outside either bar.  The estimator's table (BETA3, 2^-18) measures 343-tap sums; these are shorter.
 BETA = {1: 1e-6, 9: 1.5e-6}
-
-
-def signature(fn, args):
-    """A recorded call -> (entry point, its non-pointer arguments): what decides a launch apart from the data."""
-    types = capi._SIGNATURES[fn][1]
-    return ref.launch_signature(fn, [a for a, t in zip(args, types) if t is not capi._P])
 
 
 def _rows(fn):
@@ -82,24 +76,6 @@ def _weights(tag, cin, O, taps, g):
     return wp, b, cop
 
 
-def _launch(x, wp, b, a, N, H, W, out):
-    """r3dp_mf_conv3d with the row's arguments a (launch_plan order), N / H / W replaced."""
-    xs, xlo, cin, _, D, _, _, kd, kh, kw, up, O, cop, relu, ys, yc0, ylo, out_f32, split = a
-    capi.check(capi.lib().r3dp_mf_conv3d(capi.ptr(x, F16), xs, xlo, cin, capi.ptr(wp, F16), capi.ptr(b), None, N, D, H, W, kd, kh, kw, up, O, cop,
-                                         relu, capi.ptr(out, out.dtype), ys, yc0, ylo, out_f32, split, capi.stream()))
-
-
-def _guarded(n, dt, tail):
-    buf = torch.empty(n + GUARD + tail, device=DEV, dtype=dt)
-    buf.view(SENTINEL[dt][0]).fill_(SENTINEL[dt][1])
-    return buf, buf[GUARD:GUARD + n]
-
-
-def _untouched(t):
-    dt = t.dtype
-    return t.view(SENTINEL[dt][0]) == SENTINEL[dt][1]
-
-
 @torch.no_grad()
 @pytest.mark.parametrize('key', CONV3D_KEYS, ids=[_id(k) for k in CONV3D_KEYS])
 def test_conv3d_launch_vs_float64(key):
@@ -113,81 +89,54 @@ def test_conv3d_launch_vs_float64(key):
     M = N * D * H * W
     x = torch.randn(N, D, H, W, xs, generator=g, device=DEV).half()
     dt = F32 if out_f32 else F16
-    buf, y = _guarded(M * ys, dt, max(GUARD, (cop - O) * ys))
-    _launch(x, wp, b, a, N, H, W, y)
-    torch.cuda.synchronize()
-    inside = torch.zeros(ys, dtype=torch.bool, device=DEV)
-    inside[yc0:yc0 + O] = True
+    buf, y = guarded(M * ys, dt, tail=max(GUARD, (cop - O) * ys), device=DEV)
+    conv3d(a, x, wp, b, None, y)
+    mask = inside(ys, yc0, O, device=DEV)
+    assert_written(buf, y, ys, mask, tag)
     yv = y.view(M, ys)
-    assert not bool(_untouched(yv[:, inside]).any()), f'{tag}: an output element was not written'
-    assert bool(_untouched(yv[:, ~inside]).all()), f'{tag}: written outside the channel slice'
-    assert bool(_untouched(buf[:GUARD]).all()) and bool(_untouched(buf[GUARD + M * ys:]).all()), f'{tag}: written past the output'
     got = yv[:, yc0:yc0 + O].view(N, D, H, W, O)
     # a 256^2 last conv is checked on its last image: the float64 reference of all four would take several GB
     k0 = N - 1 if taps == 9 and H >= 256 else 0
     xd = x[k0:].double().permute(0, 4, 1, 2, 3)[:, :cin]
     wd = (wp.double().view(taps, cop, cin) if taps == 9 else wp.double().view(1, cop, cin))[None, :, :O]
     tp = (kd, kh, kw)
-    want = _ref_conv(xd, wd, tp, False, b[:O])
-    S = _ref_conv(xd.abs(), wd.abs(), tp, False, b[:O].abs())
+    want = ref_conv(xd, wd, tp, False, b[:O])
+    S = ref_conv(xd.abs(), wd.abs(), tp, False, b[:O].abs())
     alpha = scr.ALPHA_F32 if out_f32 else scr.ALPHA_F16
     extra = 0.0 if out_f32 else 2 * scr.FLOOR_F16                              # fp16 subnormal floor of the store
     scr.check_bound(got[k0:].permute(0, 4, 1, 2, 3), want, S, alpha, BETA[taps], extra, tag=_id(key))
     # bit-exact: the last image of a conv equals its N = 1 launch; the last rows of a GEMM equal a launch on those rows alone
     if taps == 9:
         if N > 1:
-            one = torch.empty(D * H * W * ys, device=DEV, dtype=dt)
-            one.view(SENTINEL[dt][0]).fill_(SENTINEL[dt][1])
-            _launch(x[N - 1:].contiguous(), wp, b, a, 1, H, W, one)
-            assert torch.equal(one.view(H * W, ys)[:, inside], yv[-H * W:, inside]), f'{tag}: last image vs its N=1 launch'
+            _, one = guarded(D * H * W * ys, dt, device=DEV)
+            conv3d(a, x[N - 1:].contiguous(), wp, b, None, one, N=1)
+            assert torch.equal(one.view(H * W, ys)[:, mask], yv[-H * W:, mask]), f'{tag}: last image vs its N=1 launch'
     else:
         r = min(W, 300)
         tail = torch.empty(r * ys, device=DEV, dtype=dt)
-        _launch(x[:, :, :, W - r:].contiguous(), wp, b, a, 1, 1, r, tail)
+        conv3d(a, x[:, :, :, W - r:].contiguous(), wp, b, None, tail, N=1, H=1, W=r)
         assert torch.equal(tail.view(r, ys), yv[-r:]), f'{tag}: last {r} rows vs a launch on them alone'
 
 
 # ---- the recorded launches -----------------------------------------------------------------------------------------------------------------
-class _Recorder:
-    """Stands in for the library object: records the arguments of every backbone entry point and passes every call on unchanged."""
-
-    def __init__(self, lib):
-        self.lib, self.calls = lib, []
-
-    def __getattr__(self, name):
-        fn = getattr(self.lib, name)
-        if not (name.startswith('r3dp_sp_') or name in ('r3dp_mf_conv3d', 'r3dp_sr_tc_conv')):
-            return fn
-
-        def call(*args):
-            self.calls.append((name, args))
-            return fn(*args)
-        return call
-
-
 @torch.no_grad()
-def test_backbone_launches_have_rows(monkeypatch):
-    import test_gpu_secc2plane_kernels as kern
-    import test_gpu_sr_conv_conformance as srcc
+def test_backbone_launches_have_rows():
     m = r3.SegFormerSECC2PlaneBackbone()
     m.load_state_dict(ref.make_params({k: v.shape for k, v in m.state_dict().items()}, 3), strict=True)
     m = m.to(DEV).eval()
     m._prepared()                                                # the weight packing launches r3dp_sr_tc_pack_weights, not recorded
-    rec = _Recorder(capi.lib())
-    monkeypatch.setattr(capi, '_lib', rec)
     launched = {}
-    for H, B in RECORDED:
-        cano, src, tgt = ref.make_inputs(B, H, 11)
-        rec.calls.clear()
-        m(torch.cat([cano.expand(B, -1, -1, -1), src.expand(B, -1, -1, -1), tgt], 1).to(DEV))
-        got = [signature(n, a) for n, a in rec.calls]
-        want = [ref.launch_signature(f, a) for _, f, a in ref.launch_plan(H, B)]
-        assert got == want, f'{H}^2 B={B}: the module launches ' + '; '.join(f'{x}' for x in got if x not in want) + \
-            ' not in launch_plan, which has ' + '; '.join(f'{x}' for x in want if x not in got)
-        for s in got:
-            launched.setdefault(s, (H, B))
-    torch.cuda.synchronize()
-    sr_rows = {srcc._signature('CASES', row) for row in srcc.CASES}
+    with Recorder(capi.lib(), lambda n: n.startswith('r3dp_sp_') or n in ('r3dp_mf_conv3d', 'r3dp_sr_tc_conv')) as rec:
+        for H, B in RECORDED:
+            cano, src, tgt = ref.make_inputs(B, H, 11)
+            rec.calls.clear()
+            m(torch.cat([cano.expand(B, -1, -1, -1), src.expand(B, -1, -1, -1), tgt], 1).to(DEV))
+            got = [call_signature(n, a) for n, a in rec.calls]
+            assert_plan(got, [ref.launch_signature(f, a) for _, f, a in ref.launch_plan(H, B)], f'{H}^2 B={B}')
+            for s in got:
+                launched.setdefault(s, (H, B))
+        torch.cuda.synchronize()
+    sr_rows = {srcc.row_signature(row) for row in srcc.CASES}
     sp_rows = kern.sp_signatures()
     missing = []
     for (fn, a), (H, B) in launched.items():
@@ -195,14 +144,13 @@ def test_backbone_launches_have_rows(monkeypatch):
             ok = (fn, a) in CONV3D
         elif fn == 'r3dp_sr_tc_conv':
             N, Nw, I, O, h, w, ksize, act = a
-            ok = srcc._signature('CASES', ('conv_res', N, Nw, I, O, h, w, {'ksize': ksize, 'act': act})) in sr_rows
+            ok = srcc.row_signature(('conv_res', N, Nw, I, O, h, w, {'ksize': ksize, 'act': act})) in sr_rows
         else:
             ok = (fn, a) in sp_rows
         if not ok:
             missing.append(f'{H}^2 B={B}: {fn}{a}')
-    assert not missing, 'backbone launches without a float64 row:\n' + '\n'.join(missing)
     stale = [f'{CONV3D[k]}: {k}' for k in CONV3D if CONV3D[k].startswith('512^2') and k not in launched]
     stale += [f'{fn}{a} ({H}^2 B={B})' for fn, a, (H, B) in kern.sp_rows_at(512) if (fn, a) not in launched]
     stale += [f'SECC_PRODUCTION {row}' for row in srcc.SECC_PRODUCTION
               if ('r3dp_sr_tc_conv', (*row[1:7], row[7].get('ksize', 3), row[7]['act'])) not in launched]
-    assert not stale, 'rows the 512^2 backbone no longer launches:\n' + '\n'.join(stale)
+    assert_rows(missing, stale, 'the 512^2 backbone')

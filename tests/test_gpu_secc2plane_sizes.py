@@ -9,7 +9,7 @@ import pytest
 import torch
 
 import secc2plane_reference as ref
-from test_gpu_secc2plane import BAR, DEV, _module, _rel
+from test_gpu_secc2plane import BAR, DEV, module, rel
 
 pytestmark = pytest.mark.gpu
 
@@ -23,13 +23,13 @@ def _input(mode, B, H, seed):
 @torch.no_grad()
 @pytest.mark.parametrize('H,mode', [(32, 'cano_src_tgt'), (96, 'cano_src_tgt'), (96, 'cano_tgt'), (480, 'cano_src_tgt')])
 def test_backbone_sizes_vs_float64(H, mode):
-    m = _module(mode)
+    m = module(mode)
     B = 3
     x, _ = _input(mode, B, H, 20 + H)
     out = m(x)
     assert out.shape == (B, 3, 32, H // 2, H // 2)
     want = ref.forward(ref.to64(m.state_dict(), DEV), x.double())
-    r = _rel(out, want)
+    r = rel(out, want)
     print(f'secc2plane {H}^2 B={B} ({mode}) vs float64: max err / range = {r:.2e}')
     assert r < BAR, r
     for k in range(B):
@@ -38,7 +38,7 @@ def test_backbone_sizes_vs_float64(H, mode):
 
 @torch.no_grad()
 def test_planes_cl_equals_forward_at_96():
-    m = _module()
+    m = module()
     x, (cano, src, tgt) = _input('cano_src_tgt', 3, 96, 31)
     full = m(x)
     m.begin_clip(cano.to(DEV), src.to(DEV))

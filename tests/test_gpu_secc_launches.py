@@ -25,14 +25,12 @@ import blink_reference as bref
 import secc2plane_reference as s2p_ref
 import secc_launch_reference as lr
 import secc_render_reference as ref
+from launch_harness import Recorder, assert_plan, assert_rows, guarded, guards_intact, untouched
 import real3dportrait_b200 as r3
 from real3dportrait_b200 import _capi as capi, engine, synthetic as syn
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
-G = 1024                                   # guard elements (a multiple of 4: the buffers between them stay 16-byte aligned)
-SENT = 0x7FC01234                          # an fp32 NaN no kernel writes
-KSENT = 0x5A5A5A5A5A5A5A5A                 # an int64 no kernel writes
 TAN = ref.TAN_HALF
 N_BFM = 150 * 238
 
@@ -58,23 +56,6 @@ def renderer(kw, S):
     if key not in _RENDERERS:
         _RENDERERS[key] = r3.SECC_Renderer(S, device=DEV, **kw)
     return _RENDERERS[key]
-
-
-def _guarded(n, dtype=torch.float32):
-    big = torch.empty(n + 2 * G, dtype=dtype, device=DEV)
-    if dtype == torch.int64:
-        big.fill_(KSENT)
-    else:
-        big.view(torch.int32).fill_(SENT)
-    return big, big[G:G + n]
-
-
-def _sentinel(t):
-    return t.view(torch.int32) == SENT if t.dtype == torch.float32 else t == KSENT
-
-
-def _guards_intact(big, n, what):
-    assert bool(_sentinel(big[:G]).all()) and bool(_sentinel(big[G + n:]).all()), f'{what}: written outside the output'
 
 
 # ---- r3dp_secc_vertices --------------------------------------------------------------------------------------------------------------------
@@ -120,13 +101,13 @@ def _pose(B, pose, seed):
 
 def _launch_vertices(basis, mean, N, n_id, n_exp, id_t, ids, exp_p, exps, euler, trans, B):
     """r3dp_secc_vertices into a buffer between guards: every element written, nothing else, w = 0."""
-    big, verts = _guarded(B * N * 4)
+    big, verts = guarded(B * N * 4, torch.float32, device=DEV)
     p = capi.ptr
     capi.check(capi.lib().r3dp_secc_vertices(p(basis), p(mean), N, n_id, n_exp, p(id_t), ids, exp_p, exps, p(euler), p(trans), B, 10.0, TAN,
                                              p(verts), capi.stream()))
     torch.cuda.synchronize()
-    _guards_intact(big, B * N * 4, 'vertices')
-    assert not bool(_sentinel(verts).any()), 'vertices: an element was not written'
+    assert guards_intact(big, B * N * 4), 'vertices: written outside the output'
+    assert not bool(untouched(verts).any()), 'vertices: an element was not written'
     v = verts.view(B, N, 4)
     assert bool((v[..., 3] == 0).all())
     return v
@@ -170,22 +151,22 @@ def _raster(verts, N, faces, ncc4, B, S, drop_face0, with_mask):
     """raster then resolve, the key buffer read back between them; every output between guards.  -> (face [B,S,S], secc, mask or None)."""
     L, p, st = capi.lib(), capi.ptr, capi.stream()
     F = faces.shape[0]
-    kbig, keys = _guarded(B * S * S, torch.int64)
+    kbig, keys = guarded(B * S * S, torch.int64, device=DEV)
     keys.fill_(-1)
     capi.check(L.r3dp_secc_raster(p(verts), N, p(faces, torch.int32), F, B, S, p(keys, torch.int64), st))
     kimg = keys.clone()
-    sbig, secc = _guarded(B * 3 * S * S)
-    mbig, mask = _guarded(B * S * S) if with_mask else (None, None)
+    sbig, secc = guarded(B * 3 * S * S, torch.float32, device=DEV)
+    mbig, mask = guarded(B * S * S, torch.float32, device=DEV) if with_mask else (None, None)
     capi.check(L.r3dp_secc_resolve(p(verts), N, p(faces, torch.int32), p(ncc4), B, S, int(drop_face0), p(keys, torch.int64), p(secc),
                                    p(mask), st))
     torch.cuda.synchronize()
     assert bool((keys == -1).all()), 'resolve leaves the key buffer empty'
-    _guards_intact(kbig, B * S * S, 'keys')
-    _guards_intact(sbig, B * 3 * S * S, 'secc')
-    assert not bool(_sentinel(secc).any()), 'secc: an element was not written'
+    assert guards_intact(kbig, B * S * S), 'keys: written outside the output'
+    assert guards_intact(sbig, B * 3 * S * S), 'secc: written outside the output'
+    assert not bool(untouched(secc).any()), 'secc: an element was not written'
     if with_mask:
-        _guards_intact(mbig, B * S * S, 'mask')
-        assert not bool(_sentinel(mask).any()), 'mask: an element was not written'
+        assert guards_intact(mbig, B * S * S), 'mask: written outside the output'
+        assert not bool(untouched(mask).any()), 'mask: an element was not written'
     k = kimg.cpu().numpy().view(np.uint64)
     face = np.where(k == np.uint64(2 ** 64 - 1), -1, (k & np.uint64(0xffffffff)).astype(np.int64)).reshape(B, S, S)
     return face, secc.view(B, 3, S, S), (mask.view(B, 1, S, S) if with_mask else None)
@@ -305,7 +286,7 @@ def _launch_blink(x, p=None, rows=ctypes.c_void_p(0), stride=0):
     """r3dp_secc_blink on x [B,3,S,S] (numpy fp32) between guards (images and scratch); p: float64 [B], or rows: the device pointer of the
     (t, T) columns of fp32 rows at the given stride."""
     B, S = x.shape[0], x.shape[-1]
-    big, secc = _guarded(x.size)
+    big, secc = guarded(x.size, torch.float32, device=DEV)
     secc.copy_(torch.from_numpy(x).reshape(-1))
     n = int(capi.lib().r3dp_secc_blink_scratch_bytes(B, S))
     sc_big = torch.full((n + 2 * 4096,), 0xA5, dtype=torch.uint8, device=DEV)
@@ -316,7 +297,7 @@ def _launch_blink(x, p=None, rows=ctypes.c_void_p(0), stride=0):
     capi.check(capi.lib().r3dp_secc_blink(capi.ptr(secc), B, S, capi.ptr(p_t, torch.float64), rows, stride,
                                           capi.ptr(sc, torch.uint8), capi.ptr(faults, torch.int32), capi.stream()))
     torch.cuda.synchronize()
-    _guards_intact(big, x.size, 'blink images')
+    assert guards_intact(big, x.size), 'blink images: written outside the output'
     assert bool((sc_big[:4096 + off] == 0xA5).all()) and bool((sc_big[4096 + off + n:] == 0xA5).all()), 'blink: written outside the scratch'
     return secc.view(x.shape).cpu().numpy(), int(faults.item())
 
@@ -413,21 +394,14 @@ def test_drop_in_control_edges(bfm):
 
 
 # ---- the recorded launches -----------------------------------------------------------------------------------------------------------------
-class _Recorder:
-    """Stands in for the library object: records every SECC renderer / blink launch and passes every call on unchanged."""
+class _SeccCalls(Recorder):
+    """Records every SECC renderer / blink launch as its secc_launch_reference signature."""
 
     def __init__(self, lib):
-        self.lib, self.calls = lib, []
+        super().__init__(lib, lr.LAUNCHES.__contains__)
 
-    def __getattr__(self, name):
-        fn = getattr(self.lib, name)
-        if name not in lr.LAUNCHES:
-            return fn
-
-        def call(*args):
-            self.calls.append(lr.signature(name, args, capi._SIGNATURES[name][1]))
-            return fn(*args)
-        return call
+    def record(self, name, args):
+        return lr.signature(name, args, capi._SIGNATURES[name][1])
 
 
 def _backbone(seed=7):
@@ -450,7 +424,7 @@ def _table_rows(N, F):
 
 
 @torch.no_grad()
-def test_secc_launches_have_rows(bfm, monkeypatch):
+def test_secc_launches_have_rows(bfm):
     kw, _ = bfm
     r = renderer(kw, 512)
     r224 = r3.SECC_Renderer(device=DEV, **kw)
@@ -468,31 +442,26 @@ def test_secc_launches_have_rows(bfm, monkeypatch):
     u_c = syn.make_jitter(4, 4096, 48, 0, seed=3)[0].to(DEV)
     img = r.render(cs)[1][0].clone()
     torch.cuda.synchronize()
-    rec = _Recorder(capi.lib())
-    monkeypatch.setattr(capi, '_lib', rec)
     recorded = []
 
     def run(shape, fn, **kw_plan):
         rec.calls.clear()
         fn()
         torch.cuda.synchronize()
-        want = lr.launch_plan(shape, N, F, r.tan_half, **kw_plan)
         got = list(rec.calls)
-        assert got == want, f'{shape}: the code launches ' + '; '.join(str(x) for x in got if x not in want) + \
-            ' not in launch_plan, which has ' + '; '.join(str(x) for x in want if x not in got) + f' (got {len(got)}, planned {len(want)})'
+        assert_plan(got, lr.launch_plan(shape, N, F, r.tan_half, **kw_plan), shape)
         recorded.extend((shape, s) for s in got)
 
-    for blink, eng in engines.items():
-        rows = torch.cat([c['id'], c['exp']] + ([torch.tensor([[1., 8.], [0., 0.], [5., 10.], [3., 9.]])] if blink else []), 1).to(DEV)
-        run('begin_planes', lambda: eng.begin_planes(cano, coeff_src=cs))
-        run('step_blink' if blink else 'step', lambda: eng.step(None, cams, u_c, coeff=rows), B=4)
-    run('forward', lambda: r224(*(c[k].to(DEV) for k in ('id', 'exp', 'euler', 'trans'))), B=4)
-    run('blink_eye_for_secc', lambda: r3.blink_eye_for_secc(img, 0.5), img_size=512)
-    monkeypatch.setattr(capi, '_lib', rec.lib)
+    with _SeccCalls(capi.lib()) as rec:
+        for blink, eng in engines.items():
+            rows = torch.cat([c['id'], c['exp']] + ([torch.tensor([[1., 8.], [0., 0.], [5., 10.], [3., 9.]])] if blink else []), 1).to(DEV)
+            run('begin_planes', lambda: eng.begin_planes(cano, coeff_src=cs))
+            run('step_blink' if blink else 'step', lambda: eng.step(None, cams, u_c, coeff=rows), B=4)
+        run('forward', lambda: r224(*(c[k].to(DEV) for k in ('id', 'exp', 'euler', 'trans'))), B=4)
+        run('blink_eye_for_secc', lambda: r3.blink_eye_for_secc(img, 0.5), img_size=512)
     table = _table_rows(N, F)
     missing = [f'{shape}: {s}' for shape, s in recorded if s not in table]
-    assert not missing, 'SECC launches without a table row:\n' + '\n'.join(missing)
     launched = {s for _, s in recorded}
     prod = ('engine', 'forward', 'class', 'drop-in')
     stale = [f'{tag}: {s}' for s, tag in table.items() if tag.startswith(prod) and s not in launched]
-    assert not stale, 'table rows the engine / class no longer launch:\n' + '\n'.join(stale)
+    assert_rows(missing, stale, 'the engine / class')

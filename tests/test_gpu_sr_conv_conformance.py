@@ -17,7 +17,6 @@
   logical output is written (canaries, the lo halves and the uint8 frames included) and every fp16 / fp32 element of it is.
 * The input and packing kernels: weight packing exactly, the composed up weights against the float64 composition, and every input
   resize against float64 bilinear interpolation and bit for bit against each other."""
-import ctypes
 import math
 import re
 
@@ -27,7 +26,7 @@ import torch.nn.functional as F
 
 from real3dportrait_b200 import _capi as capi
 import sr_conv_reference as scr
-from test_gpu_tc_exact_torso import _check_split_layout, _split
+from launch_harness import Recorder, assert_rows, bits, check_split_layout, given, guarded, guards_intact, split_cat, untouched
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
@@ -42,7 +41,7 @@ def _pad64(c):
 
 def _store(v, split):
     """fp32 NHWC -> the kernel's activation tensor: fp16, or [hi | lo] with hi = fp16(v), lo = fp16(v - hi)."""
-    return _split(v) if split else v.half().contiguous()
+    return split_cat(v) if split else v.half().contiguous()
 
 
 def _fn(name, split):
@@ -103,25 +102,14 @@ def _output_shapes(P):
     return shapes
 
 
-GUARD = 4096
-#: sentinel bit patterns of the canary buffers (fp16 and fp32 NaNs no kernel produces, and 0xA5 for the uint8 frames)
-SENTINEL = {F16: (torch.int16, 0x7E55), torch.float32: (torch.int32, 0x7FC01234), torch.uint8: (torch.uint8, 0xA5)}
-
-
-def _bits(t):
-    return t.view(SENTINEL[t.dtype][0])
-
-
 def _alloc(P, canary):
     outs, guards = {}, {}
     for name, (shape, dt) in _output_shapes(P).items():
         if not canary:
             outs[name] = torch.empty(shape, device=DEV, dtype=dt)
             continue
-        n = math.prod(shape)
-        buf = torch.empty(n + 2 * GUARD, device=DEV, dtype=dt)
-        _bits(buf).fill_(SENTINEL[dt][1])
-        outs[name], guards[name] = buf[GUARD:GUARD + n].view(shape), buf
+        buf, v = guarded(math.prod(shape), dt, device=DEV)
+        outs[name], guards[name] = v.view(shape), buf
     return outs, guards
 
 
@@ -154,11 +142,9 @@ def _run(P, canary=False):
     _launch(P, out)
     torch.cuda.synchronize()
     for name, buf in guards.items():
-        s = SENTINEL[buf.dtype][1]
-        b = _bits(buf)
-        assert bool((b[:GUARD] == s).all()) and bool((b[-GUARD:] == s).all()), f'{P["fam"]}: {name} written outside its bounds'
+        assert guards_intact(buf, out[name].numel()), f'{P["fam"]}: {name} written outside its bounds'
         if buf.dtype != torch.uint8:
-            assert not bool((b[GUARD:-GUARD] == s).any()), f'{P["fam"]}: elements of {name} left unwritten'
+            assert not bool(untouched(out[name]).any()), f'{P["fam"]}: elements of {name} left unwritten'
     return out
 
 
@@ -344,7 +330,7 @@ def test_conv_vs_float64(case, mode):
     out = _run(P, canary=True)
     _check_images(P, out, mode, tag)
     if split and 'y' in out:
-        _check_split_layout(out['y'])
+        check_split_layout(out['y'])
     if case in PRODUCTION or case in PER_SAMPLE:                      # the last image is computed by the CTAs' last units
         k = N - 1
         _assert_same_bits(_run(_slice(P, k)), {name: t[k:k + 1] for name, t in out.items()}, f'{tag}: image {k} vs its N=1 launch')
@@ -386,7 +372,7 @@ def _weights_of_set0(P, replicate):
 
 def _assert_same_bits(a, b, what):
     for name in a:
-        assert torch.equal(_bits(a[name]), _bits(b[name])), f'{what}: {name} differs'
+        assert torch.equal(bits(a[name]), bits(b[name])), f'{what}: {name} differs'
 
 
 @pytest.mark.parametrize('mode', MODES)
@@ -405,7 +391,7 @@ def test_conv_bits_slicing_shared_determinism_canaries(key, mode):
         Q = dict(P, u8=True)
         _assert_same_bits(_run(Q, canary=True), _run(Q, canary=True), f'{fam} {mode}: repeated uint8 launch')
     if split and 'y' in full:
-        _check_split_layout(full['y'])
+        check_split_layout(full['y'])
 
 
 # ---- the launches of the benchmarked step ------------------------------------------------------------------------------------------------
@@ -413,30 +399,8 @@ def test_conv_bits_slicing_shared_determinism_canaries(key, mode):
 CONV_ENTRY = re.compile(r'r3dp_sr_tcx?_(layer|layer_up_composed|layer_torgb|layer_torgb_noup|conv|conv_res|last_layer|last_layer_ex)$')
 
 
-class _Recorder:
-    """Stands in for the library object: records the arguments of every conv_tc3 entry point and passes every call on unchanged."""
-
-    def __init__(self, lib):
-        self.lib, self.calls = lib, []
-
-    def __getattr__(self, name):
-        fn = getattr(self.lib, name)
-        if not CONV_ENTRY.match(name):
-            return fn
-
-        def call(*args):
-            self.calls.append((name, args))
-            return fn(*args)
-        return call
-
-
-def _given(p):
-    """A pointer argument is not NULL (capi.ptr(None) is a NULL c_void_p; callers also pass None)."""
-    return (p.value if isinstance(p, ctypes.c_void_p) else p) is not None
-
-
 def _row_of_call(name, a):
-    """(table, row) of one recorded launch: a CASES row of this module."""
+    """The CASES row of one recorded launch."""
     op, opt = name.split('_', 3)[3], {}
     if op in ('layer', 'layer_up_composed'):
         fam = 'composed' if op == 'layer_up_composed' else ('layer1' if a[9] == 1 else 'layer2')
@@ -444,25 +408,25 @@ def _row_of_call(name, a):
     elif op in ('layer_torgb', 'layer_torgb_noup'):
         fam = 'layer_torgb' if op == 'layer_torgb' else 'noup'
         N, Nw, I, O, H, W = a[6:12]
-        opt['skip'] = _given(a[5])
+        opt['skip'] = given(a[5])
     elif op in ('conv', 'conv_res'):
         fam = 'conv_res'
         N, Nw, I, O, H, W, opt['ksize'], opt['act'] = a[3:11]
-        opt['res'] = op == 'conv_res' and _given(a[11])
+        opt['res'] = op == 'conv_res' and given(a[11])
     else:                                                             # last_layer(_ex): 128 couts, the image only
         fam, O = 'last', 128
         N, Nw, I, H, W = a[6:11]
-        opt['skip'] = _given(a[5])
+        opt['skip'] = given(a[5])
         if op == 'last_layer_ex' or name.startswith('r3dp_sr_tcx_'):
-            opt['u8'], opt['clamp'] = _given(a[12]), a[13]
-    return 'CASES', (fam, N, Nw, I, O, H, W, {k: v for k, v in opt.items() if v != DEFAULT_OPT[k]})
+            opt['u8'], opt['clamp'] = given(a[12]), a[13]
+    return fam, N, Nw, I, O, H, W, {k: v for k, v in opt.items() if v != DEFAULT_OPT[k]}
 
 
 #: the options of a CASES row that _operands() defaults
 DEFAULT_OPT = {'ksize': 3, 'act': 1, 'skip': False, 'res': False, 'clamp': 0, 'u8': False, 'same_res': 0}
 
 
-def _signature(table, row):
+def row_signature(row):
     """What decides a launch: the row with every option at its default made explicit (a uint8 launch clamps)."""
     fam, N, Nw, I, O, H, W, opt = row
     o = dict(DEFAULT_OPT, **opt)
@@ -470,42 +434,42 @@ def _signature(table, row):
             o['same_res'])
 
 
-def test_benchmarked_launches_have_rows(monkeypatch):
+def test_benchmarked_launches_have_rows():
     """Every conv_tc3 launch of the benchmarked step has a float64 row of the same shape and options: bench.py's FrameEngine(batch=4) in 'tc'
     and in 'tc_exact', and its configs[4], the torso head (stub warper, fuse mode v2) through RenderHead.synthesis without the clip's
     constants and through the engine after begin_clip().  One eager step of each, recorded at the C entry points."""
     from real3dportrait_b200 import engine, synthetic as syn
-    rec = _Recorder(capi.lib())
-    monkeypatch.setattr(capi, '_lib', rec)
     B = 4
     planes, cams = syn.make_planes(B, seed=80).to(DEV), syn.make_cameras(B, seed=81).to(DEV)
     u_c, u_f = (u.to(DEV) for u in syn.make_jitter(B, 64 * 64, 48, 48, seed=82))
     mlp = syn.make_decoder_params(seed=4)
-    for mode in ('tc', 'tc_exact'):
-        eng = engine.FrameEngine(batch=B, sr_mode=mode, use_graph=False, hp={'num_samples_fine': 0})
-        eng.load_params(mlp, syn.make_sr_params(seed=5))
-        eng.step(planes, cams, u_c)
-    eng = engine.FrameEngine(batch=B, sr_mode='tc', use_graph=False, hp=dict(syn.WARP_HPARAMS, num_samples_fine=48), torso_model=syn.StubTorsoModel())
-    eng.load_params(mlp, syn.make_sr_warp_params(seed=6))
-    inp = {k: v.to(DEV) for k, v in syn.make_warp_inputs(1, seed=7).items()}
-    kp_d = (torch.rand(B, 68, 3, generator=torch.Generator().manual_seed(9)) * 2 - 1).to(DEV)
-    cond = {'ref_torso_img': inp['ref_torso_rgb'].expand(B, -1, -1, -1).contiguous(), 'bg_img': inp['ref_bg_rgb'].expand(B, -1, -1, -1).contiguous(),
-            'segmap': inp['segmap'].expand(B, -1, -1, -1).contiguous(), 'kp_s': inp['kp_s'].expand(B, -1, -1).contiguous(), 'kp_d': kp_d}
-    eng.head.synthesis(planes, cams, cond=cond, u_coarse=u_c, u_fine=u_f)
-    eng.begin_clip(inp['ref_torso_rgb'], inp['ref_bg_rgb'], inp['segmap'], inp['kp_s'])
-    eng.step(planes, cams, u_c, u_f, kp_d=kp_d)
-    torch.cuda.synchronize()
-    have = {('CASES', _signature('CASES', row)) for row in CASES}
+    with Recorder(capi.lib(), CONV_ENTRY.match) as rec:
+        for mode in ('tc', 'tc_exact'):
+            eng = engine.FrameEngine(batch=B, sr_mode=mode, use_graph=False, hp={'num_samples_fine': 0})
+            eng.load_params(mlp, syn.make_sr_params(seed=5))
+            eng.step(planes, cams, u_c)
+        eng = engine.FrameEngine(batch=B, sr_mode='tc', use_graph=False, hp=dict(syn.WARP_HPARAMS, num_samples_fine=48),
+                                 torso_model=syn.StubTorsoModel())
+        eng.load_params(mlp, syn.make_sr_warp_params(seed=6))
+        inp = {k: v.to(DEV) for k, v in syn.make_warp_inputs(1, seed=7).items()}
+        kp_d = (torch.rand(B, 68, 3, generator=torch.Generator().manual_seed(9)) * 2 - 1).to(DEV)
+        cond = {'ref_torso_img': inp['ref_torso_rgb'].expand(B, -1, -1, -1).contiguous(),
+                'bg_img': inp['ref_bg_rgb'].expand(B, -1, -1, -1).contiguous(), 'segmap': inp['segmap'].expand(B, -1, -1, -1).contiguous(),
+                'kp_s': inp['kp_s'].expand(B, -1, -1).contiguous(), 'kp_d': kp_d}
+        eng.head.synthesis(planes, cams, cond=cond, u_coarse=u_c, u_fine=u_f)
+        eng.begin_clip(inp['ref_torso_rgb'], inp['ref_bg_rgb'], inp['segmap'], inp['kp_s'])
+        eng.step(planes, cams, u_c, u_f, kp_d=kp_d)
+        torch.cuda.synchronize()
+    have = {row_signature(row) for row in CASES}
     launches = {}
     for name, args in rec.calls:
-        t, row = _row_of_call(name, args)
-        launches.setdefault((t, _signature(t, row)), (name, t, row))
-    assert {row[0] for _, t, row in launches.values()} >= {'composed', 'layer_torgb', 'layer2', 'last', 'conv_res', 'layer1', 'noup'}
-    missing = [f'{name}: {row} (in {t})' for key, (name, t, row) in launches.items() if key not in have]
-    assert not missing, 'launches of the benchmarked step without a float64 row:\n' + '\n'.join(missing)
-    stale = [row for row in PRODUCTION if row not in SECC_PRODUCTION and row not in IMG2PLANE_PRODUCTION
-             and ('CASES', _signature('CASES', row)) not in launches]
-    assert not stale, f'PRODUCTION rows the benchmarked step no longer launches: {stale}'
+        row = _row_of_call(name, args)
+        launches.setdefault(row_signature(row), (name, row))
+    assert {row[0] for _, row in launches.values()} >= {'composed', 'layer_torgb', 'layer2', 'last', 'conv_res', 'layer1', 'noup'}
+    missing = [f'{name}: {row} (in CASES)' for key, (name, row) in launches.items() if key not in have]
+    stale = [f'PRODUCTION {row}' for row in PRODUCTION if row not in SECC_PRODUCTION and row not in IMG2PLANE_PRODUCTION
+             and row_signature(row) not in launches]
+    assert_rows(missing, stale, 'the benchmarked step')
 
 
 # ---- packing kernels ---------------------------------------------------------------------------------------------------------------------
@@ -523,8 +487,8 @@ def test_pack_weights_exact(I, mode):
         halves.append((1024 * t - halves[0].float()).half())
     for h, want in enumerate(halves):
         got = wp[..., h * Ip:(h + 1) * Ip]
-        assert torch.equal(_bits(got[..., :I].contiguous()), _bits(want.contiguous())), (mode, I, h)
-        assert bool((_bits(got[..., I:]) == 0).all()), (mode, I, h)
+        assert torch.equal(bits(got[..., :I].contiguous()), bits(want.contiguous())), (mode, I, h)
+        assert bool((bits(got[..., I:]) == 0).all()), (mode, I, h)
 
 
 @pytest.mark.parametrize('mode', MODES)
@@ -542,7 +506,7 @@ def test_pack_weights_up_composed_vs_float64(I, mode):
     floor = scr.FLOOR_F16 / (scr.SPLIT_WEIGHT_SCALE if split else 1.0)
     scr.check_bound(scr.packed_weights(wpc, I, split), ref, S, scr.alpha_store(split), 2.0 ** -21, floor, tag=f'{mode} composed weights I={I}')
     for h in range(2 if split else 1):
-        assert bool((_bits(wpc[..., h * Ip + I:(h + 1) * Ip]) == 0).all())
+        assert bool((bits(wpc[..., h * Ip + I:(h + 1) * Ip]) == 0).all())
 
 
 # ---- input resizes -----------------------------------------------------------------------------------------------------------------------
@@ -581,12 +545,12 @@ def test_input_resizes_vs_float64_and_each_other(src):
     lo = (v - hi.float()).half()
     for (name, split), y in outs.items():
         if name == 'rgb':
-            assert torch.equal(_bits(y), _bits(y32[:, :3].contiguous())), (name, split)
+            assert torch.equal(bits(y), bits(y32[:, :3].contiguous())), (name, split)
             continue
         halves = (hi, lo) if split else (hi,)
         for h, want in enumerate(halves):
             got = y[..., h * Cp:(h + 1) * Cp]
-            assert torch.equal(_bits(got[..., :C].contiguous()), _bits(want.contiguous())), (name, split, h)
-            assert bool((_bits(got[..., C:]) == 0).all()), (name, split, h)
+            assert torch.equal(bits(got[..., :C].contiguous()), bits(want.contiguous())), (name, split, h)
+            assert bool((bits(got[..., C:]) == 0).all()), (name, split, h)
         scr.check_bound(scr.nhwc(y, split)[:, :C], ref, S, scr.alpha_store(split), 2.0 ** -21, scr.FLOOR_F16,
                         tag=f'{name} split={int(split)} {src}->{size}')

@@ -9,6 +9,7 @@ import torch.nn.functional as F
 
 import real3dportrait_b200 as r3
 from real3dportrait_b200 import _capi as capi, sr_tc, synthetic as syn
+from launch_harness import check_split_layout, split_cat
 from oracle import real3d_oracle as orc
 
 pytestmark = pytest.mark.gpu
@@ -20,23 +21,10 @@ def _maxdiff(a, b):
     return float((a.detach().float().cpu() - b.detach().float().cpu()).abs().max())
 
 
-def _split(v: torch.Tensor) -> torch.Tensor:
-    """fp32 [..., C] -> fp16 [..., 2C] = [hi | lo], hi = fp16(v), lo = fp16(v - hi)."""
-    hi = v.half()
-    return torch.cat([hi, (v - hi.float()).half()], dim=-1).contiguous()
-
-
 def _join(t: torch.Tensor) -> torch.Tensor:
     """[hi | lo] fp16 [..., 2C] -> fp64 [..., C]."""
     C_ = t.shape[-1] // 2
     return t[..., :C_].double() + t[..., C_:].double()
-
-
-def _check_split_layout(t: torch.Tensor):
-    """every stored pair is hi = fp16(v), lo = fp16(v - hi): |lo| is at most half an fp16 ulp of hi."""
-    C_ = t.shape[-1] // 2
-    hi, lo = t[..., :C_].float(), t[..., C_:].float()
-    assert bool((lo.abs() <= hi.abs() * 2.0 ** -11 + 2.0 ** -24).all())
 
 
 def _exact_bars(tag, err, rng, err_tc, guard=EXACT_ABS):
@@ -167,8 +155,8 @@ def test_tcx_conv_res_relu_residual():
     torch.nn.init.uniform_(conv.bias, -0.5, 0.5)
     conv = conv.to(DEV)
     packed = sr_tc.pack_plain(conv, I, split=True)
-    xs = _split(_rand(N, H, W, I, seed=1)).to(DEV)
-    res = _split(_rand(N, H, W, O, seed=2)).to(DEV)
+    xs = split_cat(_rand(N, H, W, I, seed=1)).to(DEV)
+    res = split_cat(_rand(N, H, W, O, seed=2)).to(DEV)
     y = sr_tc.conv_plain(xs, packed, 3, residual=res, split=True)
     torch.cuda.synchronize()
     assert y.shape == (N, H, W, 2 * O)
@@ -177,14 +165,14 @@ def test_tcx_conv_res_relu_residual():
     err = _maxdiff(_join(y.cpu()), ref)
     print(f'tcx_conv_res: max-abs {err:.3e} on max |ref| {float(ref.abs().max()):.2f}')
     assert err < 2e-5 * float(ref.abs().max()), err
-    _check_split_layout(y.cpu())
+    check_split_layout(y.cpu())
 
 
 @pytest.mark.parametrize('shared', [False, True])
 def test_tcx_alpha_cat_ex(shared):
     N, H, W, Ca, Cb = 2, 3, 5, 64, 128
-    xa = _split(_rand(N, H, W, Ca, seed=3)).to(DEV)
-    xb = _split(_rand(1 if shared else N, H, W, Cb, seed=4)).to(DEV)
+    xa = split_cat(_rand(N, H, W, Ca, seed=3)).to(DEV)
+    xb = split_cat(_rand(1 if shared else N, H, W, Cb, seed=4)).to(DEV)
     al = torch.rand(N, H, W, generator=torch.Generator().manual_seed(5)).to(DEV)
     out = torch.empty(N, H, W, 2 * (Ca + Cb), device=DEV, dtype=torch.float16)
     capi.check(capi.lib().r3dp_sr_tcx_alpha_cat_ex(capi.ptr(xa, torch.float16), Ca, 2 * Ca, capi.ptr(xb, torch.float16), Cb, 2 * Cb, int(shared),
@@ -194,12 +182,12 @@ def test_tcx_alpha_cat_ex(shared):
     ref = torch.cat([_join(xa.cpu()) * a, _join(xb.cpu()).expand(N, -1, -1, -1) * (1 - a)], dim=-1)
     err = _maxdiff(_join(out.cpu()), ref)
     assert err < 1e-6 * float(ref.abs().max()), err
-    _check_split_layout(out.cpu())
+    check_split_layout(out.cpu())
 
 
 def test_tcx_alpha_mix():
     N, H, W, Cc = 2, 3, 5, 64
-    xa, xb = _split(_rand(N, H, W, Cc, seed=6)).to(DEV), _split(_rand(N, H, W, Cc, seed=7)).to(DEV)
+    xa, xb = split_cat(_rand(N, H, W, Cc, seed=6)).to(DEV), split_cat(_rand(N, H, W, Cc, seed=7)).to(DEV)
     al = torch.rand(N, H, W, generator=torch.Generator().manual_seed(8)).to(DEV)
     out = torch.empty(N, H, W, 2 * Cc, device=DEV, dtype=torch.float16)
     capi.check(capi.lib().r3dp_sr_tcx_alpha_mix(capi.ptr(xa, torch.float16), 2 * Cc, capi.ptr(xb, torch.float16), 2 * Cc, capi.ptr(al), Cc, N, H, W,
@@ -209,13 +197,13 @@ def test_tcx_alpha_mix():
     ref = _join(xa.cpu()) * a + _join(xb.cpu()) * (1 - a)
     err = _maxdiff(_join(out.cpu()), ref)
     assert err < 1e-6 * float(ref.abs().max()), err
-    _check_split_layout(out.cpu())
+    check_split_layout(out.cpu())
 
 
 @pytest.mark.parametrize('same_res', [0, 1])
 def test_tcx_torgb_ex(same_res):
     N, H, W, Cc = 2, 8, 12, 64
-    xs = _split(_rand(N, H, W, Cc, seed=9)).to(DEV)
+    xs = split_cat(_rand(N, H, W, Cc, seed=9)).to(DEV)
     wrgb, brgb = (0.1 * _rand(N, 3, Cc, seed=10)).to(DEV), _rand(3, seed=11).to(DEV)
     img_prev = _rand(N, 3, H, W, seed=12) if same_res else _rand(N, 3, H // 2, W // 2, seed=12)
     out = torch.empty(N, 3, H, W, device=DEV)
@@ -230,7 +218,7 @@ def test_tcx_torgb_ex(same_res):
 
 def test_tcx_layer_torgb_noup():
     N, H, W, I, O = 2, 4, 128, 64, 128
-    xs = _split(_rand(N, H, W, I, seed=13)).to(DEV)
+    xs = split_cat(_rand(N, H, W, I, seed=13)).to(DEV)
     wf = (_rand(1, O, I, 3, 3, seed=14) / 24.0).to(DEV)
     wp = torch.empty(1, 9, O, 2 * I, device=DEV, dtype=torch.float16)
     L = capi.lib()
@@ -249,4 +237,4 @@ def test_tcx_layer_torgb_noup():
     err_y, err_img = _maxdiff(_join(y.cpu()), v.permute(0, 2, 3, 1)), _maxdiff(img, ref_img)
     print(f'tcx_layer_torgb_noup: y max-abs {err_y:.3e}, image max-abs {err_img:.3e}')
     assert err_y < 2e-5 * float(v.abs().max()) and err_img < 2e-5 * float(ref_img.abs().max()), (err_y, err_img)
-    _check_split_layout(y.cpu())
+    check_split_layout(y.cpu())

@@ -21,8 +21,7 @@ import real3dportrait_b200 as r3
 import sr_conv_reference as scr
 import torso_fusion_reference as tfr
 from real3dportrait_b200 import _capi as capi, sr_tc, synthetic as syn
-from test_gpu_sr_conv_conformance import GUARD, SENTINEL, _bits
-from test_gpu_tc_exact_torso import _check_split_layout
+from launch_harness import bits, check_split_layout, guarded, guards_intact, untouched
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
@@ -47,19 +46,16 @@ def _run(launch, shapes, inputs=(), canary=True):
         if not canary:
             outs[name] = torch.empty(shape, device=DEV, dtype=dt)
             continue
-        n = math.prod(shape)
-        buf = torch.empty(n + 2 * GUARD, device=DEV, dtype=dt)
-        _bits(buf).fill_(SENTINEL[dt][1])
-        outs[name], guards[name] = buf[GUARD:GUARD + n].view(shape), buf
+        buf, v = guarded(math.prod(shape), dt, device=DEV)
+        outs[name], guards[name] = v.view(shape), buf
     before = [t.clone() for t in inputs]
     launch(outs)
     torch.cuda.synchronize()
     for name, buf in guards.items():
-        s, b = SENTINEL[buf.dtype][1], _bits(buf)
-        assert bool((b[:GUARD] == s).all()) and bool((b[-GUARD:] == s).all()), f'{name} written outside its bounds'
-        assert not bool((b[GUARD:-GUARD] == s).any()), f'elements of {name} left unwritten'
+        assert guards_intact(buf, outs[name].numel()), f'{name} written outside its bounds'
+        assert not bool(untouched(outs[name]).any()), f'elements of {name} left unwritten'
     for t, t0 in zip(inputs, before):
-        assert torch.equal(_bits(t), _bits(t0)), 'an operand was written'
+        assert torch.equal(bits(t), bits(t0)), 'an operand was written'
     return outs
 
 
@@ -129,16 +125,16 @@ def _check_alpha_cat(P, out):
     got = tfr.join(out['y']) if split else out['y']
     r = scr.check_bound(got, ref, ref.abs(), tfr.ALPHA_CAT[P['mode']], 0.0, tfr.FLOOR_F16, tag)
     if split:
-        _check_split_layout(out['y'])
+        check_split_layout(out['y'])
         return r
     a = P['al'][..., None]                                                   # the torch fp32 restatement: (x.float() * m).half(), bit for bit
     want = torch.cat([(P['va'].float() * a).half(), (P['vb'].float().expand(P['N'], -1, -1, -1) * (1 - a)).half()], dim=-1)
-    assert torch.equal(_bits(out['y']), _bits(want)), f'{tag}: differs from (x.float() * m).half()'
+    assert torch.equal(bits(out['y']), bits(want)), f'{tag}: differs from (x.float() * m).half()'
     if not P['shared']:                                                      # r3dp_sr_alpha_cat = alpha_cat_ex without a shared operand
         o2 = _run(lambda o: capi.check(capi.lib().r3dp_sr_alpha_cat(
             capi.ptr(P['xa'], F16), P['Ca'], P['xa'].shape[-1], capi.ptr(P['xb'], F16), P['Cb'], P['xb'].shape[-1], capi.ptr(P['al']), P['N'], P['H'],
             P['W'], capi.ptr(o['y'], F16), capi.stream())), {'y': (tuple(out['y'].shape), F16)})
-        assert torch.equal(_bits(o2['y']), _bits(out['y'])), f'{tag}: r3dp_sr_alpha_cat differs from r3dp_sr_alpha_cat_ex'
+        assert torch.equal(bits(o2['y']), bits(out['y'])), f'{tag}: r3dp_sr_alpha_cat differs from r3dp_sr_alpha_cat_ex'
     return r
 
 
@@ -170,7 +166,7 @@ def _check_cat3(P, out):
         parts = [P[k][..., h * P[k].shape[-1] // 2:][..., :P['C' + k[1]]] if halves == 2 else P[k][..., :P['C' + k[1]]] for k in ('xa', 'xb', 'xc')]
         want = tfr.cat3(*parts)
         Ct = want.shape[-1]
-        assert torch.equal(_bits(out['y'][..., h * Ct:(h + 1) * Ct]), _bits(want.contiguous())), f"cat3 {P['mode']}: half {h} differs from torch.cat"
+        assert torch.equal(bits(out['y'][..., h * Ct:(h + 1) * Ct]), bits(want.contiguous())), f"cat3 {P['mode']}: half {h} differs from torch.cat"
     return 0.0
 
 
@@ -199,7 +195,7 @@ def _check_alpha_mix(P, out):
     r = scr.check_bound(tfr.join(out['y']) if split else out['y'], ref, S, tfr.ALPHA_MIX[P['mode']], tfr.BETA_MIX[P['mode']], tfr.FLOOR_F16,
                         f"alpha_mix {P['mode']}")
     if split:
-        _check_split_layout(out['y'])
+        check_split_layout(out['y'])
     return r
 
 
@@ -259,7 +255,7 @@ def _run_person(P, canary=True):
 
 def _check_person(P, out):
     want = tfr.person_occlusion_f32(P['al'], P['torso'], P['thr'])
-    assert torch.equal(_bits(out['p']), _bits(want)), f"person_occlusion thr={P['thr']}: differs from the torch fp32 restatement"
+    assert torch.equal(bits(out['p']), bits(want)), f"person_occlusion thr={P['thr']}: differs from the torch fp32 restatement"
     return 0.0
 
 
@@ -337,8 +333,8 @@ def _check_warp_input(P, out):
     halves = (hi, (v - hi.float()).half()) if split else (hi,)
     for h, want in enumerate(halves):
         got = x0[..., h * Cp:(h + 1) * Cp]
-        assert torch.equal(_bits(got[..., :3].contiguous()), _bits(want.contiguous())), f'warp_input: x0 half {h} is not the store of rgb0'
-        assert bool((_bits(got[..., C:]) == 0).all()), f'warp_input: x0 padding channels of half {h} are not zero'
+        assert torch.equal(bits(got[..., :3].contiguous()), bits(want.contiguous())), f'warp_input: x0 half {h} is not the store of rgb0'
+        assert bool((bits(got[..., C:]) == 0).all()), f'warp_input: x0 padding channels of half {h} are not zero'
     return r
 
 
@@ -393,11 +389,11 @@ def test_fusion_bits_per_frame_and_repeat(entry, mode):
     full = run(P)
     again = run(P)
     for name in full:
-        assert torch.equal(_bits(full[name]), _bits(again[name])), f'{entry} {mode}: repeated launch differs in {name}'
+        assert torch.equal(bits(full[name]), bits(again[name])), f'{entry} {mode}: repeated launch differs in {name}'
     for k in range(P['N']):
         one = run(_frame(P, k), canary=False)
         for name in full:
-            assert torch.equal(_bits(one[name]), _bits(full[name][k:k + 1])), f'{entry} {mode}: frame {k} of the N=3 launch differs in {name}'
+            assert torch.equal(bits(one[name]), bits(full[name][k:k + 1])), f'{entry} {mode}: frame {k} of the N=3 launch differs in {name}'
 
 
 # ---- the v3 head-mask chain ------------------------------------------------------------------------------------------------------------------

@@ -8,16 +8,13 @@ import torch.nn.functional as F
 import real3dportrait_b200 as r3
 from real3dportrait_b200 import _capi as capi, synthetic as syn, torso_warp as tw
 import sr_conv_reference as scr
+import torso_motion_reference as tmr
 import torso_warper_ref as twr
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
 F16 = torch.float16
-# Accumulation term of the 3-D conv (see tests/sr_conv_reference.py for the bound): fp32 sums of up to 343 x 96 fp16 products per output
-# (x3 with split operands).  Worst ratio measured over the cases below on an H100 80GB HBM3 (700 W power limit): fp16 1.61e-6 (the K = 9
-# fuser, 114 -> 32, 7^3), split 6.84e-6 (the K = 4 fuser, 89 -> 32).  beta = 2^-18 = 3.8e-6 (2.4x) and 2^-16 = 1.5e-5 (2.2x).
-BETA3 = {False: 2.0 ** -18, True: 2.0 ** -16}
-# Measured on the same card (max-abs / range against the reference modules in fp32, TF32 off):
+# Measured on an H100 80GB HBM3, 700 W power limit (max-abs / range against the reference modules in fp32, TF32 off):
 #   estimator   K = 4  tc: deformation 7.1e-5, occlusion 4.3e-4, occlusion_2 3.7e-4    tc_exact: 1.6e-5, 5.0e-5, 4.5e-5
 #               K = 9  tc: 1.0e-4, 3.8e-4, 3.9e-4                                     tc_exact: 3.0e-5, 7.9e-5, 9.8e-5
 #   whole head  tc: image 2.8e-4, occlusion_2 2.5e-3                            tc_exact: 2.2e-5, 2.5e-4
@@ -48,23 +45,6 @@ def _store(v: torch.Tensor, split: bool) -> torch.Tensor:
 def _unpack(wp: torch.Tensor, cin: int, split: bool) -> torch.Tensor:
     """packed [nph,taps,cop,cin(x2)] -> float64 [nph,taps,cop,cin] as the kernel reads it."""
     return (wp[..., :cin].double() + wp[..., cin:].double()) / 1024.0 if split else wp.double()
-
-
-def _ref_conv(x, w, taps, up, bias=None):
-    """float64 reference: x [N,C,D,H,W], w [nph,taps,O,C] -> [N,O,D,H',W'] (up: the 4 parity phases of (kd,2,2) taps)."""
-    kd, kh, kw = taps
-    nph, _, O, C = w.shape
-    wk = w.reshape(nph, kd, kh, kw, O, C).permute(0, 4, 5, 1, 2, 3)
-    if not up:
-        y = F.conv3d(x, wk[0], padding=(kd // 2, kh // 2, kw // 2))
-    else:
-        N, _, D, H, W = x.shape
-        y = x.new_zeros(N, O, D, 2 * H, 2 * W)
-        for p in range(2):
-            for q in range(2):
-                xp = F.pad(x, (1 - q, q, 1 - p, p, kd // 2, kd // 2))
-                y[..., p::2, q::2] = F.conv3d(xp, wk[p * 2 + q])
-    return y if bias is None else y + bias.double()[None, :, None, None, None]
 
 
 def _run_conv(N, D, H, W, cin_real, cout, taps, up, split, relu=1, res=False, slice_=False, seed=0, out_f32=False):
@@ -103,8 +83,8 @@ def _run_conv(N, D, H, W, cin_real, cout, taps, up, split, relu=1, res=False, sl
     assert bool((buf[-4096:] == -7.0).all()), 'written past the output'
     xin = (scr.join(x16) if split else x16.double())[..., :cin].permute(0, 4, 1, 2, 3)
     wd = _unpack(wp, cin, split)[:, :, :O]
-    pre = _ref_conv(xin, wd, taps, up, bias[:O])
-    S = _ref_conv(xin.abs(), wd.abs(), taps, up, bias[:O].abs())
+    pre = tmr.ref_conv(xin, wd, taps, up, bias[:O])
+    S = tmr.ref_conv(xin.abs(), wd.abs(), taps, up, bias[:O].abs())
     ref = torch.relu(pre) if relu else pre
     if res:
         rv = (scr.join(r16) if split else r16.double())[..., yc0:yc0 + cout].permute(0, 4, 1, 2, 3)
@@ -119,7 +99,7 @@ def _run_conv(N, D, H, W, cin_real, cout, taps, up, split, relu=1, res=False, sl
     assert bool((raw[..., ~ins] == -7.0).all()), 'written outside the channel slice'
     alpha = scr.ALPHA_F32 if out_f32 else scr.alpha_store(split)
     extra = 0.0 if out_f32 else (2 * scr.FLOOR_F16 + (scr.ALPHA_F16 * pre.abs() if (res and not split) else 0.0))
-    return scr.check_bound(got, ref, S, alpha, BETA3[split], extra, tag=f'conv3d N{N} D{D} {H}x{W} {cin_real}->{cout} {taps} up{up} split{split}'), \
+    return scr.check_bound(got, ref, S, alpha, tmr.BETA3[split], extra, tag=f'conv3d N{N} D{D} {H}x{W} {cin_real}->{cout} {taps} up{up} split{split}'), \
         (x16, wp, bias, y)
 
 

@@ -5,7 +5,7 @@ hid_to_nchw) at its exact arguments against float64, and a recorded-launch check
   per-clip volume, N = 4 frames with a volume each, and N = 1: one row per distinct launch.
 * r3dp_mf_conv3d: the weights come from the module's own packers (pack_conv3d, compose_nearest_up3d, the fuser's channel map), so the padded
   cop rows are the module's.  The bound is sr_conv_reference's |got - ref| <= alpha |ref| + extra + beta S with
-  test_gpu_torso_motion.BETA3.  Every output sits between sentinel guards: each element of [yc0, yc0 + cout) of every voxel (and of its lo
+  torso_motion_reference.BETA3.  Every output sits between sentinel guards: each element of [yc0, yc0 + cout) of every voxel (and of its lo
   half) is written, nothing else is.  The last image of an N = 4 launch equals its N = 1 launch bit for bit.
 * The kernels around the convolutions and r3dp_tw_affine_relu: the bounds derived in tests/torso_motion_reference.py, inside the same
   guards (the fp32 outputs inside NaN guards).  Stage 2's r3dp_tw_conv, _conv_up_nearest, _narrow_conv, _gather3d and _hid_to_nchw: the
@@ -14,8 +14,6 @@ hid_to_nchw) at its exact arguments against float64, and a recorded-launch check
 * test_warper_launches_have_rows records one eager step of FrameEngine(batch=4) with the reference's warper (K = 4 and 9, `tc` and
   `tc_exact`), requires the recorded calls to equal launch_plan, fails naming a launch without a row, and fails when a row of the
   recorded plans is no longer launched."""
-import ctypes
-
 import pytest
 import torch
 
@@ -24,7 +22,8 @@ import sr_conv_reference as scr
 import test_gpu_torso_warper_layers as twl
 import torso_motion_reference as tmr
 import torso_warper_ref as twr
-from test_gpu_torso_motion import BETA3, _ref_conv
+from launch_harness import (Recorder, assert_plan, assert_rows, assert_written, call_signature, conv3d, guarded, inside, join, split_store)
+from torso_motion_reference import BETA3, ref_conv
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
@@ -32,21 +31,8 @@ F16, F32 = torch.float16, torch.float32
 #: (K, N, split, clip) of the plans the tables cover; the N = 4 per-clip ones are what test_warper_launches_have_rows records
 PLANS = [(K, N, sp, clip) for K in (4, 9) for sp in (0, 1) for N, clip in ((4, True), (4, False), (1, True))]
 RECORDED = [p for p in PLANS if p[1] == 4 and p[3]]
-SENTINEL = {F16: (torch.int16, 0x7E55), F32: (torch.int32, 0x7FC01234)}
-GUARD = 4096
 #: the argument positions of the pointers that may be NULL (torso_warper_ref.OPTIONAL_OPERANDS), per entry point
 OPTIONAL_POS = {'r3dp_mf_conv3d': (6,), 'r3dp_tw_conv': (10,), 'r3dp_tw_narrow_conv': (0, 4, 7)}
-
-
-def _given(p):
-    return (p.value if isinstance(p, ctypes.c_void_p) else p) is not None
-
-
-def signature(fn, args):
-    """A recorded call -> (entry point, its non-pointer arguments, then whether each optional operand is given), as launch_plan lists it."""
-    types = capi._SIGNATURES[fn][1]
-    a = [x for x, t in zip(args, types) if t is not capi._P] + [_given(args[i]) for i in OPTIONAL_POS.get(fn, ())]
-    return twr.launch_signature(fn, a)
 
 
 def _prefix(K, N, split, clip):
@@ -77,52 +63,6 @@ def _ids(fn):
     return [ROWS[fn][k][1] for k in ROWS[fn]]
 
 
-# ---- guarded outputs --------------------------------------------------------------------------------------------------------------------
-def _guarded(n, dt):
-    buf = torch.empty(n + 2 * GUARD, device=DEV, dtype=dt)
-    buf.view(SENTINEL[dt][0]).fill_(SENTINEL[dt][1])
-    return buf, buf[GUARD:GUARD + n]
-
-
-def _untouched(t):
-    return t.view(SENTINEL[t.dtype][0]) == SENTINEL[t.dtype][1]
-
-
-def _check_guards(buf, y, vs, inside, tag):
-    """y: the output (M voxels of vs elements); inside: bool [vs], the elements of a voxel the launch writes."""
-    torch.cuda.synchronize()
-    assert bool(_untouched(buf[:GUARD]).all()) and bool(_untouched(buf[-GUARD:]).all()), f'{tag}: written outside the output'
-    yv = y.view(-1, vs)
-    assert not bool(_untouched(yv[:, inside]).any()), f'{tag}: an output element was not written'
-    assert bool(_untouched(yv[:, ~inside]).all()), f'{tag}: written outside its channels'
-
-
-def _inside(vs, c0, n, lo, split):
-    m = torch.zeros(vs, dtype=torch.bool, device=DEV)
-    m[c0:c0 + n] = True
-    if split:
-        m[lo + c0:lo + c0 + n] = True
-    return m
-
-
-def _split_store(v: torch.Tensor, vs: int, lo: int, split: bool, c0: int = 0) -> torch.Tensor:
-    """fp32 [..., C] -> fp16 [..., vs] voxels: hi at channel c0, lo at lo + c0 when split, every other element seeded junk (never read)."""
-    g = torch.Generator(device=DEV).manual_seed(int(v.numel()) % 9973)
-    out = torch.randn(*v.shape[:-1], vs, generator=g, device=DEV).half()
-    C = v.shape[-1]
-    hi = v.half()
-    out[..., c0:c0 + C] = hi
-    if split:
-        out[..., lo + c0:lo + c0 + C] = (v - hi.float()).half()
-    return out
-
-
-def _read(y: torch.Tensor, c0: int, n: int, lo: int, split: bool) -> torch.Tensor:
-    """fp16 voxels -> float64 [..., n] of channels [c0, c0 + n) (hi + lo when split)."""
-    v = y[..., c0:c0 + n].double()
-    return v + y[..., lo + c0:lo + c0 + n].double() if split else v
-
-
 # ---- r3dp_mf_conv3d ----------------------------------------------------------------------------------------------------------------------
 def _conv3d_weights(K, tag, cin, O, taps, up, split, g):
     """The module's packing of seeded float64 weights for the layer `tag` (the logical input channels and their map as MotionWeights has
@@ -148,12 +88,6 @@ def _conv3d_weights(K, tag, cin, O, taps, up, split, g):
     return tw.pack_conv3d(w, 0.1 * rn(O), cin, bool(split), cin_map=cin_map)
 
 
-def _conv3d_launch(x, wp, bias, res, a, n, y):
-    xs, xlo, cin, _, D, H, W, kd, kh, kw, up, O, cop, relu, ys, yc0, ylo, out_f32, split, _ = a
-    capi.check(capi.lib().r3dp_mf_conv3d(capi.ptr(x, F16), xs, xlo, cin, capi.ptr(wp, F16), capi.ptr(bias), capi.ptr(res, F16), n, D, H, W, kd, kh, kw,
-                                         up, O, cop, relu, capi.ptr(y, y.dtype), ys, yc0, ylo, out_f32, split, capi.stream()))
-
-
 @torch.no_grad()
 @pytest.mark.parametrize('key', _keys('r3dp_mf_conv3d'), ids=_ids('r3dp_mf_conv3d'))
 def test_conv3d_launch(key):
@@ -164,36 +98,35 @@ def test_conv3d_launch(key):
     g = torch.Generator(device=DEV).manual_seed(_keys('r3dp_mf_conv3d').index(key) + 700)
     wp, bias, O_mod, cop_mod = _conv3d_weights(K, tag, cin, O, (kd, kh, kw), up, split, g)
     assert (O_mod, cop_mod) == (O, cop), (tag, O_mod, cop_mod)                 # the module's packing pads to the launch's cop
-    x = _split_store(torch.randn(N, D, H, W, xlo, generator=g, device=DEV), xs, xlo, split)
+    x = split_store(torch.randn(N, D, H, W, xlo, generator=g, device=DEV), xs, xlo, split)
     Ho, Wo = (2 * H, 2 * W) if up else (H, W)
     M = N * D * Ho * Wo
-    r16 = _split_store(torch.randn(N, D, Ho, Wo, O, generator=g, device=DEV), ys, ylo, split, yc0) if res else None   # the output's layout
+    r16 = split_store(torch.randn(N, D, Ho, Wo, O, generator=g, device=DEV), ys, ylo, split, yc0) if res else None   # the output's layout
     dt = F32 if out_f32 else F16
-    buf, y = _guarded(M * ys, dt)
-    _conv3d_launch(x, wp, bias, r16, a, N, y)
-    inside = _inside(ys, yc0, O, ylo, split and not out_f32)
-    _check_guards(buf, y, ys, inside, tag)
+    buf, y = guarded(M * ys, dt, device=DEV)
+    conv3d(a, x, wp, bias, r16, y)
+    mask = inside(ys, yc0, O, ylo, split and not out_f32, device=DEV)
+    assert_written(buf, y, ys, mask, tag)
     y = y.view(N, D, Ho, Wo, ys)
     wd = ((wp[..., :cin].double() + wp[..., cin:].double()) / 1024.0 if split else wp.double())[:, :, :O]
     alpha = scr.ALPHA_F32 if out_f32 else scr.alpha_store(split)
     for n in range(N):
-        xin = _read(x[n:n + 1], 0, cin, xlo, split).permute(0, 4, 1, 2, 3)
-        pre = _ref_conv(xin, wd, (kd, kh, kw), up, bias[:O])
-        S = _ref_conv(xin.abs(), wd.abs(), (kd, kh, kw), up, bias[:O].abs())
+        xin = join(x[n:n + 1], 0, cin, xlo, split).permute(0, 4, 1, 2, 3)
+        pre = ref_conv(xin, wd, (kd, kh, kw), up, bias[:O])
+        S = ref_conv(xin.abs(), wd.abs(), (kd, kh, kw), up, bias[:O].abs())
         ref = torch.relu(pre) if relu else pre
         extra = 0.0 if out_f32 else 2 * scr.FLOOR_F16
         if res:
-            rv = _read(r16[n:n + 1], yc0, O, ylo, split).permute(0, 4, 1, 2, 3)
+            rv = join(r16[n:n + 1], yc0, O, ylo, split).permute(0, 4, 1, 2, 3)
             ref, S = ref + rv, S + rv.abs()
             if not split:                                                      # tc rounds the activated value to fp16 before the add
                 extra = extra + scr.ALPHA_F16 * pre.abs()
-        got = (y[n:n + 1, ..., yc0:yc0 + O].double() if out_f32 else _read(y[n:n + 1], yc0, O, ylo, split)).permute(0, 4, 1, 2, 3)
+        got = (y[n:n + 1, ..., yc0:yc0 + O].double() if out_f32 else join(y[n:n + 1], yc0, O, ylo, split)).permute(0, 4, 1, 2, 3)
         scr.check_bound(got, ref, S, alpha, BETA3[split], extra, tag=f'{tag} image {n}')
     if N > 1:
-        one = torch.empty(D * Ho * Wo * ys, device=DEV, dtype=dt)
-        one.view(SENTINEL[dt][0]).fill_(SENTINEL[dt][1])
-        _conv3d_launch(x[N - 1:].contiguous(), wp, bias, None if r16 is None else r16[N - 1:].contiguous(), a, 1, one)
-        assert torch.equal(one.view(-1, ys)[:, inside], y[N - 1].reshape(-1, ys)[:, inside]), f'{tag}: last image vs its N=1 launch'
+        _, one = guarded(D * Ho * Wo * ys, dt, device=DEV)
+        conv3d(a, x[N - 1:].contiguous(), wp, bias, None if r16 is None else r16[N - 1:].contiguous(), one, N=1)
+        assert torch.equal(one.view(-1, ys)[:, mask], y[N - 1].reshape(-1, ys)[:, mask]), f'{tag}: last image vs its N=1 launch'
 
 
 # ---- the kernels around the convolutions ------------------------------------------------------------------------------------------------
@@ -209,15 +142,15 @@ def test_mf_input_launch(key):
     g = torch.Generator(device=DEV).manual_seed(11 + K + N + shared)
     fc = torch.randn(1 if shared else N, D, H, W, 4, generator=g, device=DEV)
     kp_s, kp_d = _kp(N, K, g)
-    buf, y = _guarded(N * D * H * W * ys, F16)
+    buf, y = guarded(N * D * H * W * ys, F16, device=DEV)
     capi.check(capi.lib().r3dp_mf_input(capi.ptr(fc), shared, capi.ptr(kp_s), capi.ptr(kp_d), N, K, D, H, W, cpad, capi.ptr(y, F16), ys, ylo, split,
                                         capi.stream()))
-    _check_guards(buf, y, ys, _inside(ys, 0, cpad, ylo, split), tag)
+    assert_written(buf, y, ys, inside(ys, 0, cpad, ylo, split, device=DEV), tag)
     y = y.view(N, D, H, W, ys)
     c0 = (K + 1) * 5
     for n in range(N):
         ref, S, extra = tmr.mf_input(fc[0 if shared else n].double(), kp_s[n].double(), kp_d[n].double())
-        got = _read(y[n], 0, c0, ylo, split)
+        got = join(y[n], 0, c0, ylo, split)
         scr.check_bound(got, ref, S, scr.alpha_store(split), tmr.BETA_SAMPLE, extra * (1 + 2.0 ** -10) + scr.FLOOR_F16, tag=f'{tag} frame {n}')
         assert bool((y[n, ..., c0:cpad] == 0).all()) and (not split or bool((y[n, ..., ylo + c0:ylo + cpad] == 0).all())), f'{tag}: pad channels'
 
@@ -228,14 +161,14 @@ def test_mf_pool_launch(key):
     _, tag = ROWS['r3dp_mf_pool'][key]
     N, D, H, W, C, xs, xlo, ys, ylo, split = key[1]
     g = torch.Generator(device=DEV).manual_seed(C + H + N)
-    x = _split_store(3 * torch.randn(N, D, 2 * H, 2 * W, C, generator=g, device=DEV), xs, xlo, split)
-    buf, y = _guarded(N * D * H * W * ys, F16)
+    x = split_store(3 * torch.randn(N, D, 2 * H, 2 * W, C, generator=g, device=DEV), xs, xlo, split)
+    buf, y = guarded(N * D * H * W * ys, F16, device=DEV)
     capi.check(capi.lib().r3dp_mf_pool(capi.ptr(x, F16), N, D, H, W, C, xs, xlo, capi.ptr(y, F16), ys, ylo, split, capi.stream()))
-    _check_guards(buf, y, ys, _inside(ys, 0, C, ylo, split), tag)
+    assert_written(buf, y, ys, inside(ys, 0, C, ylo, split, device=DEV), tag)
     y = y.view(N, D, H, W, ys)
     for n in range(N):
-        ref, S = tmr.pool(_read(x[n], 0, C, xlo, split))
-        scr.check_bound(_read(y[n], 0, C, ylo, split), ref, S, scr.alpha_store(split), tmr.BETA_POOL, scr.FLOOR_F16, tag=f'{tag} frame {n}')
+        ref, S = tmr.pool(join(x[n], 0, C, xlo, split))
+        scr.check_bound(join(y[n], 0, C, ylo, split), ref, S, scr.alpha_store(split), tmr.BETA_POOL, scr.FLOOR_F16, tag=f'{tag} frame {n}')
 
 
 @torch.no_grad()
@@ -246,13 +179,13 @@ def test_mf_head_input_launch(key):
     g = torch.Generator(device=DEV).manual_seed(5 + N)
     rgb = 2 * torch.rand(N, 3, 2 * H, 2 * W, generator=g, device=DEV) - 1
     wt = torch.rand(N, 1, 2 * H, 2 * W, generator=g, device=DEV)
-    buf, y = _guarded(N * H * W * ys, F16)
+    buf, y = guarded(N * H * W * ys, F16, device=DEV)
     capi.check(capi.lib().r3dp_mf_head_input(capi.ptr(rgb), capi.ptr(wt), N, H, W, cpad, capi.ptr(y, F16), ys, ylo, split, capi.stream()))
-    _check_guards(buf, y, ys, _inside(ys, 0, cpad, ylo, split), tag)
+    assert_written(buf, y, ys, inside(ys, 0, cpad, ylo, split, device=DEV), tag)
     y = y.view(N, H, W, ys)
     for n in range(N):
         ref, S = tmr.head_input(rgb[n:n + 1].double(), wt[n:n + 1].double())
-        scr.check_bound(_read(y[n:n + 1], 0, 4, ylo, split), ref, S, scr.alpha_store(split), tmr.BETA_HEAD_INPUT, scr.FLOOR_F16, tag=f'{tag} frame {n}')
+        scr.check_bound(join(y[n:n + 1], 0, 4, ylo, split), ref, S, scr.alpha_store(split), tmr.BETA_HEAD_INPUT, scr.FLOOR_F16, tag=f'{tag} frame {n}')
         assert bool((y[n, ..., 4:cpad] == 0).all()) and (not split or bool((y[n, ..., ylo + 4:ylo + cpad] == 0).all())), f'{tag}: pad channels'
 
 
@@ -262,14 +195,14 @@ def test_mf_head_bcast_launch(key):
     _, tag = ROWS['r3dp_mf_head_bcast'][key]
     N, D, H, W, C, xs, xlo, ys, yc0, ylo, split = key[1]
     g = torch.Generator(device=DEV).manual_seed(7 + N + ys)
-    x = _split_store(torch.randn(N, 2 * H, 2 * W, C, generator=g, device=DEV), xs, xlo, split)
-    buf, y = _guarded(N * D * H * W * ys, F16)
+    x = split_store(torch.randn(N, 2 * H, 2 * W, C, generator=g, device=DEV), xs, xlo, split)
+    buf, y = guarded(N * D * H * W * ys, F16, device=DEV)
     capi.check(capi.lib().r3dp_mf_head_bcast(capi.ptr(x, F16), N, D, H, W, C, xs, xlo, capi.ptr(y, F16), ys, yc0, ylo, split, capi.stream()))
-    _check_guards(buf, y, ys, _inside(ys, yc0, C, ylo, split), tag)
+    assert_written(buf, y, ys, inside(ys, yc0, C, ylo, split, device=DEV), tag)
     y = y.view(N, D, H, W, ys)
     for n in range(N):
-        ref, S = tmr.pool(_read(x[n], 0, C, xlo, split))
-        got = _read(y[n], yc0, C, ylo, split)
+        ref, S = tmr.pool(join(x[n], 0, C, xlo, split))
+        got = join(y[n], yc0, C, ylo, split)
         scr.check_bound(got, ref.expand(D, -1, -1, -1), S.expand(D, -1, -1, -1), scr.alpha_store(split), tmr.BETA_POOL, scr.FLOOR_F16,
                         tag=f'{tag} frame {n}')
 
@@ -283,9 +216,9 @@ def test_mf_deform_launch(key):
     logits = torch.full((N, D, H, W, ls), float('nan'), device=DEV)          # the stride's pad logits are never read
     logits[..., :K + 1] = 3 * torch.randn(N, D, H, W, K + 1, generator=g, device=DEV)
     kp_s, kp_d = _kp(N, K, g)
-    buf, y = _guarded(N * D * H * W * 3, F32)
+    buf, y = guarded(N * D * H * W * 3, F32, device=DEV)
     capi.check(capi.lib().r3dp_mf_deform(capi.ptr(logits), ls, capi.ptr(kp_s), capi.ptr(kp_d), N, K, D, H, W, capi.ptr(y), capi.stream()))
-    _check_guards(buf, y, 3, torch.ones(3, dtype=torch.bool, device=DEV), tag)
+    assert_written(buf, y, 3, torch.ones(3, dtype=torch.bool, device=DEV), tag)
     y = y.view(N, D, H, W, 3)
     for n in range(N):
         ref, S, extra = tmr.deform(logits[n, ..., :K + 1].double(), kp_s[n].double(), kp_d[n].double())
@@ -298,16 +231,16 @@ def test_mf_occlusion_launch(key):
     _, tag = ROWS['r3dp_mf_occlusion'][key]
     N, D, H, W, C, xs, xlo, split = key[1]
     g = torch.Generator(device=DEV).manual_seed(17 + N + split)
-    x = _split_store(torch.randn(N, D, H, W, C, generator=g, device=DEV), xs, xlo, split)
+    x = split_store(torch.randn(N, D, H, W, C, generator=g, device=DEV), xs, xlo, split)
     wk = (torch.randn(D, 49, C, 2, generator=g, device=DEV) / (D * 49 * C) ** 0.5 * 3).contiguous()
     bk = 0.1 * torch.randn(2, generator=g, device=DEV)
-    outs = [_guarded(N * H * W, F32) for _ in range(2)]
+    outs = [guarded(N * H * W, F32, device=DEV) for _ in range(2)]
     capi.check(capi.lib().r3dp_mf_occlusion(capi.ptr(x, F16), N, D, H, W, C, xs, xlo, split, capi.ptr(wk), capi.ptr(bk), capi.ptr(outs[0][1]),
                                             capi.ptr(outs[1][1]), capi.stream()))
     for buf, o in outs:
-        _check_guards(buf, o, 1, torch.ones(1, dtype=torch.bool, device=DEV), tag)
+        assert_written(buf, o, 1, torch.ones(1, dtype=torch.bool, device=DEV), tag)
     for n in range(N):
-        bounds = tmr.occlusion(_read(x[n], 0, C, xlo, split), wk, bk, split)
+        bounds = tmr.occlusion(join(x[n], 0, C, xlo, split), wk, bk, split)
         for (_, o), (ref, S, extra) in zip(outs, bounds):
             scr.check_bound(o.view(N, H, W)[n], ref, S, 0.0, tmr.BETA_OCC, extra, tag=f'{tag} frame {n}')
 
@@ -319,15 +252,15 @@ def test_tw_affine_relu_launch(key):
     N, H, W, C, split = key[1]
     g = torch.Generator(device=DEV).manual_seed(19 + C + N)
     cs = C * (2 if split else 1)
-    x = _split_store(3 * torch.randn(N, H, W, C, generator=g, device=DEV), cs, C, split)
+    x = split_store(3 * torch.randn(N, H, W, C, generator=g, device=DEV), cs, C, split)
     s, t = 0.5 + torch.rand(C, generator=g, device=DEV), 0.3 * torch.randn(C, generator=g, device=DEV)
-    buf, y = _guarded(N * H * W * cs, F16)
+    buf, y = guarded(N * H * W * cs, F16, device=DEV)
     capi.check(capi.lib().r3dp_tw_affine_relu(capi.ptr(x, F16), capi.ptr(s), capi.ptr(t), N, H, W, C, split, capi.ptr(y, F16), capi.stream()))
-    _check_guards(buf, y, cs, _inside(cs, 0, C, C, split), tag)
+    assert_written(buf, y, cs, inside(cs, 0, C, C, split, device=DEV), tag)
     y = y.view(N, H, W, cs)
     for n in range(N):
-        ref, S = tmr.affine_relu(_read(x[n], 0, C, C, split), s, t)
-        scr.check_bound(_read(y[n], 0, C, C, split), ref, S, scr.alpha_store(split), tmr.BETA_AFFINE, scr.FLOOR_F16, tag=f'{tag} frame {n}')
+        ref, S = tmr.affine_relu(join(x[n], 0, C, C, split), s, t)
+        scr.check_bound(join(y[n], 0, C, C, split), ref, S, scr.alpha_store(split), tmr.BETA_AFFINE, scr.FLOOR_F16, tag=f'{tag} frame {n}')
 
 
 # ---- stage 2 at the warper's launches (the layer helpers of tests/test_gpu_torso_warper_layers.py) ----------------------------------------
@@ -377,23 +310,6 @@ def test_tw_gather3d_launch(key):
 
 
 # ---- the recorded launches ---------------------------------------------------------------------------------------------------------------
-class _Recorder:
-    """Stands in for the library object: records the arguments of every r3dp_mf_* / r3dp_tw_* entry point and passes every call on."""
-
-    def __init__(self, lib):
-        self.lib, self.calls = lib, []
-
-    def __getattr__(self, name):
-        fn = getattr(self.lib, name)
-        if not name.startswith(('r3dp_mf_', 'r3dp_tw_')):
-            return fn
-
-        def call(*args):
-            self.calls.append((name, args))
-            return fn(*args)
-        return call
-
-
 def _reference_warper(K, seed, monkeypatch):
     """The reference's WarpBasedTorsoModelMediaPipe('standard') built for torso_kp_num K: its constructor copies model2.py's global hparams
     (which ref_classes() sets to K = 4, so the class is looked up first)."""
@@ -418,8 +334,7 @@ def test_warper_launches_have_rows(monkeypatch):
     planes, cam = syn.make_planes(B, seed=0).to(DEV), syn.make_cameras(B, seed=1).to(DEV)
     kp_d = (torch.rand(B, 68, 3, generator=torch.Generator().manual_seed(2)) * 2 - 1).to(DEV)
     u_c, _ = syn.make_jitter(B, 4096, 48, 0, seed=3)
-    rec = _Recorder(capi.lib())
-    launched = set()
+    launched, missing = set(), []
     for K, N, sp, clip in RECORDED:
         warper = _reference_warper(K, 41, monkeypatch)
         srp = syn.make_sr_warp_params(seed=6)
@@ -428,22 +343,16 @@ def test_warper_launches_have_rows(monkeypatch):
                                  torso_model=warper, use_graph=False, torso_stage2='cuda', torso_motion='cuda')
         eng.load_params(mlp, srp)
         eng.begin_clip(inp['ref_torso_rgb'], inp['ref_bg_rgb'], inp['segmap'], inp['kp_s'])
-        monkeypatch.setattr(capi, '_lib', rec)
-        rec.calls.clear()
-        eng.step(planes, cam, u_c.to(DEV), kp_d=kp_d)
-        torch.cuda.synchronize()
-        monkeypatch.setattr(capi, '_lib', rec.lib)
+        with Recorder(capi.lib(), lambda n: n.startswith(('r3dp_mf_', 'r3dp_tw_'))) as rec:
+            eng.step(planes, cam, u_c.to(DEV), kp_d=kp_d)
+            torch.cuda.synchronize()
         eng.end_clip()
-        got = [signature(n, a) for n, a in rec.calls]
+        got = [call_signature(n, a, OPTIONAL_POS.get(n, ())) for n, a in rec.calls]
         plan = twr.launch_plan(K, N, sp, clip)
-        want = [twr.launch_signature(f, a) for _, f, a in plan]
         where = f'K={K} N={N} {"tc_exact" if sp else "tc"}'
-        assert got == want, f'{where}: the warper launches ' + ('; '.join(f'{x}' for x in got if x not in want) or 'nothing new') + \
-            ' not in launch_plan, which has ' + ('; '.join(f'{t} {f}{a}' for (t, f, a), x in zip(plan, want) if x not in got) or 'nothing more') + \
-            f' ({len(got)} launches recorded, {len(want)} planned; where both sets agree, the order differs)'
-        missing = [f'{where}: {tag} {fn}{a}' for (tag, fn, a), s in zip(plan, got) if s not in ROWS.get(fn, {})]
-        assert not missing, 'warper launches without a float64 row:\n' + '\n'.join(missing)
+        assert_plan(got, [twr.launch_signature(f, a) for _, f, a in plan], where)
+        missing += [f'{where}: {tag} {fn}{a}' for (tag, fn, a), s in zip(plan, got) if s not in ROWS.get(fn, {})]
         launched.update(got)
     stale = [f'{tag}: {key}' for fn, rows in ROWS.items() for key, (_, tag) in rows.items()
              if any(tag.startswith(_prefix(*p)) for p in RECORDED) and key not in launched]
-    assert not stale, 'rows of the recorded plans the warper no longer launches:\n' + '\n'.join(stale)
+    assert_rows(missing, stale, 'the warper')

@@ -51,6 +51,27 @@ BETA_SAMPLE = gamma(15)
 BETA_OCC = 7 * U
 FLOOR_EXP = 2.0 ** -126
 SIGMA2 = 0.01                      # the heatmap Gaussians' variance (func_utils.py: kp_variance=0.01)
+# Accumulation term of the 3-D conv (see sr_conv_reference.py for the bound): fp32 sums of up to 343 x 96 fp16 products per output (x3
+# with split operands).  Worst ratio measured over the cases of tests/test_gpu_torso_motion.py on an H100 80GB HBM3 (700 W power limit):
+# fp16 1.61e-6 (the K = 9 fuser, 114 -> 32, 7^3), split 6.84e-6 (the K = 4 fuser, 89 -> 32).  beta = 2^-18 = 3.8e-6 (2.4x) and 2^-16 = 1.5e-5 (2.2x).
+BETA3 = {False: 2.0 ** -18, True: 2.0 ** -16}
+
+
+def ref_conv(x, w, taps, up, bias=None):
+    """float64 reference: x [N,C,D,H,W], w [nph,taps,O,C] -> [N,O,D,H',W'] (up: the 4 parity phases of (kd,2,2) taps)."""
+    kd, kh, kw = taps
+    nph, _, O, C = w.shape
+    wk = w.reshape(nph, kd, kh, kw, O, C).permute(0, 4, 5, 1, 2, 3)
+    if not up:
+        y = F.conv3d(x, wk[0], padding=(kd // 2, kh // 2, kw // 2))
+    else:
+        N, _, D, H, W = x.shape
+        y = x.new_zeros(N, O, D, 2 * H, 2 * W)
+        for p in range(2):
+            for q in range(2):
+                xp = F.pad(x, (1 - q, q, 1 - p, p, kd // 2, kd // 2))
+                y[..., p::2, q::2] = F.conv3d(xp, wk[p * 2 + q])
+    return y if bias is None else y + bias.double()[None, :, None, None, None]
 
 
 def mean2x2(x: torch.Tensor) -> torch.Tensor:
