@@ -436,6 +436,28 @@ int r3dp_sp_head_fuse(const float* g1, int h1, const float* g2, int h2, const fl
                       void* y_f16, r3dp_stream_t stream);
 int r3dp_sp_leaky(void* x_f16, long long n, float slope, r3dp_stream_t stream);
 int r3dp_sp_upsample2_flip(const void* x_f16, int N, int h, int w, int C, void* yr_f16, void* yrc_f16, r3dp_stream_t stream);
+/* The backbone in precision='tc_exact': every GEMM and conv operand split fp16 (r3dp_mf_conv3d split, r3dp_sr_tcx_conv), every activation that
+ * the `tc` path passes between launches as fp16 passed as fp32 or as split rows [hi C | lo C] (hi = fp16(v), lo = fp16(v - hi), C halves
+ * apart).  LayerNorm without a residual runs on r3dp_hb_layernorm, the embed and fp32-output LayerNorms on r3dp_sp_embed / r3dp_sp_layernorm.
+ * r3dp_sp_layernorm_split      r3dp_sp_layernorm's residual form (t required, xo may be NULL or x) with u written as split rows yh (yhs halves,
+ *                              lo at yhlo >= C)
+ * r3dp_sp_patches_split        r3dp_sp_patches of split pixels x [N,H,W][hi C | lo C] -> rows [N*Ho*Wo][hi k*k*C | lo k*k*C], the operand of
+ *                              r3dp_mf_conv3d with xs = 2K, xlo = K (K = k*k*C)
+ * r3dp_sp_attention_split      r3dp_sp_attention on fp32 q / kv (row strides qs, kvs floats) -> o split rows (os halves, lo at olo >= C)
+ * r3dp_sp_dwconv_gelu_split    r3dp_sp_dwconv_gelu on fp32 x [N,H,W,C] -> y split rows [N*H*W][hi C | lo C]
+ * r3dp_sp_head_fuse_split      r3dp_sp_head_fuse -> y split rows [N*h1*h1][hi 256 | lo 256]
+ * r3dp_sp_leaky_split          nn.LeakyReLU(slope) in place on P split rows [hi C | lo C] of the full value hi + lo
+ * r3dp_sp_upsample2_flip_split r3dp_sp_upsample2_flip on split pixels: x [N,h,w][hi C | lo C] -> yr, yrc [N,2h,2w][hi C | lo C]; C % 4 == 0 */
+int r3dp_sp_layernorm_split(const float* x, const float* t, int R, int C, const float* g, const float* b, float eps, float* xo, void* yh_f16,
+                            int yhs, int yhlo, r3dp_stream_t stream);
+int r3dp_sp_patches_split(const void* x_f16, int N, int H, int W, int C, int k, int s, int p, void* y_f16, r3dp_stream_t stream);
+int r3dp_sp_attention_split(const float* q, int qs, const float* kv, int kvs, int N, int Tq, int Tk, int heads, float scale, void* o_f16, int os,
+                            int olo, r3dp_stream_t stream);
+int r3dp_sp_dwconv_gelu_split(const float* x, int N, int H, int W, int C, const float* w, const float* b, void* y_f16, r3dp_stream_t stream);
+int r3dp_sp_head_fuse_split(const float* g1, int h1, const float* g2, int h2, const float* g3, int h3, const float* g4, int h4, int N,
+                            const float* bias, void* y_f16, r3dp_stream_t stream);
+int r3dp_sp_leaky_split(void* x_f16, long long P, int C, float slope, r3dp_stream_t stream);
+int r3dp_sp_upsample2_flip_split(const void* x_f16, int N, int h, int w, int C, void* yr_f16, void* yrc_f16, r3dp_stream_t stream);
 
 /* ------------------------------------------------ canonical plane backbone: Img2PlaneModel ---
  * (modules/img2plane/img2plane_model.py:12-81; run once per clip on the source image by cal_cano_plane, modules/real3d/secc_img2plane.py:50-62).

@@ -133,6 +133,13 @@ _SIGNATURES = {
     'r3dp_sp_head_fuse': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _I, _P, _P, _P]),
     'r3dp_sp_leaky': (_I, [_P, C.c_longlong, _F, _P]),
     'r3dp_sp_upsample2_flip': (_I, [_P, _I, _I, _I, _I, _P, _P, _P]),
+    'r3dp_sp_layernorm_split': (_I, [_P, _P, _I, _I, _P, _P, _F, _P, _P, _I, _I, _P]),
+    'r3dp_sp_patches_split': (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
+    'r3dp_sp_attention_split': (_I, [_P, _I, _P, _I, _I, _I, _I, _I, _F, _P, _I, _I, _P]),
+    'r3dp_sp_dwconv_gelu_split': (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P]),
+    'r3dp_sp_head_fuse_split': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _I, _P, _P, _P]),
+    'r3dp_sp_leaky_split': (_I, [_P, C.c_longlong, _I, _F, _P]),
+    'r3dp_sp_upsample2_flip_split': (_I, [_P, _I, _I, _I, _I, _P, _P, _P]),
     'r3dp_ip_attention': (_I, [_P, _I, _P, _I, _I, _I, _I, _I, _F, _P, _I, _P]),
     'r3dp_ip_input': (_I, [_P, _I, _I, _I, _P, _P]),
     'r3dp_ip_maxpool': (_I, [_P, _I, _I, _I, _I, _P, _P]),

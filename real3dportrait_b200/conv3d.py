@@ -54,15 +54,16 @@ def pack_conv3d(w: torch.Tensor, b: Optional[torch.Tensor], cin: int, split: boo
     return Packed(packed.contiguous(), bias, O, cop)
 
 
-def pack_gemm(w: torch.Tensor, b: Optional[torch.Tensor], dev) -> Packed:
-    """GEMM weights [O, K] (float64) -> fp16 [cop, K] on dev: pack_conv3d on 1x1x1 taps."""
-    pk = pack_conv3d(w.to(dev)[None, :, :, None, None, None], None if b is None else b.to(dev), w.shape[1], False)
+def pack_gemm(w: torch.Tensor, b: Optional[torch.Tensor], dev, split: bool = False) -> Packed:
+    """GEMM weights [O, K] (float64) -> fp16 [cop, K] ([cop, 2K] = [hi | lo] when split) on dev: pack_conv3d on 1x1x1 taps."""
+    pk = pack_conv3d(w.to(dev)[None, :, :, None, None, None], None if b is None else b.to(dev), w.shape[1], split)
     return pk._replace(w=pk.w.view(pk.cop, -1))
 
 
-def pack_taps(w: torch.Tensor, b: Optional[torch.Tensor], dev) -> Packed:
-    """3x3 conv weights [O, I, 3, 3] (float64) -> fp16 [9, cop, I] on dev, tap ky*3 + kx: pack_conv3d on 1x3x3 taps."""
-    pk = pack_conv3d(w.to(dev)[None, :, :, None], None if b is None else b.to(dev), w.shape[1], False)
+def pack_taps(w: torch.Tensor, b: Optional[torch.Tensor], dev, split: bool = False) -> Packed:
+    """3x3 conv weights [O, I, 3, 3] (float64) -> fp16 [9, cop, I] ([9, cop, 2I] = [hi | lo] when split) on dev, tap ky*3 + kx: pack_conv3d
+    on 1x3x3 taps."""
+    pk = pack_conv3d(w.to(dev)[None, :, :, None], None if b is None else b.to(dev), w.shape[1], split)
     return pk._replace(w=pk.w[0])
 
 

@@ -8,7 +8,10 @@ Weights are folded on the host in float64 and packed once per parameter set (ref
   - eval BatchNorm of fuse_head.linear_fuse goes into its weights;
   - head fold: bilinear resize (align_corners=False) is a convex combination per output pixel, so it commutes with channel mixing and passes
     constants through; ReLU(BN(W_fuse cat[R(L4 c4), R(L3 c3), R(L2 c2), L1 c1])) = ReLU(sum_i R_i(G_i c_i) + b) with G_i = diag(s) W_fuse,i L_i.
-Precision (`tc`): fp16 GEMM operands with fp32 accumulation; residual stream, LayerNorm, softmax and GELU in fp32.
+Precision (`tc`): fp16 GEMM operands with fp32 accumulation; residual stream, LayerNorm, softmax and GELU in fp32.  `tc_exact`: the same
+launch sequence with every GEMM / conv operand split into two fp16 halves ([hi | lo], weights as w * 2^10; three MMAs, fp32 accumulation)
+and every activation the `tc` path passes between launches as fp16 passed as fp32 (the GEMM outputs the attention and the DWConv read) or as
+split rows (the r3dp_sp_*_split entry points, r3dp_hb_layernorm, r3dp_sr_tcx_conv).
 """
 from __future__ import annotations
 
@@ -155,14 +158,66 @@ def plane_index_map(H: int, W: int):
     return where
 
 
+def fold_and_pack(m: 'SegFormerSECC2PlaneBackbone', dev, split: bool) -> dict:
+    """Every float64 fold of m's parameters and every r3dp_mf_conv3d weight pack, on dev (any device: nothing here launches a kernel).
+    split: the packs hold [hi | lo] of w * 2^10 (precision='tc_exact'); the fp32 tensors (prenet, patch embed 1, LayerNorms, DWConv, head
+    bias) are the same in both precisions.  The to_plane_cnn.0/2/4 packs of r3dp_sr_tc_conv are made by the module (they need CUDA)."""
+    f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()      # noqa: E731
+    d = lambda t: t.detach().double()                                   # noqa: E731
+    gemm = lambda w, b: _pack_gemm(w, b, dev, split)                    # noqa: E731
+    P = {}
+    wpre, bpre = fold_prenet(m.prenet.weight, m.prenet.bias)
+    nconst = wpre.shape[1] - 3
+    P['wpre'], P['bpre'] = f32(wpre), f32(bpre)
+    P['wpre_const'], P['wpre_tgt'] = f32(wpre[:, :nconst]), f32(wpre[:, nconst:])
+    mv = m.mix_vit
+    P['pe1'] = (f32(mv.patch_embed1.proj.weight), f32(mv.patch_embed1.proj.bias))
+    ln = lambda n: (f32(n.weight), f32(n.bias), float(n.eps))          # noqa: E731
+    stages = []
+    for s in range(4):
+        pe = getattr(mv, f'patch_embed{s + 1}')
+        st = {'pe_norm': ln(pe.norm), 'norm': ln(getattr(mv, f'norm{s + 1}'))}
+        if s > 0:
+            st['pe'] = gemm(_conv_rows(d(pe.proj.weight)), d(pe.proj.bias))
+        blocks = []
+        for blk in getattr(mv, f'block{s + 1}'):
+            at = blk.attn
+            b = {'norm1': ln(blk.norm1), 'norm2': ln(blk.norm2),
+                 'q': gemm(d(at.q.weight), d(at.q.bias)), 'kv': gemm(d(at.kv.weight), d(at.kv.bias)),
+                 'proj': gemm(d(at.proj.weight), d(at.proj.bias)),
+                 'fc1': gemm(d(blk.mlp.fc1.weight), d(blk.mlp.fc1.bias)),
+                 'fc2': gemm(d(blk.mlp.fc2.weight), d(blk.mlp.fc2.bias)),
+                 'dw': (f32(blk.mlp.dwconv.dwconv.weight.reshape(-1, 9)), f32(blk.mlp.dwconv.dwconv.bias))}
+            if SR[s] > 1:
+                b['sr'] = gemm(_conv_rows(d(at.sr.weight)), d(at.sr.bias))
+                b['sr_norm'] = ln(at.norm)
+            blocks.append(b)
+        st['blocks'] = blocks
+        stages.append(st)
+    P['stages'] = stages
+    G, hb = fold_head(m.fuse_head)
+    P['G'] = [gemm(g, None) for g in G]
+    P['head_bias'] = f32(hb)
+    P['convs'] = [{'mf': _pack_taps(d(c.weight), d(c.bias), dev, split)} for c in (m.to_plane_cnn[i] for i in (0, 2, 4))]
+    last = m.to_plane_cnn[7]
+    w7, b7 = d(last.weight), d(last.bias)
+    P['last_r'] = _pack_taps(w7[:64].flip(2), b7[:64], dev, split)          # planes 0, 1: rows mirrored
+    P['last_rc'] = _pack_taps(w7[64:].flip(2, 3), b7[64:], dev, split)      # plane 2: rows and columns mirrored
+    return P
+
+
 class SegFormerSECC2PlaneBackbone(nn.Module):
     """SegFormerSECC2PlaneBackbone(mode='b0', out_channels=96, pncc_cond_mode='cano_src_tgt') (segformer.py:673-733) on sm_90a kernels.
 
     forward(x [B, 9|6, H, W]) -> [B, 3, 32, H/2, W/2] (the reference's flipped planes), a view of channels-last data;
     begin_clip(cond_cano, cond_src) then planes_cl(cond_tgt) -> PlanesCL('hwpc') [B, H/2, W/2, 3, 32]: the per-clip prenet part folded into
-    one cached image, and the planes written by the last conv's epilogue in the render's zero-copy layout."""
+    one cached image, and the planes written by the last conv's epilogue in the render's zero-copy layout.
 
-    def __init__(self, mode='b0', out_channels=96, pncc_cond_mode='cano_src_tgt'):
+    precision: 'tc' (fp16 GEMM / conv operands, fp32 accumulation) or 'tc_exact' (fp32-grade: every GEMM and conv operand split into two
+    fp16 halves, three MMAs per product; every activation passed between launches as fp32 or split fp16).  The parameters and state_dict
+    are the same in both."""
+
+    def __init__(self, mode='b0', out_channels=96, pncc_cond_mode='cano_src_tgt', *, precision='tc'):
         super().__init__()
         if mode != 'b0':
             raise NotImplementedError(f'SegFormerSECC2PlaneBackbone: only MiT-b0 is built (got mode={mode!r})')
@@ -170,7 +225,9 @@ class SegFormerSECC2PlaneBackbone(nn.Module):
             raise NotImplementedError(f'SegFormerSECC2PlaneBackbone: only out_channels=96 (tri-planes of 32 channels) is built, got {out_channels}')
         if pncc_cond_mode not in ('cano_src_tgt', 'cano_tgt'):
             raise NotImplementedError(f'pncc_cond_mode={pncc_cond_mode!r}')
-        self.mode, self.pncc_cond_mode = mode, pncc_cond_mode
+        if precision not in ('tc', 'tc_exact'):
+            raise ValueError(f"SegFormerSECC2PlaneBackbone: precision must be 'tc' or 'tc_exact', got {precision!r}")
+        self.mode, self.pncc_cond_mode, self.precision = mode, pncc_cond_mode, precision
         in_dim = 9 if pncc_cond_mode == 'cano_src_tgt' else 6
         self.prenet = _Prenet(in_dim)
         self.mix_vit = _MiTb0()
@@ -199,47 +256,10 @@ class SegFormerSECC2PlaneBackbone(nn.Module):
             return self._prep
         if dev.type != 'cuda':
             raise RuntimeError('real3dportrait_b200 runs on CUDA tensors only (no CPU fallback); move the module to a CUDA device')
-        f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()      # noqa: E731
-        d = lambda t: t.detach().double()                                   # noqa: E731
-        P = {}
-        wpre, bpre = fold_prenet(self.prenet.weight, self.prenet.bias)
-        nconst = wpre.shape[1] - 3
-        P['wpre'], P['bpre'] = f32(wpre), f32(bpre)
-        P['wpre_const'], P['wpre_tgt'] = f32(wpre[:, :nconst]), f32(wpre[:, nconst:])
-        mv = self.mix_vit
-        P['pe1'] = (f32(mv.patch_embed1.proj.weight), f32(mv.patch_embed1.proj.bias))
-        ln = lambda m: (f32(m.weight), f32(m.bias), float(m.eps))          # noqa: E731
-        stages = []
-        for s in range(4):
-            pe = getattr(mv, f'patch_embed{s + 1}')
-            st = {'pe_norm': ln(pe.norm), 'norm': ln(getattr(mv, f'norm{s + 1}'))}
-            if s > 0:
-                st['pe'] = _pack_gemm(_conv_rows(d(pe.proj.weight)), d(pe.proj.bias), dev)
-            blocks = []
-            for blk in getattr(mv, f'block{s + 1}'):
-                at = blk.attn
-                b = {'norm1': ln(blk.norm1), 'norm2': ln(blk.norm2),
-                     'q': _pack_gemm(d(at.q.weight), d(at.q.bias), dev), 'kv': _pack_gemm(d(at.kv.weight), d(at.kv.bias), dev),
-                     'proj': _pack_gemm(d(at.proj.weight), d(at.proj.bias), dev),
-                     'fc1': _pack_gemm(d(blk.mlp.fc1.weight), d(blk.mlp.fc1.bias), dev),
-                     'fc2': _pack_gemm(d(blk.mlp.fc2.weight), d(blk.mlp.fc2.bias), dev),
-                     'dw': (f32(blk.mlp.dwconv.dwconv.weight.reshape(-1, 9)), f32(blk.mlp.dwconv.dwconv.bias))}
-                if SR[s] > 1:
-                    b['sr'] = _pack_gemm(_conv_rows(d(at.sr.weight)), d(at.sr.bias), dev)
-                    b['sr_norm'] = ln(at.norm)
-                blocks.append(b)
-            st['blocks'] = blocks
-            stages.append(st)
-        P['stages'] = stages
-        G, hb = fold_head(self.fuse_head)
-        P['G'] = [_pack_gemm(g, None, dev) for g in G]
-        P['head_bias'] = f32(hb)
-        P['convs'] = [{'tc': sr_tc.pack_plain(c, EMB), 'mf': _pack_taps(d(c.weight), d(c.bias), dev)}
-                      for c in (self.to_plane_cnn[i] for i in (0, 2, 4))]
-        last = self.to_plane_cnn[7]
-        w7, b7 = d(last.weight), d(last.bias)
-        P['last_r'] = _pack_taps(w7[:64].flip(2), b7[:64], dev)          # planes 0, 1: rows mirrored
-        P['last_rc'] = _pack_taps(w7[64:].flip(2, 3), b7[64:], dev)      # plane 2: rows and columns mirrored
+        split = self.precision == 'tc_exact'
+        P = fold_and_pack(self, dev, split)
+        for cv, c in zip(P['convs'], (self.to_plane_cnn[i] for i in (0, 2, 4))):
+            cv['tc'] = sr_tc.pack_plain(c, EMB, split=split)            # r3dp_sr_tc_conv / r3dp_sr_tcx_conv (act 2) where W % 128 == 0
         self._prep = P
         return P
 
@@ -297,21 +317,36 @@ class SegFormerSECC2PlaneBackbone(nn.Module):
         P, L, st, dev = self._prepared(), capi.lib(), capi.stream(), x.device
         B, cin, H, W = x.shape
         ptr = capi.ptr
+        ex = self.precision == 'tc_exact'
+        wide = 2 if ex else 1               # halves per channel of an activation passed as fp16: 2 = split rows [hi C | lo C]
+
+        def act(*shape):
+            """An activation the tc path passes as fp16; split rows (twice as wide) in tc_exact."""
+            return torch.empty(*shape[:-1], wide * shape[-1], device=dev, dtype=F16)
 
         def gemm(a, R, pk, out_f32):
-            K = pk.w.shape[1]
-            y = torch.empty(R, pk.cout, device=dev, dtype=torch.float32 if out_f32 else F16)
-            conv3d.launch(pk, a, K, 0, K, (1, 1, 1, R), (1, 1, 1), y, pk.cout, stream=st)
+            """Token GEMM on r3dp_mf_conv3d.  tc_exact: split operands, and every output fp32 (the attention and the DWConv read q, kv, fc1
+            at fp32 grade)."""
+            K = pk.w.shape[1] // wide
+            y = torch.empty(R, pk.cout, device=dev, dtype=torch.float32 if out_f32 or ex else F16)
+            conv3d.launch(pk, a, wide * K, K if ex else 0, K, (1, 1, 1, R), (1, 1, 1), y, pk.cout, stream=st)
             return y
 
         def layernorm(xv, t, R, C, p, xo=None, yf=None, yh=None):
             g, b, eps = p
-            capi.check(L.r3dp_sp_layernorm(ptr(xv), ptr(t), R, C, ptr(g), ptr(b), eps, ptr(xo), ptr(yf), ptr(yh, F16), C, st))
+            if not ex or yh is None:
+                capi.check(L.r3dp_sp_layernorm(ptr(xv), ptr(t), R, C, ptr(g), ptr(b), eps, ptr(xo), ptr(yf), ptr(yh, F16), C, st))
+            elif t is None:
+                assert xo is None and yf is None
+                capi.check(L.r3dp_hb_layernorm(ptr(xv), R, C, ptr(g), ptr(b), eps, 0, None, 0, ptr(yh, F16), 2 * C, C, st))
+            else:
+                assert yf is None
+                capi.check(L.r3dp_sp_layernorm_split(ptr(xv), ptr(t), R, C, ptr(g), ptr(b), eps, ptr(xo), ptr(yh, F16), 2 * C, C, st))
 
         def patches(a, h, C, k, s, p):
             ho = (h + 2 * p - k) // s + 1
-            y = torch.empty(B * ho * ho, k * k * C, device=dev, dtype=F16)
-            capi.check(L.r3dp_sp_patches(ptr(a, F16), B, h, h, C, k, s, p, ptr(y, F16), st))
+            y = act(B * ho * ho, k * k * C)
+            capi.check((L.r3dp_sp_patches_split if ex else L.r3dp_sp_patches)(ptr(a, F16), B, h, h, C, k, s, p, ptr(y, F16), st))
             return y, ho
 
         with capi.region('secc2plane'):
@@ -327,59 +362,72 @@ class SegFormerSECC2PlaneBackbone(nn.Module):
                 R = B * h * h
                 xres = torch.empty(R, C, device=dev)
                 layernorm(t0, None, R, C, S['pe_norm'], yf=xres)
-                a = torch.empty(R, C, device=dev, dtype=F16)
+                a = act(R, C)
                 layernorm(xres, None, R, C, S['blocks'][0]['norm1'], yh=a)
                 for bi, bw in enumerate(S['blocks']):
                     q = gemm(a, R, bw['q'], False)
                     if SR[s] > 1:
                         pt, hk = patches(a, h, C, SR[s], SR[s], 0)
                         r = gemm(pt, B * hk * hk, bw['sr'], True)
-                        a2 = torch.empty(B * hk * hk, C, device=dev, dtype=F16)
+                        a2 = act(B * hk * hk, C)
                         layernorm(r, None, B * hk * hk, C, bw['sr_norm'], yh=a2)
                         kv, tk = gemm(a2, B * hk * hk, bw['kv'], False), hk * hk
                     else:
                         kv, tk = gemm(a, R, bw['kv'], False), h * h
-                    o = torch.empty(R, C, device=dev, dtype=F16)
-                    capi.check(L.r3dp_sp_attention(ptr(q, F16), C, ptr(kv, F16), 2 * C, B, h * h, tk, HEADS[s], HEAD_DIM ** -0.5, ptr(o, F16), C, st))
+                    o = act(R, C)
+                    if ex:
+                        capi.check(L.r3dp_sp_attention_split(ptr(q), C, ptr(kv), 2 * C, B, h * h, tk, HEADS[s], HEAD_DIM ** -0.5, ptr(o, F16), 2 * C,
+                                                             C, st))
+                    else:
+                        capi.check(L.r3dp_sp_attention(ptr(q, F16), C, ptr(kv, F16), 2 * C, B, h * h, tk, HEADS[s], HEAD_DIM ** -0.5, ptr(o, F16), C,
+                                                       st))
                     t = gemm(o, R, bw['proj'], True)
                     layernorm(xres, t, R, C, bw['norm2'], xo=xres, yh=a)
                     f1 = gemm(a, R, bw['fc1'], False)
-                    f2 = torch.empty_like(f1)
-                    capi.check(L.r3dp_sp_dwconv_gelu(ptr(f1, F16), B, h, h, 4 * C, ptr(bw['dw'][0]), ptr(bw['dw'][1]), ptr(f2, F16), st))
+                    f2 = act(R, 4 * C)
+                    if ex:
+                        capi.check(L.r3dp_sp_dwconv_gelu_split(ptr(f1), B, h, h, 4 * C, ptr(bw['dw'][0]), ptr(bw['dw'][1]), ptr(f2, F16), st))
+                    else:
+                        capi.check(L.r3dp_sp_dwconv_gelu(ptr(f1, F16), B, h, h, 4 * C, ptr(bw['dw'][0]), ptr(bw['dw'][1]), ptr(f2, F16), st))
                     t = gemm(f2, R, bw['fc2'], True)
                     if bi + 1 < len(S['blocks']):
                         layernorm(xres, t, R, C, S['blocks'][bi + 1]['norm1'], xo=xres, yh=a)
                     else:
-                        prev = torch.empty(R, C, device=dev, dtype=F16)
+                        prev = act(R, C)
                         layernorm(xres, t, R, C, S['norm'], yh=prev)
                 feats.append((prev, h))
             g = [(gemm(c, B * hh * hh, P['G'][i], True), hh) for i, (c, hh) in enumerate(feats)]
             h1 = feats[0][1]
-            y = torch.empty(B, h1, h1, EMB, device=dev, dtype=F16)
-            capi.check(L.r3dp_sp_head_fuse(ptr(g[0][0]), g[0][1], ptr(g[1][0]), g[1][1], ptr(g[2][0]), g[2][1], ptr(g[3][0]), g[3][1], B,
-                                           ptr(P['head_bias']), ptr(y, F16), st))
+            y = act(B, h1, h1, EMB)
+            capi.check((L.r3dp_sp_head_fuse_split if ex else L.r3dp_sp_head_fuse)(ptr(g[0][0]), g[0][1], ptr(g[1][0]), g[1][1], ptr(g[2][0]), g[2][1],
+                                                                                ptr(g[3][0]), g[3][1], B, ptr(P['head_bias']), ptr(y, F16), st))
             for ci, cv in enumerate(P['convs']):
                 z = torch.empty_like(y)
                 with capi.region(f'secc2plane.conv{2 * ci}'):         # per-launch times of the conv stack (tools/bench_secc.py)
                     if h1 % 128 == 0:          # r3dp_sr_tc_conv tiles 128-pixel rows
                         wp, bias, _ = cv['tc']
-                        capi.check(L.r3dp_sr_tc_conv(ptr(y, F16), ptr(wp, F16), ptr(bias), B, 1, EMB, EMB, h1, h1, 3, 2, ptr(z, F16), st))
+                        capi.check((L.r3dp_sr_tcx_conv if ex else L.r3dp_sr_tc_conv)(ptr(y, F16), ptr(wp, F16), ptr(bias), B, 1, EMB, EMB, h1, h1, 3,
+                                                                                    2, ptr(z, F16), st))
+                    elif ex:
+                        conv3d.launch(cv['mf'], y, 2 * EMB, EMB, EMB, (B, 1, h1, h1), (1, 3, 3), z, 2 * EMB, 0, EMB, stream=st)
+                        capi.check(L.r3dp_sp_leaky_split(ptr(z, F16), B * h1 * h1, EMB, 0.01, st))
                     else:
                         conv3d.launch(cv['mf'], y, EMB, 0, EMB, (B, 1, h1, h1), (1, 3, 3), z, EMB, stream=st)
                         capi.check(L.r3dp_sp_leaky(ptr(z, F16), z.numel(), 0.01, st))
                 y = z
             H2 = 2 * h1
-            ur = torch.empty(B, H2, H2, EMB, device=dev, dtype=F16)
+            ur = act(B, H2, H2, EMB)
             urc = torch.empty_like(ur)
             with capi.region('secc2plane.upsample'):
-                capi.check(L.r3dp_sp_upsample2_flip(ptr(y, F16), B, h1, h1, EMB, ptr(ur, F16), ptr(urc, F16), st))
+                capi.check((L.r3dp_sp_upsample2_flip_split if ex else L.r3dp_sp_upsample2_flip)(ptr(y, F16), B, h1, h1, EMB, ptr(ur, F16), ptr(urc, F16),
+                                                                                              st))
             if out is None:
                 out = torch.empty(B, H2, H2, 3, 32, device=dev)
             elif tuple(out.shape) != (B, H2, H2, 3, 32) or out.dtype != torch.float32 or not out.is_contiguous():
                 raise ValueError(f'planes_cl: out must be a contiguous fp32 [{B},{H2},{H2},3,32] tensor')
             with capi.region('secc2plane.conv7'):
                 for src, pk, c0 in ((ur, P['last_r'], 0), (urc, P['last_rc'], 64)):
-                    conv3d.launch(pk, src, EMB, 0, EMB, (B, 1, H2, H2), (1, 3, 3), out, 96, c0, stream=st)
+                    conv3d.launch(pk, src, wide * EMB, EMB if ex else 0, EMB, (B, 1, H2, H2), (1, 3, 3), out, 96, c0, stream=st)
         return out
 
 
