@@ -367,16 +367,14 @@ class Img2PlaneModel(nn.Module):
             act: None, 'relu' or 'leaky' (nn.LeakyReLU(0.01), only into a tensor of its own)."""
             ho = cv.out_size(h)
             own = y is None
+            if cv.tc is not None and xs == cv.cin and h % 128 == 0 and own and res is None and not out_f32:
+                # r3dp_sr_tc_conv (tiles of 128-pixel rows) on the dense input; epilogue act 3 = ReLU, 2 = LeakyReLU(0.01)
+                return sr_tc.conv_plain(src, (cv.tc, cv.pk.bias, 3), {None: 0, 'leaky': 2, 'relu': 3}[act]), ho
             if own:
                 y = torch.empty(B, ho, ho, cv.cout, device=dev, dtype=torch.float32 if out_f32 else F16)
                 ys = cv.cout
             assert act != 'leaky' or (own and not out_f32)
             relu = int(act == 'relu')
-            if cv.tc is not None and xs == cv.cin and h % 128 == 0 and own and res is None and not out_f32:
-                # r3dp_sr_tc_conv (tiles of 128-pixel rows); epilogue act 3 = ReLU, 2 = LeakyReLU(0.01)
-                capi.check(L.r3dp_sr_tc_conv(xp, ptr(cv.tc, F16), ptr(cv.pk.bias), B, 1, cv.cin, cv.cout, h, h, 3, {None: 0, 'leaky': 2, 'relu': 3}[act],
-                                             ptr(y, F16), st))
-                return y, ho
             if cv.box:
                 conv3d.launch(cv.pk, xp, xs, 0, cv.cin, (B, 1, h, h), (1, 3, 3), y, ys, yc0, relu=relu, res=res, stream=st)
             elif cv.gemm:

@@ -402,16 +402,15 @@ class SegFormerSECC2PlaneBackbone(nn.Module):
             capi.check((L.r3dp_sp_head_fuse_split if ex else L.r3dp_sp_head_fuse)(ptr(g[0][0]), g[0][1], ptr(g[1][0]), g[1][1], ptr(g[2][0]), g[2][1],
                                                                                 ptr(g[3][0]), g[3][1], B, ptr(P['head_bias']), ptr(y, F16), st))
             for ci, cv in enumerate(P['convs']):
-                z = torch.empty_like(y)
                 with capi.region(f'secc2plane.conv{2 * ci}'):         # per-launch times of the conv stack (tools/bench_secc.py)
                     if h1 % 128 == 0:          # r3dp_sr_tc_conv tiles 128-pixel rows
-                        wp, bias, _ = cv['tc']
-                        capi.check((L.r3dp_sr_tcx_conv if ex else L.r3dp_sr_tc_conv)(ptr(y, F16), ptr(wp, F16), ptr(bias), B, 1, EMB, EMB, h1, h1, 3,
-                                                                                    2, ptr(z, F16), st))
+                        z = sr_tc.conv_plain(y, cv['tc'], 2, split=ex)
                     elif ex:
+                        z = torch.empty_like(y)
                         conv3d.launch(cv['mf'], y, 2 * EMB, EMB, EMB, (B, 1, h1, h1), (1, 3, 3), z, 2 * EMB, 0, EMB, stream=st)
                         capi.check(L.r3dp_sp_leaky_split(ptr(z, F16), B * h1 * h1, EMB, 0.01, st))
                     else:
+                        z = torch.empty_like(y)
                         conv3d.launch(cv['mf'], y, EMB, 0, EMB, (B, 1, h1, h1), (1, 3, 3), z, EMB, stream=st)
                         capi.check(L.r3dp_sp_leaky(ptr(z, F16), z.numel(), 0.01, st))
                 y = z

@@ -187,39 +187,9 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
 
     @staticmethod
     def _conv(x16: torch.Tensor, packed, act: int, split: bool = False) -> torch.Tensor:
-        """x16 [N,H,W,Ct] fp16 -> [N,H,W,Opad] fp16; act 0 linear, 2 nn.LeakyReLU(0.01).  split: [hi | lo] tensors of twice the channels (fp32-grade)."""
-        wp, bias, k = packed
-        N, H, W, Ct = x16.shape
-        wide = 2 if split else 1
-        y = torch.empty(N, H, W, wp.shape[2] * wide, device=x16.device, dtype=torch.float16)
-        fn = capi.lib().r3dp_sr_tcx_conv if split else capi.lib().r3dp_sr_tc_conv
+        """sr_tc.conv_plain (no residual), timed in the 'sr_conv' profiler stage."""
         with capi.region('sr_conv'):
-            capi.check(fn(capi.ptr(x16, torch.float16), capi.ptr(wp, torch.float16), capi.ptr(bias), N, 1, Ct // wide, wp.shape[2], H, W, k, act,
-                          capi.ptr(y, torch.float16), capi.stream()))
-        return y
-
-    @staticmethod
-    def _alpha_cat(xa16, Ca, xb16, Cb, alpha, split: bool = False) -> torch.Tensor:
-        """cat[xa*alpha, xb*(1-alpha)]; xb may hold ONE frame shared by the whole batch (per-clip constant features).  split: [hi | lo] inputs,
-        output = the [hi | lo] layout of the (Ca + Cb)-channel result."""
-        N, H, W, _ = xa16.shape
-        out = torch.empty(N, H, W, (Ca + Cb) * (2 if split else 1), device=xa16.device, dtype=torch.float16)
-        fn = capi.lib().r3dp_sr_tcx_alpha_cat_ex if split else capi.lib().r3dp_sr_alpha_cat_ex
-        capi.check(fn(capi.ptr(xa16, torch.float16), Ca, xa16.shape[-1], capi.ptr(xb16, torch.float16), Cb, xb16.shape[-1],
-                      int(xb16.shape[0] == 1 and N > 1), capi.ptr(alpha), N, H, W, capi.ptr(out, torch.float16), capi.stream()))
-        return out
-
-    @staticmethod
-    def _cat3(xa16, xb16, xc16, split: bool = False) -> torch.Tensor:
-        """cat[xa, xb, xc] of three 256-channel NHWC fp16 tensors, unweighted; xc may hold ONE frame shared by the whole batch (per-clip constant
-        features).  split: [hi | lo] inputs, output = the [hi | lo] layout of the 768-channel result."""
-        N, H, W, _ = xa16.shape
-        out = torch.empty(N, H, W, 768 * (2 if split else 1), device=xa16.device, dtype=torch.float16)
-        fn = capi.lib().r3dp_sr_tcx_cat3 if split else capi.lib().r3dp_sr_cat3
-        capi.check(fn(capi.ptr(xa16, torch.float16), 256, xa16.shape[-1], capi.ptr(xb16, torch.float16), 256, xb16.shape[-1],
-                      capi.ptr(xc16, torch.float16), 256, xc16.shape[-1], int(xc16.shape[0] == 1 and N > 1), N, H, W, capi.ptr(out, torch.float16),
-                      capi.stream()))
-        return out
+            return sr_tc.conv_plain(x16, packed, act, split=split)
 
     # ---- per-clip constants (SURVEY.md §8f #2) -------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -312,7 +282,6 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
             raise NotImplementedError('reference images must be 512x512 (antialiased 1/2 resize is the only down-scaling built)')
         ws3 = ws[:, -1:, :].expand(N, 3, -1)
         sp = self._split
-        wide = 2 if sp else 1
         prep = getattr(self, 'static_prepared_warp', None)
         if prep is not None and prep['main'].split != sp:
             prep = None
@@ -325,7 +294,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
             if x_nhwc is not None:                                       # one launch, bit-identical to the three below
                 xn = capi.f32(x_nhwc)
                 _, h, w, Cc = xn.shape
-                x0 = torch.empty(N, R, R, (Cc + 63) // 64 * 64 * wide, device=xn.device, dtype=torch.float16)
+                x0 = sr_tc.activation(N, R, R, (Cc + 63) // 64 * 64, sp, xn.device)
                 rgb0 = torch.empty(N, 3, R, R, device=xn.device)
                 rgb_256 = torch.empty(N, 3, 256, 256, device=xn.device)
                 weights_256 = torch.empty(N, 1, 256, 256, device=xn.device)
@@ -345,16 +314,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
                 ref_torso_256, ref_bg_256 = cc['batch']
             else:                                                        # per-clip constants, one frame broadcast over the batch (0.8 MB copies)
                 ref_torso_256, ref_bg_256 = cc['ref_torso_256'].expand(N, -1, -1, -1).contiguous(), cc['ref_bg_256'].expand(N, -1, -1, -1).contiguous()
-        main, Nw = prep['main'], prep['main'].Nw
-        b0 = self.block0
-        # block0: 128^2 -> 256^2 head features + head rgb
-        a0 = sr_tc.layer(x0, b0.conv0, main.wp[0], 2, sp)
-        xh = torch.empty(N, 256, 256, 256 * wide, device=x.device, dtype=torch.float16)
-        rgb_h = torch.empty(N, 3, 256, 256, device=x.device)
-        with capi.region('sr_conv'):
-            capi.check(sr_tc._fn('layer_torgb', sp)(capi.ptr(a0, torch.float16), capi.ptr(main.wp[1], torch.float16), capi.ptr(capi.f32(b0.conv1.bias)),
-                                                capi.ptr(main.wrgb0), capi.ptr(capi.f32(b0.torgb.bias)), capi.ptr(rgb0), N, Nw, 256, 256, 256, 256,
-                                                capi.ptr(xh, torch.float16), capi.ptr(rgb_h), capi.stream()))
+        xh, rgb_h = sr_tc.block0(self.block0, prep['main'], x0, rgb0)   # 128^2 -> 256^2 head features + head rgb
         return {'N': N, 'split': sp, 'prep': prep, 'plain': plain, 'cc': cc, 'device': x.device, 'xh': xh, 'rgb_h': rgb_h, 'ref_bg_256': ref_bg_256,
                 'weights_256': weights_256, 'out_clamp': bool(block_kwargs.pop('out_clamp', False)), 'out_uint8': bool(block_kwargs.pop('out_uint8', False)),
                 'torso_args': (ref_torso_256, segmap, kp_s, kp_d, rgb_256, weights_256), 'target_torso_mask': target_torso_mask}
@@ -383,9 +343,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         rgb_torso nor facev2v_ret['occlusion_2']."""
         L = capi.lib()
         N, sp, prep, plain, cc, dev = st['N'], st['split'], st['prep'], st['plain'], st['cc'], st['device']
-        wide = 2 if sp else 1
         xh, rgb_h, weights_256 = st['xh'], st['rgb_h'], st['weights_256']
-        Nw = prep['main'].Nw
         hb = getattr(self, 'head_torso_block', None)
         x_torso = self._conv(sr_tc.to_nhwc_f16(facev2v_ret['deformed_torso_hid'], 256, sp), plain['te'], 0, sp)       # 1x1, 64 -> 256
         if cc is None:
@@ -394,15 +352,13 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
             x_bg = cc['x_bg']                                            # [1,256,256,256 (x2 split)] fp16, read by every frame of the batch
         if not self.weight_fuse:
             # sr_with_ref.py:159-161: cat[x, x_torso, x_bg] unweighted, and block1 without a skip image
-            return self._fg_bg_block1(st, self._cat3(xh, x_torso, x_bg, sp), None)
+            return self._fg_bg_block1(st, sr_tc.cat3(xh, x_torso, x_bg, sp), None)
         thr = float(self.hparams['htbsr_head_threshold'])
         if self.fuse_mode == 'v1':
             # head/torso fusion v1 (sr_with_ref.py:96-98): plain alpha blend of the rgb images AND of the feature maps; no fusing convs, no head_torso_block
             alpha = weights_256
             rgb_p2 = self._blend(rgb_h, rgb_torso, alpha)
-            xp = torch.empty(N, 256, 256, 256 * wide, device=dev, dtype=torch.float16)
-            capi.check((L.r3dp_sr_tcx_alpha_mix if sp else L.r3dp_sr_alpha_mix)(capi.ptr(xh, torch.float16), xh.shape[-1], capi.ptr(x_torso, torch.float16), x_torso.shape[-1], capi.ptr(alpha), 256,
-                                           N, 256, 256, capi.ptr(xp, torch.float16), capi.stream()))
+            xp = sr_tc.alpha_mix(xh, x_torso, alpha, sp)
         else:
             if self.fuse_mode == 'v3':
                 # sr_with_ref.py:129-132: a 3-conv net post-processes the head mask from (head rgb, weights, torso rgb); capped by the weights.  The net runs
@@ -421,14 +377,9 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
                 alpha = weights_256                                 # v2, sr_with_ref.py:108-109 (the masked assignment is a no-op)
             # alpha-cat fusion of the head and torso features (sr_with_ref.py:110-113 | 133-136)
             rgb_p = self._blend(rgb_h, rgb_torso, alpha)
-            xf = self._conv(self._conv(self._alpha_cat(xh, 256, x_torso, 256, alpha, sp), plain['fh0'], 2, sp), plain['fh2'], 0, sp)
+            xf = self._conv(self._conv(sr_tc.alpha_cat(xh, 256, x_torso, 256, alpha, sp), plain['fh0'], 2, sp), plain['fh2'], 0, sp)
             c0 = sr_tc.layer(xf, hb.conv0, prep['ht0'], 1, sp)
-            xp = torch.empty(N, 256, 256, 256 * wide, device=dev, dtype=torch.float16)
-            rgb_p2 = torch.empty(N, 3, 256, 256, device=dev)
-            with capi.region('sr_conv'):
-                capi.check(sr_tc._fn('layer_torgb_noup', sp)(capi.ptr(c0, torch.float16), capi.ptr(prep['ht1'], torch.float16), capi.ptr(capi.f32(hb.conv1.bias)),
-                                                         capi.ptr(prep['htrgb']), capi.ptr(capi.f32(hb.torgb.bias)), capi.ptr(rgb_p), N, Nw, 256, 256, 256, 256,
-                                                         capi.ptr(xp, torch.float16), capi.ptr(rgb_p2), capi.stream()))
+            xp, rgb_p2 = sr_tc.layer_torgb(c0, hb, prep['ht1'], prep['htrgb'], rgb_p, sp, noup=True)
         # person / background fusion, sr_with_ref.py:115-124
         occ = capi.f32(facev2v_ret['occlusion_2'])
         torso_occ = occ if occ.shape[-1] == 256 else self._resize(occ, 256)
@@ -436,22 +387,11 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         capi.check(L.r3dp_sr_person_occlusion(capi.ptr(alpha), capi.ptr(torso_occ), thr, N, 256, 256,
                                               capi.ptr(person), capi.stream()))
         rgb_f = self._blend(rgb_p2, st['ref_bg_256'], person)
-        return self._fg_bg_block1(st, self._alpha_cat(xp, 256, x_bg, 256, person, sp), rgb_f)
+        return self._fg_bg_block1(st, sr_tc.alpha_cat(xp, 256, x_bg, 256, person, sp), rgb_f)
 
     def _fg_bg_block1(self, st: Dict, xg: torch.Tensor, rgb_f: Optional[torch.Tensor]) -> torch.Tensor:
         """fuse_fg_bg_convs and block1 on the fused features xg; rgb_f = block1's skip image (None: no skip, the image is ToRGB alone)."""
-        L = capi.lib()
-        N, sp, plain, dev = st['N'], st['split'], st['plain'], st['device']
-        main, Nw = st['prep']['main'], st['prep']['main'].Nw
-        b1 = self.block1
+        sp, plain = st['split'], st['plain']
         xg = self._conv(self._conv(self._conv(xg, plain['ff0'], 2, sp), plain['ff2'], 2, sp), plain['ff4'], 0, sp)
         # block1: 256^2 -> 512^2; with out_uint8 the last epilogue writes the video frames (real3d_infer.py:515-519)
-        a2 = sr_tc.layer(xg, b1.conv0, main.wp[2], 2, sp)
-        u8 = st['out_uint8']
-        out = torch.empty(N, 512, 512, 3, device=dev, dtype=torch.uint8) if u8 else torch.empty(N, 3, 512, 512, device=dev)
-        with capi.region('sr_conv'):
-            capi.check((L.r3dp_sr_tcx_last_layer if sp else L.r3dp_sr_tc_last_layer_ex)(
-                capi.ptr(a2, torch.float16), capi.ptr(main.wp[3], torch.float16), capi.ptr(capi.f32(b1.conv1.bias)), capi.ptr(main.wrgb1),
-                capi.ptr(capi.f32(b1.torgb.bias)), capi.ptr(rgb_f), N, Nw, 128, 512, 512, None if u8 else capi.ptr(out),
-                capi.ptr(out, torch.uint8) if u8 else None, int(st['out_clamp'] or u8), capi.stream()))
-        return out
+        return sr_tc.block1(self.block1, st['prep']['main'], xg, rgb_f, st['out_clamp'], st['out_uint8'])
