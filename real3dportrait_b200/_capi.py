@@ -224,6 +224,13 @@ def ptr(t: Optional[torch.Tensor], dtype=torch.float32) -> C.c_void_p:
     return C.c_void_p(t.data_ptr())
 
 
+def cuda_device(t: torch.Tensor) -> torch.device:
+    """The device of a module's parameter t, which must be a CUDA device (prepared weights are built there)."""
+    if not t.is_cuda:
+        raise RuntimeError('real3dportrait_b200 runs on CUDA tensors only (no CPU fallback); move the module to a CUDA device')
+    return t.device
+
+
 def f32(t: torch.Tensor) -> torch.Tensor:
     """Borrow as dense fp32 (no copy when already so); detached — this path is inference-only."""
     t = t.detach()

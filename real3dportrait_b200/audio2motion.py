@@ -31,6 +31,7 @@ import torch.nn as nn
 
 from . import _capi as capi, conv3d
 from .conv3d import pack_conv3d
+from .prepared import PreparedMixin
 
 F16 = torch.float16
 LATENT = 16
@@ -253,7 +254,7 @@ def f0_to_coarse(f0: torch.Tensor) -> torch.Tensor:
 
 
 # ---- the models --------------------------------------------------------------------------------------------------------------------------
-class _Audio2Motion(nn.Module):
+class _Audio2Motion(PreparedMixin, nn.Module):
     pitch = False
 
     def _check_config(self, in_out_dim, audio_in_dim, sqz_prior):
@@ -269,21 +270,11 @@ class _Audio2Motion(nn.Module):
     def device(self):
         return next(self.vae.parameters()).device
 
-    # prepared weights belong to one parameter set on one device
-    def _load_from_state_dict(self, *a, **k):
-        self._prep = None
-        return super()._load_from_state_dict(*a, **k)
-
-    def _apply(self, fn, *a, **k):
-        self._prep = None
-        return super()._apply(fn, *a, **k)
-
     def _prepared(self):
-        if self._prep is not None:
-            return self._prep
-        dev = self.device
-        if dev.type != 'cuda':
-            raise RuntimeError('real3dportrait_b200 runs on CUDA tensors only (no CPU fallback); move the module to a CUDA device')
+        return self.prepared('weights', self._build)
+
+    def _build(self):
+        dev = capi.cuda_device(next(self.vae.parameters()))
         with torch.no_grad():
             P = fold_weights(self)
 
@@ -313,7 +304,6 @@ class _Audio2Motion(nn.Module):
             Q['dec_cond'] = conv(P['dec_cond'], Q['gin'])
             Q['dec_wn'] = wn(P['dec_wn'])
             Q['out_proj'] = conv(P['out_proj'], 256)
-        self._prep = Q
         return Q
 
     # ---- input checks --------------------------------------------------------------------------------------------------------------
@@ -508,7 +498,6 @@ class PitchContourVAEModel(_Audio2Motion):
         self.in_dim = self.out_dim = in_out_dim
         self.sqz_prior, self.use_prior_flow = sqz_prior, use_prior_flow
         self.vae = FVAE(feat, use_prior_flow)
-        self._prep = None
 
 
 class VAEModel(_Audio2Motion):
@@ -527,4 +516,3 @@ class VAEModel(_Audio2Motion):
         self.in_dim = self.out_dim = in_out_dim
         self.sqz_prior, self.use_prior_flow = sqz_prior, use_prior_flow
         self.vae = FVAE(feat, use_prior_flow)
-        self._prep = None

@@ -119,7 +119,7 @@ class _TorsoGraphs:
 
 class FrameEngine:
     """batch: frames per step; static_styles: the SR styles are constant (Real3D passes ws == 1, img2plane_baseline.py:142) so
-    the folded fp16 weights are prepared once per parameter load; use_graph: replay the step as CUDA graphs.
+    the folded fp16 weights are prepared once per parameter load or move; use_graph: replay the step as CUDA graphs.
     torso_model: run the torso head with this warper (WarpBasedTorsoModelMediaPipe or a module with its forward signature);
     warper_in_graph: capture the warper inside the step's single graph (only for capturable warpers; the default runs it eagerly
     between two graphs).  torso_stage2='cuda': the warper's stage 2 on this library's kernels, its appearance features cached per clip by
@@ -171,7 +171,8 @@ class FrameEngine:
         self.batch, self.world, self.rank, self.dist = batch, world, rank, dist
         self.device = device if device is not None else torch.device('cuda', torch.cuda.current_device())
         self.head = RenderHead(hp=hp, sr_mode=sr_mode, torso_model=torso_model).to(self.device).eval()
-        self.static_styles, self.use_graph = static_styles, use_graph
+        self.head.superresolution.static_styles = bool(static_styles)
+        self.use_graph = use_graph
         self.torso, self.warper_in_graph = self.head.torso, bool(warper_in_graph)
         if torso_stage2 != 'torch':
             if not self.torso:
@@ -226,16 +227,7 @@ class FrameEngine:
         self.graph = None
         self.inplace = {}
         self._consts = None                                            # loading dropped the head's per-clip cache: begin_clip() again
-        sr = self.head.superresolution
-        sr.static_prepared = None
-        if self.static_styles and sr.sr_mode in ('tc', 'tc_exact'):
-            from . import sr_tc
-            ones = torch.ones(1, 3, self.head.hparams['w_dim'], device=self.device)
-            with torch.no_grad():
-                if self.torso:
-                    sr.static_prepared_warp = sr.prepare_styles(ones)
-                else:
-                    sr.static_prepared = sr_tc.Prepared(sr, ones, sr.sr_mode == 'tc_exact')
+        self.head.superresolution.prepared_styles()                    # folded now, so that no step or captured graph does it
 
     # ---- torso head: per-clip constants --------------------------------------------------------------------------------------------------
     @torch.no_grad()

@@ -23,6 +23,7 @@ import torch
 import torch.nn as nn
 
 from . import _capi as capi
+from .prepared import PreparedMixin
 
 F16 = torch.float16
 SEG = 1000                    # frames per encoder segment (extract_hubert.py: clip_length = 320 * 1000)
@@ -247,7 +248,7 @@ class _Output:
         return (self.last_hidden_state,)[i]
 
 
-class HubertModel(nn.Module):
+class HubertModel(PreparedMixin, nn.Module):
     """transformers.HubertModel(config) at inference, for the hubert-large-ls960-ft architecture (see the module docstring)."""
 
     def __init__(self, config):
@@ -260,7 +261,6 @@ class HubertModel(nn.Module):
         self.feature_extractor = _FeatureExtractor(c)
         self.feature_projection = _FeatureProjection(c)
         self.encoder = _Encoder(c)
-        self._prep = None
         self.eval()
 
     @classmethod
@@ -285,20 +285,11 @@ class HubertModel(nn.Module):
     def device(self):
         return self.feature_projection.projection.weight.device
 
-    def _load_from_state_dict(self, *a, **k):
-        self._prep = None
-        return super()._load_from_state_dict(*a, **k)
-
-    def _apply(self, fn, *a, **k):
-        self._prep = None
-        return super()._apply(fn, *a, **k)
-
     def _prepared(self):
-        if self._prep is not None:
-            return self._prep
-        dev = self.device
-        if dev.type != 'cuda':
-            raise RuntimeError('real3dportrait_b200 runs on CUDA tensors only (no CPU fallback); move the module to a CUDA device')
+        return self.prepared('weights', self._build)
+
+    def _build(self):
+        dev = capi.cuda_device(self.feature_projection.projection.weight)
         c = self.config
         C, H = c.conv_dim[0], c.hidden_size
         Cp = _ceil64(C)
@@ -317,7 +308,6 @@ class HubertModel(nn.Module):
             Q['layers'] = [tuple(pack_split(w).to(dev) if j % 2 == 0 else f32(w) for j, w in enumerate(lay)) for lay in P['layers']]
             Q['ln_f'] = (f32(P['ln_f'].weight), f32(P['ln_f'].bias), float(P['ln_f'].eps))
             Q['unit'] = torch.tensor([0.0, 1.0], dtype=torch.float64, device=dev)
-        self._prep = Q
         return Q
 
     def train(self, mode: bool = True):

@@ -26,6 +26,7 @@ import torch.nn as nn
 
 from . import _capi as capi, conv3d, sr_tc
 from .conv3d import pack_gemm, pack_taps
+from .prepared import PreparedMixin
 from .renderer import PlanesCL
 from .secc2plane import _conv_rows
 
@@ -198,7 +199,7 @@ class _Conv:
         return (h + 2 * self.p - self.d * (self.k - 1) - 1) // self.s + 1
 
 
-class Img2PlaneModel(nn.Module):
+class Img2PlaneModel(PreparedMixin, nn.Module):
     """Img2PlaneModel(out_channels=96, hp=None) (img2plane_model.py:12-35) on sm_90a kernels, for img2plane_input_mode 'rgb',
     triplane_feature_type 'triplane', triplane_depth 1 and img2plane_backbone_scale 'small' | 'standard' | 'large' (read from hp).
 
@@ -231,24 +232,13 @@ class Img2PlaneModel(nn.Module):
         self.high_reso_encoder = _HighResoEncoder(cin)
         self.low_reso_vit = _LowResolutionViT(nlow)
         self.triplane_predictor_vit = _TriplanePredictorViT(ntri, out_channels)
-        self._prep = None
-
-    # prepared weights belong to one parameter set on one device
-    def _load_from_state_dict(self, *a, **k):
-        self._prep = None
-        return super()._load_from_state_dict(*a, **k)
-
-    def _apply(self, fn, *a, **k):
-        self._prep = None
-        return super()._apply(fn, *a, **k)
 
     def _prepared(self):
-        if self._prep is not None:
-            return self._prep
+        return self.prepared('weights', self._build)
+
+    def _build(self):
         enc = self.low_reso_encoder.encoder
-        dev = enc.conv1.weight.device
-        if dev.type != 'cuda':
-            raise RuntimeError('real3dportrait_b200 runs on CUDA tensors only (no CPU fallback); move the module to a CUDA device')
+        dev = capi.cuda_device(enc.conv1.weight)
         d = lambda t: None if t is None else t.detach().double()           # noqa: E731
         f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()     # noqa: E731
 
@@ -311,7 +301,6 @@ class Img2PlaneModel(nn.Module):
         P['tri_pre'] = [conv(tv.first_conv), conv(tv.second_conv)]
         P['tri_post'] = [conv(tv.first_conv_after_cat), conv(tv.second_conv_after_cat), conv(tv.third_conv_after_cat)]
         P['tri_final'] = conv(tv.final_conv)
-        self._prep = P
         return P
 
     # ---- input checks ------------------------------------------------------------------------------------------------------------------

@@ -23,6 +23,7 @@ import torch.nn as nn
 
 from . import _capi as capi, conv3d, sr_tc
 from .conv3d import pack_gemm as _pack_gemm, pack_taps as _pack_taps
+from .prepared import PreparedMixin
 from .renderer import PlanesCL, producer_view
 
 F16 = torch.float16
@@ -206,7 +207,7 @@ def fold_and_pack(m: 'SegFormerSECC2PlaneBackbone', dev, split: bool) -> dict:
     return P
 
 
-class SegFormerSECC2PlaneBackbone(nn.Module):
+class SegFormerSECC2PlaneBackbone(PreparedMixin, nn.Module):
     """SegFormerSECC2PlaneBackbone(mode='b0', out_channels=96, pncc_cond_mode='cano_src_tgt') (segformer.py:673-733) on sm_90a kernels.
 
     forward(x [B, 9|6, H, W]) -> [B, 3, 32, H/2, W/2] (the reference's flipped planes), a view of channels-last data;
@@ -238,29 +239,15 @@ class SegFormerSECC2PlaneBackbone(nn.Module):
             nn.Conv2d(256, 256, 3, 1, 1), nn.LeakyReLU(0.01, inplace=True),
             nn.UpsamplingBilinear2d(scale_factor=2.),
             nn.Conv2d(256, out_channels, 3, 1, 1))
-        self._prep = None
-        self._clip_base = None
-
-    # prepared weights belong to one parameter set on one device
-    def _load_from_state_dict(self, *a, **k):
-        self._prep, self._clip_base = None, None
-        return super()._load_from_state_dict(*a, **k)
-
-    def _apply(self, fn, *a, **k):
-        self._prep, self._clip_base = None, None
-        return super()._apply(fn, *a, **k)
 
     def _prepared(self):
-        dev = self.prenet.weight.device
-        if self._prep is not None:
-            return self._prep
-        if dev.type != 'cuda':
-            raise RuntimeError('real3dportrait_b200 runs on CUDA tensors only (no CPU fallback); move the module to a CUDA device')
+        return self.prepared('weights', self._build)
+
+    def _build(self):
         split = self.precision == 'tc_exact'
-        P = fold_and_pack(self, dev, split)
+        P = fold_and_pack(self, capi.cuda_device(self.prenet.weight), split)
         for cv, c in zip(P['convs'], (self.to_plane_cnn[i] for i in (0, 2, 4))):
             cv['tc'] = sr_tc.pack_plain(c, EMB, split=split)            # r3dp_sr_tc_conv / r3dp_sr_tcx_conv (act 2) where W % 128 == 0
-        self._prep = P
         return P
 
     # ---- input checks ------------------------------------------------------------------------------------------------------------------
@@ -294,23 +281,23 @@ class SegFormerSECC2PlaneBackbone(nn.Module):
         P = self._prepared()
         xc = torch.cat(parts, 1).contiguous() if len(parts) > 1 else parts[0]
         _, cin, H, W = xc.shape
-        base = self._clip_base
+        base = self.cached('clip')
         if base is None or base.shape[2:] != (H, W) or base.device != xc.device:
-            base = torch.empty(1, 3, H, W, device=xc.device)
+            base = self.store('clip', torch.empty(1, 3, H, W, device=xc.device))
         # a later clip of the same size refills the same image in place: CUDA graphs captured over planes_cl() read its address
         capi.check(capi.lib().r3dp_sp_prenet(capi.ptr(xc), 1, cin, H, W, capi.ptr(P['wpre_const']), capi.ptr(P['bpre']), capi.ptr(base),
                                              capi.stream()))
-        self._clip_base = base
 
     def planes_cl(self, cond_tgt: torch.Tensor, out: Optional[torch.Tensor] = None) -> PlanesCL:
         """cond_tgt [B,3,H,W] (after begin_clip) -> PlanesCL('hwpc') [B,H/2,W/2,3,32] fp32, the same values as forward(cat[cano, src, tgt])."""
-        if self._clip_base is None:
+        base = self.cached('clip')
+        if base is None:
             raise RuntimeError('planes_cl: call begin_clip(cond_cano, cond_src) first')
         x = self._check_image(cond_tgt, 3, 'planes_cl')
-        if x.shape[2:] != self._clip_base.shape[2:]:
+        if x.shape[2:] != base.shape[2:]:
             raise ValueError('planes_cl: cond_tgt must have the size of the clip images')
         P = self._prepared()
-        return PlanesCL(self._run(x, P['wpre_tgt'], self._clip_base, None, out), 'hwpc')
+        return PlanesCL(self._run(x, P['wpre_tgt'], base, None, out), 'hwpc')
 
     # ---- the launch sequence -----------------------------------------------------------------------------------------------------------
     def _run(self, x, wpre, base, bpre, out=None):

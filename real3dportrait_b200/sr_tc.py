@@ -238,15 +238,13 @@ def forward(sr, rgb: Optional[torch.Tensor], x: torch.Tensor, ws3: Optional[torc
     x_nhwc: the same features channels-last [N,h,w,C] (the renderer's native output) - skips a layout round trip.
     out_clamp: the image leaves the last epilogue clamped to [-1,1]; out_uint8: it leaves as uint8 HWC frames [N,512,512,3]
     (the caller loop's conversion, inference/real3d_infer.py:515-519, fused).
-    If `sr.static_prepared` is set (caller guarantees constant styles, e.g. Real3D's ws == 1) the weight preparation
-    (styles -> fold -> demod -> fp16 pack) is skipped."""
+    With `sr.static_styles` (the caller guarantees constant styles, e.g. Real3D's ws == 1) the weight preparation
+    (styles -> fold -> demod -> fp16 pack) is done once, by sr.prepared_styles()."""
     from .superresolution import SuperresolutionHybrid8XDC
     N, R = x.shape[0], sr.input_resolution
     split = getattr(sr, 'sr_mode', 'tc') == 'tc_exact'          # fp32-grade: split fp16 operands, three MMAs per product
-    prep = getattr(sr, 'static_prepared', None)
-    if prep is not None and prep.split != split:
-        prep = None
     with capi.region('sr_prep'):
+        prep = sr.prepared_styles()
         if prep is None:
             if shared_styles is None:
                 shared_styles = N == 1 or getattr(sr, 'assume_shared_styles', False)
@@ -265,15 +263,15 @@ def forward(sr, rgb: Optional[torch.Tensor], x: torch.Tensor, ws3: Optional[torc
 
 
 def _large_packed(sr, split: bool = False):
-    """Packed plain convolutions of the large_sr residual blocks / to_rgb layers (cached until the parameters are reloaded or the mode changes)."""
-    c = getattr(sr, '_large_cache', None)
-    if c is None or c['split'] != split:
-        c = {'split': split}
+    """Packed plain convolutions of the large_sr residual blocks / to_rgb layers (cached until the parameters are loaded or moved or the
+    mode changes)."""
+    def build():
+        c = {}
         for name, blk, ch in (('b0', sr.block0, 256), ('b1', sr.block1, 128)):
             c[name] = [(pack_plain(rb.conv1, ch, split=split), pack_plain(rb.conv2, ch, split=split)) for rb in blk.resblocks]
             c[name + '_rgb'] = (blk.to_rgb.weight.detach().float().reshape(1, 3, ch).contiguous(), blk.to_rgb.bias.detach().float().contiguous())
-        sr._large_cache = c
-    return c
+        return c
+    return sr.prepared('large', build, split)
 
 
 def _forward_large_tail(sr, b1, a1, img1, prep, out_clamp, out_uint8):

@@ -74,12 +74,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         self.fuse_in_dim = 512 if self.weight_fuse else 768      # weight_fuse=False: cat[x, x_torso, x_bg] (sr_with_ref.py:57-58)
         self.fuse_fg_bg_convs = nn.Sequential(nn.Conv2d(self.fuse_in_dim, 64, 1, 1, padding=0), nn.LeakyReLU(), nn.Conv2d(64, 256, 3, 1, padding=1),
                                               nn.LeakyReLU(), nn.Conv2d(256, 256, 3, 1, padding=1))
-        self._plain_cache = None
-        self._clip_cache = None
-        self.static_prepared_warp = None
-        self._stage2_cache = None
         self._warper = None
-        self._motion_cache = None
         self.torso_motion = 'torch'
         self.set_torso_stage2(torso_stage2)
         self.set_torso_motion(torso_motion)
@@ -95,7 +90,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         if mode == 'torch' and getattr(self, 'torso_motion', 'torch') == 'cuda':
             raise ValueError("torso_motion='cuda' needs torso_stage2='cuda': call set_torso_motion('torch') first")
         self.torso_stage2 = mode
-        self._stage2_cache = None
+        self.forget('stage2')
 
     def set_torso_motion(self, mode: str) -> None:
         """'torch': the warper calls the caller's motion_field_estimator.  'cuda': the estimator (network2.py:162-244) runs on this library's
@@ -115,18 +110,15 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
                 if err is not None:
                     raise NotImplementedError(f"torso_motion='cuda' is built for MotionFieldEstimator('standard'): {err}")
         self.torso_motion = mode
-        self._motion_cache = None
+        self.forget('motion')
 
     def _motion_weights(self):
         """Folded + packed estimator weights (torso_warp.MotionWeights), keyed like _stage2_weights(); None unless torso_motion='cuda'."""
         if self.torso_motion != 'cuda':
             return None
         from . import torso_warp
-        mfe = self.torso_model.motion_field_estimator
-        key = (self._split, tuple((t.data_ptr(), t._version) for t in list(mfe.parameters()) + list(mfe.buffers())))
-        if self._motion_cache is None or self._motion_cache[0] != key:
-            self._motion_cache = (key, torso_warp.MotionWeights(mfe, self._split))
-        return self._motion_cache[1]
+        sp, mfe = self._split, self.torso_model.motion_field_estimator
+        return self.prepared('motion', lambda: torso_warp.MotionWeights(mfe, sp), sp, watch=(mfe,))
 
     def _stage2_weights(self):
         """Folded + packed stage-2 weights, rebuilt when the mode, the device or any of the warper's parameters / buffers changed (a
@@ -135,10 +127,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         from . import torso_warp
         sp, tm = self._split, self.torso_model
         mods = (tm.deform_based_generator, tm.occlusion_2_predictor)
-        key = (sp, tuple((t.data_ptr(), t._version) for m in mods for t in list(m.parameters()) + list(m.buffers())))
-        if self._stage2_cache is None or self._stage2_cache[0] != key:
-            self._stage2_cache = (key, torso_warp.Stage2Weights(*mods, sp))
-        return self._stage2_cache[1]
+        return self.prepared('stage2', lambda: torso_warp.Stage2Weights(*mods, sp), sp, watch=mods)
 
     @property
     def _split(self) -> bool:
@@ -147,43 +136,34 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
 
     # ---- weight preparation ------------------------------------------------------------------------------------------------
     def _plain(self) -> Dict[str, tuple]:
+        return self.prepared('plain', self._build_plain, self._split)
+
+    def _build_plain(self) -> Dict[str, tuple]:
         sp = self._split
-        if self._plain_cache is None or self._plain_cache['split'] != sp:
-            te, bg, ff = self.torso_encoder, self.bg_encoder, self.fuse_fg_bg_convs
-            self._plain_cache = {
-                'split': sp,
-                'te': _pack_plain(te[0], 64, split=sp), 'bg0': _pack_plain(bg[0], 64, split=sp), 'bg2': _pack_plain(bg[2], 128, split=sp),
-                'bg4': _pack_plain(bg[4], 256, split=sp),
-                'ff0': _pack_plain(ff[0], self.fuse_in_dim, split=sp), 'ff2': _pack_plain(ff[2], 128, split=sp), 'ff4': _pack_plain(ff[4], 256, split=sp),
-            }
-            if self.fuse_mode in ('v2', 'v3'):
-                fh = self.fuse_head_torso_convs
-                self._plain_cache.update({'fh0': _pack_plain(fh[0], 512, split=sp), 'fh2': _pack_plain(fh[2], 256, split=sp)})
-            if self.fuse_mode == 'v3':                             # the mask predictor runs with split fp16 operands (its output is thresholded)
-                ap = self.head_torso_alpha_predictor
-                self._plain_cache.update({'ap0': sr_tc.pack_plain(ap[0], 64, split=True), 'ap2': sr_tc.pack_plain(ap[2], 128, split=True),
-                                          'ap4': sr_tc.pack_plain(ap[4], 128, split=True)})
-        return self._plain_cache
+        te, bg, ff = self.torso_encoder, self.bg_encoder, self.fuse_fg_bg_convs
+        P = {
+            'te': _pack_plain(te[0], 64, split=sp), 'bg0': _pack_plain(bg[0], 64, split=sp), 'bg2': _pack_plain(bg[2], 128, split=sp),
+            'bg4': _pack_plain(bg[4], 256, split=sp),
+            'ff0': _pack_plain(ff[0], self.fuse_in_dim, split=sp), 'ff2': _pack_plain(ff[2], 128, split=sp), 'ff4': _pack_plain(ff[4], 256, split=sp),
+        }
+        if self.fuse_mode in ('v2', 'v3'):
+            fh = self.fuse_head_torso_convs
+            P.update({'fh0': _pack_plain(fh[0], 512, split=sp), 'fh2': _pack_plain(fh[2], 256, split=sp)})
+        if self.fuse_mode == 'v3':                             # the mask predictor runs with split fp16 operands (its output is thresholded)
+            ap = self.head_torso_alpha_predictor
+            P.update({'ap0': sr_tc.pack_plain(ap[0], 64, split=True), 'ap2': sr_tc.pack_plain(ap[2], 128, split=True),
+                      'ap4': sr_tc.pack_plain(ap[4], 128, split=True)})
+        return P
 
     def prepare_styles(self, wsel: torch.Tensor) -> Dict:
-        """Folded + packed weights of block0/1 and head_torso_block for styles wsel [Nw,3,512].  Assign the result to
-        `static_prepared_warp` when the styles are constant (Real3D passes ws == 1): forward() then stops preparing them per call."""
+        """Folded + packed weights of block0/1 and head_torso_block for styles wsel [Nw,3,512] (with static_styles, prepared_styles()
+        keeps those of the all-ones styles)."""
         sp = self._split
         prep = {'main': sr_tc.Prepared(self, wsel, sp)}
         if self.fuse_mode in ('v2', 'v3'):
             prep.update({'ht0': sr_tc.pack_for(self.head_torso_block.conv0, wsel[:, 0], sp), 'ht1': sr_tc.pack_for(self.head_torso_block.conv1, wsel[:, 1], sp),
                          'htrgb': self.head_torso_block.torgb.folded_weight(wsel[:, 2])})
         return prep
-
-    def _load_from_state_dict(self, *a, **k):
-        # runs for THIS module whenever it or any parent (RenderHead, FrameEngine.load_params) loads a state_dict: every cache that was
-        # derived from the parameters is dropped (packed fp16 conv weights, per-clip constants, prepared styles)
-        self._plain_cache = None
-        self._clip_cache = None
-        self.static_prepared_warp = None
-        self._stage2_cache = None
-        self._motion_cache = None
-        return super()._load_from_state_dict(*a, **k)
 
     @staticmethod
     def _conv(x16: torch.Tensor, packed, act: int, split: bool = False) -> torch.Tensor:
@@ -207,7 +187,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         assert ref_torso_rgb.shape[0] == 1 and ref_bg_rgb.shape[0] == 1, 'one reference image per clip'
         plain, sp = self._plain(), self._split
         t256, b256 = self._aa_down2(ref_torso_rgb), self._aa_down2(ref_bg_rgb)
-        cc = {'ref_torso_256': t256, 'ref_bg_256': b256, 'x_bg': self._bg_features(b256, plain, sp), 'split': sp, 'batch': None, 'torso_app': None}
+        cc = {'ref_torso_256': t256, 'ref_bg_256': b256, 'x_bg': self._bg_features(b256, plain, sp), 'batch': None, 'torso_app': None}
         if segmap is not None and self.torso_stage2 == 'cuda':
             from . import torso_warp
             assert segmap.shape[0] == 1, 'one segmap per clip'
@@ -215,7 +195,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
         if batch is not None:
             cc['batch'] = (t256.expand(batch, -1, -1, -1).contiguous(), b256.expand(batch, -1, -1, -1).contiguous())
         old = self._clip_cache
-        if in_place and old is not None and old['split'] == sp and (old['batch'] is None) == (batch is None) and \
+        if in_place and old is not None and (old['batch'] is None) == (batch is None) and \
                 (batch is None or old['batch'][0].shape[0] == batch) and (old['torso_app'] is None) == (cc['torso_app'] is None) and \
                 (cc['torso_app'] is None or old['torso_app'].keys() == cc['torso_app'].keys()):
             for k in ('ref_torso_256', 'ref_bg_256', 'x_bg'):
@@ -227,11 +207,16 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
                 for dst, src in zip(old['batch'], cc['batch']):
                     dst.copy_(src)
             return True
-        self._clip_cache = cc
+        self.store('clip', cc, sp)
         return False
 
     def end_clip(self) -> None:
-        self._clip_cache = None
+        self.forget('clip')
+
+    @property
+    def _clip_cache(self) -> Optional[Dict]:
+        """The constants of the clip begun in the current sr_mode (None outside a clip)."""
+        return self.cached('clip', self._split)
 
     def _bg_features(self, ref_bg_256, plain, split: bool) -> torch.Tensor:
         """bg_encoder(ref_bg) on the tensor cores: [N,256,256,256] fp16 ([N,256,256,512] = [hi | lo] when split)."""
@@ -282,10 +267,8 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
             raise NotImplementedError('reference images must be 512x512 (antialiased 1/2 resize is the only down-scaling built)')
         ws3 = ws[:, -1:, :].expand(N, 3, -1)
         sp = self._split
-        prep = getattr(self, 'static_prepared_warp', None)
-        if prep is not None and prep['main'].split != sp:
-            prep = None
         with capi.region('sr_prep'):
+            prep = self.prepared_styles()
             if prep is None:
                 shared = N == 1 or getattr(self, 'assume_shared_styles', False)
                 prep = self.prepare_styles(ws3[:1] if shared else ws3)
@@ -305,9 +288,7 @@ class SuperresolutionHybrid8XDC_Warp(SuperresolutionHybrid8XDC):
                 rgb0 = self._resize(rgb, R) if rgb.shape[-1] != R else capi.f32(rgb)
                 rgb_256 = self._resize(rgb0, 256)
                 weights_256 = self._resize(weights_img.detach(), 256)
-            cc = self._clip_cache
-            if cc is not None and cc['split'] != sp:                    # begun in another sr_mode: run uncached
-                cc = None
+            cc = self._clip_cache                                        # None when begun in another sr_mode: run uncached
             if cc is None:
                 ref_torso_256, ref_bg_256 = self._aa_down2(ref_torso_rgb), self._aa_down2(ref_bg_rgb)
             elif cc['batch'] is not None and cc['batch'][0].shape[0] == N:  # per-clip constants, broadcast over the batch once per clip

@@ -16,6 +16,7 @@ import torch
 
 from . import _capi as capi
 from .decoder import FullyConnectedLayer
+from .prepared import PreparedMixin
 
 
 def setup_filter(f=(1, 3, 3, 1)) -> torch.Tensor:
@@ -174,7 +175,7 @@ class LargeSynthesisBlock1(torch.nn.Module):
         self.to_rgb = torch.nn.Conv2d(128, 3, kernel_size=1)
 
 
-class SuperresolutionHybrid8XDC(torch.nn.Module):
+class SuperresolutionHybrid8XDC(PreparedMixin, torch.nn.Module):
     def __init__(self, channels, img_resolution, sr_num_fp16_res, sr_antialias, large_sr=False, sr_mode='fp32', resblocks_in_large_sr=None,
                  **block_kwargs):
         """large_sr=True (superresolution.py:263-345) needs `resblocks_in_large_sr` (the reference reads hparams['resblocks_in_large_sr']) and
@@ -198,13 +199,23 @@ class SuperresolutionHybrid8XDC(torch.nn.Module):
                                          conv_clamp=None, **block_kwargs)
             self.block1 = SynthesisBlock(256, 128, w_dim=512, resolution=512, img_channels=3, is_last=True, use_fp16=False,
                                          conv_clamp=None, **block_kwargs)
-        self.static_prepared = None
-        self._large_cache = None
+        self.static_styles = False       # the caller passes constant styles (Real3D's ws == 1): the tensor-core path prepares them once
 
-    def _load_from_state_dict(self, *a, **k):
-        self.static_prepared = None          # prepared (folded + packed) weights belong to the parameters being replaced
-        self._large_cache = None
-        return super()._load_from_state_dict(*a, **k)
+    def prepare_styles(self, wsel: torch.Tensor):
+        """Folded + packed weights of the tensor-core path for styles wsel [Nw,3,512]."""
+        from . import sr_tc
+        return sr_tc.Prepared(self, wsel, self.sr_mode == 'tc_exact')
+
+    def prepared_styles(self):
+        """With static_styles on the tensor-core path: prepare_styles() of the all-ones styles, cached until the parameters are loaded or
+        moved; None otherwise (the styles are then prepared per call)."""
+        if not self.static_styles or self.sr_mode not in ('tc', 'tc_exact'):
+            return None
+
+        def build():
+            with torch.no_grad():
+                return self.prepare_styles(torch.ones(1, 3, 512, device=next(self.parameters()).device))
+        return self.prepared('styles', build, self.sr_mode == 'tc_exact')
 
     @staticmethod
     def _resize(x: torch.Tensor, size: int) -> torch.Tensor:
@@ -222,8 +233,7 @@ class SuperresolutionHybrid8XDC(torch.nn.Module):
             raise NotImplementedError('fused clamp / uint8 output is an option of the tensor-core SR path')
         rgb_from_x = bool(block_kwargs.pop('rgb_from_x', False))   # tensor-core path: the caller states rgb == x[:, :3] (one fused input launch)
         block_kwargs = {k: v for k, v in block_kwargs.items() if k != 'sr_mode'}
-        prep = self.static_prepared
-        if not (self.sr_mode in ('tc', 'tc_exact') and prep is not None and prep.split == (self.sr_mode == 'tc_exact')):     # prepared weights: the styles are not read again
+        if not (self.sr_mode in ('tc', 'tc_exact') and self.static_styles):     # prepared weights: the styles are not read again
             ws = ws[:, -1:, :].repeat(1, 3, 1)
         if x.shape[-1] > self.input_resolution:
             raise NotImplementedError('down-scaling inputs (antialiased) is not on the Real3D path')

@@ -96,7 +96,7 @@ def test_engine_graph_paths_match_eager_and_synthesis():
     engs = {'eager': _engine(use_graph=False), 'split': _engine(), 'whole': _engine(warper_in_graph=True), 'prepared': _engine()}
     for e in engs.values():
         e.begin_clip(*consts)
-    assert engs['split'].head.superresolution.static_prepared_warp is not None
+    assert engs['split'].head.superresolution.cached('styles', False) is not None
     ref = _run(engs['eager'], frames)
     got_split, got_whole = _run(engs['split'], frames), _run(engs['whole'], frames)
     assert isinstance(engs['split'].graph, engine._TorsoGraphs) and isinstance(engs['whole'].graph, torch.cuda.CUDAGraph)
